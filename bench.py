@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the forward hot path on B200, one BASELINE.json config per --workload.
+"""bench.py -- throughput of the forward hot path on H100, one BASELINE.json config per --workload.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -22,6 +22,8 @@ collective; one all-gather of the [B, classes] logits per step.  Prints ONE JSON
   cpu_baseline  the reference's own CPU forward on the host cores (oracle/_ref = the byte-compiled reference), bounded sample
 
 ``--impl reference`` times the reference's CPU fp32 forward itself (rank 0 only) on a bounded sample of the same workload.
+``--dump-outputs DIR`` writes what each timed forward returned in its last timed step to DIR/<workload>.npy (float32; see
+dump_output) so that two builds can be compared output for output: inputs and weights are seeded, identical from run to run.
 """
 import argparse
 import json
@@ -67,7 +69,30 @@ def load_peaks():
             pk = json.load(fh)
         return dict(hbm_gbs=pk["hbm_gbs"], tflops=pk.get("bf16_tflops_sustained", pk["bf16_tflops"]),
                     tflops_burst=pk["bf16_tflops"], source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, tflops_burst=1590.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 -- not reached, and a card with a lower
+    # power limit clocks down under sustained load
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_burst=989.0, source="fallback (H100 SXM data sheet)")
+
+
+DUMP_MAX_ELEMS = 4 << 20          # per output: 16 MB of float32, so the (at most four) dumps of one line stay under 64 MB
+
+
+def dump_output(args, name, t, max_elems=DUMP_MAX_ELEMS):
+    """--dump-outputs: write tensor ``t`` (what the timed path returned in its last step) to DIR/<name>.npy as float32.  An
+    output of more than ``max_elems`` elements is replaced by a fixed sample: the elements at ``max_elems`` sorted positions
+    drawn from a generator seeded with 0 (the same positions in every run of the same workload)."""
+    if not args.dump_outputs:
+        return
+    import numpy as np
+    import torch
+    flat = t.detach().float().reshape(-1)
+    if flat.numel() > max_elems:
+        idx = torch.randint(0, flat.numel(), (max_elems,), generator=torch.Generator().manual_seed(0)).sort().values
+        arr = flat[idx.to(flat.device)].cpu().numpy()
+    else:
+        arr = flat.cpu().numpy().reshape(tuple(t.shape))
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    np.save(os.path.join(args.dump_outputs, name + ".npy"), arr.astype(np.float32))
 
 
 class ClockSampler(threading.Thread):
@@ -337,10 +362,12 @@ def run_ours(args, spec, rank, world, local, secondary=False):
     for _ in range(args.steps):
         out = graphed()
         if world > 1:
-            parallel.gather_logits(out, total)
+            out = parallel.gather_logits(out, total)      # what a caller receives: the whole batch's logits, in batch order
     e1.record()
     barrier()
     clocks = sampler.stop() if sampler else None
+    if rank == 0:
+        dump_output(args, args.workload, out)
     ms = e0.elapsed_time(e1)
     t = torch.tensor([ms], dtype=torch.float64, device=dev)
     if world > 1:
@@ -398,7 +425,7 @@ def run_ours(args, spec, rank, world, local, secondary=False):
     if args.workload == DEFAULT_WORKLOAD and not secondary:
         del host_in
         x_keep = x_dev
-        sub_steps = max(5, min(args.steps, 20))
+        sub_steps = args.steps
         todo = ([] if args.no_biggan else ["biggan256"]) + ([] if args.no_others else ["r2plus1d34", "nonlocal50"])
         for name in todo:
             torch.cuda.empty_cache()
@@ -439,10 +466,10 @@ def run_ours(args, spec, rank, world, local, secondary=False):
     whole = spec["gflop"] * 1e9 * value / world / 1e12
     roofline.update({
         "kernel": "%s (%d launch per forward; %s)" % (top_desc, top["n"] // nrep, kernel_of(top_desc)),
-        "traffic": None,      # dram bytes need an ncu pass (profiles/ncu_traffic_r02.json); not measurable inside an un-profiled run
+        "traffic": None,      # dram bytes need a profiler pass; not measurable inside an un-profiled run
         "algorithmic_bytes": top["bytes"] / top["n"], "algorithmic_flop": top["flops"] / top["n"],
         "ms_per_launch": top["ms"] / top["n"], "share_of_step": top["ms"] / nrep / all_ms,
-        "family": {"kernels": "all %d tcgen05 conv / GEMM / attention launches of one forward" % (len(conv_rows) // nrep),
+        "family": {"kernels": "all %d tensor-core conv / GEMM / attention launches of one forward" % (len(conv_rows) // nrep),
                    "achieved": family_tflops, "frac": family_tflops / peaks["tflops"], "share_of_step": conv_ms / all_ms},
         "whole_step_tflops": whole, "whole_step_frac": whole / peaks["tflops"],
         "mixed": mixed_roofline(rows, nrep, peaks, ms_total / args.steps),
@@ -458,7 +485,7 @@ def run_ours(args, spec, rank, world, local, secondary=False):
                        spec["arch"], ("B=%d in total (%d per GPU)" % (total, B)) if strong else ("B=%d per GPU" % B),
                        "x".join(map(str, spec["sample"])), spec["config"]),
                    "global_batch": total, "parallelism": "dp%d" % world,
-                   "l2": "input (%.0f MB fp32) and the activations of one step (%.0f MB) exceed the 126 MB L2; no flush needed"
+                   "l2": "input (%.0f MB fp32) and the activations of one step (%.0f MB) exceed the 50 MB L2; no flush needed"
                          % (h2d_bytes / 1e6, spec["act_elems"] * 2 * B / 1e6),
                    "schedule": schedule,
                    "timing": "CUDA events around %d CUDA-graph replays, max over ranks" % args.steps},
@@ -617,10 +644,13 @@ def run_biggan(args, rank, world, local, emit=True, steps=None):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
-        graphed()
+        imgs = graphed()
     e1.record()
     barrier()
     clocks = sampler.stop() if sampler else None
+    # no collective on this path: each rank's caller receives its own shard of the images
+    # (the ranks share one output budget)
+    dump_output(args, "biggan256" if world == 1 else "biggan256_rank%d" % rank, imgs, DUMP_MAX_ELEMS // world)
     t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -693,7 +723,7 @@ def run_biggan(args, rank, world, local, emit=True, steps=None):
                                "(BASELINE.json configs[4]); architecture absent from the reference tree: parity is against "
                                "oracle/biggan.py (unpinned)" % (gflop, B),
                    "global_batch": B * world, "parallelism": "dp%d" % world,
-                   "l2": "activations of one step (tens of GB) exceed the 126 MB L2; no flush needed",
+                   "l2": "activations of one step (tens of GB) exceed the 50 MB L2; no flush needed",
                    "schedule": schedule,
                    "timing": "CUDA events around %d CUDA-graph replays, max over ranks" % steps},
         "clocks": clocks,
@@ -742,7 +772,7 @@ def kernel_of(desc):
     if desc.startswith("conv 1x1x1 s111") or desc.startswith("gemm"):
         return "pgemm_kernel"
     if desc.startswith("attention"):
-        return "nonlocal_attention_online_kernel"
+        return "nonlocal_attention_kernel"
     return "slabconv_kernel" if desc.startswith("conv") else "?"
 
 
@@ -760,6 +790,8 @@ def main():
     ap.add_argument("--no-others", action="store_true", help="skip the secondary r2plus1d34 / nonlocal50 measurements of the default line")
     ap.add_argument("--workload", default=DEFAULT_WORKLOAD, choices=list(WORKLOADS) + ["biggan256"],
                     help="which BASELINE.json config to time (default resnet3d50 = configs[1], the contract's line)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write each timed forward's output of the last timed step to DIR/<workload>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 

@@ -1,4 +1,4 @@
-/* b2_pretorched.h -- C ABI of the B200-native forward engine for pretorched-x's video-ConvNet hot path.
+/* b2_pretorched.h -- C ABI of the H100-native forward engine for pretorched-x's video-ConvNet hot path.
  *
  * The reference (alexandonian/pretorched-x @ 36a5754) has no FFI layer of its own: every FLOP of
  * its hot path is a torch.nn call inside a Python `forward` body.  Each entry point below therefore
@@ -14,7 +14,7 @@
  *     pitch `ld` (elements) a multiple of 8.  Channels in [C, ld) must be zero.
  *   - Returns 0 on success, a negative B2_ERR_* code otherwise; b2_last_error() returns a
  *     thread-local message.  No C++ exception crosses the ABI.
- *   - There is NO CPU fallback: on a machine without an sm_100 GPU every compute call fails with
+ *   - There is NO CPU fallback: on a machine without an sm_90 GPU every compute call fails with
  *     B2_ERR_CUDA / B2_ERR_UNSUPPORTED.
  */
 #ifndef B2_PRETORCHED_H_
@@ -41,7 +41,7 @@ const char* b2_last_error(void);
 uint64_t b2_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------
- * Convolution as implicit GEMM on tcgen05 tensor cores, with the eval-mode BatchNorm affine
+ * Convolution as implicit GEMM on wgmma tensor cores, with the eval-mode BatchNorm affine
  * (scale/shift), the residual add and the ReLU fused into the epilogue:
  *     y[m, k] = act( scale[k] * sum_{tap,c} x[m @ tap, c] * w[k, tap, c] + shift[k] + residual[m, k] )
  * Replaces nn.Conv3d -> nn.BatchNorm3d -> (+=residual) -> nn.ReLU chains at
@@ -145,7 +145,7 @@ typedef struct b2_gemm_args {
   int32_t aff2_ld, aff2_rows;
 } b2_gemm_args;
 int b2_gemm_f16(const b2_gemm_args* a, void* stream);
-/* D = act(scale * (A.B^T + A2.B2^T) + shift + residual): both products accumulate in the same TMEM tile.  Used to
+/* D = act(scale * (A.B^T + A2.B2^T) + shift + residual): both products accumulate in the same accumulator tile.  Used to
  * fuse the type-B shortcut projection (resnet3D.py:176-185) into the block-closing 1x1x1 convolution
  * (resnet3D.py:136-143) with the two BatchNorm scales folded into B and B2: the shortcut never touches HBM.
  * fp16 output, per-column affine only. */

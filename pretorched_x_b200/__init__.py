@@ -1,8 +1,8 @@
-"""pretorched_x_b200 -- B200-native forward engine for pretorched-x's video-ConvNet hot path.
+"""pretorched_x_b200 -- H100-native forward engine for pretorched-x's video-ConvNet hot path.
 
 Drop-in for the reference's factory API: ``pretorched_x_b200.__dict__[name](num_classes=..., pretrained=...)``
 returns a module with ``features / logits / forward / last_linear`` and the reference's ``state_dict`` layout
-(reference: pretorched/__init__.py:11-83).  The block bodies are hand-written sm_100a kernels reached through
+(reference: pretorched/__init__.py:11-83).  The block bodies are hand-written sm_90a kernels reached through
 the C ABI in ``include/b2_pretorched.h``; there is no CPU or library fallback.
 """
 from .__version__ import __version__  # noqa: F401

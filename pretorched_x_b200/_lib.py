@@ -1,8 +1,8 @@
 """ctypes binding of libb2pretorched.so -- the C-ABI boundary declared in include/b2_pretorched.h.
 
 This is the only place Python touches native code.  There is deliberately no fallback: if the shared
-library is missing it is built with nvcc (sm_100a); if that is impossible, or a compute entry point
-is called without a B200, a RuntimeError carrying b2_last_error() is raised.
+library is missing it is built with nvcc (sm_90a); if that is impossible, or a compute entry point
+is called without an H100, a RuntimeError carrying b2_last_error() is raised.
 """
 import ctypes
 import os

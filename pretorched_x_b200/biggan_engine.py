@@ -1,4 +1,4 @@
-"""BigGAN-deep generator forward on the B200 kernels (BASELINE.json configs[4]).
+"""BigGAN-deep generator forward on the H100 kernels (BASELINE.json configs[4]).
 
 There is no reference code for this path (SURVEY.md section 8a row a14): the block bodies below implement the published
 GBlock / SAGAN-attention / class-conditional-BN arithmetic restated in ``oracle/biggan.py`` (test infrastructure), on the
@@ -11,7 +11,7 @@ How the pieces map:
   + Wb y`` is an affine map per (sample, channel): ``scale = rstd + (rstd * Wg) y`` and ``shift = (Wb - m * rstd * Wg) y
   - m * rstd`` are both linear in the conditioning vector y, so the (spectrally normalised) gain / bias matrices of every
   ccbn are stacked, with ``rstd`` and the mean folded in, into one fp16 matrix ``[2 * sum(C)][3 * 256]`` and a single
-  tcgen05 GEMM with fp32 output produces every scale and shift of the network: ``aff[B][2 * sum(C)]`` (operands split
+  wgmma GEMM with fp32 output produces every scale and shift of the network: ``aff[B][2 * sum(C)]`` (operands split
   into fp16 hi + lo parts, K = 3 x 256, so the gains carry ~22 bits).
 * ccbn -> ReLU that FOLLOWS a convolution is that convolution's epilogue (per-sample affine, ``b2_conv_args.aff_ld``):
   conv2 carries bn3, conv3 carries bn4, conv1 carries bn2 (from 16x16 images on: a 128-row tile must stay inside one
@@ -20,10 +20,9 @@ How the pieces map:
   2x2 convolutions of the low-res image (one per output phase, filters summed when packed), which the slab kernel runs
   as 4 x 4 taps with a strided output write -- 2.25x fewer MACs and a quarter of the input bytes.
 * bn1 + ReLU of block i+1 CAN be a second output of block i's conv4 (or of the attention's output GEMM): a second epilogue
-  pass over the accumulator that is still in TMEM writes relu(ccbn1_next(h + skip)) next to h + skip (``next_affine``,
-  ``dual_output=True``).  Measured on B200 it does not pay -- these layers are write-bound and the second 2-byte-per-element
-  stream costs the 1x1 kernel as much as the stand-alone read+write pass it replaces (27.3 vs 26.5 ms per 256 images) -- so
-  it is off by default; the stand-alone ``b2_ccbn_act_ndhwc`` pass runs at ~5 TB/s.
+  pass over the accumulator tile writes relu(ccbn1_next(h + skip)) next to h + skip (``next_affine``,
+  ``dual_output=True``).  These layers are write-bound and the second 2-byte-per-element stream costs the 1x1 kernel about as
+  much as the stand-alone ``b2_ccbn_act_ndhwc`` read+write pass it replaces, so it is off by default.
 * conv4's epilogue adds the skip path: channel drop = the residual pitch, and for the upsampling block the epilogue reads
   the LOW-res x and upsamples on the fly (``residual_up``), so ``upsample(x)`` is never written either.
 * Tail: the output BatchNorm + ReLU is folded into the last block's conv4 (``residual_pre``: the skip joins before the
@@ -285,10 +284,9 @@ _DFS_SPEC = os.environ.get("B2_GAN_DFS", "off")
 
 
 def set_dfs(spec):
-    """Schedule of the generator's high-resolution tail: ``"off"`` (whole batch per launch: the default and the measured optimum,
+    """Schedule of the generator's high-resolution tail: ``"off"`` (whole batch per launch: the default,
     see ``engine.set_dfs``) or ``"res:images,res:images"`` -- modules whose OUTPUT resolution is at least ``res`` (up to the next
-    listed resolution) run depth-first on chunks of ``images``.  Measured at B = 256 (profiles/dfs_sweep_r02.txt): 22.5 ms whole
-    batch; the last block alone in chunks of 16 / 8 / 4 / 2 images: 23.1 / 23.8 / 24.4 / 25.8 ms."""
+    listed resolution) run depth-first on chunks of ``images``."""
     global _DFS_SPEC
     _DFS_SPEC = str(spec)
 
@@ -296,7 +294,7 @@ def set_dfs(spec):
 def dfs_plan(model, B, mods):
     """[(first module, end module, images per chunk)] covering a suffix of ``mods`` (empty = whole batch everywhere)."""
     spec = _DFS_SPEC.strip().lower()
-    if spec in ("0", "off", "none", "", "auto"):      # "auto" = the measured rule: never chunk
+    if spec in ("0", "off", "none", "", "auto"):      # "auto" = the default rule: never chunk
         return []
     levels = sorted(tuple(int(v) for v in part.split(":")) for part in spec.split(","))
     res, out_res = model.bottom_width, []
@@ -325,9 +323,9 @@ def generator_forward(model, z, y, out_dtype=torch.float32, stages=None, fuse_ou
     convolution writes relu(bn_out(.)) directly), so 'stage{last}' is only recorded when it is off; with ``split_head``
     (default) the RGB convolution runs as a 1x1 GEMM + gather and 'pre_tanh' is only recorded when it is off."""
     if model.training:
-        raise RuntimeError("the B200 engine is inference-only: call model.eval() (standing statistics, no SN update)")
+        raise RuntimeError("the H100 engine is inference-only: call model.eval() (standing statistics, no SN update)")
     if not z.is_cuda:
-        raise RuntimeError("the generator runs on a CUDA (sm_100a) device only: this engine has no CPU path")
+        raise RuntimeError("the generator runs on a CUDA (sm_90a) device only: this engine has no CPU path")
     dev = z.device
     pk = _packed(model, dev)
     B = z.shape[0]
@@ -369,7 +367,7 @@ def generator_forward(model, z, y, out_dtype=torch.float32, stages=None, fuse_ou
             stages['pre_tanh'] = t
         return ops.tanh_to_nchw(t, out_dtype, out=out)
 
-    # Optional depth-first tail (set_dfs; off by default -- measured slower, see engine.set_dfs): the modules of the listed
+    # Optional depth-first tail (set_dfs; off by default, see engine.set_dfs): the modules of the listed
     # resolutions run on chunks of images, every intermediate a write-then-read inside L2; chunk outputs land in their slice of the
     # next segment's input (or of the image tensor).  Not with ``stages`` (whole-batch stage tensors wanted) or ``dual_output``.
     plan = [] if (stages is not None or dual_output) else dfs_plan(model, B, mods)

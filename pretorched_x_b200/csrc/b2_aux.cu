@@ -309,7 +309,7 @@ __global__ void ncdhw_to_ndhwc_kernel(const TIn* __restrict__ x, __half* __restr
 }
 
 // Stem input, fp32 NCDHW with C <= 4 -> fp16 NDHWC4, four pixels per thread: one 16-byte load per channel plane and one 32-byte
-// store (the per-pixel version keeps 12 B of loads in flight per thread and tops out at ~4.4 TB/s; S % 4 == 0 and 16-byte aligned
+// store (the per-pixel version keeps only 12 B of loads in flight per thread; S % 4 == 0 and 16-byte aligned
 // planes are checked by the launcher).
 __global__ void __launch_bounds__(256)
 ncdhw_f32_to_ndhwc4_x4_kernel(const float* __restrict__ x, __half* __restrict__ y, int C, long long S, long long total_q) {

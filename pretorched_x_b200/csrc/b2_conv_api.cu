@@ -1,4 +1,4 @@
-// b2_conv_api.cu -- C-ABI entry points for the tcgen05 implicit-GEMM convolution and the dense GEMM,
+// b2_conv_api.cu -- C-ABI entry points for the wgmma implicit-GEMM convolution and the dense GEMM,
 // plus library-wide error/launch bookkeeping and the CUtensorMap builder.
 #include <atomic>
 #include <mutex>
@@ -31,16 +31,19 @@ int set_error(int code, const char* fmt, ...) {
 }
 void count_launch(int n) { g_launches.fetch_add(static_cast<uint64_t>(n), std::memory_order_relaxed); }
 
-int require_sm100() {
+int require_sm90() {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return set_error(B2_ERR_CUDA, "no CUDA device: %s", cudaGetErrorString(e));
   int major = 0;
   e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   if (e != cudaSuccess) return set_error(B2_ERR_CUDA, "cudaDeviceGetAttribute: %s", cudaGetErrorString(e));
-  if (major != 10)
-    return set_error(B2_ERR_UNSUPPORTED, "this library targets sm_100a (B200); device is sm_%d0 and there is no fallback",
-                     major);
+  int minor = 0;
+  e = cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (e != cudaSuccess) return set_error(B2_ERR_CUDA, "cudaDeviceGetAttribute: %s", cudaGetErrorString(e));
+  if (major != 9 || minor != 0)
+    return set_error(B2_ERR_UNSUPPORTED, "this library targets sm_90a (H100); device is sm_%d%d and there is no fallback",
+                     major, minor);
   return B2_OK;
 }
 
@@ -55,7 +58,7 @@ int sm_count() {               // per device ordinal (a process may drive severa
   const int dev = current_device() & 63;
   int n = cache[dev].load(std::memory_order_relaxed);
   if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cache[dev].store(n, std::memory_order_relaxed);
   }
   return n;
@@ -127,7 +130,8 @@ int make_tmap_ndhwc_slab(CUtensorMap* out, const void* base, uint64_t C, uint64_
 // slab convolution launcher (stride 1, "same" padding)
 // ------------------------------------------------------------------------------------------
 static int g_conv_algo = 0;   // 0 auto, 1 force gather (debug / A-B comparisons)
-static int g_slab_wide = -1;       // 256-column N tiles for channel counts that are multiples of 256: -1 rule below, 0 never, 1 always (tuning)
+static int g_slab_wide = -1;       // 1: request 256-column N tiles for channel counts that are multiples of 256 (tuning; they only run
+                                   // where their accumulator tile fits in shared memory), otherwise the 128-column rule
 static int g_slab_force_mt = -1;   // M tiles per slab work item: -1 read B2_SLAB_MT once, 0 cost model, > 0 forced (tuning)
 
 static int slab_naff(int ldy) { return (ldy + 31) / 32 * 32 + 256; }   // chunk reads may run past ldy inside the last N tile
@@ -233,7 +237,8 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.plane_stride = R * p.PW * 128;
   p.slab_bytes = ((R * p.PW * 128 * (p.mp > 1 ? p.mp : 1)) + 1023) / 1024 * 1024;
   p.MT = MT;
-  p.nacc = (MT * p.accs <= 256) ? 2 : 1;
+  const int smem_one = kSlabSStages * p.slab_bytes + kSlabWStages * p.wbytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024;
+  p.nacc = (smem_one + acc_bytes(2 * MT * p.accs) <= 227 * 1024) ? 2 : 1;
   p.Ncols = a->K;
   p.scale = a->scale; p.shift = a->shift;
   p.residual = reinterpret_cast<const __half*>(a->residual);
@@ -253,7 +258,7 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.fd_To = make_fastdiv(p.To); p.fd_PW = make_fastdiv(p.PW);
   if (a->aff_ld && ((a->aff_ld & 3) || (reinterpret_cast<uintptr_t>(a->scale) & 15) || (reinterpret_cast<uintptr_t>(a->shift) & 15)))
     return set_error(B2_ERR_INVALID, "per-sample scale/shift must be 16-byte aligned with a pitch that is a multiple of 4 floats");
-  const int smem_bytes = kSlabSStages * p.slab_bytes + kSlabWStages * p.wbytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024;
+  const int smem_bytes = smem_one + acc_bytes(p.nacc * MT * p.accs);
   B2_OPT_IN_SMEM(slabconv_kernel<BNT>, 227 * 1024);
   CUtensorMap tmX, tmB;
   int rc;
@@ -271,7 +276,7 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
 
 // Picks the N tile (fixed 64 / 128 or runtime), the M tiles per work item and the slab rows for a geometry; *best_mt == 0
 // when no configuration fits in shared memory.
-static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out, bool* flex_out, int* best_mt_out, int* best_R_out, bool wide = false) {
+static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out, bool* flex_out, int* best_mt_out, int* best_R_out) {
   int BN = (a->ldy <= 64) ? 64 : 128;
   const int planes = a->N * p.To;
   int ntn = (a->ldy + BN - 1) / BN;
@@ -281,7 +286,7 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   if (a->ldy > 128) {
     const int tn = (a->ldy + 255) / 256;
     const int bn = (((a->ldy + tn - 1) / tn) + 15) / 16 * 16;
-    if ((long long)bn * tn * 21 <= (long long)ntn * 128 * 20 || ((wide || g_slab_wide == 1) && a->ldy % 256 == 0)) {
+    if ((long long)bn * tn * 21 <= (long long)ntn * 128 * 20 || (g_slab_wide == 1 && a->ldy % 256 == 0)) {
       flex = true; BN = bn; ntn = tn;
       p.bn = bn; p.wbytes = (bn * 128 + 1023) / 1024 * 1024; p.accs = (bn + 31) / 32 * 32;
     }
@@ -294,8 +299,9 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   const int acc_stride = flex ? p.accs : BN;
   const int w_stage = flex ? p.wbytes : BN * 128;
   // Pick the M tiles per work item from a cycle model of one SM's share: rounds of items x the slower of the MMA
-  // stream and the slab/weight loads, plus the epilogue when a single accumulator set leaves it exposed.  (Constants
-  // from ncu: a 128xNx16 MMA retires in ~40 + N/2 cycles, TMA delivers ~48 B/cycle/SM out of L2.)
+  // stream and the slab/weight loads, plus the epilogue when shared memory holds a single accumulator set (the rule of
+  // launch_slab) and the epilogue is therefore exposed.  (Model constants:
+  // a 128xNx16 MMA retires in ~40 + N/2 cycles, TMA delivers ~48 B/cycle/SM out of L2; not re-fitted on H100.)
   int best_mt = 0, best_R = 0;
   double best_cost = 0.0;
   int& force_mt = g_slab_force_mt;
@@ -311,43 +317,42 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   const bool mp_ok = mp_env && p.P <= 128 && (a->kt == 1 || a->T == 1) && p.ss == 1 && !p.up && p.wchunks == 1 && planes > 1 &&
                      !a->aff_ld;      // (a per-sample affine is read once per item: its tiles must belong to one image)
   p.mp = 0;
-  for (int MT = 512 / acc_stride > 4 ? 4 : 512 / acc_stride; MT >= 1; --MT) {
+  for (int MT = 4; MT >= 1; --MT) {
     if (force_mt > 0 && MT != force_mt && MT != 1) continue;
     // (multi-plane: rows one plane's positions and taps can touch -- slab_rows assumes a full 128-position tile)
     const int R = mp_ok ? (p.P - 1 + p.reach) / p.PW + (p.reach + p.PW - 1) / p.PW + 1 : slab_rows(MT, p.PW, p.reach, p.P);
     if (p.ss * (R - 1) + 1 > 256) continue;
     const long long slab_b = ((long long)R * p.PW * 128 * (mp_ok ? MT : 1) + 1023) / 1024 * 1024;
-    const long long smem = 2ll * slab_b + kSlabWStages * w_stage + 256 + 2 * slab_naff(a->ldy) * 4 + 1024;
-    if (smem > 227 * 1024) continue;
+    const long long smem_one = 2ll * slab_b + kSlabWStages * w_stage + 256 + 2 * slab_naff(a->ldy) * 4 + 1024;
+    if (smem_one + acc_bytes(MT * acc_stride) > 227 * 1024) continue;
+    const bool two_sets = smem_one + acc_bytes(2 * MT * acc_stride) <= 227 * 1024;
     const long long tq = mp_ok ? 1 : (p.P + MT * 128 - 1) / (MT * 128);
     const long long items = (long long)ntn * tq * (mp_ok ? (planes + MT - 1) / MT : planes) * p.wchunks * (p.up ? 4 : 1);
     const double rounds = (double)((items + sm_count() - 1) / sm_count());
     const double tiles_per_item = mp_ok ? (double)MT : (double)((p.P + 127) / 128) / (double)tq;   // average (the last item of a plane is short)
-    // (A per-weight-tile issue floor of ~650 cycles was tried here after profiles/ncu_r02 showed the issuing warp, not the tensor
-    // pipe, pacing one-tile items with a narrow N; it moved the (1,3,3) C64->144 layer from MT = 1 with two accumulator sets to MT = 2
-    // with one, which measured 59 us instead of 44 us -- losing the epilogue overlap costs more than the amortised issue work gains.)
     const double mma = tiles_per_item * p.kt * taps_hw * ksteps * (40.0 + 0.5 * BN);
     // small planes: every SM streams the whole filter per item at the same time, and what bounds that is the aggregate L2 -> SM rate
-    // (~7 TB/s = 26 B/cycle/SM: 192 items x 884 KB in 25 us on the 7x7 C256->576 layer), not one SM's TMA rate
+    // (modelled as 26 B/cycle/SM), not one SM's TMA rate
     const double bpc = mp_ok ? 26.0 : 48.0;
     const double load = (double)p.kt * p.n_sub * p.cchunks * slab_b / bpc + (double)p.kt * taps_hw * p.cchunks * w_stage / bpc;
-    const double epi = (MT * acc_stride <= 256) ? 0.0 : tiles_per_item * ((BN + 31) / 32) * 250.0;
+    const double epi = two_sets ? 0.0 : tiles_per_item * ((BN + 31) / 32) * 250.0;
     const double cost = rounds * ((mma > load ? mma : load) + epi + 1500.0);
     if (force_mt == -1) {                                   // previous rule (A/B): largest power-of-two MT with >= 2 rounds of items
       if ((MT & (MT - 1)) != 0 && !flex) continue;
       best_mt = MT; best_R = R;
-      if (items >= 2 * 148) break;
+      if (items >= 2 * sm_count()) break;
       continue;
     }
     if (best_mt == 0 || cost < best_cost || (force_mt > 0 && MT == force_mt)) { best_mt = MT; best_R = R; best_cost = cost; }
     if (force_mt > 0 && MT == force_mt) break;
   }
-  if (mp_ok && best_mt >= 2 && best_mt < 4 && force_mt <= 0 && 4 * acc_stride <= 512) {
-    // measured (profiles/slab_mp_sweep_r02.txt): four planes per item beat two by ~10% as long as a full wave of items remains
+  if (mp_ok && best_mt >= 2 && best_mt < 4 && force_mt <= 0) {
+    // four planes per item share each weight tile twice as often as two, as long as a full wave of items remains
     const int R4 = (p.P - 1 + p.reach) / p.PW + (p.reach + p.PW - 1) / p.PW + 1;
     const long long slab4 = ((long long)R4 * p.PW * 128 * 4 + 1023) / 1024 * 1024;
     const long long items4 = (long long)ntn * ((planes + 3) / 4);
-    if (2ll * slab4 + kSlabWStages * w_stage + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 <= 227 * 1024 && items4 >= sm_count()) { best_mt = 4; best_R = R4; }
+    if (2ll * slab4 + kSlabWStages * w_stage + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 + acc_bytes(4 * acc_stride) <= 227 * 1024 &&
+        items4 >= sm_count()) { best_mt = 4; best_R = R4; }
   }
   p.mp = (mp_ok && best_mt > 1) ? best_mt : 0;
   *BN_out = BN; *flex_out = flex; *best_mt_out = best_mt; *best_R_out = best_R;
@@ -387,22 +392,7 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream) {
     if (g_conv_algo == 2 && q.ss != 1) return 0;              // debug: strided convs through the gather kernel
     int bn_c = 0, mt_c = 0, r_c = 0;
     bool flex_c = false;
-    double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c);
-    if (g_slab_wide < 0 && a->ldy % 256 == 0 && !flex_c) {
-      // 256-column N tiles (one A read per 256 output channels instead of per 128): measured with tools/conv_sweep.py
-      // (profiles/slab_wide_sweep_r02.txt) they win by 5-35% wherever at least 64 work items of at least two M tiles remain, and lose
-      // when halving the number of N tiles leaves SMs idle (M = 6272: 33 -> 41 us) or an item is a single tile (7x7 planes: 23 -> 29 us)
-      SlabParams qw = q;
-      int bn_w = 0, mt_w = 0, r_w = 0;
-      bool flex_w = false;
-      const double cost_w = slab_pick_tiles(a, qw, &bn_w, &flex_w, &mt_w, &r_w, true);
-      if (mt_w != 0 && flex_w) {
-        const long long tq = (qw.P + mt_w * 128 - 1) / (mt_w * 128);
-        const long long items_w = (long long)((a->ldy + bn_w - 1) / bn_w) * tq * a->N * qw.To * qw.wchunks * (qw.up ? 4 : 1);
-        const double tiles_per_item = (double)((qw.P + 127) / 128) / (double)tq;
-        if (items_w >= 64 && tiles_per_item >= 2.0) { q = qw; bn_c = bn_w; flex_c = flex_w; mt_c = mt_w; r_c = r_w; cost = cost_w * 0.8; }
-      }
-    }
+    const double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c);
     if (mt_c == 0) continue;
     if (best_mt == 0 || cost < best_cost) { best_p = q; BN = bn_c; flex = flex_c; best_mt = mt_c; best_R = r_c; best_cost = cost; }
   }
@@ -423,11 +413,9 @@ static int try_slabts(const b2_conv_args* a, cudaStream_t stream) {
   if (!g_slabts || g_conv_algo != 0) return 0;
   if (a->mode != B2_CONV_AUTO || a->out_f32 || a->upsample || a->aff_ld || a->y2 || a->residual_up || a->residual_pre || a->in_scale) return 0;
   if (a->kt != 3 || a->st != 1 || a->pt != 1 || a->sh != 1 || a->sw != 1 || a->ldy > 64 || a->T < 3) return 0;
-  // Measured (CUDA-graph replays, profiles/README_r02.md): 180 vs 186 us on the 3x3x3 C64->64 layer of resnet3d50 -- the operand
-  // traffic it saves in shared memory comes back as 2.5x more weight bytes per output tile from L2 (one 24 KB stack per tap and input
-  // frame, two M tiles per item) -- and it LOSES where the single accumulator set exposes a residual read (243 vs 190 us) or the
-  // in-plane filter is 1x1 (the (3,1,1) convolutions of R(2+1)D: 64 vs 31 us against the frames-as-rows remap).  So: true 3-D
-  // filters without a residual only.
+  // The operand traffic it saves in shared memory comes back as 2.5x more weight bytes per output tile from L2 (one 24 KB stack per
+  // tap and input frame), the single accumulator set exposes a residual read, and with a 1x1 in-plane filter the frames-as-rows remap
+  // of the slab kernel has less to gain from.  So: true 3-D filters without a residual only.
   if (a->kh * a->kw < 9 || a->residual) return 0;
   SlabParams p;
   if (!slab_geometry(a, &p, 0) || p.n_sub != 1) return 0;
@@ -436,7 +424,7 @@ static int try_slabts(const b2_conv_args* a, cudaStream_t stream) {
   for (; MT >= 1; --MT) {
     R = slab_rows(MT, p.PW, p.reach, p.P);
     const long long slab_b = ((long long)R * p.PW * 128 + 1023) / 1024 * 1024;
-    smem = kSlabSStages * slab_b + kSlabWStages * kTsWBytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024;
+    smem = kSlabSStages * slab_b + kSlabWStages * kTsWBytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 + acc_bytes(MT * kTsGroup * kTsBN);
     if (R <= 256 && smem <= 227 * 1024) break;
   }
   if (MT < 1) return 0;
@@ -487,7 +475,7 @@ static bool tstack_plan(const b2_conv_args* a, TstackParams* out, size_t* smem_o
     return false;
   const int cchunks = (a->C + 63) / 64;
   const long long wbytes = (long long)cchunks * a->kt * kTkWBlock;
-  if (wbytes > 144 * 1024) return false;                     // the filter must stay resident next to the A ring
+  if (wbytes > 112 * 1024) return false;                     // the filter must stay resident next to the A ring and the accumulators
   const long long HW = (long long)a->H * a->W;
   if (HW >= (1ll << 24)) return false;
   TstackParams p;
@@ -498,8 +486,7 @@ static bool tstack_plan(const b2_conv_args* a, TstackParams* out, size_t* smem_o
   p.tiles_q = (int)((HW + 127) / 128);
   const long long items = (long long)a->N * p.groups * p.tiles_q;
   if (items >= (1ll << 31)) return false;
-  // Below one work item per SM the frames-as-rows form of the slab kernel (more, smaller items) keeps more SMs busy
-  // (2 clips of the (3,1,1) C144 layer, 56 items: 9.6 vs 11.0 us, profiles/tstack_sweep_r02.txt).
+  // Below one work item per SM the frames-as-rows form of the slab kernel (more, smaller items) keeps more SMs busy.
   if (g_tstack < 0 && items < sm_count()) return false;
   p.items_total = (int)items;
   p.Ncols = a->K; p.ldy = a->ldy; p.ldr = a->ldr; p.relu = a->relu;
@@ -508,7 +495,7 @@ static bool tstack_plan(const b2_conv_args* a, TstackParams* out, size_t* smem_o
   p.y = reinterpret_cast<__half*>(a->y);
   p.fd_tiles_q = make_fastdiv(p.tiles_q); p.fd_groups = make_fastdiv(p.groups);
   *out = p;
-  *smem_out = 1024 + (size_t)kTkStages * kTkABytes + (size_t)wbytes + 128 + 512 + 64;
+  *smem_out = 1024 + (size_t)kTkStages * kTkABytes + (size_t)wbytes + 128 + 512 + acc_bytes(kTkSetCols);
   return true;
 }
 
@@ -545,7 +532,7 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   p.Ho = (a->H + 2 * a->ph - a->kh) / 2 + 1;
   p.Wo = (a->W + 6 - 7) / 2 + 1;
   p.kt = a->kt; p.kh = a->kh; p.pt = a->pt; p.ph = a->ph;
-  p.G = 256 / BN;
+  p.G = kStemAccCols / BN;
   p.rows = 2 * (p.G - 1) + a->kh;
   if (p.rows > kStemMaxRows) return set_error(B2_ERR_UNSUPPORTED, "stem kernel height %d too large", a->kh);
   for (int i = 0; i < p.rows; ++i) {
@@ -559,7 +546,7 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   }
   p.w_bytes = a->kh * BN * 64;
   p.stage_bytes = ((p.rows * kStemPitch + p.w_bytes) + 127) / 128 * 128;
-  const int tail_bytes = 128 + 2048 + 1024 + 256;     // barriers, scale / shift, W-pool exchange slots
+  const int tail_bytes = 128 + 2048 + 1024 + acc_bytes(2 * kStemAccCols) + 256;   // barriers, scale / shift, W-pool exchange slots, accumulators
   p.nstages = (227 * 1024 - tail_bytes) / p.stage_bytes;
   if (p.nstages > kStemMaxStages) p.nstages = kStemMaxStages;
   if (p.nstages < 1) return set_error(B2_ERR_UNSUPPORTED, "stem slab does not fit in shared memory (kh=%d)", a->kh);
@@ -660,7 +647,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------
 // small-M path: dense-M implicit GEMM, split-K over a thread-block cluster (b2_densem.cuh)
 // ------------------------------------------------------------------------------------------
-// Which layers take the dense-M kernel (measured with tools/conv_sweep.py as CUDA-graph replays, profiles/smallm_sweep_r02.txt):
+// Which layers take the dense-M kernel (tools/conv_sweep.py times single layers as CUDA-graph replays to re-check the rule):
 // it beats the slab kernel only where a plane fills a small part of a 128-row tile AND the K loop is long enough to split --
 // stride-1 multi-tap convolutions with M <= 1024 output positions (4x4 planes: 12% tile fill), strided multi-tap convolutions
 // (whose slab form needs four phase sub-images per tap) with M <= 8192.  1x1x1 convolutions stay on the persistent GEMM.
@@ -681,8 +668,9 @@ static bool densem_wanted(long long M, int taps, bool strided) {
   return strided ? M <= 8192 : M <= 1024;
 }
 
-// N tile (multiple of 32, <= 256, least padding then widest) and cluster size S (bn / S a multiple of 32, >= 2 K blocks per CTA):
-// the smallest S that gives every SM a work unit, else the largest admissible one.
+// N tile (multiple of 32, <= 128, least padding then widest) and cluster size S (bn / S a multiple of 32, >= 2 K blocks per CTA):
+// the smallest S that gives every SM a work unit, else the largest admissible one.  128 columns at most: the shared-memory
+// accumulator tile of a wider N tile leaves too little room for the operand ring and for the peers' partials, which alias it.
 static bool densem_split_ok(int bn, int S, int nkb) {      // bn / S a multiple of 32 and every CTA of the cluster gets >= 1 K block
   if (S < 1 || bn % (32 * S) != 0 || S > nkb) return false;
   const int per = (nkb + S - 1) / S;
@@ -690,8 +678,8 @@ static bool densem_split_ok(int bn, int S, int nkb) {      // bn / S a multiple 
 }
 static int g_densem_force_s = -1;
 static void densem_plan(int M, int ldy, int nkb, int* bn_out, int* S_out) {
-  int best_bn = 256, best_waste = 1 << 30;
-  for (int bn = 256; bn >= 64; bn -= 32) {
+  int best_bn = 128, best_waste = 1 << 30;
+  for (int bn = 128; bn >= 64; bn -= 32) {
     const int tn = (ldy + bn - 1) / bn;
     const int waste = tn * bn - ldy;
     if (waste < best_waste) { best_waste = waste; best_bn = bn; }
@@ -704,7 +692,7 @@ static void densem_plan(int M, int ldy, int nkb, int* bn_out, int* S_out) {
     if (!densem_split_ok(best_bn, cand, nkb) || (cand > 1 && nkb / cand < 2)) continue;
     if (g_densem_force_s > 0) { if (cand <= g_densem_force_s) S = cand; continue; }
     S = cand;
-    if (tiles * cand >= 64) break;                  // measured: beyond ~half the SMs the cluster / DSMEM cost outgrows the gain
+    if (tiles * cand >= 64) break;                  // beyond ~half the SMs the cluster / DSMEM cost outgrows the gain
   }
   *bn_out = best_bn; *S_out = S;
 }
@@ -718,12 +706,12 @@ static int launch_densem(const IgemmLaunch& L, cudaStream_t stream) {
   int bn = 0, S = 1;
   densem_plan(p.M_total, width, p.nkb, &bn, &S);
   dp.bn = bn; dp.bbytes = bn * 128; dp.stage_bytes = kBM * kBK * 2 + dp.bbytes;
-  dp.tmem_cols = bn <= 32 ? 32 : bn <= 64 ? 64 : bn <= 128 ? 128 : 256;
   dp.ksplit = S;
   dp.kb_per = (p.nkb + S - 1) / S;
-  dp.nstages = (227 * 1024 - 256 - 1024) / dp.stage_bytes;
+  dp.nstages = (227 * 1024 - 256 - 1024 - acc_bytes(bn)) / dp.stage_bytes;
   if (dp.nstages > kDmMaxStages) dp.nstages = kDmMaxStages;
-  const int smem_bytes = dp.nstages * dp.stage_bytes + 256 + 1024;
+  dp.acc_off = dp.nstages * dp.stage_bytes + 256;
+  const int smem_bytes = dp.acc_off + acc_bytes(bn) + 1024;
   B2_OPT_IN_SMEM(densem_kernel, 227 * 1024);
   CUtensorMap tmA, tmB;
   int rc;
@@ -814,10 +802,9 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
 static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   if (g_gemm_algo == 0 && densem_applies(L.p, L.k2)) return launch_densem(L, stream);
   if (g_gemm_algo == 0 && L.p.amode == AMODE_TMA && L.p.epi == EPI_TMA_F16 && !L.p.per_row) {
-    if (L.p.y2) return launch_pgemm<64, 1>(L, stream);       // second output: the 64-wide instance has a second staging tile
-    if (L.p.res_up || L.p.res_pre || L.p.in_scale)
-      return L.p.ldy <= 64 ? launch_pgemm<64, 1>(L, stream) : launch_pgemm<128, 1>(L, stream);
-    return L.p.ldy <= 64 ? launch_pgemm<64, 0>(L, stream) : launch_pgemm<128, 0>(L, stream);
+    // 64-wide N tiles only (see b2_pgemm.cuh: the accumulator tiles of a 128-wide instance do not fit in shared memory)
+    if (L.p.y2 || L.p.res_up || L.p.res_pre || L.p.in_scale) return launch_pgemm<64, 1>(L, stream);
+    return launch_pgemm<64, 0>(L, stream);
   }
   if (L.p.aff_ld)
     return set_error(B2_ERR_UNSUPPORTED, "per-sample affine is implemented by the slab convolution and the persistent GEMM only");
@@ -875,7 +862,7 @@ int b2_debug_slab_plan(const b2_conv_args* a_in, int* out) {
   return B2_OK;
 }
 /* debug knobs of the small-M path: layers with M <= maxm take the dense-M kernel (0 = never); force_s > 0 caps the cluster size */
-int b2_debug_set_slab_wide(int on) { g_slab_wide = on; return B2_OK; }   /* -1 rule, 0 never, 1 always */
+int b2_debug_set_slab_wide(int on) { g_slab_wide = on; return B2_OK; }   /* 1: request 256-column tiles; -1 / 0: the rule */
 /* host-only view of the temporal stack kernel's decision for a convolution (no launch, no GPU needed): out = {applies, items, frame
    groups per clip, position tiles per frame, channel chunks, resident filter bytes, dynamic shared memory bytes} */
 int b2_debug_tstack_plan(const b2_conv_args* a, int* out) {
@@ -940,7 +927,7 @@ static int validate_conv(const b2_conv_args* a) {
 int b2_conv_ndhwc_fprop(const b2_conv_args* a, void* stream) {
   int rc = validate_conv(a);
   if (rc != B2_OK) return rc;
-  if ((rc = require_sm100()) != B2_OK) return rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
   const long long M_out = (long long)a->N * conv_out_dim(a->T, a->kt, a->st, a->pt) * conv_out_dim(a->H, a->kh, a->sh, a->ph) *
                           conv_out_dim(a->W, a->kw, a->sw, a->pw);
   const bool small_m = a->mode == B2_CONV_AUTO && !a->upsample && !a->aff_ld && !a->out_f32 && !a->y2 && !a->residual_up &&
@@ -1047,7 +1034,7 @@ static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const vo
     B2_CHECK_ARG(g->residual == nullptr || (g->ldr % 8 == 0 && g->ldr >= g->N), "bad residual pitch");
   }
   int rc;
-  if ((rc = require_sm100()) != B2_OK) return rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
 
   IgemmLaunch L;
   memset(&L, 0, sizeof(L));

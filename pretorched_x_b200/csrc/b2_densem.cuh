@@ -1,7 +1,7 @@
 // b2_densem.cuh -- dense-M implicit GEMM with split-K across a thread-block cluster, for the SMALL-M regime.
 //
 // The slab kernel (b2_slabconv.cuh) tiles one (n, t) plane at a time: a 7x7 plane fills 49 of the 128 rows of an MMA tile and a
-// 4x4 plane 16 of them, and a layer with M = N*T*H*W of a few thousand positions yields far fewer work items than the 148 SMs --
+// 4x4 plane 16 of them, and a layer with M = N*T*H*W of a few thousand positions yields far fewer work items than the 132 SMs --
 // the late stages of every video net here (resnet3d50 layer3/4, all of R(2+1)D-34 beyond layer2, everything at 2 clips per GPU).
 // Those layers are bound by streaming their WEIGHTS (2.6 - 10.6 MB per launch) through few SMs.  This kernel:
 //   * packs output positions densely: tile row r is output pixel m0 + r whatever plane it lies in (im2col gather by cp.async,
@@ -10,24 +10,25 @@
 //     the weights, so tiles x S >= #SMs work units exist even for a 4-tile layer;
 //   * reduces the S partial accumulators through distributed shared memory, reduce-scatter style: CTA r owns the column slice
 //     [r*bn/S, (r+1)*bn/S) of the tile; every peer writes its partial of that slice into r's shared memory
-//     (st.shared::cluster), one cluster barrier later r adds them to its own TMEM partial, applies BN / residual / ReLU and
+//     (st.shared::cluster), one cluster barrier later r adds them to its own partial, applies BN / residual / ReLU and
 //     stores the slice.  No global workspace, no second pass, no atomics; the epilogue work is spread over all S CTAs.
-// Operands as everywhere else: fp16, K-major SWIZZLE_128B tiles, fp32 accumulation in TMEM, one elected MMA-issuing lane.
+// Operands as everywhere else: fp16, K-major SWIZZLE_128B tiles, fp32 accumulation in a shared-memory AccTile, one MMA warpgroup.
 #pragma once
 
 #include "b2_igemm.cuh"
 
 namespace b2 {
 
-constexpr int kDmThreads = 192;    // warps 0-3: A gather producers, then epilogue; warp 4: TMA producer; warp 5: MMA issuer
+constexpr int kDmThreads = 288;    // warps 0-3: A gather producers, then epilogue; warps 4-7: MMA warpgroup; warp 8: TMA producer
+constexpr int kDmTmaWarp = 8;
 constexpr int kDmMaxStages = 6;
 
 struct DensemParams {
   IgemmParams g;           // geometry / epilogue description shared with the gather kernel (epi is ignored: direct stores)
-  int bn;                  // N per tile (multiple of 32, <= 256); bn / ksplit is a multiple of 32
+  int bn;                  // N per tile (multiple of 32, <= 128); bn / ksplit is a multiple of 32
   int bbytes;              // weight stage bytes: bn * 128
   int stage_bytes;         // 16 KB (A) + bbytes, multiple of 1024
-  int tmem_cols;           // power of two >= bn
+  int acc_off;             // byte offset of the AccTile (bn columns) behind the ring and the barriers
   int ksplit;              // cluster size along K (gridDim.z)
   int kb_per;              // K blocks per CTA (the last CTA may get fewer)
   int nstages;             // operand ring depth (as many as fit: the loop is latency-bound, bytes in flight are what count)
@@ -62,8 +63,8 @@ densem_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C
   const int ring_bytes = kDmStages * dp.stage_bytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + ring_bytes);
   uint64_t* empty_bar = full_bar + kDmMaxStages;
-  uint64_t* tmem_full_bar = empty_bar + kDmMaxStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+  uint64_t* acc_full_bar = empty_bar + kDmMaxStages;
+  const AccTile at{reinterpret_cast<float*>(smem + dp.acc_off), acc_ld(dp.bn)};
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int bn = dp.bn;
@@ -77,16 +78,12 @@ densem_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C
 
   if (tid == 128) {
     for (int s = 0; s < kDmStages; ++s) { mbar_init(&full_bar[s], gather ? (128 + 1) : 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(tmem_full_bar, 1);
+    mbar_init(acc_full_bar, 1);
     fence_mbar_init();
     tma_prefetch_desc(&tmB);
     if (!gather) tma_prefetch_desc(&tmA);
   }
-  if (warp == 5) { tmem_alloc(tmem_slot, static_cast<uint32_t>(dp.tmem_cols)); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();
 
@@ -132,7 +129,7 @@ densem_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C
         }
       }
     }
-  } else if (warp == 4) {
+  } else if (warp == kDmTmaWarp) {
     // ================================ TMA producer ======================================
     const uint32_t tx = static_cast<uint32_t>(dp.bbytes) + (gather ? 0u : static_cast<uint32_t>(kBM * kBK * 2));
     for (int i = 0; i < nkb_here; ++i) {
@@ -153,40 +150,30 @@ densem_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C
       __syncwarp();
     }
   } else {
-    // ================================ MMA issuer ========================================
-    const uint32_t idesc = make_idesc_f16(kBM, static_cast<uint32_t>(bn), 0);
-    const uint32_t tm = warp_uniform(tmem_base);
+    // ================================ MMA warpgroup =====================================
     const uint32_t ring = smem_u32(smem);
     for (int i = 0; i < nkb_here; ++i) {
       const int s = i % kDmStages;
       mbar_wait(&full_bar[s], (i / kDmStages) & 1);
-      tc_fence_after();
       if (gather) fence_proxy_async();
       const uint32_t a_lo = sw128_desc_lo(ring + s * dp.stage_bytes);
       const uint32_t b_lo = sw128_desc_lo(ring + s * dp.stage_bytes + kBM * kBK * 2);
-      if (elect_one()) {
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo), idesc, i != 0 ? 1u : 0u);
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo + 2), desc_from(kSw128DescHi, b_lo + 2), idesc, 1u);
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo + 4), desc_from(kSw128DescHi, b_lo + 4), idesc, 1u);
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo + 6), desc_from(kSw128DescHi, b_lo + 6), idesc, 1u);
-        umma_commit(&empty_bar[s]);
-        if (i == nkb_here - 1) umma_commit(tmem_full_bar);
-      }
-      __syncwarp();
+      wg_mma(at, 0, bn, wg_sw128(desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo)), 4, i != 0);
+      wg_sync();
+      wg_arrive(&empty_bar[s]);
+      if (i == nkb_here - 1) wg_arrive(acc_full_bar);
     }
-    if (nkb_here == 0 && elect_one()) mbar_arrive(tmem_full_bar);      // (cannot happen: the host gives every CTA >= 1 block)
+    if (nkb_here == 0) wg_arrive(acc_full_bar);      // (cannot happen: the host gives every CTA >= 1 block)
   }
 
   // ---- everyone: this CTA's partial accumulator is complete (its operand ring is no longer read) ----
-  mbar_wait(tmem_full_bar, 0);
-  tc_fence_after();
+  mbar_wait(acc_full_bar, 0);
   const int S = dp.ksplit;
   const int slice = bn / S;                         // columns this CTA finalises (multiple of 32)
   float* stage = reinterpret_cast<float*>(smem);    // [S - 1][128][slice] fp32 partials from the peers, aliasing the ring
   if (S > 1) {
     cluster_sync_all();                             // B0: every CTA of the cluster is done with its ring -> safe to overwrite
     if (warp < 4) {
-      const uint32_t lane_taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
       for (int peer = 0; peer < S; ++peer) {
         if (peer == static_cast<int>(rank)) continue;
         const int slot = static_cast<int>(rank) < peer ? static_cast<int>(rank) : static_cast<int>(rank) - 1;   // my slot in the peer's staging area
@@ -195,8 +182,7 @@ densem_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C
                                            static_cast<uint32_t>(peer));
         for (int c = 0; c < slice; c += 32) {
           uint32_t v[32];
-          tmem_ld32(lane_taddr + peer * slice + c, v);
-          tmem_ld_wait();
+          acc_ld32(at, tid, peer * slice + c, v);
 #pragma unroll
           for (int q = 0; q < 8; ++q)
             st_cluster_v4(remote + static_cast<uint32_t>(c / 4 + q) * (kBM * 16u), v[q * 4], v[q * 4 + 1], v[q * 4 + 2], v[q * 4 + 3]);
@@ -211,12 +197,10 @@ densem_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C
     const int r = tid;
     const int m = m0 + r;
     const bool row_ok = m < p.M_total;
-    const uint32_t lane_taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
     const int col0 = static_cast<int>(rank) * slice;              // first tile column of my slice
     for (int c = 0; c < slice; c += 32) {
       uint32_t v[32];
-      tmem_ld32(lane_taddr + col0 + c, v);
-      tmem_ld_wait();
+      acc_ld32(at, r, col0 + c, v);
       float acc[32];
 #pragma unroll
       for (int i = 0; i < 32; ++i) acc[i] = __uint_as_float(v[i]);
@@ -275,9 +259,6 @@ densem_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, static_cast<uint32_t>(dp.tmem_cols));
 }
 
 }  // namespace b2

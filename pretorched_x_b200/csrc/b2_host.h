@@ -65,7 +65,7 @@ int make_tmap_2d_f16(CUtensorMap* out, const void* base, uint64_t inner, uint64_
 int make_tmap_ndhwc_slab(CUtensorMap* out, const void* base, uint64_t C, uint64_t W, uint64_t H, uint64_t planes,
                          uint32_t box_w, uint32_t box_h, uint32_t stride_hw, uint32_t box_planes = 1);
 
-int require_sm100();
+int require_sm90();
 
 // Launch with programmatic stream serialization (see pdl_wait() in b2_ptx.cuh).  B2_PDL=0 in the environment turns
 // the attribute off (A/B measurements).

@@ -1,14 +1,14 @@
-// b2_igemm.cuh -- implicit-GEMM convolution / GEMM on tcgen05 with a fused BN/residual/ReLU epilogue.
+// b2_igemm.cuh -- implicit-GEMM convolution / GEMM on wgmma with a fused BN/residual/ReLU epilogue.
 //
 //   D[M][N] = act( scale * (A_im2col[M][Ktot] . W[N][Ktot]^T) + shift + residual )
 //
-// One CTA computes one 128 x BN output tile.  6 warps:
+// One CTA computes one 128 x BN output tile.  9 warps:
 //   warps 0-3  A producers in gather mode (cp.async im2col, one output row per thread), then
-//              the epilogue (thread = accumulator row = TMEM lane)
-//   warp  4    TMA producer (weights always; activations too in AMODE_TMA)
-//   warp  5    TMEM allocation + the single MMA-issuing thread
+//              the epilogue (thread = accumulator row)
+//   warps 4-7  MMA warpgroup (wgmma)
+//   warp  8    TMA producer (weights always; activations too in AMODE_TMA)
 // K is consumed in blocks of 64 fp16 (one 128-byte swizzle row) through a STAGES-deep smem ring
-// guarded by full/empty mbarriers; accumulators live in TMEM (BN fp32 columns x 128 lanes).
+// guarded by full/empty mbarriers; accumulators live in a shared-memory AccTile (BN fp32 columns x 128 rows).
 //
 // smem tiles use the canonical K-major SWIZZLE_128B layout: row r at r*128 B, 16-byte chunk j of a
 // row stored at chunk (j ^ (r & 7)).  TMA produces that layout natively; the gather producers
@@ -22,7 +22,9 @@ namespace b2 {
 constexpr int kBM = 128;     // output rows (pixels) per CTA
 constexpr int kBK = 64;      // K elements per pipeline stage
 constexpr int kStages = 3;   // smem ring depth
-constexpr int kThreads = 192;
+constexpr int kThreads = 288;
+constexpr int kIgMmaWarp0 = 4;
+constexpr int kIgTmaWarp = 8;
 
 enum : int { AMODE_TMA = 0, AMODE_GATHER = 1 };
 enum : int { EPI_TMA_F16 = 0, EPI_DIRECT_F16 = 1, EPI_DIRECT_F32 = 2 };
@@ -72,7 +74,8 @@ struct IgemmSmem {
   static constexpr int kCTileBytes = kBM * BN * 2;
   static_assert(2 * kCTileBytes <= kRingBytes, "epilogue staging must fit in the ring");
   static constexpr int kBarOffset = kRingBytes;          // barriers + scale/shift after the ring
-  static constexpr int kTotalBytes = kRingBytes + 256 + 2 * BN * 4 + 2 * kBM * 4 + 1024 /*align slack*/;
+  static constexpr int kAccOffset = kRingBytes + 256 + 2 * BN * 4 + 2 * kBM * 4;
+  static constexpr int kTotalBytes = kAccOffset + acc_bytes(BN) + 1024 /*align slack*/;
 };
 
 template <int BN>
@@ -89,9 +92,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
 
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full_bar = empty_bar + kStages;
-  uint64_t* res_bar = tmem_full_bar + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_bar + 1);
+  uint64_t* acc_full_bar = empty_bar + kStages;
+  uint64_t* res_bar = acc_full_bar + 1;
+  const AccTile acc{reinterpret_cast<float*>(smem + S::kAccOffset), acc_ld(BN)};
   float* s_scale = reinterpret_cast<float*>(smem + S::kBarOffset + 256);
   float* s_shift = s_scale + (BN > kBM ? BN : kBM);  // per-column needs BN entries, per-row kBM
 
@@ -107,15 +110,11 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
       mbar_init(&full_bar[s], gather ? (128 + 1) : 1);
       mbar_init(&empty_bar[s], 1);
     }
-    mbar_init(tmem_full_bar, 1);
+    mbar_init(acc_full_bar, 1);
     mbar_init(res_bar, 1);
     fence_mbar_init();
     tma_prefetch_desc(&tmB);
     if (!gather) tma_prefetch_desc(&tmA);
-  }
-  if (warp == 5) {
-    tmem_alloc(tmem_slot, BN);   // BN fp32 accumulator columns (power of two >= 32)
-    tmem_relinquish();
   }
   // folded-BN affine for this tile
   if (p.per_row) {
@@ -131,10 +130,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
       s_shift[i] = (c < p.Ncols) ? __ldg(&p.shift[c]) : 0.f;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();                       // everything above touched only weights / on-chip state
 
@@ -191,11 +187,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
     }
 
     // ================================ epilogue ==========================================
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const int r = tid;                      // accumulator row == TMEM lane
+    mbar_wait(acc_full_bar, 0);
+    const int r = tid;                      // accumulator row
     const int m = m0 + r;
-    const uint32_t taddr_row = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
     const uint32_t swz = static_cast<uint32_t>(r & 7);
     uint8_t* c_stage = smem;                          // BN/64 boxes of [128][64] fp16, 128B swizzle
     uint8_t* r_stage = smem + S::kCTileBytes;
@@ -212,8 +206,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
 #pragma unroll 1
       for (int j = 0; j < BN / 32; ++j) {
         uint32_t v[32];
-        tmem_ld32(taddr_row + j * 32, v);
-        tmem_ld_wait();
+        acc_ld32(acc, r, j * 32, v);
         const int box = j >> 1;
         const int chunk0 = (j & 1) * 4;
         uint8_t* crow = c_stage + box * (kBM * 128) + r * 128;
@@ -261,8 +254,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
 #pragma unroll 1
       for (int j = 0; j < BN / 32; ++j) {
         uint32_t v[32];
-        tmem_ld32(taddr_row + j * 32, v);
-        tmem_ld_wait();
+        acc_ld32(acc, r, j * 32, v);
         if (row_ok) {
 #pragma unroll 4
           for (int i = 0; i < 32; ++i) {
@@ -287,7 +279,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
         }
       }
     }
-  } else if (warp == 4) {
+  } else if (warp == kIgTmaWarp) {
     // ================================ TMA producer ======================================
     // (whole warp with warp-uniform operands; one elected lane issues -- see elect_one())
     const uint32_t tx = S::kBBytes + (gather ? 0 : S::kABytes);
@@ -309,34 +301,21 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
       __syncwarp();
     }
   } else {
-    // ================================ MMA issuer ========================================
-    constexpr uint32_t idesc = make_idesc_f16(kBM, BN, 0);
-    const uint32_t tm = warp_uniform(tmem_base);
+    // ================================ MMA warpgroup =====================================
     const uint32_t ring = smem_u32(smem);
     for (int kb = 0; kb < p.nkb; ++kb) {
       const int s = kb % kStages;
       const uint32_t par = (kb / kStages) & 1;
       mbar_wait(&full_bar[s], par);
-      tc_fence_after();
       if (gather) fence_proxy_async();
       const uint32_t a_lo = sw128_desc_lo(ring + s * S::kStageBytes);
       const uint32_t b_lo = sw128_desc_lo(ring + s * S::kStageBytes + S::kABytes);
-      if (elect_one()) {
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo), idesc, kb != 0 ? 1u : 0u);
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo + 2), desc_from(kSw128DescHi, b_lo + 2), idesc, 1u);
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo + 4), desc_from(kSw128DescHi, b_lo + 4), idesc, 1u);
-        umma_f16(tm, desc_from(kSw128DescHi, a_lo + 6), desc_from(kSw128DescHi, b_lo + 6), idesc, 1u);
-        umma_commit(&empty_bar[s]);            // frees the smem slot once these MMAs retire
-        if (kb == p.nkb - 1) umma_commit(tmem_full_bar);   // accumulator complete -> epilogue
-      }
-      __syncwarp();
+      wg_mma(acc, 0, BN, wg_sw128(desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo)), 4, kb != 0);
+      wg_sync();
+      wg_arrive(&empty_bar[s]);                          // frees the smem slot
+      if (kb == p.nkb - 1) wg_arrive(acc_full_bar);     // accumulator complete -> epilogue
     }
   }
-
-  // ---- teardown -------------------------------------------------------------------------
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, BN);
 }
 
 }  // namespace b2

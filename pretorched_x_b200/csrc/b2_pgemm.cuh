@@ -2,31 +2,36 @@
 //
 //     D[M][N] = act( scale[n] * (A[M][K] . B[N][K]^T  [+ A2[M][K2] . B2[N][K2]^T]) + shift[n] + residual[M][N] )
 //                                                                                   (fp16 in/out, fp32 accumulate)
-// The optional second operand pair accumulates into the same TMEM tile: it fuses the type-B shortcut projection of a
+// The optional second operand pair accumulates into the same accumulator tile: it fuses the type-B shortcut projection of a
 // bottleneck into its closing 1x1x1 convolution (BN scales folded into the two weight matrices), so the projected
 // shortcut never goes through HBM.
 //
 // These layers are HBM-bound (K is 64..2048 while every output element is written once and, for the block-closing
 // conv3, a residual element is read once), so the kernel is organised around keeping the memory system busy rather
 // than the tensor core: one CTA per SM loops over output tiles, and the three stages of a tile -- TMA loads of A/B
-// (and of the residual tile), the tcgen05 MMAs, and the epilogue (TMEM -> registers -> BN/residual/ReLU -> smem ->
-// TMA store) -- belong to different warps and overlap across consecutive tiles through double-buffered TMEM
-// accumulators, a double-buffered residual tile and an smem operand ring.  The non-persistent igemm_kernel pays the
-// TMEM allocation, barrier set-up and a cold pipeline for every 128 x 128 tile; with K = 64 that prologue dominates.
+// (and of the residual tile), the wgmma MMAs, and the epilogue (accumulators -> registers -> BN/residual/ReLU -> smem ->
+// TMA store) -- belong to different warps and overlap across consecutive tiles through double-buffered accumulator
+// tiles in shared memory, a double-buffered residual tile and an smem operand ring.  The non-persistent igemm_kernel
+// pays the barrier set-up and a cold pipeline for every tile; with K = 64 that prologue dominates.
+// Only the 64-wide instance fits: two 128 x 128 fp32 accumulator tiles beside the ring and the staging tiles of a
+// 128-wide tile would exceed 227 KB.
 //
-//   warp 8   producer: residual tile of tile i, then its K blocks (A and B boxes, 128B-swizzled)
-//   warp 9   MMA issuer: accumulates tile i into TMEM buffer i & 1
-//   warps 0-7 epilogue of tile i (thread = accumulator row x one half of the columns), TMA store from a staging tile
+//   warps 8-11  MMA warpgroup: accumulates tile i into accumulator buffer i & 1
+//   warp 12     producer: residual tile of tile i, then its K blocks (A and B boxes, 128B-swizzled)
+//   warps 0-7   epilogue of tile i (thread = accumulator row x one half of the columns), TMA store from a staging tile
 #pragma once
 
 #include "b2_ptx.cuh"
 
 namespace b2 {
 
-constexpr int kPgEpiWarps = 8;                       // two warps per TMEM lane quarter, each takes half of the columns
-constexpr int kPgThreads = (kPgEpiWarps + 2) * 32;
+constexpr int kPgEpiWarps = 8;                       // two warps per 32 accumulator rows, each takes half of the columns
+constexpr int kPgMmaWarp0 = kPgEpiWarps;
+constexpr int kPgProdWarp = kPgMmaWarp0 + 4;
+constexpr int kPgXformWarp0 = kPgProdWarp + 1;
+constexpr int kPgThreads = (kPgProdWarp + 1) * 32;
 constexpr int kPgXformWarps = 4;                     // generator instance only: A-operand transform warps (see PgemmParams::in_scale)
-constexpr int kPgThreadsGan = (kPgEpiWarps + 2 + kPgXformWarps) * 32;
+constexpr int kPgThreadsGan = (kPgXformWarp0 + kPgXformWarps) * 32;
 constexpr int kPgStages = 3;
 
 struct PgemmParams {
@@ -79,7 +84,9 @@ struct PgemmSmem {
                                                              // 128-wide one has no room and falls back to re-using C)
   static constexpr int kBarOff = kC2Off + (BN == 64 ? kTile : 0);
   static constexpr int kAffOff = kBarOff + 256;              // scale[BN], shift[BN] (+ scale2[BN], shift2[BN]) of the current tile
-  static constexpr int kTotal = kAffOff + 4 * BN * 4 + 1024;
+  static constexpr int kAccOff = kAffOff + 4 * BN * 4;       // two accumulator tiles of BN columns
+  static constexpr int kTotal = kAccOff + acc_bytes(2 * BN) + 1024;
+  static_assert(kTotal <= 227 * 1024, "shared memory budget");
 };
 
 template <int BN, int GAN>   // GAN = 1: instance with the generator extras (res_up gather, res_pre, A transform); 0: the classic epilogue
@@ -97,7 +104,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   uint64_t* acc_empty = acc_full + 2;                                // [2]
   uint64_t* res_full = acc_empty + 2;                                // [2]
   uint64_t* res_empty = res_full + 2;                                // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_empty + 2);
+  const AccTile at{reinterpret_cast<float*>(smem + S::kAccOff), acc_ld(2 * BN)};
   uint64_t* xf_full = reinterpret_cast<uint64_t*>(smem + S::kBarOff + 128);   // [3] A tile transformed (generator instance)
   const bool xform = GAN && p.in_scale != nullptr;
 
@@ -112,15 +119,11 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     fence_mbar_init();
     tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); tma_prefetch_desc(&tmC);
   }
-  if (warp == kPgEpiWarps + 1) { tmem_alloc(tmem_slot, 2 * BN); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();                       // everything above touched only weights / on-chip state
 
-  if (warp == kPgEpiWarps) {
+  if (warp == kPgProdWarp) {
     // ================================ producer ==========================================
     int it = 0, lt = 0;
     for (int tile = blockIdx.x; tile < p.tiles_total; tile += gridDim.x, ++lt) {
@@ -161,44 +164,34 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         __syncwarp();
       }
     }
-  } else if (warp == kPgEpiWarps + 1) {
-    // ================================ MMA issuer ========================================
-    constexpr uint32_t idesc = make_idesc_f16(128, BN, 0);
-    const uint32_t tm = warp_uniform(tmem_base);
+  } else if (warp >= kPgMmaWarp0 && warp < kPgMmaWarp0 + 4) {
+    // ================================ MMA warpgroup =====================================
     const uint32_t ring = smem_u32(smem);
     int it = 0, lt = 0;
     for (int tile = blockIdx.x; tile < p.tiles_total; tile += gridDim.x, ++lt) {
       const int ab = lt & 1;
       mbar_wait(&acc_empty[ab], ((lt >> 1) & 1) ^ 1);        // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t d = tm + ab * BN;
       const int nkb_all = p.nkb + p.nkb2;
       for (int kb = 0; kb < nkb_all; ++kb, ++it) {
         const int s = it % kPgStages;
         if (xform && kb < p.nkb) mbar_wait(&xf_full[s], (it / kPgStages) & 1);     // operands landed AND the A tile was rewritten
         else mbar_wait(&full[s], (it / kPgStages) & 1);
-        tc_fence_after();
         const uint32_t a_lo = sw128_desc_lo(ring + s * S::kStage);
         const uint32_t b_lo = sw128_desc_lo(ring + s * S::kStage + S::kABytes);
-        if (elect_one()) {
-          umma_f16(d, desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo), idesc, kb != 0 ? 1u : 0u);
-          umma_f16(d, desc_from(kSw128DescHi, a_lo + 2), desc_from(kSw128DescHi, b_lo + 2), idesc, 1u);
-          umma_f16(d, desc_from(kSw128DescHi, a_lo + 4), desc_from(kSw128DescHi, b_lo + 4), idesc, 1u);
-          umma_f16(d, desc_from(kSw128DescHi, a_lo + 6), desc_from(kSw128DescHi, b_lo + 6), idesc, 1u);
-          umma_commit(&empty[s]);
-          if (kb == nkb_all - 1) umma_commit(&acc_full[ab]);
-        }
-        __syncwarp();
+        wg_mma(at, ab * BN, BN, wg_sw128(desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo)), 4, kb != 0);
+        wg_sync();
+        wg_arrive(&empty[s]);
+        if (kb == nkb_all - 1) wg_arrive(&acc_full[ab]);
       }
     }
-  } else if (GAN && warp >= kPgEpiWarps + 2) {
+  } else if (GAN && warp >= kPgXformWarp0) {
     // ================================ A-operand transform (generator instance) ==========
     if (xform) {
       // thread t owns logical 8-channel chunk j = t & 7 (its 8 scale + 8 shift values stay in registers for the K block) of the
       // rows (t >> 3) + 16 i, i = 0..7.  The eight threads of a quarter-warp cover one 128-byte row: conflict-free; all loads of a K
       // block are issued before the first use and all stores after the last (one row per thread with load -> store per chunk
       // serialised on shared-memory latency: 2x slower layers than the stand-alone pass it replaces).
-      const int t = tid - (kPgEpiWarps + 2) * 32;
+      const int t = tid - kPgXformWarp0 * 32;
       const int j = t & 7, r0 = t >> 3;
       const uint32_t coff = (static_cast<uint32_t>(j) ^ static_cast<uint32_t>(r0 & 7)) << 4;     // (r0 + 16 i) & 7 == r0 & 7
       int it = 0;
@@ -226,7 +219,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           }
 #pragma unroll
           for (int i = 0; i < 8; ++i) *reinterpret_cast<uint4*>(base + i * (16 * 128)) = v[i];
-          fence_proxy_async();                        // generic-proxy writes -> visible to tcgen05.mma's shared-memory reads
+          fence_proxy_async();                        // generic-proxy writes -> visible to wgmma's shared-memory reads
           mbar_arrive(&xf_full[s]);
         }
       }
@@ -237,9 +230,8 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     float* s_shift = s_scale + BN;
     float* s_scale2 = s_shift + BN;
     float* s_shift2 = s_scale2 + BN;
-    const int r = (warp & 3) * 32 + (tid & 31);        // accumulator row == TMEM lane
+    const int r = (warp & 3) * 32 + (tid & 31);        // accumulator row
     const int half = warp >> 2;                        // which half of the tile's columns this warp handles
-    const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
     const uint32_t swz = static_cast<uint32_t>(r & 7);
     uint8_t* c_stage0 = smem + S::kCOff;
     uint8_t* c_stage1 = smem + (BN == 64 ? S::kC2Off : S::kCOff);
@@ -248,7 +240,6 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       const int m0 = (tile / p.tiles_n) * 128, n0 = (tile % p.tiles_n) * BN;
       const int ab = lt & 1;
       mbar_wait(&acc_full[ab], (lt >> 1) & 1);
-      tc_fence_after();
       const uint8_t* r_stage = smem + S::kResOff + ab * S::kTile;
       int rsrc = r;                                        // row of the residual box this thread's output row adds
       if (GAN && p.res_up) {
@@ -287,8 +278,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 #pragma unroll 1
         for (int j = half * (BN / 64); j < (half + 1) * (BN / 64); ++j) {
           uint32_t v[32];
-          tmem_ld32(tmem_base + lane_off + ab * BN + j * 32, v);
-          tmem_ld_wait();
+          acc_ld32(at, r, ab * BN + j * 32, v);
           const int box = j >> 1, chunk0 = (j & 1) * 4;
           uint8_t* crow = c_stage + box * (128 * 128) + r * 128;
           const uint8_t* rrow = r_stage + box * (128 * 128) + rsrc * 128;
@@ -323,7 +313,6 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         }
         if (pass == npass - 1) {
           // accumulator and residual buffers are free for tile lt + 2
-          tc_fence_before();
           mbar_arrive(&acc_empty[ab]);
           if (p.has_residual) mbar_arrive(&res_empty[ab]);
         }
@@ -339,10 +328,6 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     }
     if (tid == 0) tma_store_wait_read0();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kPgEpiWarps + 1) tmem_dealloc(tmem_base, 2 * BN);
 }
 
 }  // namespace b2

@@ -1,4 +1,4 @@
-// b2_probe.cu -- single-CTA experiments that pin down tcgen05 shared-memory descriptor semantics the
+// b2_probe.cu -- single-CTA experiments that pin down the wgmma shared-memory descriptor semantics the
 // convolution kernels rely on.  Not part of the product path; exercised by tools/probe_umma.py.
 //
 //   mode 0: K-major SWIZZLE_128B A operand whose start address is shifted by `shift` rows (128 B each)
@@ -6,7 +6,7 @@
 //           D[r][n] = sum_k A[shift + r][k] * B[n][k]   (A is 256 x 64, loaded by TMA as two boxes).
 //   mode 2: MN-major SWIZZLE_128B B operand.  B is given as V[K = 64][N = 128] row-major (N contiguous), loaded
 //           by TMA as two [64 n x 64 k-rows] boxes 8 KB apart; descriptor: LBO = 8192 (next 64-wide N block),
-//           SBO = 1024 (next 8 K rows), K step of 16 = +2048 B; instruction descriptor has b_major = MN.
+//           SBO = 1024 (next 8 K rows), K step of 16 = +2048 B; B transposed (MN-major) in the instruction.
 //           Expected: D[r][n] = sum_k A[r][k] * V[k][n]  with N = 128.
 //   mode 1: K-major SWIZZLE_NONE A operand built as an overlapping (Toeplitz) view of a linear buffer:
 //           row r starts at byte 16*r, K = 32 elements: LBO = 16 B, SBO = 128 B.
@@ -19,64 +19,46 @@
 namespace b2 {
 
 __global__ void __launch_bounds__(128, 1)
-umma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __half* __restrict__ lin_a, const __half* __restrict__ lin_b, float* __restrict__ out,
-                  int mode, int shift, int base_off) {
+mma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __half* __restrict__ lin_a, const __half* __restrict__ lin_b, float* __restrict__ out,
+                 int mode, int shift, int base_off) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align<1024>(smem_raw);
   uint8_t* sA = smem;                 // 256 rows x 128 B = 32 KB
   uint8_t* sB = smem + 32768;         // 64 rows x 128 B  = 8 KB (mode 0) / no-swizzle B (mode 1)
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 32768 + 8192);
-  uint64_t* mma_bar = bar + 1;
-  uint32_t* slot = reinterpret_cast<uint32_t*>(bar + 2);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const AccTile at{reinterpret_cast<float*>(smem + 32768 + 8192 + 64), acc_ld(128)};
+  const int tid = threadIdx.x;
 
-  if (tid == 0) { mbar_init(bar, 1); mbar_init(mma_bar, 1); fence_mbar_init(); }
-  if (warp == 0) { tmem_alloc(slot, 128); tmem_relinquish(); }
-  tc_fence_before();
+  if (tid == 0) { mbar_init(bar, 1); fence_mbar_init(); }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *slot;
 
+  const int ncol = (mode == 2) ? 128 : 64;
   if (mode == 0) {
     if (tid == 0) {
       mbar_expect_tx(bar, 32768 + 8192);
       tma_load_2d(sA, &tmA, bar, 0, 0);
       tma_load_2d(sA + 16384, &tmA, bar, 0, 128);
       tma_load_2d(sB, &tmB, bar, 0, 0);
-      mbar_wait(bar, 0);
-      tc_fence_after();
-      constexpr uint32_t idesc = make_idesc_f16(128, 64, 0);
-      const uint32_t a_addr = smem_u32(sA) + shift * 128;
-      const uint32_t b_addr = smem_u32(sB);
-      for (int k = 0; k < 4; ++k) {
-        uint64_t ad = make_desc_sw128_kmajor(a_addr + k * 32) | (static_cast<uint64_t>(base_off & 7) << 49);
-        umma_f16(tmem, ad, make_desc_sw128_kmajor(b_addr + k * 32), idesc, k != 0);
-      }
-      umma_commit(mma_bar);
     }
+    mbar_wait(bar, 0);
+    const uint64_t ad = make_desc_sw128_kmajor(smem_u32(sA) + shift * 128) | (static_cast<uint64_t>(base_off & 7) << 49);
+    wg_mma(at, 0, 64, wg_sw128(ad, make_desc_sw128_kmajor(smem_u32(sB))), 4, false);
   } else if (mode == 2) {
     if (tid == 0) {
       mbar_expect_tx(bar, 16384 + 16384);
       tma_load_2d(sA, &tmA, bar, 0, 0);                 // A: 128 x 64 K-major
       tma_load_2d(sA + 16384, &tmB, bar, 0, 0);         // V block n in [0,64):   64 k-rows x 128 B
       tma_load_2d(sA + 16384 + 8192, &tmB, bar, 64, 0); // V block n in [64,128)
-      mbar_wait(bar, 0);
-      tc_fence_after();
-      const uint32_t idesc = make_idesc_f16(128, 128, 0) | (1u << 16);   // b_major = MN
-      const uint32_t a_addr = smem_u32(sA);
-      const uint32_t b_addr = smem_u32(sA + 16384);
-      for (int k = 0; k < 4; ++k) {
-        uint64_t bd = 0;
-        bd |= static_cast<uint64_t>(((b_addr + k * 2048) & 0x3FFFF) >> 4);
-        bd |= static_cast<uint64_t>(8192 >> 4) << 16;   // LBO: next 64-wide N block
-        bd |= static_cast<uint64_t>(1024 >> 4) << 32;   // SBO: next 8 K rows
-        bd |= static_cast<uint64_t>(1) << 46;
-        bd |= static_cast<uint64_t>(2) << 61;
-        umma_f16(tmem, make_desc_sw128_kmajor(a_addr + k * 32), bd, idesc, k != 0);
-      }
-      umma_commit(mma_bar);
     }
+    mbar_wait(bar, 0);
+    uint64_t bd = 0;
+    bd |= static_cast<uint64_t>(((smem_u32(sA + 16384)) & 0x3FFFF) >> 4);
+    bd |= static_cast<uint64_t>(8192 >> 4) << 16;   // LBO: next 64-wide N block
+    bd |= static_cast<uint64_t>(1024 >> 4) << 32;   // SBO: next 8 K rows
+    bd |= static_cast<uint64_t>(1) << 62;           // SWIZZLE_128B
+    const WgOperands ops{make_desc_sw128_kmajor(smem_u32(sA)), bd, 2u, 512u, 128u, 512u, 0u};
+    wg_mma<1>(at, 0, 128, ops, 4, false);
   } else {
     // linear buffers copied with plain stores: A buffer 4 KB (2048 halfs), B = 64 rows x 32 k in the
     // canonical no-swizzle K-major layout: chunk (n, j) at (n/8)*SBO_B + j*LBO_B + (n%8)*16, LBO_B = 128,
@@ -89,31 +71,17 @@ umma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     fence_proxy_async();
     __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      constexpr uint32_t idesc = make_idesc_f16(128, 64, 0);
-      const uint32_t a_addr = smem_u32(sA);
-      const uint32_t b_addr = smem_u32(sB);
-      for (int k = 0; k < 2; ++k) {   // K = 32 -> two K=16 MMAs; each advances two 16-byte chunks
-        uint64_t ad = make_desc_noswz_kmajor(a_addr + k * 32, /*LBO*/ 16, /*SBO*/ 128);
-        uint64_t bd = make_desc_noswz_kmajor(b_addr + k * 256, /*LBO*/ 128, /*SBO*/ 512);
-        umma_f16(tmem, ad, bd, idesc, k != 0);
-      }
-      umma_commit(mma_bar);
-    }
+    // K = 32 -> two K=16 steps; A advances two 16-byte chunks (32 B), B two 128-byte chunk columns (256 B)
+    const WgOperands ops{make_desc_noswz_kmajor(smem_u32(sA), /*LBO*/ 16, /*SBO*/ 128),
+                         make_desc_noswz_kmajor(smem_u32(sB), /*LBO*/ 128, /*SBO*/ 512), 2u, 64u, 16u, 256u, 64u};
+    wg_mma(at, 0, 64, ops, 2, false);
   }
-  mbar_wait(mma_bar, 0);
-  tc_fence_after();
+  __syncthreads();
   uint32_t v[32];
-  const int ncol = (mode == 2) ? 128 : 64;
   for (int j = 0; j < ncol / 32; ++j) {
-    tmem_ld32(tmem + (static_cast<uint32_t>(warp * 32) << 16) + j * 32, v);
-    tmem_ld_wait();
+    acc_ld32(at, tid, j * 32, v);
     for (int i = 0; i < 32; ++i) out[tid * ncol + j * 32 + i] = __uint_as_float(v[i]);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 128);
 }
 
 }  // namespace b2
@@ -125,9 +93,9 @@ extern "C" int b2_debug_umma_probe(const void* a, const void* b, float* out, int
                                    void* stream) {
   B2_CHECK_ARG(a && b && out, "null pointer");
   int rc;
-  if ((rc = require_sm100()) != B2_OK) return rc;
-  const int smem_bytes = 32768 + 8192 + 64 + 1024;
-  B2_OPT_IN_SMEM(umma_probe_kernel, smem_bytes);
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  const int smem_bytes = 32768 + 8192 + 64 + acc_bytes(128) + 1024;
+  B2_OPT_IN_SMEM(mma_probe_kernel, smem_bytes);
   CUtensorMap tmA, tmB;
   memset(&tmA, 0, sizeof(tmA)); memset(&tmB, 0, sizeof(tmB));
   if (mode == 0) {
@@ -137,8 +105,8 @@ extern "C" int b2_debug_umma_probe(const void* a, const void* b, float* out, int
     if ((rc = make_tmap_2d_f16(&tmA, a, 64, 128, 64, 64, 128, true)) != B2_OK) return rc;
     if ((rc = make_tmap_2d_f16(&tmB, b, 128, 64, 128, 64, 64, true)) != B2_OK) return rc;   // V[64][128]
   }
-  umma_probe_kernel<<<1, 128, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(
+  mma_probe_kernel<<<1, 128, smem_bytes, reinterpret_cast<cudaStream_t>(stream)>>>(
       tmA, tmB, reinterpret_cast<const __half*>(a), reinterpret_cast<const __half*>(b), out, mode, shift, base_off);
-  B2_CHECK_LAUNCH("umma_probe_kernel");
+  B2_CHECK_LAUNCH("mma_probe_kernel");
   return B2_OK;
 }

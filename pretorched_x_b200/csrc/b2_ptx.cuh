@@ -1,9 +1,8 @@
-// b2_ptx.cuh -- thin inline-PTX wrappers for the sm_100a features the hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), cp.async, tcgen05 (alloc / mma / commit / ld) and the
-// shared-memory / instruction descriptors that tcgen05.mma consumes.
+// b2_ptx.cuh -- thin inline-PTX wrappers for the sm_90a features the hot path uses:
+// mbarrier, TMA (cp.async.bulk.tensor), cp.async, wgmma and the shared-memory matrix descriptors it consumes.
 //
 // Everything here is device-side and header-only.  No CUTLASS/CuTe is used; the bit layouts
-// follow the PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor" tables.
+// follow the PTX ISA "matrix descriptor" table of the warpgroup-level MMA.
 #pragma once
 
 #include <cuda.h>
@@ -21,10 +20,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 
 // Aligns the dynamic shared-memory base with pointer arithmetic on the __shared__ array itself.  Going through
-// uintptr_t makes the compiler lose the address space: every later access became a generic LD/ST plus an R2UR
-// (measured: 2 generic loads per output element in the conv epilogues).
+// uintptr_t makes the compiler lose the address space: every later access becomes a generic LD/ST.
 // Programmatic dependent launch: the tensor-core kernels are launched with programmatic stream serialization, so a
-// CTA of launch i+1 starts (barrier init, TMEM allocation, tensor-map prefetch, BN-affine staging) on every SM that
+// CTA of launch i+1 starts (barrier init, tensor-map prefetch, BN-affine staging) on every SM that
 // launch i has vacated and only then waits for launch i to finish; without the attribute both are no-ops.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -77,7 +75,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// generic-proxy writes (st.shared / cp.async) -> async-proxy readers (TMA store, tcgen05.mma)
+// generic-proxy writes (st.shared / cp.async) -> async-proxy readers (TMA store, wgmma)
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -145,77 +143,176 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05: tensor memory + 5th-gen tensor core MMA
+// Warpgroup MMA (wgmma) into an accumulator tile in shared memory
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {  // whole warp
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// Hopper has no tensor memory: the fp32 accumulators of a 128-row MMA tile live in shared memory as [128 rows][ld]
+// ("AccTile", ld = columns + 4 so that neither the fragment stores nor the row-per-thread reads of the epilogue
+// conflict).  One warpgroup (4 warps, 128 threads) issues the MMAs: wg_mma() loads a 64 x <=64 piece of the tile
+// into registers, accumulates one K block with wgmma (both operands from shared memory, K-major or, for B, MN-major
+// descriptors), waits for it and stores the piece back.  An epilogue thread owns tile row r and reads / writes
+// 32 consecutive columns at a time (acc_ld32 / acc_st32 / acc_zero32).
+struct AccTile {
+  float* p;   // row 0, column 0
+  int ld;     // row pitch in floats
+};
+__host__ __device__ constexpr int acc_ld(int cols) { return cols + 4; }
+__host__ __device__ constexpr int acc_bytes(int cols) { return 128 * acc_ld(cols) * 4; }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, fp16/bf16 inputs, fp32 accumulate; single thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+__device__ __forceinline__ void acc_ld32(const AccTile& t, int row, int col, uint32_t (&v)[32]) {
+  const float4* s = reinterpret_cast<const float4*>(t.p + static_cast<size_t>(row) * t.ld + col);
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float4 f = s[q];
+    v[4 * q] = __float_as_uint(f.x); v[4 * q + 1] = __float_as_uint(f.y);
+    v[4 * q + 2] = __float_as_uint(f.z); v[4 * q + 3] = __float_as_uint(f.w);
+  }
+}
+__device__ __forceinline__ void acc_st32(const AccTile& t, int row, int col, const uint32_t (&v)[32]) {
+  float4* s = reinterpret_cast<float4*>(t.p + static_cast<size_t>(row) * t.ld + col);
+#pragma unroll
+  for (int q = 0; q < 8; ++q)
+    s[q] = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
+                       __uint_as_float(v[4 * q + 3]));
+}
+__device__ __forceinline__ void acc_zero32(const AccTile& t, int row, int col) {
+  float4* s = reinterpret_cast<float4*>(t.p + static_cast<size_t>(row) * t.ld + col);
+#pragma unroll
+  for (int q = 0; q < 8; ++q) s[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+template <int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b) {
   asm volatile(
       "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, 0, %34;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "n"(TB));
 }
-// mbarrier arrives once every tcgen05.mma issued so far by this thread has completed
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+template <int TB>
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1, 1, 1, 0, %18;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "n"(TB));
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 1, 1, 1, 0, %10;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "n"(TB));
 }
 
-// TMEM -> registers: warp w reads lanes [32*(w%4), +32); thread = one lane (one accumulator row),
-// 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+// D[64 x 128] += A[64 x 16] . B[128 x 16]^T, both operands K-major in shared memory (descriptors), D in registers
+__device__ __forceinline__ void wgmma_n128_ss(float (&d)[64], uint64_t a, uint64_t b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM: zero 32 consecutive fp32 columns of this thread's lane
-__device__ __forceinline__ void tmem_st32_zero(uint32_t taddr) {
+// D[64 x 64] += A[64 x 16] . B, A from registers (four fp16x2 per thread in the accumulator-fragment layout of its
+// columns), B a shared-memory descriptor (TB = 1: MN-major)
+template <int TB>
+__device__ __forceinline__ void wgmma_n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, "
-      "%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr),
-      "r"(0u)
-      : "memory");
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1, %37;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "n"(TB));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// registers -> TMEM: 32 consecutive fp32 columns of this thread's lane
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-      "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-      "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-      "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
+
+// Operand walk of wg_mma: descriptor of rows / columns 0 at K step 0 and the descriptor increments (16-byte units)
+// per 16-element K step, per 64 rows of A, per 64 and per 16 columns of B.
+struct WgOperands {
+  uint64_t a, b;
+  uint32_t a_k, a_m64, b_k, b_n64, b_n16;
+};
+// K-major SWIZZLE_128B tiles (rows 128 B apart): K step +32 B, 16 rows +2 KB
+__device__ __forceinline__ WgOperands wg_sw128(uint64_t a, uint64_t b) {
+  return WgOperands{a, b, 2u, 512u, 2u, 512u, 128u};
+}
+
+// Fragment <-> tile: thread t of the warpgroup holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) of a 64-row piece and
+// column pairs 8 j + 2 (t % 4).
+template <int W>
+__device__ __forceinline__ void frag_io(const AccTile& t, int row0, int col0, float (&d)[W / 2], bool load, bool zero) {
+  const int wt = threadIdx.x & 127;
+  const int row = row0 + (wt >> 5) * 16 + ((wt & 31) >> 2);
+  float* p0 = t.p + static_cast<size_t>(row) * t.ld + col0 + 2 * (wt & 3);
+  float* p1 = p0 + 8 * t.ld;
+#pragma unroll
+  for (int j = 0; j < W / 8; ++j) {
+    if (load) {
+      float2 u = zero ? make_float2(0.f, 0.f) : *reinterpret_cast<const float2*>(p0 + 8 * j);
+      float2 w = zero ? make_float2(0.f, 0.f) : *reinterpret_cast<const float2*>(p1 + 8 * j);
+      d[4 * j] = u.x; d[4 * j + 1] = u.y; d[4 * j + 2] = w.x; d[4 * j + 3] = w.y;
+    } else {
+      *reinterpret_cast<float2*>(p0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+      *reinterpret_cast<float2*>(p1 + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+  }
+}
+
+template <int W, int TB>
+__device__ __forceinline__ void wg_mma_piece(const AccTile& t, int row0, int col0, uint64_t a, uint64_t b, uint32_t a_k,
+                                             uint32_t b_k, int ksteps, bool accumulate) {
+  float d[W / 2];
+  frag_io<W>(t, row0, col0, d, true, !accumulate);
+  wgmma_fence();
+  for (int k = 0; k < ksteps; ++k) {
+    if constexpr (W == 64) wgmma_n64<TB>(d, a + k * a_k, b + k * b_k);
+    else if constexpr (W == 32) wgmma_n32<TB>(d, a + k * a_k, b + k * b_k);
+    else wgmma_n16<TB>(d, a + k * a_k, b + k * b_k);
+  }
+  wgmma_commit();
+  wgmma_wait0();
+  frag_io<W>(t, row0, col0, d, false, false);
+}
+
+// D[128 rows][col0, col0 + n) (+)= A[128][16 ksteps] . B[n][16 ksteps]^T.  Called by all 128 threads of the MMA
+// warpgroup with warp-uniform arguments; n is a multiple of 16 (of 64 for an MN-major B, TB = 1).  Synchronous: the
+// operands have been read and the tile updated when every thread has returned.
+template <int TB = 0>
+__device__ __forceinline__ void wg_mma(const AccTile& t, int col0, int n, const WgOperands& o, int ksteps, bool accumulate) {
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    const uint64_t a = o.a + h * o.a_m64;
+    int c = 0;
+#pragma unroll 1
+    for (; c + 64 <= n; c += 64)
+      wg_mma_piece<64, TB>(t, h * 64, col0 + c, a, o.b + (c / 64) * o.b_n64, o.a_k, o.b_k, ksteps, accumulate);
+    if (c + 32 <= n) {
+      wg_mma_piece<32, TB>(t, h * 64, col0 + c, a, o.b + (c / 64) * o.b_n64, o.a_k, o.b_k, ksteps, accumulate);
+      c += 32;
+    }
+    if (c < n)
+      wg_mma_piece<16, TB>(t, h * 64, col0 + c, a, o.b + (c / 64) * o.b_n64 + ((c % 64) / 16) * o.b_n16, o.a_k, o.b_k,
+                           ksteps, accumulate);
+  }
+}
+
+// The MMA warpgroup has finished with what it read and wrote: one thread arrives on `bar` (expected count 1).
+// Named barrier 15 is reserved for the MMA warpgroup.
+__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync 15, 128;" ::: "memory"); }
+__device__ __forceinline__ void wg_arrive(uint64_t* bar) {
+  if ((threadIdx.x & 127) == 0) mbar_arrive(bar);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -223,8 +320,10 @@ __device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32
 // ------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor (64 bit):
 //   [ 0,14) start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset>>4 [46,48) version (1 on sm_100)
-//   [49,52) base offset               [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
+//   [32,46) stride-dim byte offset>>4 [49,52) base offset
+//   [62,64) layout: 0 none, 1 = 128B swizzle, 2 = 64B, 3 = 32B
+// The swizzle is a function of the absolute shared-memory address bits, so a start address moved by whole 128-byte
+// rows or by 32-byte K steps inside a row addresses the same TMA-written tile.
 //
 // K-major, 128B swizzle (what TMA SWIZZLE_128B writes for a [rows][64 x fp16] box): rows are 128 B
 // apart, 8-row groups are SBO = 1024 B apart, the 16 B chunk index is XORed with (row & 7).
@@ -234,8 +333,7 @@ __device__ __forceinline__ uint64_t make_desc_sw128_kmajor(uint32_t smem_addr) {
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;            // LBO (unused for swizzled K-major; 1 like CuTe)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;    // SBO
-  d |= static_cast<uint64_t>(1) << 46;            // version
-  d |= static_cast<uint64_t>(2) << 61;            // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;            // SWIZZLE_128B
   return d;
 }
 // K-major, no swizzle ("interleave"): core matrix = 8 rows x 16 B with rows 16 B apart;
@@ -246,20 +344,12 @@ __device__ __forceinline__ uint64_t make_desc_noswz_kmajor(uint32_t smem_addr, u
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
   return d;
-}
-
-// Instruction descriptor for kind::f16 (32 bit):
-//   [4,6) D format (1 = f32)  [7,10) A format (0 = f16, 1 = bf16)  [10,13) B format
-//   [15] A major (0 = K)  [16] B major (0 = K)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t ab_fmt /*0 f16, 1 bf16*/) {
-  return (1u << 4) | (ab_fmt << 7) | (ab_fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // Cheap descriptor arithmetic for issue loops: the high word of a K-major SWIZZLE_128B descriptor is a
 // constant, the low word is (addr >> 4) | LBO; stepping K by 16 elements (+32 B) is "+2" on the low word.
-constexpr uint32_t kSw128DescHi = (1024u >> 4) | (1u << 14) | (2u << 29);
+constexpr uint32_t kSw128DescHi = (1024u >> 4) | (1u << 30);
 __device__ __forceinline__ uint32_t sw128_desc_lo(uint32_t smem_addr) {
   return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16);
 }
@@ -267,9 +357,7 @@ __device__ __forceinline__ uint64_t desc_from(uint32_t hi, uint32_t lo) {
   return (static_cast<uint64_t>(hi) << 32) | lo;
 }
 
-// One lane of a fully converged warp.  Issue loops run on the whole warp with warp-uniform operands and wrap only
-// the tcgen05 / TMA instructions in `if (elect_one())`: that keeps descriptors in uniform registers (a loop nested
-// under `if (lane == 0)` makes ptxas emit an ELECT/R2UR "waterfall" around every UTCHMMA, ~100 cycles per MMA).
+// One lane of a fully converged warp (TMA issue from a whole producer warp with warp-uniform operands).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -281,7 +369,6 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
 
 // ------------------------------------------------------------------------------------------
 // small numeric helpers
@@ -297,7 +384,7 @@ __device__ __forceinline__ float2 unpack_half2(uint32_t u) {
 
 // Division by a run-time constant as a 64-bit multiply + shift (exact for 0 <= n < 2^31): the work-item decode and the
 // epilogue's position -> (row, column) split run once per item in every warp; with few-tap 2-D filters an item is short
-// enough that the ~25-instruction integer division sequences showed up in the issue-slot budget (profiles/NOTES_r01.md).
+// enough that the ~25-instruction integer division sequences show up in the issue-slot budget.
 struct FastDiv {
   unsigned long long M;
   int s, d;

@@ -16,20 +16,22 @@
 // (1 + 2 + 2 + 4 taps for 3x3); the 1x1x1 stride-2 shortcut projection is the one-phase, one-tap special case.
 //
 // Output positions are enumerated in *padded-row* coordinates q = h*(W+2pw) + w' of one (n,t) plane; a work item
-// is MT consecutive 128-position M tiles (MT accumulators in TMEM share every weight tile) x one N tile, and the
+// is MT consecutive 128-position M tiles (MT accumulators share every weight tile) x one N tile, and the
 // positions that fall on halo columns are discarded.  Rows longer than a TMA box are cut into W chunks (each with
 // its own halo); a purely temporal (kt,1,1) filter is run as a (1,kt,1) filter over the image "frames x (H*W)",
 // so its slab holds MT+kt-1 frames of one position chunk and every temporal tap is a whole-row shift of it.
 // CTAs are persistent (one per SM): the producer runs ahead
-// into the next item's slabs, and when MT*BN <= 256 two accumulator sets let the epilogue of item i overlap the
-// MMAs of item i+1.
+// into the next item's slabs, and when shared memory has room for two accumulator sets (AccTile, b2_ptx.cuh) the
+// epilogue of item i overlaps the MMAs of item i+1.
 #pragma once
 
 #include "b2_ptx.cuh"
 
 namespace b2 {
 
-constexpr int kSlabThreads = 320;   // warps 0-3 and 6-9: epilogue (even / odd 32-column chunks), 4: TMA producer, 5: MMA issuer
+constexpr int kSlabThreads = 416;   // warps 0-7: epilogue (even / odd 32-column chunks), 8-11: MMA warpgroup, 12: TMA producer
+constexpr int kSlabMmaWarp0 = 8;
+constexpr int kSlabTmaWarp = 12;
 constexpr int kSlabWStages = 4;     // weight-tile ring depth
 constexpr int kSlabSStages = 2;     // slab ring depth
 
@@ -55,13 +57,13 @@ struct SlabParams {
   unsigned char sub_tap[kSlabMaxSub][kSlabMaxTaps];
   int reach;               // max |sub_off|
   int slab_bytes;          // R * PW * 128, rounded up to 1024
-  int MT;                  // M tiles per work item (MT * accs <= 512)
-  int nacc;                // accumulator sets in TMEM: 2 when MT * accs <= 256 (epilogue overlaps the next item)
+  int MT;                  // M tiles per work item
+  int nacc;                // accumulator sets: 2 when they fit in shared memory (epilogue overlaps the next item)
   // runtime N tile (slabconv_kernel<0> only; the <64>/<128> instances use their template value): Cout = 144, 288,
   // 576 ... of the (2+1)D factorisation would waste up to 44% of the MMA columns on 128-wide tiles
   int bn;                  // N per MMA / per tile, multiple of 16, <= 256
   int wbytes;              // weight stage stride in smem: bn * 128 rounded up to 1024
-  int accs;                // TMEM column stride between the MT accumulators: bn rounded up to 32
+  int accs;                // accumulator column stride between the MT accumulators: bn rounded up to 32
   int P;                   // Ho * PW: padded positions per output plane
   int Ncols;               // logical output channels
   int tiles_n, tiles_q, items_total;
@@ -87,7 +89,8 @@ struct SlabParams {
   FastDiv fd_tiles_n, fd_tiles_q, fd_wchunks, fd_To, fd_PW;   // dividers of the item decode (set by launch_slab)
 };
 
-// scale/shift live in smem for all (padded) output channels: SlabParams::naff = round_up(ldy, 32) + 32 entries each
+// scale/shift live in smem for all (padded) output channels: SlabParams::naff = round_up(ldy, 32) + 32 entries each; the
+// accumulator tile (nacc * MT * accs columns) follows them
 
 struct SlabItem {
   int n0, q0, wc, plane_o, plane_i0, r_lo, dt_lo, n_dt, n_slabs, mt_valid;   // plane_i0: input plane of temporal tap 0
@@ -140,12 +143,12 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
   uint64_t* w_empty = w_full + kSlabWStages;
   uint64_t* acc_full = w_empty + kSlabWStages;      // [2]
   uint64_t* acc_empty = acc_full + 2;               // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_scale = reinterpret_cast<float*>(tail + 256);     // barriers + TMEM slot occupy the first 132 bytes
+  float* s_scale = reinterpret_cast<float*>(tail + 256);     // barriers occupy the first 128 bytes
   float* s_shift = s_scale + p.naff;
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int acc_cols = p.MT * accs;
+  const AccTile at{s_shift + p.naff, acc_ld(p.nacc * acc_cols)};
 
   if (tid == 128) {
     for (int s = 0; s < kSlabSStages; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 1); }
@@ -155,22 +158,18 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 5) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
   for (int i = tid; i < p.naff; i += kSlabThreads) {
     s_scale[i] = (i < p.Ncols && !p.aff_ld) ? __ldg(&p.scale[i]) : 0.f;
     s_shift[i] = (i < p.Ncols && !p.aff_ld) ? __ldg(&p.shift[i]) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();                       // everything above touched only weights / on-chip state
 
-  if (warp == 4) {
+  if (warp == kSlabTmaWarp) {
     // ================================ TMA producer ======================================
     // Walks (item, slab) pairs; the slab after the current one -- possibly the first slab of the NEXT item -- is
-    // requested once the weight ring (kSlabWStages deep) guarantees the MMA warp has retired the slab that
+    // requested once the weight ring (kSlabWStages deep) guarantees the MMA warpgroup has retired the slab that
     // occupied the target slot, so that wait never stalls weight issue.
     int wit = 0, sg = 0;                     // global weight-tile / slab counters (ring phases persist across items)
     int item = blockIdx.x;
@@ -221,11 +220,8 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
         }
       }
     }
-  } else if (warp == 5) {
-    // ================================ MMA issuer ========================================
-    // whole warp, warp-uniform operands; one elected lane issues (see elect_one())
-    const uint32_t idesc = make_idesc_f16(128, bn, 0);
-    const uint32_t tm = warp_uniform(tmem_base);
+  } else if (warp >= kSlabMmaWarp0) {
+    // ================================ MMA warpgroup =====================================
     const uint32_t slab0 = smem_u32(slab_base), w0s = smem_u32(w_base);
     const uint32_t tile_stride16 = (p.mp > 1 ? static_cast<uint32_t>(p.plane_stride) : 128u * 128u) >> 4;   // A start of tile j, in 16-byte units
     int wit = 0, sg = 0, lt = 0;
@@ -233,8 +229,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
       const SlabItem w = slab_item(p, item, bn);
       const int ab = lt % p.nacc;
       mbar_wait(&acc_empty[ab], (((lt / p.nacc) & 1) ^ 1));      // epilogue drained this accumulator set
-      tc_fence_after();
-      const uint32_t acc = tm + ab * acc_cols;
+      const int acc = ab * acc_cols;
       int wl = 0;                                                // weight step within the item
       for (int si = 0; si < w.n_slabs; ++si, ++sg) {
         const int sub = p.up ? w.phase : si % p.n_sub;
@@ -247,46 +242,32 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
         for (int ti = 0; ti < ntaps; ++ti, ++wit, ++wl) {
           const int ws = wit % kSlabWStages;
           mbar_wait(&w_full[ws], (wit / kSlabWStages) & 1);
-          tc_fence_after();
           // slab-local pixel index of padded output position q0 under this tap
           const int pix0 = w.q0 + p.sub_off[sub][ti] - w.r_lo * p.PW;
           const uint32_t b_lo = sw128_desc_lo(w0s + ws * kWBytes);
           const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u);
-          if (elect_one()) {
-            for (int j = 0; j < w.mt_valid; ++j) {
-              const uint32_t a_lo = a_lo0 + j * tile_stride16;
-              const uint32_t d = acc + j * accs;
-              umma_f16(d, desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo), idesc, wl != 0 ? 1u : 0u);
-              if (ksteps == 4) {
-                umma_f16(d, desc_from(kSw128DescHi, a_lo + 2), desc_from(kSw128DescHi, b_lo + 2), idesc, 1u);
-                umma_f16(d, desc_from(kSw128DescHi, a_lo + 4), desc_from(kSw128DescHi, b_lo + 4), idesc, 1u);
-                umma_f16(d, desc_from(kSw128DescHi, a_lo + 6), desc_from(kSw128DescHi, b_lo + 6), idesc, 1u);
-              } else {                                     // last channel chunk of C = 144, 288, 232 ...: skip all-zero K steps
-                for (int k = 1; k < ksteps; ++k)
-                  umma_f16(d, desc_from(kSw128DescHi, a_lo + 2 * k), desc_from(kSw128DescHi, b_lo + 2 * k), idesc, 1u);
-              }
-            }
-            umma_commit(&w_empty[ws]);
-            if (ti == ntaps - 1) umma_commit(&slab_empty[s]);
-            if (ti == ntaps - 1 && si == w.n_slabs - 1) umma_commit(&acc_full[ab]);
-          }
-          __syncwarp();
+          // (the last channel chunk of C = 144, 288, 232 ... skips its all-zero K steps)
+          for (int j = 0; j < w.mt_valid; ++j)
+            wg_mma(at, acc + j * accs, bn, wg_sw128(desc_from(kSw128DescHi, a_lo0 + j * tile_stride16), desc_from(kSw128DescHi, b_lo)),
+                   ksteps, wl != 0);
+          wg_sync();
+          wg_arrive(&w_empty[ws]);
+          if (ti == ntaps - 1) wg_arrive(&slab_empty[s]);
+          if (ti == ntaps - 1 && si == w.n_slabs - 1) wg_arrive(&acc_full[ab]);
         }
       }
     }
   } else {
     // ================================ epilogue ==========================================
-    // a warp may only touch TMEM lanes 32*(warp%4)..+31; the two warpgroups split the accumulator columns
+    // thread = accumulator row; the two warpgroups split the accumulator columns
     const int erow = (warp & 3) * 32 + (tid & 31);
-    const int egroup = warp >= 6 ? 1 : 0;
-    const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
+    const int egroup = warp >= 4 ? 1 : 0;
     int lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const SlabItem w = slab_item(p, item, bn);
       const int ab = lt % p.nacc;
       mbar_wait(&acc_full[ab], (lt / p.nacc) & 1);
-      tc_fence_after();
-      const uint32_t acc = tmem_base + lane_off + ab * acc_cols;
+      const int acc = ab * acc_cols;
       const int ncols_here = min(bn, p.ldy - w.n0);     // columns of this tile that exist in y (incl. zero padding)
       // output row of this thread in each of the item's M tiles
       size_t row[4];
@@ -333,8 +314,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
           }
         }
         // residual rows are requested one M tile AHEAD of their use (two register sets): the loads are independent of the MMAs,
-        // and issued load -> use per tile each exposed ~1 us of HBM latency to the epilogue warps (73% of their stall samples on
-        // the temporal convolutions of R(2+1)D, profiles/ncu_r02)
+        // and issued load -> use per tile each would expose the HBM latency to the epilogue warps
         uint4 rres[2][4];
         auto load_res = [&](int j) {
           if (p.residual && j < w.mt_valid && ok[j]) {
@@ -350,8 +330,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
           if (j < w.mt_valid) {                            // warp-uniform
             if (j + 1 < 4) load_res(j + 1);
             uint32_t v[32];
-            tmem_ld32(acc + j * accs + jc * 32, v);        // warp-collective: outside the `ok` branch
-            tmem_ld_wait();
+            acc_ld32(at, erow, acc + j * accs + jc * 32, v);
             if (ok[j]) {
               __half* yrow = p.y + row[j] * p.ldy + c0;
               if (p.residual) {                              // uniform: residual added in fp32 before the single rounding
@@ -396,14 +375,9 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
           }
         }
       }
-      tc_fence_before();
       mbar_arrive(&acc_empty[ab]);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace b2

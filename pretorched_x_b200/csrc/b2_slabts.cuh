@@ -1,8 +1,7 @@
 // b2_slabts.cuh -- 3 x kh x kw "same" convolution with <= 64 output channels, temporal-group form of the slab kernel.
 //
 // The slab kernel (b2_slabconv.cuh) reads the A tile of every (dt, dh, dw) tap from shared memory for an MMA of N = Cout columns.
-// With Cout = 64 a 128 x 64 x 16 MMA moves 4 KB of A + 2 KB of B per 32 math cycles: it is shared-memory-operand bound (ncu:
-// tensor pipe 41% active on the 3x3x3 C64 layers, 14% of the resnet3d50 step).  An input frame f contributes to the three output
+// With Cout = 64 a 128 x 64 x 16 MMA moves 4 KB of A + 2 KB of B per 32 math cycles: it is shared-memory-operand bound.  An input frame f contributes to the three output
 // frames f-1, f, f+1 through the temporal taps dt = 2, 1, 0 with the SAME in-plane shift, so here a work item owns a group of three
 // consecutive output frames (to0, to0+1, to0+2) of one spatial tile and walks the five input frames to0-1 .. to0+3:
 //     input frame (relative) fr = 0..4 feeds output slots s in [max(0, fr-2), min(2, fr)] with temporal tap dt = fr - s,
@@ -10,11 +9,11 @@
 // a CONTIGUOUS row range of that stack and a contiguous column range of the accumulator [tile][slot][64]: one MMA of N = 64, 128 or
 // 192 per (in-plane tap, K step) instead of one N = 64 MMA per (temporal tap, in-plane tap, K step).  Five A tiles are read where the
 // plain form reads nine, and the operand bytes per MMA column drop from 96 to 53 (N = 192): 304 instead of 432 shared-memory cycles
-// per in-plane tap.  Accumulators start from zero (tcgen05.st by the epilogue, as in the stem kernel), so every MMA accumulates and
+// per in-plane tap.  Accumulators start from zero (stored by the epilogue, as in the stem kernel), so every MMA accumulates and
 // slots may receive their first contribution from different input frames.
 //
 // Same building blocks as the slab kernel: 4-D TMA halo slabs (SWIZZLE_128B, zero-filled padding), shifted descriptors for the
-// in-plane taps, persistent CTAs, TMA producer warp / MMA warp / 8 epilogue warps.  Stride 1, kt = 3, pt = 1, plain per-channel affine.
+// in-plane taps, persistent CTAs, TMA producer warp / MMA warpgroup / 8 epilogue warps.  Stride 1, kt = 3, pt = 1, plain per-channel affine.
 #pragma once
 
 #include "b2_slabconv.cuh"
@@ -72,12 +71,12 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
   uint64_t* w_empty = w_full + kSlabWStages;
   uint64_t* acc_full = w_empty + kSlabWStages;      // [1]
   uint64_t* acc_empty = acc_full + 2;               // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   float* s_scale = reinterpret_cast<float*>(tail + 256);
   float* s_shift = s_scale + p.naff;
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int tile_cols = kTsGroup * kTsBN;            // accumulator columns of one M tile: [slot][64]
+  const AccTile at{s_shift + p.naff, acc_ld(p.MT * tile_cols)};
 
   if (tid == 128) {
     for (int s = 0; s < kSlabSStages; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 1); }
@@ -87,19 +86,15 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 5) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
   for (int i = tid; i < p.naff; i += kSlabThreads) {
     s_scale[i] = (i < p.Ncols) ? __ldg(&p.scale[i]) : 0.f;
     s_shift[i] = (i < p.Ncols) ? __ldg(&p.shift[i]) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();
 
-  if (warp == 4) {
+  if (warp == kSlabTmaWarp) {
     // ================================ TMA producer ======================================
     int wit = 0, sg = 0;
     int item = blockIdx.x;
@@ -150,22 +145,19 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
         }
       }
     }
-  } else if (warp == 5) {
-    // ================================ MMA issuer ========================================
-    const uint32_t tm = warp_uniform(tmem_base);
+  } else if (warp >= kSlabMmaWarp0) {
+    // ================================ MMA warpgroup =====================================
     const uint32_t slab0 = smem_u32(slab_base), w0s = smem_u32(w_base);
     const int ntaps = p.sub_ntaps[0];
     int wit = 0, sg = 0, lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const SlabTsItem w = slabts_item(p, item);
       mbar_wait(&acc_empty[0], lt & 1);                    // the epilogue has drained AND re-zeroed the accumulators
-      tc_fence_after();
       const int nfr = w.fr_hi - w.fr_lo + 1;
       for (int si = 0; si < w.n_slabs; ++si, ++sg) {
         const int cc = si / nfr, fr = w.fr_lo + (si - cc * nfr);
         const int s_lo = max(0, fr - 2), s_hi = min(w.nf - 1, fr);          // output slots this input frame feeds
         const int nslots = s_hi - s_lo + 1;                                 // >= 1 for every valid frame
-        const uint32_t idesc = make_idesc_f16(128, static_cast<uint32_t>(nslots * kTsBN), 0);
         const uint32_t b_row = static_cast<uint32_t>(2 - (fr - s_lo));      // first row block of the stack: dt = fr - s_lo
         const int ksteps = min(4, (p.C - cc * 64 + 15) >> 4);
         const int s = sg % kSlabSStages;
@@ -174,35 +166,25 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
         for (int ti = 0; ti < ntaps; ++ti, ++wit) {
           const int ws = wit % kSlabWStages;
           mbar_wait(&w_full[ws], (wit / kSlabWStages) & 1);
-          tc_fence_after();
           const int pix0 = w.q0 + p.sub_off[0][ti] - w.r_lo * p.PW;
           const uint32_t b_lo = sw128_desc_lo(w0s + ws * kTsWBytes + b_row * (kTsBN * 128));
           const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u);
-          if (elect_one()) {
-            for (int j = 0; j < w.mt_valid; ++j) {
-              const uint32_t a_lo = a_lo0 + j * (128u * 128u >> 4);
-              const uint32_t d = tm + j * tile_cols + s_lo * kTsBN;
-              for (int k = 0; k < ksteps; ++k)
-                umma_f16(d, desc_from(kSw128DescHi, a_lo + 2 * k), desc_from(kSw128DescHi, b_lo + 2 * k), idesc, 1u);
-            }
-            umma_commit(&w_empty[ws]);
-            if (ti == ntaps - 1) umma_commit(&slab_empty[s]);
-            if (ti == ntaps - 1 && si == w.n_slabs - 1) umma_commit(&acc_full[0]);
-          }
-          __syncwarp();
+          for (int j = 0; j < w.mt_valid; ++j)
+            wg_mma(at, j * tile_cols + s_lo * kTsBN, nslots * kTsBN,
+                   wg_sw128(desc_from(kSw128DescHi, a_lo0 + j * (128u * 128u >> 4)), desc_from(kSw128DescHi, b_lo)), ksteps, true);
+          wg_sync();
+          wg_arrive(&w_empty[ws]);
+          if (ti == ntaps - 1) wg_arrive(&slab_empty[s]);
+          if (ti == ntaps - 1 && si == w.n_slabs - 1) wg_arrive(&acc_full[0]);
         }
       }
     }
   } else {
     // ================================ epilogue ==========================================
     const int erow = (warp & 3) * 32 + (tid & 31);
-    const int egroup = warp >= 6 ? 1 : 0;
-    const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t acc = tmem_base + lane_off;
+    const int egroup = warp >= 4 ? 1 : 0;
     const int used_cols = p.MT * tile_cols;
-    for (int c = egroup * 32; c < used_cols; c += 64) tmem_st32_zero(acc + c);     // accumulators start at zero
-    tmem_st_wait();
-    tc_fence_before();
+    for (int c = egroup * 32; c < used_cols; c += 64) acc_zero32(at, erow, c);     // accumulators start at zero
     mbar_arrive(&acc_empty[0]);
     const size_t plane_rows = static_cast<size_t>(p.Ho) * p.Wo;
     int lt = 0;
@@ -225,15 +207,13 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
       for (int c = 0; c < 32; ++c) { sc[c] = s_scale[c0 + c]; sh[c] = s_shift[c0 + c]; }
       const int ncols_here = min(kTsBN, p.ldy);
       mbar_wait(&acc_full[0], lt & 1);
-      tc_fence_after();
 #pragma unroll 1
       for (int s = 0; s < w.nf; ++s) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           if (j < w.mt_valid) {                            // warp-uniform
             uint32_t v[32];
-            tmem_ld32(acc + j * tile_cols + s * kTsBN + c0, v);
-            tmem_ld_wait();
+            acc_ld32(at, erow, j * tile_cols + s * kTsBN + c0, v);
             if (ok[j]) {
               const size_t r = row[j] + s * plane_rows;
               __half* yrow = p.y + r * p.ldy + c0;
@@ -263,16 +243,10 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
           }
         }
       }
-      for (int c = egroup * 32; c < used_cols; c += 64) tmem_st32_zero(acc + c);   // hand the accumulators back zeroed (this group's chunks)
-      tmem_st_wait();
-      tc_fence_before();
+      for (int c = egroup * 32; c < used_cols; c += 64) acc_zero32(at, erow, c);   // hand the accumulators back zeroed (this group's chunks)
       mbar_arrive(&acc_empty[0]);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace b2

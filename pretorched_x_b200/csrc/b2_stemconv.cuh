@@ -4,31 +4,33 @@
 // Input is NDHWC4 (8 bytes per pixel).  For a fixed temporal/vertical tap (dt, dh) the 7 horizontal taps of
 // output pixel wo read the 8 consecutive pixels [2wo-4, 2wo+4) (pixel 2wo-4 carries a zero weight; it only keeps
 // the run 16-byte aligned): 32 fp16 = 64 contiguous bytes, and the run of output pixel wo+1 starts exactly
-// 16 bytes later.  A K-major SWIZZLE_NONE tcgen05 operand is addressed as
+// 16 bytes later.  A K-major SWIZZLE_NONE wgmma operand is addressed as
 //     byte(row r, 16-byte chunk j) = start + (r % 8) * 16 + (r / 8) * SBO + j * LBO,
 // so with LBO = 16 and SBO = 128 the 128 x 32 im2col tile of one input row is an overlapping (Toeplitz) view of
 // the raw row sitting in shared memory (verified by tools/probe_umma.py, mode 1): no thread touches the data on
 // its way to the tensor core.
 //
 // Input-row-stationary schedule.  Slab row i (input row 2*ho0 - ph + i) feeds local output row g through vertical
-// tap dh = i - 2g, i.e. up to 4 consecutive output rows.  The per-row accumulators sit side by side in TMEM (row g
-// at column BN*g) and the weight image stores the taps of one parity class in *decreasing* dh order, so all of
-// those contributions are ONE MMA: A = the Toeplitz tile of slab row i, B = [W(dh_max); W(dh_max-2); ...]
-// (N = BN x #taps, up to 256), D = the accumulator columns of the touched output rows.  Compared with one N=64
-// MMA per (output row, dh) every A tile is read from shared memory once instead of up to 4 times and 4x fewer
-// instructions are issued: the kernel moves from smem-operand-bound to tensor-bound.  Accumulators start from
-// zero (tcgen05.st by the epilogue warps), so every MMA accumulates.
+// tap dh = i - 2g, i.e. up to G consecutive output rows.  The per-row accumulators sit side by side in the accumulator
+// tile (row g at column BN*g) and the weight image stores the taps of one parity class in *decreasing* dh order, so
+// all of those contributions are ONE MMA: A = the Toeplitz tile of slab row i, B = [W(dh_max); W(dh_max-2); ...]
+// (N = BN x #taps, up to kStemAccCols), D = the accumulator columns of the touched output rows.  Every A tile is read
+// from shared memory once per slab row instead of once per (output row, dh).  Accumulators start from zero (stored
+// by the epilogue warps), so every MMA accumulates.
 //
-// Persistent CTAs (one per SM) walk (plane, row-group, column-tile) work items; TMEM holds two accumulator sets
-// so the epilogue of item i (BN + ReLU -> fp16 NDHWC) overlaps the MMAs of item i+1.
-// Warps 0-3 and 6-9: epilogue (the two warpgroups split the 32-column chunks), warp 4: TMA/bulk-copy producer, warp 5: MMA issuer.
+// Persistent CTAs (one per SM) walk (plane, row-group, column-tile) work items; two accumulator sets in shared memory
+// let the epilogue of item i (BN + ReLU -> fp16 NDHWC) overlap the MMAs of item i+1.
+// Warps 0-7: epilogue (the two warpgroups split the 32-column chunks), 8-11: MMA warpgroup, 12: TMA/bulk-copy producer.
 #pragma once
 
 #include "b2_ptx.cuh"
 
 namespace b2 {
 
-constexpr int kStemThreads = 320;       // warps 0-3 and 6-9: epilogue (even / odd 32-column chunks), 4: producer, 5: MMA issuer
+constexpr int kStemThreads = 416;       // warps 0-7: epilogue (even / odd 32-column chunks), 8-11: MMA warpgroup, 12: producer
+constexpr int kStemMmaWarp0 = 8;
+constexpr int kStemTmaWarp = 12;
+constexpr int kStemAccCols = 128;       // one accumulator set: G * BN columns
 constexpr int kStemPitch = 2048;        // bytes per slab row: 256 pixels [2*w0-4, 2*w0+252) of 8 bytes
 constexpr int kStemRowPx = 256;         // TMA box width (the maximum box extent), one 8-byte element per pixel
 constexpr int kStemTileW = 120;         // output columns per item: rows r < 124 of the 128-row MMA tile see complete runs
@@ -40,7 +42,7 @@ struct StemParams {
   int To, Ho, Wo;
   int kt, kh;              // kw == 7, strides (1, 2, 2)
   int pt, ph;
-  int G;                   // output rows per item (G * BN <= 256)
+  int G;                   // output rows per item (G * BN <= kStemAccCols)
   int rows;                // slab rows = 2*(G-1) + kh
   int stage_bytes;         // slab + weights of one temporal tap, multiple of 128
   int w_bytes;             // kh * BN * 64: weight image of one temporal tap for one N tile
@@ -109,14 +111,14 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
   uint64_t* empty = full + kStemMaxStages;
   uint64_t* acc_full = empty + kStemMaxStages;                 // [2]
   uint64_t* acc_empty = acc_full + 2;                          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   float* s_scale = reinterpret_cast<float*>(tail + 128);       // [256] (ntiles_n * BN <= 256 is enforced by the host)
   float* s_shift = s_scale + 256;
   uint32_t* s_xchg = reinterpret_cast<uint32_t*>(s_shift + 256);   // [2 groups][2][4][16]: lane 31 of each epilogue warp, for the W pool
+  const AccTile at{reinterpret_cast<float*>(s_xchg + 256), acc_ld(2 * kStemAccCols)};
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int slab_bytes = p.rows * kStemPitch;
-  constexpr int kAccCols = 256;                                // one accumulator set: G * BN <= 256 columns
+  constexpr int kAccCols = kStemAccCols;
 
   if (tid == 128) {
     for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
@@ -124,19 +126,15 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
     fence_mbar_init();
     tma_prefetch_desc(&tmX);
   }
-  if (warp == 5) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
   for (int i = tid; i < 256; i += kStemThreads) {
     s_scale[i] = (i < p.Ncols) ? __ldg(&p.scale[i]) : 0.f;
     s_shift[i] = (i < p.Ncols) ? __ldg(&p.shift[i]) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();                       // everything above touched only weights / on-chip state
 
-  if (warp == 4) {
+  if (warp == kStemTmaWarp) {
     // ================================ producer ==========================================
     int it = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x) {
@@ -156,12 +154,12 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
         __syncwarp();
       }
     }
-  } else if (warp == 5) {
-    // ================================ MMA issuer ========================================
-    // SWIZZLE_NONE K-major descriptors: hi = SBO >> 4 | version; lo = addr >> 4 | (LBO >> 4) << 16
-    constexpr uint32_t a_hi = (128u >> 4) | (1u << 14), b_hi = (512u >> 4) | (1u << 14);
+  } else if (warp >= kStemMmaWarp0) {
+    // ================================ MMA warpgroup =====================================
+    // SWIZZLE_NONE K-major descriptors: hi = SBO >> 4; lo = addr >> 4 | (LBO >> 4) << 16.  A: SBO 128 B (64 rows = 1 KB),
+    // K step 32 B; B: SBO 512 B (16 rows = 1 KB), LBO 128 B, K step 256 B.
+    constexpr uint32_t a_hi = 128u >> 4, b_hi = 512u >> 4;
     constexpr uint32_t kTapBytes = BN * 64;            // weight image of one (dt, dh) tap: BN rows x 32 k
-    const uint32_t tm = warp_uniform(tmem_base);
     const uint32_t base = smem_u32(smem);
     int it = 0, lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
@@ -170,41 +168,32 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
       const int g_valid = min(p.G, p.Ho - w.ho0);
       const int ab = lt & 1;
       mbar_wait(&acc_empty[ab], (lt >> 1) & 1);            // the epilogue has drained and re-zeroed this set
-      tc_fence_after();
-      const uint32_t acc = tm + ab * kAccCols;
+      const int acc = ab * kAccCols;
       for (int dt = dt_lo; dt <= dt_hi; ++dt, ++it) {
         const int s = it % p.nstages;
         mbar_wait(&full[s], (it / p.nstages) & 1);
-        tc_fence_after();
         const uint32_t slab = base + s * p.stage_bytes;
         const uint32_t wbase = slab + slab_bytes;
-        if (elect_one()) {
-          for (int i = 0; i < p.rows; ++i) {
-            const int g_lo = p.row_glo[i];
-            const int g_hi = min(static_cast<int>(p.row_ghi[i]), g_valid - 1);
-            if (g_lo > g_hi) continue;
-            const uint32_t idesc = make_idesc_f16(128, static_cast<uint32_t>(g_hi - g_lo + 1) * BN, 0);
-            const uint32_t a_lo = ((slab + static_cast<uint32_t>(i) * kStemPitch) >> 4) | ((16u >> 4) << 16);
-            const uint32_t b_lo = ((wbase + static_cast<uint32_t>(p.row_slot[i]) * kTapBytes) >> 4) | ((128u >> 4) << 16);
-            const uint32_t d = acc + g_lo * BN;
-            umma_f16(d, desc_from(a_hi, a_lo), desc_from(b_hi, b_lo), idesc, 1u);
-            umma_f16(d, desc_from(a_hi, a_lo + 2), desc_from(b_hi, b_lo + 16), idesc, 1u);
-          }
-          umma_commit(&empty[s]);
-          if (dt == dt_hi) umma_commit(&acc_full[ab]);
+        for (int i = 0; i < p.rows; ++i) {
+          const int g_lo = p.row_glo[i];
+          const int g_hi = min(static_cast<int>(p.row_ghi[i]), g_valid - 1);
+          if (g_lo > g_hi) continue;
+          const uint32_t a_lo = ((slab + static_cast<uint32_t>(i) * kStemPitch) >> 4) | ((16u >> 4) << 16);
+          const uint32_t b_lo = ((wbase + static_cast<uint32_t>(p.row_slot[i]) * kTapBytes) >> 4) | ((128u >> 4) << 16);
+          const WgOperands ops{desc_from(a_hi, a_lo), desc_from(b_hi, b_lo), 2u, 64u, 16u, 256u, 64u};
+          wg_mma(at, acc + g_lo * BN, (g_hi - g_lo + 1) * BN, ops, 2, true);
         }
-        __syncwarp();
+        wg_sync();
+        wg_arrive(&empty[s]);
+        if (dt == dt_hi) wg_arrive(&acc_full[ab]);
       }
     }
   } else {
     // ================================ epilogue ==========================================
-    // a warp may only touch TMEM lanes 32*(warp%4)..+31: pixel (row) index of this thread, and its warpgroup's column chunks
-    const int ew = warp & 3, egroup = warp >= 6 ? 1 : 0;
+    // pixel (accumulator row) index of this thread, and its warpgroup's column chunks
+    const int ew = warp & 3, egroup = warp >= 4 ? 1 : 0;
     const int erow = ew * 32 + (tid & 31);
-    const uint32_t lane_off = static_cast<uint32_t>(ew * 32) << 16;
-    for (int c = egroup * 32; c < 512; c += 64) tmem_st32_zero(tmem_base + lane_off + c);   // both accumulator sets start at zero
-    tmem_st_wait();
-    tc_fence_before();
+    for (int c = egroup * 32; c < 2 * kAccCols; c += 64) acc_zero32(at, erow, c);   // both accumulator sets start at zero
     mbar_arrive(&acc_empty[0]);
     mbar_arrive(&acc_empty[1]);
     int lt = 0;
@@ -218,8 +207,7 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
       const int plane_out = p.pair ? 2 * w.plane_o + (erow >> 6) : w.plane_o;
       const bool col_ok = p.pair ? (wo < p.Wo && plane_out < p.planes_total) : ((erow < kStemTileW) && (wo < p.Wo));
       mbar_wait(&acc_full[ab], (lt >> 1) & 1);
-      tc_fence_after();
-      const uint32_t acc = tmem_base + lane_off + ab * kAccCols;
+      const int acc = ab * kAccCols;
       if (p.pool_w) {
         // ---- BN + ReLU, then max over the 3-wide / stride-2 window along W before anything is written ----
         // thread tid holds output column wo = tid (one column tile per row); even columns 2wp produce pooled column wp from
@@ -233,8 +221,7 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
 #pragma unroll 1
           for (int jc = egroup; jc < BN / 32; jc += 2, ++xit) {
             uint32_t v[32];
-            tmem_ld32(acc + g * BN + jc * 32, v);
-            tmem_ld_wait();
+            acc_ld32(at, erow, acc + g * BN + jc * 32, v);
             uint32_t h[16];
 #pragma unroll
             for (int e = 0; e < 16; ++e) {
@@ -277,8 +264,7 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
 #pragma unroll 1
         for (int jc = egroup; jc < BN / 32; jc += 2) {
           uint32_t v[32];
-          tmem_ld32(acc + g * BN + jc * 32, v);
-          tmem_ld_wait();
+          acc_ld32(at, erow, acc + g * BN + jc * 32, v);
           if (col_ok) {
 #pragma unroll
             for (int c8 = 0; c8 < 4; ++c8) {
@@ -299,16 +285,10 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
           }
         }
       }
-      for (int c = egroup * 32; c < kAccCols; c += 64) tmem_st32_zero(acc + c);   // hand the set back zeroed (this group's chunks)
-      tmem_st_wait();
-      tc_fence_before();
+      for (int c = egroup * 32; c < kAccCols; c += 64) acc_zero32(at, erow, acc + c);   // hand the set back zeroed (this group's chunks)
       mbar_arrive(&acc_empty[ab]);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace b2

@@ -2,36 +2,36 @@
 // SpatioTemporalConv of R(2+1)D whose output is 64 wide (r2plus1d.py:85-88 -- the stem's (7,1,1) C110->64 and the twelve
 // (3,1,1) C144->64 of layer1 in R(2+1)D-34), with the outer BN / residual / ReLU in the epilogue.
 //
-// Why its own kernel.  With Cout = 64 a 128 x 64 x 16 MMA is bound by the A-operand feed from shared memory, not by math: ~75
-// cycles against 32 (ncu: tensor pipe 41% active; DESIGN.md section 3c), so the slab kernel -- one N = 64 MMA per (temporal tap, K step)
-// -- runs these layers at 0.36-0.41 of their roofline.  An input frame f contributes to the output frames f-pt .. f+pt through the
-// taps dt = kt-1 .. 0 with the SAME A tile (128 positions x 64 channels of frame f), so here the accumulators of G = 4 consecutive
-// output frames sit side by side in TMEM ([slot][64 columns]) and the weights are stacked [W(dt=kt-1); ...; W(dt=0)] (64 rows each):
-// the slots an input frame feeds are a CONTIGUOUS row range of that stack and a contiguous column range of the accumulator set,
-// and one MMA of N = 64 x (slots fed) <= 256 replaces up to four N = 64 MMAs on the same A tile.  Per output frame a (3,1,1) filter
-// issues 1.5 A-tile passes instead of 3, a (7,1,1) filter 2.5 instead of 7, most of them at N = 192 / 256 where the feed is paid once.
+// Why its own kernel.  With Cout = 64 a 128 x 64 x 16 MMA is bound by the A-operand feed from shared memory, not by math, so the
+// slab kernel -- one N = 64 MMA per (temporal tap, K step) -- pays that feed once per tap.  An input frame f contributes to the output frames f-pt .. f+pt through the
+// taps dt = kt-1 .. 0 with the SAME A tile (128 positions x 64 channels of frame f), so here the accumulators of G = 2 consecutive
+// output frames sit side by side in the accumulator tile ([slot][64 columns]) and the weights are stacked [W(dt=kt-1); ...; W(dt=0)]
+// (64 rows each): the slots an input frame feeds are a CONTIGUOUS row range of that stack and a contiguous column range of the
+// accumulator tile, and one MMA of N = 64 x (slots fed) <= 128 replaces up to two N = 64 MMAs on the same A tile.
 // b2_slabts.cuh does the same for 3 x kh x kw filters but streams a 24 KB weight stack per (tap, input frame) from L2, which is what
-// made it lose on 1x1 in-plane filters (64 vs 31 us, DESIGN.md section 3c).  Here the in-plane filter is 1x1: the whole filter is
+// made it lose on 1x1 in-plane filters.  Here the in-plane filter is 1x1: the whole filter is
 // kt x ceil(C/64) blocks of 8 KB (72 KB for C144, 112 KB for C110 x 7 taps) and stays RESIDENT in shared memory, loaded once per CTA
 // before griddepcontrol.wait (weights do not depend on the previous kernel); A tiles are plain [128 positions][64 channels] TMA boxes
-// (no halo, rows past the end of a frame zero-filled), and with one M tile per item TWO accumulator sets (2 x 256 TMEM columns) let
-// the epilogue of item i -- residual rows requested before the accumulators are even complete -- overlap the MMAs of item i + 1.
+// (no halo, rows past the end of a frame zero-filled).  The accumulator tile (128 x 128 fp32, 66 KB) shares the 227 KB of shared
+// memory with the resident filter (up to 112 KB) and a 2-stage A ring, which is what bounds G and leaves room for one set only.
 //
-//   warp 4   TMA producer: resident weights once, then the A tiles of (item, input frame, channel chunk) through a 4-stage ring
-//   warp 5   MMA issuer: per input frame one MMA of N = 64 x slots per K step into accumulator set (item & 1); all MMAs accumulate
-//            (the epilogue hands accumulators back zeroed, tcgen05.st, so slots may start from different input frames)
-//   warps 0-3, 6-9   epilogue: thread = one position (TMEM lane) x 32 channels; affine (+ residual) (+ ReLU), 16-byte stores
+//   warp 12      TMA producer: resident weights once, then the A tiles of (item, input frame, channel chunk) through the ring
+//   warps 8-11   MMA warpgroup: per input frame one MMA of N = 64 x slots per K step; all MMAs accumulate
+//                (the epilogue hands the accumulators back zeroed, so slots may start from different input frames)
+//   warps 0-7    epilogue: thread = one position (accumulator row) x 32 channels; affine (+ residual) (+ ReLU), 16-byte stores
 #pragma once
 
 #include "b2_ptx.cuh"
 
 namespace b2 {
 
-constexpr int kTkThreads = 320;
-constexpr int kTkStages = 4;                 // A-tile ring depth
+constexpr int kTkThreads = 416;
+constexpr int kTkMmaWarp0 = 8;
+constexpr int kTkTmaWarp = 12;
+constexpr int kTkStages = 2;                 // A-tile ring depth
 constexpr int kTkABytes = 128 * 128;         // one A tile: 128 positions x 64 fp16 channels, SWIZZLE_128B
-constexpr int kTkG = 4;                      // output frames (accumulator slots) per work item
-constexpr int kTkSetCols = kTkG * 64;        // TMEM columns of one accumulator set
+constexpr int kTkG = 2;                      // output frames (accumulator slots) per work item
+constexpr int kTkSetCols = kTkG * 64;        // accumulator columns
 constexpr int kTkWBlock = 64 * 128;          // one (channel chunk, temporal tap) weight block: 64 output rows x 128 B
 
 struct TstackParams {
@@ -83,33 +83,29 @@ tstack_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, HW, 1, 
   uint64_t* a_full = reinterpret_cast<uint64_t*>(tail);
   uint64_t* a_empty = a_full + kTkStages;
   uint64_t* w_full = a_empty + kTkStages;             // [1]
-  uint64_t* acc_full = w_full + 1;                    // [2]
-  uint64_t* acc_empty = acc_full + 2;                 // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* s_scale = reinterpret_cast<float*>(tail + 128);   // barriers + TMEM slot occupy the first 108 bytes
+  uint64_t* acc_full = w_full + 1;                    // [1]
+  uint64_t* acc_empty = acc_full + 1;                 // [1]
+  float* s_scale = reinterpret_cast<float*>(tail + 128);   // barriers occupy the first 64 bytes
   float* s_shift = s_scale + 64;
+  const AccTile at{reinterpret_cast<float*>(tail + 128 + 512), acc_ld(kTkSetCols)};
 
   const int tid = threadIdx.x, warp = tid >> 5;
 
   if (tid == 128) {
     for (int s = 0; s < kTkStages; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
     mbar_init(&w_full[0], 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 256); }
+    mbar_init(acc_full, 1); mbar_init(acc_empty, 256);
     fence_mbar_init();
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 5) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
   if (tid < 64) {
     s_scale[tid] = (tid < p.Ncols) ? __ldg(&p.scale[tid]) : 0.f;
     s_shift[tid] = (tid < p.Ncols) ? __ldg(&p.shift[tid]) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
-  if (warp == 4) {
+  if (warp == kTkTmaWarp) {
     // resident filter: block (cc, r) holds W(dt = kt-1-r) for channels [64 cc, 64 cc + 64); rows >= K and columns past the
     // tensor's extent are zero-filled by TMA (columns past C inside a tap hold the next tap's weights: the activation side
     // zero-fills channels >= C and the K loop stops at the last 16-channel step that holds real channels)
@@ -123,7 +119,7 @@ tstack_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, HW, 1, 
   }
   pdl_wait();                       // everything above touched only weights / on-chip state
 
-  if (warp == 4) {
+  if (warp == kTkTmaWarp) {
     // ================================ TMA producer ======================================
     int it = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x) {
@@ -140,54 +136,39 @@ tstack_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, HW, 1, 
         }
       }
     }
-  } else if (warp == 5) {
-    // ================================ MMA issuer ========================================
-    // whole warp, warp-uniform operands; one elected lane issues (see elect_one())
-    const uint32_t tm = warp_uniform(tmem_base);
+  } else if (warp >= kTkMmaWarp0) {
+    // ================================ MMA warpgroup =====================================
     const uint32_t a0s = smem_u32(a_base), w0s = smem_u32(w_base);
     mbar_wait(&w_full[0], 0);
-    tc_fence_after();
     int it = 0, lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const TstackItem w = tstack_item(p, item);
-      const int ab = lt & 1;
-      mbar_wait(&acc_empty[ab], (lt >> 1) & 1);            // the epilogue has drained AND re-zeroed this accumulator set
-      tc_fence_after();
-      const uint32_t dset = tm + ab * kTkSetCols;
+      mbar_wait(acc_empty, lt & 1);                        // the epilogue has drained AND re-zeroed the accumulators
       for (int fr = w.fr_lo; fr <= w.fr_hi; ++fr) {
         const int s_lo = max(0, fr - (p.kt - 1)), s_hi = min(w.nf - 1, fr);   // output slots this input frame feeds (>= 1)
-        const uint32_t idesc = make_idesc_f16(128, static_cast<uint32_t>((s_hi - s_lo + 1) * 64), 0);
         const int r0 = p.kt - 1 - (fr - s_lo);                              // first block of the stack: dt = fr - s_lo
-        const uint32_t d = dset + s_lo * 64;
         for (int cc = 0; cc < p.cchunks; ++cc, ++it) {
           const int ksteps = min(4, (p.C - cc * 64 + 15) >> 4);              // 16-channel K steps that hold real channels
           const int s = it % kTkStages;
           mbar_wait(&a_full[s], (it / kTkStages) & 1);
-          tc_fence_after();
           const uint32_t a_lo = sw128_desc_lo(a0s + s * kTkABytes);
           const uint32_t b_lo = sw128_desc_lo(w0s + (cc * p.kt + r0) * kTkWBlock);
-          if (elect_one()) {
-            for (int k = 0; k < ksteps; ++k)
-              umma_f16(d, desc_from(kSw128DescHi, a_lo + 2 * k), desc_from(kSw128DescHi, b_lo + 2 * k), idesc, 1u);
-            umma_commit(&a_empty[s]);
-            if (fr == w.fr_hi && cc == p.cchunks - 1) umma_commit(&acc_full[ab]);
-          }
-          __syncwarp();
+          wg_mma(at, s_lo * 64, (s_hi - s_lo + 1) * 64, wg_sw128(desc_from(kSw128DescHi, a_lo), desc_from(kSw128DescHi, b_lo)), ksteps,
+                 true);
+          wg_sync();
+          wg_arrive(&a_empty[s]);
+          if (fr == w.fr_hi && cc == p.cchunks - 1) wg_arrive(acc_full);
         }
       }
     }
   } else {
     // ================================ epilogue ==========================================
-    // a warp may only touch TMEM lanes 32*(warp%4)..+31; the two warpgroups split the 64 channels of a slot
+    // thread = accumulator row; the two warpgroups split the 64 channels of a slot
     const int erow = (warp & 3) * 32 + (tid & 31);
-    const int egroup = warp >= 6 ? 1 : 0;
+    const int egroup = warp >= 4 ? 1 : 0;
     const int c0 = egroup * 32;
-    const uint32_t acc = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-    for (int c = c0; c < 2 * kTkSetCols; c += 64) tmem_st32_zero(acc + c);     // both sets start at zero (this group's chunks)
-    tmem_st_wait();
-    tc_fence_before();
-    mbar_arrive(&acc_empty[0]);
-    mbar_arrive(&acc_empty[1]);
+    for (int c = c0; c < kTkSetCols; c += 64) acc_zero32(at, erow, c);     // the accumulators start at zero (this group's chunks)
+    mbar_arrive(acc_empty);
     float sc[32], sh[32];
 #pragma unroll
     for (int c = 0; c < 32; ++c) { sc[c] = s_scale[c0 + c]; sh[c] = s_shift[c0 + c]; }
@@ -195,31 +176,26 @@ tstack_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, HW, 1, 
     int lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const TstackItem w = tstack_item(p, item);
-      const int ab = lt & 1;
       const bool ok = w.q0 + erow < p.HW;
       const size_t row0 = static_cast<size_t>(w.plane_o0) * p.HW + w.q0 + erow;     // slot s: + s * HW
-      // residual rows of the first two slots are requested before the accumulators are complete, slot s + 2 while slot s is processed
-      uint4 rres[3][4];
+      // residual rows of both slots are requested before the accumulators are complete
+      uint4 rres[kTkG][4];
       auto load_res = [&](int s) {
         if (p.residual && ok && s < w.nf) {
           const __half* rrow = p.residual + (row0 + static_cast<size_t>(s) * p.HW) * p.ldr + c0;
 #pragma unroll
           for (int c8 = 0; c8 < 4; ++c8)
-            if (c0 + c8 * 8 < ncols_here) rres[s % 3][c8] = __ldg(reinterpret_cast<const uint4*>(rrow + c8 * 8));
+            if (c0 + c8 * 8 < ncols_here) rres[s][c8] = __ldg(reinterpret_cast<const uint4*>(rrow + c8 * 8));
         }
       };
       load_res(0);
       load_res(1);
-      mbar_wait(&acc_full[ab], (lt >> 1) & 1);
-      tc_fence_after();
-      const uint32_t aset = acc + ab * kTkSetCols + c0;
+      mbar_wait(acc_full, lt & 1);
 #pragma unroll
       for (int s = 0; s < kTkG; ++s) {
         if (s < w.nf) {                                      // warp-uniform
-          load_res(s + 2);
           uint32_t v[32];
-          tmem_ld32(aset + s * 64, v);                       // warp-collective: outside the `ok` branch
-          tmem_ld_wait();
+          acc_ld32(at, erow, s * 64 + c0, v);
           if (ok) {
             __half* yrow = p.y + (row0 + static_cast<size_t>(s) * p.HW) * p.ldy + c0;
 #pragma unroll
@@ -227,7 +203,7 @@ tstack_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, HW, 1, 
               if (c0 + c8 * 8 < ncols_here) {
                 uint32_t rr[4] = {0u, 0u, 0u, 0u};
                 if (p.residual) {
-                  const uint4 rv = rres[s % 3][c8];
+                  const uint4 rv = rres[s][c8];
                   rr[0] = rv.x; rr[1] = rv.y; rr[2] = rv.z; rr[3] = rv.w;
                 }
                 uint32_t o[4];
@@ -246,16 +222,10 @@ tstack_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, HW, 1, 
           }
         }
       }
-      for (int c = 0; c < kTkSetCols; c += 64) tmem_st32_zero(aset + c);   // hand the set back zeroed (this group's chunks)
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(&acc_empty[ab]);
+      for (int c = c0; c < kTkSetCols; c += 64) acc_zero32(at, erow, c);   // hand the accumulators back zeroed (this group's chunks)
+      mbar_arrive(acc_empty);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace b2

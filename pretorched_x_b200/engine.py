@@ -1,5 +1,5 @@
 """Forward engine: walks a (reference-layout) module tree and replaces the bodies of its hot blocks by
-fused sm_100a kernels.
+fused sm_90a kernels.
 
 The nn.Modules in ``models/`` are *parameter containers* that keep the reference's ``state_dict``
 layout; nothing in them computes.  This file holds the block bodies:
@@ -21,7 +21,7 @@ NOT seen: ``model.invalidate()`` / ``engine.invalidate(model)`` drops every pack
 Every block body is entered through a ``torch.autograd.Function`` (``functions.py``, SURVEY.md section 8b-ii): the
 Function's ``forward`` is the ctypes call sequence, its outputs are marked non-differentiable (frozen-backbone
 semantics: the engine has no backward for the convolutional trunk), and the dense heads (``last_linear``, the TRN
-relation MLPs) have a real backward on the same tcgen05 GEMM so that a head can be trained on engine features.
+relation MLPs) have a real backward on the same wgmma GEMM so that a head can be trained on engine features.
 """
 import os
 
@@ -179,7 +179,7 @@ def _plain_1x1(conv):
 def _fused_close_with_projection(block, a, h, out=None):
     """conv3 + bn3 + (downsample conv + bn)(x) + ReLU as ONE two-operand GEMM (resnet3D.py:136-143 with the type-B
     shortcut of resnet3D.py:176-185): both BatchNorm scales are folded into the fp16 weight matrices, both products
-    accumulate in the same TMEM tile, and the projected shortcut never goes through HBM."""
+    accumulate in the same accumulator tile, and the projected shortcut never goes through HBM."""
     ds_conv, ds_bn = block.downsample[0], block.downsample[1]
     stride = _conv_geometry(ds_conv)[0]
     xs = a if stride == (1, 1, 1) else ops.shortcut_a(a, stride[0], a.C)
@@ -446,19 +446,16 @@ def _stem_body(model, a, simt=False, out=None):
 # Clips are independent in every layer (eval-mode BN, per-clip attention), so the trunk may be walked in any clip order.  The
 # breadth-first walk (one launch per layer over the whole batch) is the default.  ``set_dfs("units:clips,...")`` walks consecutive
 # segments of trunk units DEPTH-first instead -- a chunk of a few clips goes through stem, pool and a run of residual blocks before
-# the next chunk starts, so that a chunk's intermediates are write-then-read inside the 126 MB L2 (the allocator hands the next
+# the next chunk starts, so that a chunk's intermediates are write-then-read inside the 50 MB L2 (the allocator hands the next
 # chunk the same addresses) and only a segment's first input and last output cross HBM; the last kernel of a chunk writes straight
-# into its row range of the whole-batch tensor (``out=``).  MEASURED on B200 (tools/dfs_sweep.py, profiles/dfs_sweep_r02.txt): it
-# never pays.  resnet3d50 at 32 clips of 16x224x224: 3.72 ms breadth-first; stem + layer1 in chunks of 8 / 4 / 2 / 1 clips: 4.07 /
-# 4.25 / 4.88 / 6.53 ms; same picture for R(2+1)D-34, the non-local net, resnet18 and the BigGAN generator.  Every extra launch of
-# these persistent kernels costs 6-9 us of pipeline fill, drain and tile quantisation, and the layers that look HBM-bound (1x1x1
-# convolutions at 0.83 of the copy rate) do not speed up when their operands are L2-resident.  The schedule stays as an opt-in
-# (same kernels per output element: results equal the breadth-first walk up to kernel-dispatch boundaries) with the evidence.
+# into its row range of the whole-batch tensor (``out=``).  Every extra launch of these persistent kernels costs pipeline fill,
+# drain and tile quantisation, so breadth-first is the default; tools/dfs_sweep.py times the alternatives.  The schedule stays as
+# an opt-in (same kernels per output element: results equal the breadth-first walk up to kernel-dispatch boundaries).
 _DFS_SPEC = os.environ.get("B2_DFS", "off")
 
 
 def set_dfs(spec):
-    """Trunk schedule: ``"off"`` (breadth-first, the default and the measured optimum) or an explicit
+    """Trunk schedule: ``"off"`` (breadth-first, the default) or an explicit
     ``"units:clips,units:clips"`` list -- consecutive segments of trunk units (unit 0 = stem + pool, then the residual blocks in
     order), each walked depth-first in chunks of ``clips``; units not covered run breadth-first."""
     global _DFS_SPEC
@@ -475,7 +472,7 @@ def _trunk_units(model):
 def dfs_plan(model=None, N=None, geom=None):
     """[(units, clips per chunk)] for ``run_trunk`` (empty = breadth-first)."""
     spec = _DFS_SPEC.strip().lower()
-    if spec in ("0", "off", "none", "", "auto"):       # "auto" = the measured rule: never chunk
+    if spec in ("0", "off", "none", "", "auto"):       # "auto" = the default rule: never chunk
         return []
     return [tuple(int(v) for v in part.split(":")) for part in spec.split(",")]
 

@@ -11,7 +11,7 @@ Two kinds:
   ``last_linear``, README.md:520-547).  There is no backward for the convolutional trunk: asking for one raises.
 * **Dense heads with a real backward** -- ``LinearFunction`` (``last_linear`` / ``fc``: resnet3D.py:162,
   torchvision_models.py:463-464) and, built from it, the TRN relation MLP (trn.py:39-49).  ``forward`` and both
-  gradient products run on the same tcgen05 GEMM (``b2_gemm_f16``: fp16 operands, fp32 accumulation and output), so a
+  gradient products run on the same wgmma GEMM (``b2_gemm_f16``: fp16 operands, fp32 accumulation and output), so a
   head can be trained on engine features without leaving the library.
 
 Tensors cross a Function boundary as the raw ``[N*T*H*W][ld]`` fp16 matrix of an ``ops.Act`` plus its geometry tuple.
@@ -126,7 +126,7 @@ def _unit_affine(n, dev):
 
 
 class LinearFunction(torch.autograd.Function):
-    """y = x W^T + b on tcgen05 (fp16 operands, fp32 accumulate / output), with
+    """y = x W^T + b on wgmma (fp16 operands, fp32 accumulate / output), with
     dL/dx = g W, dL/dW = g^T x, dL/db = sum_rows g computed by the same kernel (D = A . B^T with K-major operands:
     the gradient products take the transposed fp16 copies as their operands)."""
 

@@ -1,7 +1,7 @@
 """CUDA-graph replay of a whole forward pass.
 
 A forward of resnet3d50 is ~75 kernel launches, each preceded by a Python -> ctypes crossing and a host-side
-CUtensorMap encode; at B200 speeds that host work is comparable to the device time.  Capturing the launch
+CUtensorMap encode; at H100 speeds that host work is comparable to the device time.  Capturing the launch
 sequence once (static shapes, buffers from the graph's private pool) removes it: the timed step is one
 ``cudaGraphLaunch``.  All C-ABI entry points are capture-safe (no syncs, no allocations).
 """

@@ -1,4 +1,4 @@
-"""BigGAN-deep generator on the B200 engine (BASELINE.json configs[4]; SURVEY.md section 8a row a14 / 8f row n1).
+"""BigGAN-deep generator on the H100 engine (BASELINE.json configs[4]; SURVEY.md section 8a row a14 / 8f row n1).
 
 The reference tree has **no GAN code** (nothing to be a drop-in for), so the boundary kept here is the one the public
 BigGAN-deep implementation established and that published checkpoints use: a ``Generator`` whose ``state_dict`` has
@@ -12,7 +12,7 @@ BigGAN-deep implementation established and that published checkpoints use: a ``G
 
 and whose ``forward(z, y)`` takes z fp32 ``[B, dim_z]`` and either class indices (int64 ``[B]``) or an already embedded
 ``[B, shared_dim]`` tensor.  The modules below are *parameter containers* only (like every other model in this
-package); the arithmetic is ``pretorched_x_b200/biggan_engine.py`` on hand-written sm_100a kernels.  Evaluation mode
+package); the arithmetic is ``pretorched_x_b200/biggan_engine.py`` on hand-written sm_90a kernels.  Evaluation mode
 only: BatchNorm uses ``stored_mean/var`` (standing statistics), spectral norm divides by the sigma obtained from one
 power-iteration step off the stored ``u0`` (no update).
 """

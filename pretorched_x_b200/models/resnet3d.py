@@ -3,7 +3,7 @@
 The classes here are parameter containers: they create exactly the tensors of the reference's
 ``state_dict`` (same names, shapes, registration and RNG order, so a seeded random init is
 bit-identical and zoo checkpoints load unchanged), while every ``forward`` body delegates to
-``pretorched_x_b200.engine`` -- fused sm_100a kernels, fp16 NDHWC activations.
+``pretorched_x_b200.engine`` -- fused sm_90a kernels, fp16 NDHWC activations.
 
 Drop-in surface kept (SURVEY.md section 8b): ``resnet3d10..200`` / ``resneti3d50`` factories with the
 reference signatures, ``features / logits / forward``, a swappable ``last_linear`` (``fc`` is None as

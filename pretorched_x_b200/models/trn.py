@@ -3,7 +3,7 @@
 ``Relation`` (trn.py:20-56) is ReLU -> Linear(T*F, bottleneck) -> ReLU -> Linear(bottleneck, out) over the
 concatenated frame features; ``MultiScaleRelation`` (trn.py:59-113) sums such MLPs over sub-sampled frame
 tuples of every scale.  Both keep the reference's parameter names (``relate.1.*``, ``relate.3.*``,
-``relations.{i}.relate.*``); the bodies run as tcgen05 GEMMs with the bias / ReLU in the epilogue and the
+``relations.{i}.relate.*``); the bodies run as wgmma GEMMs with the bias / ReLU in the epilogue and the
 cross-tuple sum accumulated in fp32 by the second GEMM.
 
 Upstream defects mirrored, not fixed (SURVEY.md section 0.6-0.8): ``HierarchicalRelation`` with depth > 0

@@ -51,7 +51,7 @@ def _on_device(fn):
 
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise RuntimeError("%s must live on a CUDA (sm_100a) device: this engine has no CPU path" % what)
+        raise RuntimeError("%s must live on a CUDA (sm_90a) device: this engine has no CPU path" % what)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -330,7 +330,7 @@ def conv(a, pc, residual=None, relu=False, simt=False, sample_affine=None, resid
 @_on_device
 def gemm(a2d, b2d, scale, shift, M, N, Kd, residual=None, relu=False, per_row=False, out=None, out_f32=False,
          accumulate=False, second=None, aff_rows=0, next_affine=None):
-    """D[M][N] = act(scale * A[M][Kd] . B[N][Kd]^T + shift + residual) on tcgen05 (b2_gemm_f16).
+    """D[M][N] = act(scale * A[M][Kd] . B[N][Kd]^T + shift + residual) on wgmma (b2_gemm_f16).
     ``second=(A2, B2, K2)`` adds A2[M][K2] . B2[N][K2]^T into the same accumulator (b2_gemm2_f16)."""
     dev = a2d.device
     if out is None:

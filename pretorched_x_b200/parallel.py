@@ -1,7 +1,7 @@
 """Data-parallel inference over the GPUs of one box: one process per GPU, clips sharded on dim 0, weights
 replicated by one broadcast, a single all-gather of the logits per step.
 
-This is the B200 counterpart of the reference's only multi-GPU construct, ``torch.nn.DataParallel(model)``
+This is the H100 counterpart of the reference's only multi-GPU construct, ``torch.nn.DataParallel(model)``
 (examples/imagenet_eval.py:136, nonlocalnet.py:604): scatter the batch, run replicas, gather outputs.  Clips are
 independent (eval-mode BN, per-sample attention), so the data path needs no collective until the
 ``[B/world, num_classes]`` fp32 logits are gathered -- a few KB per rank, latency-bound, issued on NCCL over

@@ -141,7 +141,7 @@ class TransformImage(object):
 
     def _to_device_u8(self, img):
         if self.device is None:
-            raise RuntimeError("TransformImage runs on a CUDA (sm_100a) device: this engine has no CPU path")
+            raise RuntimeError("TransformImage runs on a CUDA (sm_90a) device: this engine has no CPU path")
         if isinstance(img, torch.Tensor):
             t = img
         else:

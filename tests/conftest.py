@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100a) GPU; run with `-m gpu` on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU; run with `-m gpu`")
 
 
 @pytest.fixture(scope="session")
@@ -17,9 +17,9 @@ def golden_dir():
     return os.path.join(ROOT, "tests", "golden")
 
 
-def has_b200():
+def has_h100():
     try:
         import torch
-        return torch.cuda.is_available() and torch.cuda.get_device_capability(0)[0] == 10
+        return torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (9, 0)
     except Exception:
         return False

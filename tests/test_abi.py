@@ -1,4 +1,4 @@
-"""CPU: the C-ABI shared library builds for sm_100a, loads, and exports every symbol include/b2_pretorched.h
+"""CPU: the C-ABI shared library builds for sm_90a, loads, and exports every symbol include/b2_pretorched.h
 declares; the ctypes struct mirrors match the C layout.  No compute call is made (no GPU here)."""
 import ctypes
 import os
@@ -49,16 +49,15 @@ def test_ctypes_structs_match_c_layout(tmp_path):
                     ctypes.sizeof(_lib.GemmArgs), _lib.GemmArgs.M.offset, _lib.GemmArgs.accumulate.offset]
 
 
-def test_sass_contains_blackwell_tensor_core_and_tma_instructions():
+def test_sass_contains_hopper_tensor_core_and_tma_instructions():
     cuobjdump = "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", _lib.lib_path()], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass      # tcgen05.mma
-    assert "LDTM" in sass         # tcgen05.ld
+    assert "HGMMA" in sass        # wgmma
     assert "UTMALDG" in sass      # TMA load
     assert "UTMASTG" in sass      # TMA store
-    assert "HMMA." not in sass.replace("UTCHMMA", "")   # no legacy mma.sync path
+    assert "HMMA." not in sass    # no legacy mma.sync path
 
 
 def test_argument_validation_needs_no_gpu():

@@ -30,7 +30,7 @@ FIX = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "biggan
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     return torch.device("cuda:0")
 
 

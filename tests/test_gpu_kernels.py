@@ -18,7 +18,7 @@ TOL_F32 = 1e-4
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     from pretorched_x_b200 import _lib
     _lib.load()
     return torch.device("cuda:0")
@@ -230,7 +230,8 @@ def test_nonlocal_attention_matches_oracle(dev, case):
 @pytest.mark.parametrize("two_pass", [False, True], ids=["single_pass", "two_pass"])
 def test_attention_with_growing_logits(dev, two_pass):
     """Keys whose norm grows along the sequence: the running row maximum jumps by far more than 2^8 several times, so
-    the single-pass kernel must rescale its TMEM accumulator (lazy rescaling) -- and agree with the exact two-pass one."""
+    the single-pass kernel must rescale its register-resident output accumulator (lazy rescaling) -- and agree with the exact
+    two-pass one."""
     from pretorched_x_b200 import ops, _lib
     B, Npos, d, dv = 2, 700, 128, 256
     g = torch.Generator().manual_seed(77)

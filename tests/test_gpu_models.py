@@ -28,7 +28,7 @@ MODEL_FIX = [g for g in GOLDEN if torch.load(g, weights_only=False)["kind"] == "
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     return torch.device("cuda:0")
 
 
@@ -360,7 +360,7 @@ def test_multiscale_relation_is_graph_capturable(dev):
 
 def test_trainable_head_on_frozen_engine_features(dev):
     """torch.autograd.Function boundary: the trunk is a frozen feature extractor (non-differentiable outputs), the dense head has
-    a real backward on the tcgen05 GEMM.  Gradients of last_linear match torch's fp32 autograd on the same pooled features."""
+    a real backward on the wgmma GEMM.  Gradients of last_linear match torch's fp32 autograd on the same pooled features."""
     torch.manual_seed(0)
     m = OF.randomize_bn_(P.resnet3d18(num_classes=7, pretrained=None), 1).eval().to(dev)
     x = OF.seeded_input((3, 3, 8, 64, 64), 4).to(dev).requires_grad_(True)

@@ -19,7 +19,7 @@ FIX = [g for g in sorted(glob.glob(os.path.join(os.path.dirname(__file__), "gold
 @pytest.mark.timeout(240, method="thread")        # first hardware run of this family: a stuck kernel must fail, not hang the tier
 @pytest.mark.parametrize("path", FIX, ids=[os.path.basename(p)[:-3] for p in FIX])
 def test_resnext3d_forward_matches_reference_golden(path):
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     dev = torch.device("cuda:0")
     fx = torch.load(path, weights_only=False)
     torch.manual_seed(fx["seeds"]["init"])

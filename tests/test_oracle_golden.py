@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from oracle import functional as OF
-from oracle import reference_loader as RL
+from oracle.make_golden_state import state_sha256
 import pretorched_x_b200 as P
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.pt")))
@@ -79,19 +79,21 @@ def test_multiscale_relation_fixture():
     assert torch.equal(y, y2)
 
 
-@pytest.mark.skipif(not RL.available(), reason="/root/reference not present (GPU box)")
+def assert_state_identical_to_reference(arch, build):
+    """The seeded state_dict equals the reference's: same keys in the same order, same dtypes, shapes and bytes (one SHA-256 over
+    all of them, recorded from the unmodified reference by oracle/make_golden_state.py)."""
+    import json
+    with open(os.path.join(os.path.dirname(__file__), "golden", "reference_state_sha256.json")) as fh:
+        case = next(c for c in json.load(fh) if c["arch"] == arch)
+    torch.manual_seed(case["seed"])
+    sd = build(**case["kwargs"]).state_dict()
+    assert len(sd) == case["n_state"] and state_sha256(sd) == case["sha256"], arch
+
+
 def test_state_dict_identical_to_live_reference():
-    RL.load(); RL.load_r2plus1d()
-    for arch, kw in [("r2plus1d18", dict(num_classes=400)), ("resnet3d50", dict(num_classes=400)),
-                     ("nonlocalresnet3d50", dict())]:
-        torch.manual_seed(3)
-        ref = RL.build(arch, **kw)
-        torch.manual_seed(3)
-        ours = getattr(P, arch)(**kw) if arch.startswith("r2") else getattr(P, arch)(pretrained=None, **kw)
-        a, b = ref.state_dict(), ours.state_dict()
-        assert list(a) == list(b)
-        for k in a:
-            assert torch.equal(a[k], b[k]), (arch, k)
+    for arch in ("r2plus1d18", "resnet3d50", "nonlocalresnet3d50"):
+        fn = getattr(P, arch)
+        assert_state_identical_to_reference(arch, fn if arch.startswith("r2") else (lambda fn=fn, **kw: fn(pretrained=None, **kw)))
 
 
 SF_FIX = [g for g in GOLDEN if torch.load(g, weights_only=False)["kind"] == "slowfast"]
@@ -173,22 +175,9 @@ def test_resnext_fixtures_present():
     assert len(RX_FIX) >= 2
 
 
-@pytest.mark.skipif(not RL.available(), reason="/root/reference not present (GPU box)")
 def test_resnext3d_state_dict_identical_to_live_reference():
-    import warnings
-    RL.load()
-    for arch, kw in [("resnext3d50", dict(num_classes=400)), ("resnext3d18", dict(num_classes=10, shortcut_type="A")),
-                     ("resnext3d101", dict())]:
-        with warnings.catch_warnings():
-            warnings.simplefilter("ignore")
-            torch.manual_seed(5)
-            ref = RL.build(arch, **kw)
-        torch.manual_seed(5)
-        ours = getattr(P, arch)(**kw)
-        a, b = ref.state_dict(), ours.state_dict()
-        assert list(a) == list(b)
-        for k in a:
-            assert torch.equal(a[k], b[k]), (arch, k)
+    for arch in ("resnext3d50", "resnext3d18", "resnext3d101"):
+        assert_state_identical_to_reference(arch, getattr(P, arch))
     assert P.models.resnext3d.pretrained_settings["resnext3d101"]["kinetics-400"]["url"].endswith("resnext3d101_kinetics-8e57b772.pth")
     assert P.models.resnext3d.pretrained_settings["resnext3d50"]["kinetics-400"]["url"] is None
 

@@ -1,4 +1,4 @@
-"""Probe tcgen05 smem-descriptor semantics on the GPU (see csrc/b2_probe.cu).  Prints which variants are exact."""
+"""Probe wgmma smem-descriptor semantics on the GPU (see csrc/b2_probe.cu).  Prints which variants are exact."""
 import ctypes
 import os
 import sys

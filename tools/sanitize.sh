@@ -1,7 +1,7 @@
 #!/bin/bash
 # compute-sanitizer passes over one small forward of every model family (SURVEY.md section 5 "race detection / sanitizers").
 # Only this library's kernels (namespace b2) are instrumented; torch's own element-wise kernels are skipped to keep the run short.
-# memcheck / synccheck gate (exit code 7 on a finding).  racecheck (`all`) is logged for reading: tcgen05 / TMA traffic runs through
+# memcheck / synccheck gate (exit code 7 on a finding).  racecheck (`all`) is logged for reading: wgmma / TMA traffic runs through
 # the async proxy and cluster barriers order DSMEM traffic, neither of which it models.  initcheck is not run: with only this
 # library's kernels instrumented every buffer written by a torch kernel (inputs, folded BN affines) reads as "uninitialised".
 O=gpurun_out/sanitizer; mkdir -p $O

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """SASS instruction counts per kernel of the shipped library (cuobjdump -sass; runs without a GPU): the mnemonics that prove
-tcgen05 / TMEM / TMA are what the kernels execute (B200_PROFILING.md), and that no mma.sync (HMMA) path exists.
+wgmma / TMA are what the kernels execute, and that no mma.sync (HMMA) path exists.
 usage: python tools/sass_summary.py [out.txt]"""
 import collections
 import os
@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from pretorched_x_b200 import _lib  # noqa: E402
 
-COLS = ["UTCHMMA", "UTCBAR", "UTMALDG", "UTMASTG", "UTMAPF", "LDTM", "STTM", "UTCATOM", "SYNCS", "LDGSTS", "HMMA", "MUFU", "LDS", "STS",
+COLS = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "SYNCS", "LDGSTS", "HMMA", "MUFU", "LDS", "STS",
         "LDG", "STG"]
 
 
@@ -37,8 +37,8 @@ def main():
             for c in COLS:
                 if op.startswith(c):
                     counts[cur][c] += 1
-    out = ["SASS instruction counts per kernel of libb2pretorched.so (cuobjdump -sass, sm_100a): tcgen05.mma = UTCHMMA, tcgen05.commit = UTCBAR,",
-           "TMA load / store / prefetch = UTMALDG / UTMASTG / UTMAPF, tcgen05.ld / st = LDTM / STTM, TMEM alloc = UTCATOMSWS, mbarrier = SYNCS,",
+    out = ["SASS instruction counts per kernel of libb2pretorched.so (cuobjdump -sass, sm_90a): wgmma = HGMMA, wgmma fence / wait = WARPGROUP,",
+           "TMA load / store / prefetch = UTMALDG / UTMASTG / UTMAPF, mbarrier = SYNCS,",
            "cp.async = LDGSTS; HMMA (mma.sync) must be 0 everywhere.", "",
            "%-60s" % "kernel" + "".join("%8s" % c for c in COLS) + "%8s" % "total"]
     for name in order:
