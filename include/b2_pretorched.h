@@ -97,6 +97,11 @@ typedef struct b2_conv_args {
                             To*Ho*Wo % 128 == 0                                                                           */
   const float* in_shift;
   int32_t in_aff_ld;
+  const void* mask;     /* nullable fp16 [M][ldm] (ldm % 8 == 0, ldm >= ldy): y = (scale * acc + shift + residual) where mask > 0,
+                           else 0, in fp32 before the single rounding -- the ReLU derivative of the fine-tuning backward.  fp16
+                           output without relu / per-sample affine / generator extras; taken by the persistent GEMM and the
+                           implicit-GEMM kernel only (the dispatcher skips every other path for a masked call)              */
+  int32_t ldm;
 } b2_conv_args;
 
 int b2_conv_ndhwc_fprop(const b2_conv_args* a, void* stream);
@@ -143,6 +148,8 @@ typedef struct b2_gemm_args {
   const float* scale2;
   const float* shift2;
   int32_t aff2_ld, aff2_rows;
+  const void* mask;     /* nullable fp16 [M][ldm] ReLU-derivative mask of the output, see b2_conv_args.mask */
+  int32_t ldm;
 } b2_gemm_args;
 int b2_gemm_f16(const b2_gemm_args* a, void* stream);
 /* D = act(scale * (A.B^T + A2.B2^T) + shift + residual): both products accumulate in the same accumulator tile.  Used to
@@ -198,6 +205,37 @@ int b2_gather_frames(const void* x, void* y, const int32_t* idx_dev, int N, int 
  * device (one table for the whole forward, filled by a single host->device copy: trn.py:100-110 without a copy per tuple). */
 int b2_gather_frame_tuples(const void* x, void* y, const int32_t* idx_dev, int N, int T, int F, int n_idx, int n_tuples,
                            void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Fine-tuning backward of the residual blocks (the backward of resnet3D.py:91-143 with eval-mode BatchNorm).  Gradients
+ * travel between kernels as fp16 NDHWC matrices multiplied by a device-resident power-of-two loss scale; the fp32 results
+ * (weight, gamma and beta gradients) divide it out.  `inv_loss_scale` / `scale_pair` are DEVICE pointers.
+ * ------------------------------------------------------------------------------------------- */
+/* Weight gradient of a k x k x k convolution (k = 1, padding 0, or k = 3, padding 1; stride 1 or 2) on wgmma:
+ *     G[co][ci][tap] = sum over output positions p of g[p][co] * x[stride * p + tap - pad][ci]
+ *     dw[co][ci][tap] = scale[co] * G * inv_loss_scale      (fp32, nn.Conv3d.weight layout [Cout][Cin][k][k][k])
+ *     wdot[co]        = sum_{ci,tap} w[co][ci][tap] * G * inv_loss_scale      (nullable; needs w, fp32 same layout)
+ * g: fp16 [N*To*Ho*Wo][ldg] (gradient at the convolution output), x: fp16 [N*T*H*W][ldx] (its input).  scale and
+ * inv_loss_scale nullable (= 1).  ws: fp32 workspace of b2_conv_wgrad_workspace_elems(...) elements; the result does not
+ * depend on how the position sum is split (fixed-order reduction, no atomics). */
+size_t b2_conv_wgrad_workspace_elems(int N, int T, int H, int W, int Cin, int Cout, int k, int stride, int pad);
+int b2_conv_wgrad(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
+                  float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int Cin, int Cout, int k,
+                  int stride, int pad, void* stream);
+/* Adjoint of b2_shortcut_a_ndhwc: y[n, s*to, s*ho, s*wo, 0:C] = g[n, to, ho, wo, 0:C] for the low-resolution extent
+ * To = (T-1)/s + 1 (etc.), every other pixel and channels [C, ldy) zero; y is [N*T*H*W][ldy].  The backward of the type-A
+ * shortcut, the placement of the type-B projection gradient, and the zero-insertion that turns the input gradient of a
+ * stride-2 3x3x3 convolution into a stride-1 convolution with the flipped filter. */
+int b2_zero_insert_ndhwc(const void* g, int ldg, int C, void* y, int ldy, int N, int T, int H, int W, int stride, void* stream);
+/* out[c] = inv_loss_scale * sum_r g[r][c] (fp32, fixed-order two-pass reduction; ws: b2_colsum_workspace_elems(C) floats). */
+size_t b2_colsum_workspace_elems(int C);
+int b2_colsum_f16(const void* g, int ldg, long long rows, int C, const float* inv_loss_scale, float* out, float* ws, void* stream);
+/* scale_pair = [2^k, 2^-k] with max |g| * 2^k in [2^7, 2^8) (k = 0 when g is all zero or has a non-finite entry). */
+int b2_loss_scale_f32(const float* g, int rows, int cols, int ldg, float* scale_pair, void* stream);
+/* Backward of b2_avgpool_global_ndhwc followed by the block's closing ReLU: y[n*S + p][c] = fp16(gf[n][c] * scale_pair[0] / S)
+ * where out[n*S + p][c] > 0, else 0 (channels [C, ld) zero).  gf fp32 [N][ldf]; out, y fp16 [N*S][ld]. */
+int b2_avgpool_global_backward(const float* gf, int ldf, const float* scale_pair, const void* out, void* y, int N, int S, int C,
+                               int ld, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Image preprocessing on the device -- TransformImage (pretorched/transforms/utils.py:34-81; used by

@@ -38,6 +38,7 @@ class ConvArgs(ctypes.Structure):
         ("relu", c_i32), ("out_f32", c_i32), ("accumulate", c_i32), ("mode", c_i32), ("aff_ld", c_i32), ("upsample", c_i32), ("residual_up", c_i32), ("residual_pre", c_i32),
         ("y2", c_void_p), ("scale2", c_void_p), ("shift2", c_void_p), ("aff2_ld", c_i32), ("pool_w", c_i32),
         ("in_scale", c_void_p), ("in_shift", c_void_p), ("in_aff_ld", c_i32),
+        ("mask", c_void_p), ("ldm", c_i32),
     ]
 
 
@@ -51,6 +52,7 @@ class GemmArgs(ctypes.Structure):
         ("per_row", c_i32), ("relu", c_i32), ("out_f32", c_i32), ("accumulate", c_i32),
         ("aff_ld", c_i32), ("aff_rows", c_i32),
         ("d2", c_void_p), ("scale2", c_void_p), ("shift2", c_void_p), ("aff2_ld", c_i32), ("aff2_rows", c_i32),
+        ("mask", c_void_p), ("ldm", c_i32),
     ]
 
 
@@ -85,6 +87,13 @@ SYMBOLS = {
     "b2_ccbn_act_ndhwc": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p]),
     "b2_rgb_head_gather_tanh": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "b2_tanh_nhwc_to_nchw": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, ctypes.c_longlong, c_int, c_void_p]),
+    "b2_conv_wgrad_workspace_elems": (ctypes.c_size_t, [c_int] * 9),
+    "b2_conv_wgrad": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 6 + [ctypes.c_size_t] + [c_int] * 9 + [c_void_p]),
+    "b2_zero_insert_ndhwc": (c_int, [c_void_p, c_int, c_int, c_void_p] + [c_int] * 6 + [c_void_p]),
+    "b2_colsum_workspace_elems": (ctypes.c_size_t, [c_int]),
+    "b2_colsum_f16": (c_int, [c_void_p, c_int, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_loss_scale_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "b2_avgpool_global_backward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
 }
 
 

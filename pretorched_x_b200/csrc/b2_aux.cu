@@ -414,6 +414,109 @@ __global__ void gather_frames_kernel(const __half* __restrict__ x, __half* __res
   reinterpret_cast<uint4*>(y)[i] = __ldg(reinterpret_cast<const uint4*>(x + (n * T + idx[t * n_idx + j]) * (long long)(F8 * 8)) + f8);
 }
 
+// ------------------------------------------------------------------------------------------
+// fine-tuning backward helpers
+// ------------------------------------------------------------------------------------------
+// Adjoint of shortcut_a_kernel: y[n, s*to, s*ho, s*wo, 0:C] = g[n, to, ho, wo, 0:C], every other pixel and channels [C, ldy)
+// zero.  y has the full-resolution extent (T, H, W); s * (To - 1) <= T - 1 for To = (T - 1) / s + 1.
+__global__ void zero_insert_kernel(const __half* __restrict__ g, int ldg8, int C8, __half* __restrict__ y, int ldy8, int T, int H,
+                                   int W, int s, int To, int Ho, int Wo, long long total) {
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c8 = (int)(i % ldy8);
+  long long q = i / ldy8;
+  const int w = (int)(q % W); q /= W;
+  const int h = (int)(q % H); q /= H;
+  const int t = (int)(q % T);
+  const long long n = q / T;
+  uint4 v = make_uint4(0, 0, 0, 0);
+  if (c8 < C8 && t % s == 0 && h % s == 0 && w % s == 0 && t / s < To && h / s < Ho && w / s < Wo)
+    v = __ldg(reinterpret_cast<const uint4*>(g) + (((n * To + t / s) * Ho + h / s) * Wo + w / s) * ldg8 + c8);
+  reinterpret_cast<uint4*>(y)[i] = v;
+}
+
+// Column sums of an fp16 matrix in two fixed-order passes: CTA (column block of 32, row chunk) -> part[chunk][c], then
+// out[c] = inv * sum_chunk part[chunk][c].
+constexpr int kColsumChunks = 128;
+__global__ void __launch_bounds__(256) colsum_partial_kernel(const __half* __restrict__ g, int ldg, long long rows, int C,
+                                                             float* __restrict__ part) {
+  __shared__ float red[8][33];
+  const int c = blockIdx.x * 32 + threadIdx.x;
+  const long long r0 = rows * blockIdx.y / kColsumChunks, r1 = rows * (blockIdx.y + 1) / kColsumChunks;
+  float acc = 0.f;
+  if (c < C)
+    for (long long r = r0 + threadIdx.y; r < r1; r += 8) acc += __half2float(g[r * ldg + c]);
+  red[threadIdx.y][threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.y == 0 && c < C) {
+    float t = 0.f;
+    for (int j = 0; j < 8; ++j) t += red[j][threadIdx.x];
+    part[(long long)blockIdx.y * C + c] = t;
+  }
+}
+__global__ void colsum_final_kernel(const float* __restrict__ part, int C, const float* __restrict__ inv, float* __restrict__ out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  float t = 0.f;
+  for (int j = 0; j < kColsumChunks; ++j) t += part[(long long)j * C + c];
+  out[c] = t * (inv ? *inv : 1.f);
+}
+
+// Power-of-two loss scale from the largest |g| of the gradient entering the trunk: max|g| lands in [2^7, 2^8), leaving 2^8
+// of fp16 headroom for growth through the blocks.  sc = [scale, 1 / scale].  Non-finite values leave the scale at 2^0 so
+// that they reach the parameter gradients unchanged.
+__global__ void __launch_bounds__(1024) loss_scale_kernel(const float* __restrict__ g, int rows, int cols, int ldg,
+                                                          float* __restrict__ sc) {
+  __shared__ float red[32];
+  __shared__ int bad_any;
+  if (threadIdx.x == 0) bad_any = 0;
+  __syncthreads();
+  float m = 0.f;
+  int bad = 0;
+  const long long total = (long long)rows * cols;
+  for (long long i = threadIdx.x; i < total; i += blockDim.x) {
+    const float v = fabsf(g[(i / cols) * ldg + i % cols]);
+    if (!(v <= FLT_MAX)) bad = 1;
+    else m = fmaxf(m, v);
+  }
+  if (bad) atomicOr(&bad_any, 1);
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_down_sync(0xffffffffu, m, off));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int j = 1; j < (int)(blockDim.x >> 5); ++j) m = fmaxf(m, red[j]);
+    int e = 0;
+    if (m > 0.f && !bad_any) frexpf(m, &e);              // m = f * 2^e, f in [0.5, 1)
+    int k = (m > 0.f && !bad_any) ? 8 - e : 0;
+    k = k > 100 ? 100 : (k < -100 ? -100 : k);
+    sc[0] = ldexpf(1.f, k);
+    sc[1] = ldexpf(1.f, -k);
+  }
+}
+
+// Backward of the global average pool: y[n*S + p][c] = fp16(gf[n][c] * scale / S) where the pooled block output was
+// positive (its closing ReLU), 0 elsewhere and in channels [C, ld).
+__global__ void pool_backward_kernel(const float* __restrict__ gf, int ldf, const float* __restrict__ sc, const __half* __restrict__ out,
+                                     __half* __restrict__ y, int S, int C, int ld8, long long total) {
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c8 = (int)(i % ld8);
+  const long long r = i / ld8;
+  const long long n = r / S;
+  const float f = sc[0] / (float)S;
+  const uint4 mk = __ldg(reinterpret_cast<const uint4*>(out) + i);
+  const __half* mh = reinterpret_cast<const __half*>(&mk);
+  uint4 v;
+  __half* vh = reinterpret_cast<__half*>(&v);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int c = c8 * 8 + j;
+    vh[j] = __float2half_rn((c < C && __half2float(mh[j]) > 0.f) ? gf[n * ldf + c] * f : 0.f);
+  }
+  reinterpret_cast<uint4*>(y)[i] = v;
+}
+
 }  // namespace b2
 
 using namespace b2;
@@ -574,6 +677,47 @@ int b2_gather_frame_tuples(const void* x, void* y, const int32_t* idx_dev, int N
 
 int b2_gather_frames(const void* x, void* y, const int32_t* idx_dev, int N, int T, int F, int n_idx, void* stream) {
   return b2_gather_frame_tuples(x, y, idx_dev, N, T, F, n_idx, 1, stream);
+}
+
+int b2_zero_insert_ndhwc(const void* g, int ldg, int C, void* y, int ldy, int N, int T, int H, int W, int stride, void* stream) {
+  B2_CHECK_ARG(g && y && N > 0 && T > 0 && H > 0 && W > 0 && stride > 0, "bad argument");
+  B2_CHECK_ARG(C % 8 == 0 && ldg % 8 == 0 && ldy % 8 == 0 && ldg >= C && ldy >= C, "channel counts and pitches must be multiples of 8");
+  const int To = (T - 1) / stride + 1, Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  const long long total = (long long)N * T * H * W * (ldy / 8);
+  zero_insert_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      (const __half*)g, ldg / 8, C / 8, (__half*)y, ldy / 8, T, H, W, stride, To, Ho, Wo, total);
+  B2_CHECK_LAUNCH("zero_insert");
+  return B2_OK;
+}
+
+size_t b2_colsum_workspace_elems(int C) { return (size_t)kColsumChunks * (C > 0 ? C : 0); }
+
+int b2_colsum_f16(const void* g, int ldg, long long rows, int C, const float* inv_loss_scale, float* out, float* ws, void* stream) {
+  B2_CHECK_ARG(g && out && ws && rows > 0 && C > 0 && ldg >= C, "bad argument");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  colsum_partial_kernel<<<dim3(div_up(C, 32), kColsumChunks), dim3(32, 8), 0, st>>>((const __half*)g, ldg, rows, C, ws);
+  B2_CHECK_LAUNCH("colsum_partial");
+  colsum_final_kernel<<<div_up(C, 256), 256, 0, st>>>(ws, C, inv_loss_scale, out);
+  B2_CHECK_LAUNCH("colsum_final");
+  return B2_OK;
+}
+
+int b2_loss_scale_f32(const float* g, int rows, int cols, int ldg, float* scale_pair, void* stream) {
+  B2_CHECK_ARG(g && scale_pair && rows > 0 && cols > 0 && ldg >= cols, "bad argument");
+  loss_scale_kernel<<<1, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>(g, rows, cols, ldg, scale_pair);
+  B2_CHECK_LAUNCH("loss_scale");
+  return B2_OK;
+}
+
+int b2_avgpool_global_backward(const float* gf, int ldf, const float* scale_pair, const void* out, void* y, int N, int S, int C,
+                               int ld, void* stream) {
+  B2_CHECK_ARG(gf && scale_pair && out && y && N > 0 && S > 0 && C > 0 && ldf >= C, "bad argument");
+  B2_CHECK_ARG(ld % 8 == 0 && ld >= C, "channel pitch %d is not a multiple of 8 >= C", ld);
+  const long long total = (long long)N * S * (ld / 8);
+  pool_backward_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      gf, ldf, scale_pair, (const __half*)out, (__half*)y, S, C, ld / 8, total);
+  B2_CHECK_LAUNCH("pool_backward");
+  return B2_OK;
 }
 
 }  // extern "C"

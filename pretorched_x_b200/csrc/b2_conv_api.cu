@@ -126,6 +126,27 @@ int make_tmap_ndhwc_slab(CUtensorMap* out, const void* base, uint64_t C, uint64_
   return B2_OK;
 }
 
+int make_tmap_ndhwc_5d(CUtensorMap* out, const void* base, uint64_t C, uint64_t ld, uint64_t W, uint64_t H, uint64_t T,
+                       uint64_t N, uint32_t box_w, uint32_t box_h, uint32_t stride_hw) {
+  PFN_encodeTiled enc = get_encode_tiled();
+  if (!enc) return set_error(B2_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no driver?)");
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0) return set_error(B2_ERR_INVALID, "tensor base not 16-byte aligned");
+  if (ld % 8 != 0 || ld < C) return set_error(B2_ERR_INVALID, "channel pitch %llu must be a multiple of 8 and >= %llu",
+                                              (unsigned long long)ld, (unsigned long long)C);
+  cuuint64_t dims[5] = {C, W, H, T, N};
+  cuuint64_t strides[4] = {ld * 2, W * ld * 2, H * W * ld * 2, T * H * W * ld * 2};
+  cuuint32_t box[5] = {64, stride_hw * (box_w - 1) + 1, stride_hw * (box_h - 1) + 1, 1, 1};
+  cuuint32_t estr[5] = {1, stride_hw, stride_hw, 1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(base), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return set_error(B2_ERR_CUDA, "cuTensorMapEncodeTiled(5d) failed (%d) C=%llu ld=%llu W=%llu H=%llu T=%llu N=%llu", (int)r,
+                     (unsigned long long)C, (unsigned long long)ld, (unsigned long long)W, (unsigned long long)H,
+                     (unsigned long long)T, (unsigned long long)N);
+  return B2_OK;
+}
+
 // ------------------------------------------------------------------------------------------
 // slab convolution launcher (stride 1, "same" padding)
 // ------------------------------------------------------------------------------------------
@@ -609,10 +630,10 @@ struct IgemmLaunch {
   int b_cols;             // logical K extent of B
 };
 
-template <int BN>
+template <int BN, int MASK>
 static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   using S = IgemmSmem<BN>;
-  B2_OPT_IN_SMEM(igemm_kernel<BN>, S::kTotalBytes);
+  B2_OPT_IN_SMEM((igemm_kernel<BN, MASK>), S::kTotalBytes);
   const IgemmParams& p = L.p;
   CUtensorMap tmA, tmB, tmC, tmR;
   memset(&tmA, 0, sizeof(tmA)); memset(&tmC, 0, sizeof(tmC)); memset(&tmR, 0, sizeof(tmR));
@@ -638,7 +659,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     tmC = tmB; tmR = tmB;
   }
   dim3 grid((p.epi == EPI_TMA_F16 ? (p.ldy + BN - 1) / BN : (p.Ncols + BN - 1) / BN), (p.M_total + kBM - 1) / kBM, 1);
-  B2_CHECK_CUDA(launch_pdl(igemm_kernel<BN>, grid, dim3(kThreads), S::kTotalBytes, stream, tmA, tmB, tmC, tmR, p));
+  B2_CHECK_CUDA(launch_pdl(igemm_kernel<BN, MASK>, grid, dim3(kThreads), S::kTotalBytes, stream, tmA, tmB, tmC, tmR, p));
   B2_CHECK_LAUNCH("igemm_kernel");
   return B2_OK;
 }
@@ -749,10 +770,10 @@ static bool densem_applies(const IgemmParams& p, int k2) {
 
 static int g_gemm_algo = 0;   // 0 auto (persistent kernel where it applies), 1 force the per-tile kernel
 
-template <int BN, int GAN>
+template <int BN, int GAN, int MASK = 0>
 static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
   using S = PgemmSmem<BN>;
-  B2_OPT_IN_SMEM((pgemm_kernel<BN, GAN>), S::kTotal);
+  B2_OPT_IN_SMEM((pgemm_kernel<BN, GAN, MASK>), S::kTotal);
   const IgemmParams& ip = L.p;
   CUtensorMap tmA, tmB, tmC, tmR;
   int rc;
@@ -793,16 +814,30 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.res_pre = ip.res_pre;
   p.in_scale = GAN ? ip.in_scale : nullptr; p.in_shift = ip.in_shift; p.in_ld = ip.in_ld; p.in_rows = ip.in_rows > 0 ? ip.in_rows : 128;
   p.dual = ip.y2 != nullptr; p.scale2 = ip.scale2; p.shift2 = ip.shift2; p.aff2_ld = ip.aff2_ld; p.aff2_rows = ip.aff2_rows > 0 ? ip.aff2_rows : 128;
+  p.mask = ip.mask; p.ldm = ip.ldm;
   const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
-  B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, GAN>, dim3(grid), dim3(GAN ? kPgThreadsGan : kPgThreads), S::kTotal, stream, tmA, tmB, tmA2, tmB2, tmC, tmR, tmC2, p));
+  B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, GAN, MASK>, dim3(grid), dim3(GAN ? kPgThreadsGan : kPgThreads), S::kTotal, stream, tmA, tmB, tmA2, tmB2, tmC, tmR, tmC2, p));
   B2_CHECK_LAUNCH("pgemm_kernel");
   return B2_OK;
 }
 
+static int g_last_gemm_path = 0;   // kernel of the last GEMM-family launch: 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (tests pin it)
+
 static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
-  if (g_gemm_algo == 0 && densem_applies(L.p, L.k2)) return launch_densem(L, stream);
+  if (L.p.mask) {
+    // ReLU-derivative mask (fine-tuning backward): the persistent GEMM and the implicit-GEMM kernel carry the masked epilogue
+    if (L.p.epi != EPI_TMA_F16 || L.p.per_row || L.p.relu || L.p.aff_ld || L.p.res_up || L.p.res_pre || L.p.y2 || L.p.in_scale)
+      return set_error(B2_ERR_UNSUPPORTED, "a masked output needs fp16 output without ReLU, per-row / per-sample affines or generator extras");
+    if (L.p.ldm % 8 || L.p.ldm < L.p.ldy) return set_error(B2_ERR_INVALID, "mask pitch %d must be a multiple of 8 and >= ldy %d", L.p.ldm, L.p.ldy);
+    if (g_gemm_algo == 0 && L.p.amode == AMODE_TMA) { g_last_gemm_path = 2; return launch_pgemm<64, 0, 1>(L, stream); }
+    if (L.k2 > 0) return set_error(B2_ERR_UNSUPPORTED, "two-operand GEMM needs the persistent kernel");
+    g_last_gemm_path = 3;
+    return L.p.ldy <= 64 ? launch_igemm<64, 1>(L, stream) : launch_igemm<128, 1>(L, stream);
+  }
+  if (g_gemm_algo == 0 && densem_applies(L.p, L.k2)) { g_last_gemm_path = 1; return launch_densem(L, stream); }
   if (g_gemm_algo == 0 && L.p.amode == AMODE_TMA && L.p.epi == EPI_TMA_F16 && !L.p.per_row) {
     // 64-wide N tiles only (see b2_pgemm.cuh: the accumulator tiles of a 128-wide instance do not fit in shared memory)
+    g_last_gemm_path = 2;
     if (L.p.y2 || L.p.res_up || L.p.res_pre || L.p.in_scale) return launch_pgemm<64, 1>(L, stream);
     return launch_pgemm<64, 0>(L, stream);
   }
@@ -812,8 +847,9 @@ static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     return set_error(B2_ERR_UNSUPPORTED, "upsampled / pre-scale residuals, second outputs and input affines are implemented by the persistent GEMM (1x1 convolutions, fp16) only");
   // 64-wide tiles for narrow outputs, 128 otherwise
   const int width = (L.p.epi == EPI_TMA_F16) ? L.p.ldy : L.p.Ncols;
-  if (width <= 64) return launch_igemm<64>(L, stream);
-  return launch_igemm<128>(L, stream);
+  g_last_gemm_path = 3;
+  if (width <= 64) return launch_igemm<64, 0>(L, stream);
+  return launch_igemm<128, 0>(L, stream);
 }
 
 bool pdl_enabled() {
@@ -875,7 +911,8 @@ int b2_debug_tstack_plan(const b2_conv_args* a, int* out) {
   out[5] = ok ? p.cchunks * p.kt * kTkWBlock : 0; out[6] = ok ? (int)smem : 0;
   return B2_OK;
 }
-int b2_debug_last_conv_path(void) { return g_last_conv_path; }   /* 1: the temporal stack kernel took the last convolution */
+int b2_debug_last_conv_path(void) { return g_last_conv_path; }
+int b2_debug_last_gemm_path(void) { return g_last_gemm_path; }   /* 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (last GEMM-family launch) */   /* 1: the temporal stack kernel took the last convolution */
 int b2_debug_set_tstack(int mode) { g_tstack = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }   /* temporal stack kernel: -1 rule, 0 never, 1 whenever eligible */
 int b2_debug_set_slab_mt(int mt) { g_slab_force_mt = mt < 0 ? 0 : mt; return B2_OK; }
 int b2_debug_set_densem(int maxm, int force_s) { g_densem_maxm = maxm < 0 ? -2 : maxm; g_densem_force_s = force_s; return B2_OK; }
@@ -896,6 +933,7 @@ static int validate_conv(const b2_conv_args* a) {
                    conv_out_dim(a->W, a->kw, a->sw, a->pw) > 0,
                "empty output");
   B2_CHECK_ARG(!a->pool_w || a->mode == B2_CONV_STEM7, "pool_w is implemented by the stem convolution only");
+  B2_CHECK_ARG(!a->mask || (a->mode == B2_CONV_AUTO && !a->upsample), "a masked output needs a plain (B2_CONV_AUTO) convolution");
   if (a->mode == B2_CONV_STEM7) {
     B2_CHECK_ARG(a->C == 4, "STEM7 needs NDHWC4 input (C == 4), got %d", a->C);
     B2_CHECK_ARG(a->kw == 7 && a->sw == 2 && a->pw == 3, "STEM7 needs kw=7, sw=2, pw=3");
@@ -934,11 +972,13 @@ int b2_conv_ndhwc_fprop(const b2_conv_args* a, void* stream) {
                        !a->residual_pre && !a->in_scale && g_gemm_algo == 0 &&
                        densem_wanted(M_out, a->kt * a->kh * a->kw, a->st > 1 || a->sh > 1 || a->sw > 1);
   g_last_conv_path = 0;
-  rc = small_m ? 0 : try_tstack(a, reinterpret_cast<cudaStream_t>(stream));
+  g_last_gemm_path = 0;
+  const bool skip_slab = small_m || a->mask != nullptr;     // the slab / temporal kernels have no masked epilogue
+  rc = skip_slab ? 0 : try_tstack(a, reinterpret_cast<cudaStream_t>(stream));
   if (rc != 0) return rc < 0 ? rc : B2_OK;
-  rc = small_m ? 0 : try_slabts(a, reinterpret_cast<cudaStream_t>(stream));
+  rc = skip_slab ? 0 : try_slabts(a, reinterpret_cast<cudaStream_t>(stream));
   if (rc != 0) return rc < 0 ? rc : B2_OK;
-  rc = small_m ? 0 : try_slab(a, reinterpret_cast<cudaStream_t>(stream));
+  rc = skip_slab ? 0 : try_slab(a, reinterpret_cast<cudaStream_t>(stream));
   if (rc != 0) return rc < 0 ? rc : B2_OK;
   if (a->upsample) return set_error(B2_ERR_UNSUPPORTED, "fused upsampling needs the slab kernel, which does not take this shape");
 
@@ -983,6 +1023,7 @@ int b2_conv_ndhwc_fprop(const b2_conv_args* a, void* stream) {
     p.in_scale = a->in_scale; p.in_shift = a->in_shift; p.in_ld = a->in_aff_ld; p.in_rows = p.To * p.Ho * p.Wo;
   }
   p.aff_rows = p.To * p.Ho * p.Wo;
+  p.mask = reinterpret_cast<const __half*>(a->mask); p.ldm = a->ldm;
   if (a->aff_ld && p.aff_rows % 128 != 0)
     return set_error(B2_ERR_UNSUPPORTED, "per-sample affine on a 1x1x1 convolution needs To*Ho*Wo %% 128 == 0 (got %d)", p.aff_rows);
   L.w = a->w;
@@ -1053,6 +1094,7 @@ static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const vo
                                                      !g->out_f32 && !g->per_row)),
                "bad per-sample affine (pitch %d, rows per sample %d)", g->aff_ld, g->aff_rows);
   p.aff_ld = g->aff_ld; p.aff_rows = g->aff_rows;
+  p.mask = reinterpret_cast<const __half*>(g->mask); p.ldm = g->ldm;
   if (g->d2) {
     B2_CHECK_ARG(g->scale2 && g->shift2 && g->aff2_ld >= g->N && g->aff2_rows > 0 && g->aff2_rows % 128 == 0 && !g->out_f32 && !g->per_row,
                  "second output needs scale2 / shift2 (fp32 [M / aff2_rows][aff2_ld >= N], aff2_rows %% 128 == 0) and fp16 output");

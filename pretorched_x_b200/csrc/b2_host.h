@@ -65,6 +65,11 @@ int make_tmap_2d_f16(CUtensorMap* out, const void* base, uint64_t inner, uint64_
 int make_tmap_ndhwc_slab(CUtensorMap* out, const void* base, uint64_t C, uint64_t W, uint64_t H, uint64_t planes,
                          uint32_t box_w, uint32_t box_h, uint32_t stride_hw, uint32_t box_planes = 1);
 
+// 5-D fp16 tensor map over an NDHWC activation viewed as (C, W, H, T, N) with channel pitch `ld`; smem box = (64, box_w,
+// box_h, 1, 1) pixels taken every stride_hw-th column / row, SWIZZLE_128B, zeros outside the tensor (including channels >= C).
+int make_tmap_ndhwc_5d(CUtensorMap* out, const void* base, uint64_t C, uint64_t ld, uint64_t W, uint64_t H, uint64_t T,
+                       uint64_t N, uint32_t box_w, uint32_t box_h, uint32_t stride_hw);
+
 int require_sm90();
 
 // Launch with programmatic stream serialization (see pdl_wait() in b2_ptx.cuh).  B2_PDL=0 in the environment turns

@@ -62,7 +62,20 @@ struct IgemmParams {
   const float* in_scale;   // persistent GEMM (generator instance) only: per-sample affine + ReLU on the A operand, see PgemmParams
   const float* in_shift;
   int in_ld, in_rows;
+  const __half* mask;      // MASK instances only: fp16 [M][ldm]; the output is zeroed where mask <= 0 (ReLU derivative)
+  int ldm;
 };
+
+// Eight mask entries of output row m, columns [c, c + 8) (zeros past the mask's rows / pitch), and the masked pair select.
+__device__ __forceinline__ uint4 load_mask8(const IgemmParams& p, int m, int c) {
+  if (m >= p.M_total || c >= p.ldm) return make_uint4(0, 0, 0, 0);
+  return __ldg(reinterpret_cast<const uint4*>(p.mask + static_cast<size_t>(m) * p.ldm + c));
+}
+__device__ __forceinline__ void apply_mask2(uint32_t mk, float& a0, float& a1) {
+  const float2 mf = unpack_half2(mk);
+  a0 = mf.x > 0.f ? a0 : 0.f;
+  a1 = mf.y > 0.f ? a1 : 0.f;
+}
 
 template <int BN>
 struct IgemmSmem {
@@ -78,7 +91,7 @@ struct IgemmSmem {
   static constexpr int kTotalBytes = kAccOffset + acc_bytes(BN) + 1024 /*align slack*/;
 };
 
-template <int BN>
+template <int BN, int MASK = 0>   // MASK = 1: ReLU-derivative mask operand in the fp16 epilogue (fine-tuning backward)
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C] matrix (AMODE_TMA only)
              const __grid_constant__ CUtensorMap tmB,   // weights [N][Ktot]
@@ -217,6 +230,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
           uint4 rv = make_uint4(0, 0, 0, 0);
           if (p.residual != nullptr) rv = *reinterpret_cast<const uint4*>(rrow + coff);
           const uint32_t rr[4] = {rv.x, rv.y, rv.z, rv.w};
+          uint4 mv = make_uint4(0, 0, 0, 0);
+          if constexpr (MASK) mv = load_mask8(p, m, n0 + j * 32 + q * 8);
+          const uint32_t mm[4] = {mv.x, mv.y, mv.z, mv.w};
           uint32_t out[4];
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
@@ -233,6 +249,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmA,   // activations as [M][C]
             const float2 rf = unpack_half2(rr[e]);
             a0 += rf.x; a1 += rf.y;
             if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+            if constexpr (MASK) apply_mask2(mm[e], a0, a1);
             out[e] = pack_half2(a0, a1);
           }
           *reinterpret_cast<uint4*>(crow + coff) = make_uint4(out[0], out[1], out[2], out[3]);

@@ -69,6 +69,8 @@ struct PgemmParams {
   const float* in_scale;
   const float* in_shift;
   int in_ld, in_rows;
+  const __half* mask;       // pgemm_kernel<BN, 0, 1> only: fp16 [M][ldm] ReLU-derivative mask of the output (see IgemmParams)
+  int ldm;
 };
 
 template <int BN>
@@ -89,7 +91,8 @@ struct PgemmSmem {
   static_assert(kTotal <= 227 * 1024, "shared memory budget");
 };
 
-template <int BN, int GAN>   // GAN = 1: instance with the generator extras (res_up gather, res_pre, A transform); 0: the classic epilogue
+template <int BN, int GAN, int MASK = 0>   // GAN = 1: instance with the generator extras (res_up gather, res_pre, A transform); 0: the classic
+                                           // epilogue.  MASK = 1 (with GAN = 0): ReLU-derivative mask operand (fine-tuning backward)
 __global__ void __launch_bounds__(GAN ? kPgThreadsGan : kPgThreads, 1)
 pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -288,6 +291,12 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             uint4 rv = make_uint4(0, 0, 0, 0);
             if (p.has_residual) rv = *reinterpret_cast<const uint4*>(rrow + ((static_cast<uint32_t>(chunk0 + q) ^ rswz) << 4));
             const uint32_t rr[4] = {rv.x, rv.y, rv.z, rv.w};
+            uint4 mv = make_uint4(0, 0, 0, 0);
+            if constexpr (MASK) {
+              const int mrow = m0 + r, mcol = n0 + j * 32 + q * 8;
+              if (mrow < p.M && mcol < p.ldm) mv = __ldg(reinterpret_cast<const uint4*>(p.mask + static_cast<size_t>(mrow) * p.ldm + mcol));
+            }
+            const uint32_t mm[4] = {mv.x, mv.y, mv.z, mv.w};
             uint32_t out[4];
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
@@ -302,6 +311,11 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                 a1 = a1 * s_scale[ci + 1] + s_shift[ci + 1] + rf.y;
               }
               if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+              if constexpr (MASK) {
+                const float2 mf = unpack_half2(mm[e]);
+                a0 = mf.x > 0.f ? a0 : 0.f;
+                a1 = mf.y > 0.f ? a1 : 0.f;
+              }
               if (GAN && pass == 1) {                          // second output: next block's ccbn + ReLU on the fp32 value
                 a0 = fmaxf(a0 * s_scale2[ci] + s_shift2[ci], 0.f);
                 a1 = fmaxf(a1 * s_scale2[ci + 1] + s_shift2[ci + 1], 0.f);

@@ -20,7 +20,7 @@ NOT seen: ``model.invalidate()`` / ``engine.invalidate(model)`` drops every pack
 
 Every block body is entered through a ``torch.autograd.Function`` (``functions.py``, SURVEY.md section 8b-ii): the
 Function's ``forward`` is the ctypes call sequence, its outputs are marked non-differentiable (frozen-backbone
-semantics: the engine has no backward for the convolutional trunk), and the dense heads (``last_linear``, the TRN
+semantics), except for the stages a ``ResNet3D.fine_tune(k)`` call made trainable (``block_backward``), and the dense heads (``last_linear``, the TRN
 relation MLPs) have a real backward on the same wgmma GEMM so that a head can be trained on engine features.
 """
 import os
@@ -165,9 +165,12 @@ def run_basic(block, a, simt=False, out=None):
     return Fn.BasicBlockFunction.run(block, a, simt, out)
 
 
-def _basic_body(block, a, simt=False, out=None):
+def _basic_body(block, a, simt=False, out=None, keep=None):
+    """``keep``: a list that receives the post-ReLU intermediate (the fine-tuning backward reads it)."""
     res = _shortcut(block, a, simt)
     h = conv_bn_act(block.conv1, block.bn1, a, relu=True, simt=simt)
+    if keep is not None:
+        keep.append(h)
     return conv_bn_act(block.conv2, block.bn2, h, residual=res, relu=True, simt=simt, out=out)
 
 
@@ -212,18 +215,20 @@ def run_bottleneck(block, a, simt=False, out=None):
     return Fn.BottleneckFunction.run(block, a, simt, out)
 
 
-def _bottleneck_body(block, a, simt=False, out=None):
+def _bottleneck_body(block, a, simt=False, out=None, keep=None):
+    """``keep``: a list that receives the two post-ReLU intermediates (the fine-tuning backward reads them)."""
+    keep = [] if keep is None else keep
     ds = block.downsample
     if (not simt and isinstance(ds, nn.Sequential) and len(ds) == 2 and _plain_1x1(ds[0]) and _plain_1x1(block.conv3)
             and not ds[1].training and len(set(_conv_geometry(ds[0])[0])) == 1 and (a.T > 1 or _conv_geometry(ds[0])[0][0] == 1)
             and isinstance(ds[0], nn.Conv3d)):
-        h = conv_bn_act(block.conv1, block.bn1, a, relu=True)
-        h = conv_bn_act(block.conv2, block.bn2, h, relu=True)
-        return _fused_close_with_projection(block, a, h, out)
+        keep.append(conv_bn_act(block.conv1, block.bn1, a, relu=True))
+        keep.append(conv_bn_act(block.conv2, block.bn2, keep[-1], relu=True))
+        return _fused_close_with_projection(block, a, keep[-1], out)
     res = _shortcut(block, a, simt)
-    h = conv_bn_act(block.conv1, block.bn1, a, relu=True, simt=simt)
-    h = conv_bn_act(block.conv2, block.bn2, h, relu=True, simt=simt)
-    return conv_bn_act(block.conv3, block.bn3, h, residual=res, relu=True, simt=simt, out=out)
+    keep.append(conv_bn_act(block.conv1, block.bn1, a, relu=True, simt=simt))
+    keep.append(conv_bn_act(block.conv2, block.bn2, keep[-1], relu=True, simt=simt))
+    return conv_bn_act(block.conv3, block.bn3, keep[-1], residual=res, relu=True, simt=simt, out=out)
 
 
 def _bn_relu(bn, a):
@@ -521,8 +526,176 @@ def run_trunk(model, x, simt=False):
     return _run_units(units[ui:], a, simt) if ui < len(units) else a
 
 
+# ---------------------------------------------------------------------------------------------
+# fine-tuning: backward through plain BasicBlock / Bottleneck blocks with eval-mode ("frozen") BatchNorm
+# ---------------------------------------------------------------------------------------------
+# Notation for one conv -> BN -> (+res) -> ReLU: s = gamma / sqrt(var + eps), g = gradient at the BN output (already through
+# the ReLU mask), G = sum_m g (x) x_tap the UNSCALED weight gradient (b2_conv_wgrad).  Then dW = s G, dbeta = sum_m g,
+# dgamma = (<W, G> - mean dbeta) / sqrt(var + eps) (sum g conv(x) = <W, G>: no pre-BN tensor is kept), and the input gradient
+# is the convolution of g with the transposed, flipped, s-folded filter on the forward kernels.  Gradients cross kernels as
+# fp16 times a power-of-two loss scale chosen on the device where the gradient enters the trunk (ops.loss_scale_); every fp32
+# result divides it out.
+class TrainAct(Act):
+    """Act produced by the fine-tuned part of the trunk: ``data`` carries the autograd graph and ``loss_scale`` is the
+    device pair [scale, 1/scale] its backward fills in."""
+    __slots__ = ("loss_scale",)
+
+
+def check_trainable_block(block):
+    """Raise NotImplementedError unless ``block`` is a plain 3-D ResNet BasicBlock / Bottleneck the backward covers."""
+    from .models.resnet3d import BasicBlock, Bottleneck, ShortcutA
+    name = type(block).__name__
+    ok = type(block) in (BasicBlock, Bottleneck) and getattr(block, "nonlocalblock", None) is None
+    convs = [(block.conv1, block.bn1), (block.conv2, block.bn2)] + ([(block.conv3, block.bn3)] if ok and hasattr(block, "conv3") else [])
+    ds = getattr(block, "downsample", None)
+    if isinstance(ds, nn.Sequential):
+        ok = ok and len(ds) == 2 and _plain_1x1(ds[0])
+        convs.append((ds[0], ds[1]) if ok else (None, None))
+    elif ds is not None and not isinstance(ds, ShortcutA):
+        ok = False
+    for conv, bn in convs if ok else ():
+        k = tuple(conv.weight.shape[2:])
+        ok = ok and type(conv) is nn.Conv3d and conv.groups == 1 and conv.bias is None and all(d == 1 for d in conv.dilation)
+        ok = ok and k in ((1, 1, 1), (3, 3, 3)) and tuple(conv.padding) == (k[0] // 2,) * 3
+        ok = ok and len(set(conv.stride)) == 1 and conv.stride[0] in (1, 2)
+        ok = ok and isinstance(bn, nn.BatchNorm3d) and bn.affine and bn.running_var is not None
+    if not ok:
+        raise NotImplementedError("fine-tuning backward covers the plain BasicBlock / Bottleneck of the 3-D ResNets (shortcut A, B or "
+                                  "identity); got a %s" % name)
+
+
+def _train_units(block):
+    """(conv, bn) pairs of a block in parameter order: conv1, conv2[, conv3][, downsample projection]."""
+    units = [(block.conv1, block.bn1), (block.conv2, block.bn2)]
+    if hasattr(block, "conv3"):
+        units.append((block.conv3, block.bn3))
+    if isinstance(block.downsample, nn.Sequential):
+        units.append((block.downsample[0], block.downsample[1]))
+    return units
+
+
+def train_params(block):
+    return [t for conv, bn in _train_units(block) for t in (conv.weight, bn.weight, bn.bias)]
+
+
+def _bn_scale(bn):
+    return (bn.weight.detach().float() * torch.rsqrt(bn.running_var.float() + bn.eps)).contiguous()
+
+
+def _dgrad_1x1(conv, s):
+    """B operand [Cin][Cout] (fp16) of the input gradient g . (s W) of a 1x1x1 convolution."""
+    w = conv.weight.detach().reshape(conv.weight.shape[0], -1).float() * s[:, None]
+    return w.t().contiguous().to(torch.float16)
+
+
+def _dgrad_3x3(conv, s, g_pitch):
+    """The input gradient of a 3x3x3 convolution as a stride-1, padding-1 convolution with the transposed, flipped, s-folded filter."""
+    w = conv.weight.detach().float() * s[:, None, None, None, None]
+    return ops.PackedConv(w.flip(2, 3, 4).transpose(0, 1).contiguous(), None, None, (1, 1, 1), (1, 1, 1), in_pitch=g_pitch)
+
+
+def _gemm_dgrad(g, wt, residual=None, second=None, mask=None):
+    """g . wt^T (+ residual), zeroed where ``mask`` (an Act of the result's shape) is not positive."""
+    C = wt.shape[0]
+    one = torch.ones(C, dtype=torch.float32, device=g.data.device)
+    zero = torch.zeros(C, dtype=torch.float32, device=g.data.device)
+    y = ops.gemm(g.data, wt, one, zero, g.M, C, g.C, residual=residual.data if residual is not None else None, second=second,
+                 mask=mask.data if mask is not None else None)
+    return Act(y, g.N, g.T, g.H, g.W, C)
+
+
+def _conv_dgrad(conv, s, g, x):
+    """Gradient at the input ``x`` of a 3x3x3 convolution for the gradient ``g`` at its (BN-scaled) output, before any residual."""
+    stride = conv.stride[0]
+    z = g if stride == 1 else ops.zero_insert(g, x.T, x.H, x.W, stride)
+    return z, _dgrad_3x3(conv, s, z.ld)
+
+
+def _param_grads(conv, bn, g, x, ls, needs):
+    """(dW, dgamma, dbeta) of conv -> eval-mode bn for the gradient ``g`` at the BN output; None where not needed."""
+    need_w, need_g, need_b = needs
+    dw = wdot = dbeta = dgamma = None
+    inv = ls[1:]
+    if need_w or need_g:
+        k = conv.weight.shape[2]
+        dw, wdot = ops.conv_wgrad(g, x, k, conv.stride[0], k // 2, weight=conv.weight if need_g else None, scale=_bn_scale(bn),
+                                  inv_loss_scale=inv)
+    if need_b or need_g:
+        dbeta = ops.colsum(g, inv)
+    if need_g:
+        dgamma = (wdot - bn.running_mean.float() * dbeta) * torch.rsqrt(bn.running_var.float() + bn.eps)
+    return [dw if need_w else None, dgamma, dbeta if need_b else None]
+
+
+def _shortcut_grad(block, g, x):
+    """Gradient the shortcut sends to the block input (``g`` itself for the identity)."""
+    ds = block.downsample
+    if ds is None:
+        return g
+    if isinstance(ds, nn.Sequential):
+        stride = ds[0].stride[0]
+        pg = _gemm_dgrad(g, _dgrad_1x1(ds[0], _bn_scale(ds[1])))
+        return pg if stride == 1 else ops.zero_insert(pg, x.T, x.H, x.W, stride, ld=x.ld)
+    return ops.zero_insert(g, x.T, x.H, x.W, ds.stride, channels=x.C, ld=x.ld)       # type A: subsample + zero channels
+
+
+def block_backward(block, x, hs, gy, ls, need_x, needs):
+    """Backward of one fine-tuned block.  ``gy``: loss-scaled fp16 gradient at the block output, already multiplied by the
+    block's closing ReLU mask; ``hs``: the post-ReLU intermediates of the forward; ``needs``: needs_input_grad of the
+    parameters in ``train_params`` order.  Returns (gradient at the block input times [x > 0], or None; parameter grads)."""
+    units = _train_units(block)
+    grads = [None] * (3 * len(units))
+    if hasattr(block, "conv3"):
+        h1, h2 = hs
+        grads[6:9] = _param_grads(block.conv3, block.bn3, gy, h2, ls, needs[6:9])
+        g2 = _gemm_dgrad(gy, _dgrad_1x1(block.conv3, _bn_scale(block.bn3)), mask=h2)
+        grads[3:6] = _param_grads(block.conv2, block.bn2, g2, h1, ls, needs[3:6])
+        z, pc = _conv_dgrad(block.conv2, _bn_scale(block.bn2), g2, h1)
+        g1 = ops.conv(z, pc, mask=h1)
+    else:
+        (h1,) = hs
+        grads[3:6] = _param_grads(block.conv2, block.bn2, gy, h1, ls, needs[3:6])
+        g1 = ops.conv(gy, _dgrad_3x3(block.conv2, _bn_scale(block.bn2), gy.ld), mask=h1)
+    grads[0:3] = _param_grads(block.conv1, block.bn1, g1, x, ls, needs[0:3])
+    if isinstance(block.downsample, nn.Sequential):
+        ds = block.downsample
+        grads[-3:] = _param_grads(ds[0], ds[1], gy, x, ls, needs[-3:])
+    if not need_x:
+        return None, grads
+    s1 = _bn_scale(block.bn1)
+    ds = block.downsample
+    if hasattr(block, "conv3"):
+        w1 = _dgrad_1x1(block.conv1, s1)
+        if isinstance(ds, nn.Sequential) and ds[0].stride[0] == 1:     # both 1x1 products in one two-operand GEMM
+            dx = _gemm_dgrad(g1, w1, second=(gy.data, _dgrad_1x1(ds[0], _bn_scale(ds[1])), gy.C), mask=x)
+        else:
+            dx = _gemm_dgrad(g1, w1, residual=_shortcut_grad(block, gy, x), mask=x)
+    else:
+        z, pc = _conv_dgrad(block.conv1, s1, g1, x)
+        dx = ops.conv(z, pc, residual=_shortcut_grad(block, gy, x), mask=x)
+    return dx, grads
+
+
+def run_trunk_finetune(model, x, k):
+    """Stem and layer1..layer{k-1} frozen (the forward path), layer{k}..layer4 through the differentiable block Functions.
+    The depth-first schedule is not used."""
+    units = _trunk_units(model)
+    n_frozen = 1 + sum(len(getattr(model, "layer%d" % i)) for i in range(1, k))
+    a = _run_units(units[:n_frozen], x, simt=False)
+    ls = torch.ones(2, dtype=torch.float32, device=a.data.device)
+    for _, blk in units[n_frozen:]:
+        a = Fn.BlockTrainFunction.run(blk, a, ls)
+    out = TrainAct(a.data, a.N, a.T, a.H, a.W, a.C)
+    out.loss_scale = ls
+    return out
+
+
 def run_head(model, a, head):
     """avgpool -> view(B,-1) -> last_linear (torchvision_models.py:460-464).  Returns fp32 [N][classes]."""
+    if isinstance(a, TrainAct):
+        # fine-tuning: fp32 pooled features, so that the head's input gradient reaches the pool backward unrounded
+        pooled = Fn.FineTunePoolFunction.apply(a.data, (a.N, a.T, a.H, a.W, a.C), a.loss_scale)
+        return Fn.linear(pooled, head.weight, head.bias) if isinstance(head, nn.Linear) else head(pooled)
     pooled = ops.avgpool_global(a)                     # fp16 [N][ld]
     if isinstance(head, nn.Linear) and torch.is_grad_enabled() and any(p.requires_grad for p in head.parameters()):
         # trainable head on frozen engine features: differentiable GEMM (functions.LinearFunction), same kernel

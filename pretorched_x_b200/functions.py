@@ -8,7 +8,9 @@ Two kinds:
   ``GBlockFunction`` (BigGAN-deep GBlock).  ``forward`` is the ctypes launch sequence of ``engine.py`` /
   ``biggan_engine.py`` on fp16 NDHWC matrices; every output is marked non-differentiable, so the modules can sit inside
   an autograd graph as a frozen feature extractor (the way the reference's zoo models are used with a replaced
-  ``last_linear``, README.md:520-547).  There is no backward for the convolutional trunk: asking for one raises.
+  ``last_linear``, README.md:520-547).  These frozen bodies have no backward: asking for one raises.
+* **Fine-tuned residual blocks** -- ``BlockTrainFunction`` / ``FineTunePoolFunction``, used instead of the frozen bodies for
+  ``layer{k}..layer4`` after ``ResNet3D.fine_tune(k)`` (engine.block_backward).
 * **Dense heads with a real backward** -- ``LinearFunction`` (``last_linear`` / ``fc``: resnet3D.py:162,
   torchvision_models.py:463-464) and, built from it, the TRN relation MLP (trn.py:39-49).  ``forward`` and both
   gradient products run on the same wgmma GEMM (``b2_gemm_f16``: fp16 operands, fp32 accumulation and output), so a
@@ -108,6 +110,63 @@ class GBlockFunction(_FrozenFunction):
             return out[0].data, _geom(out[0]), out[1].data, _geom(out[1])
         ctx.mark_non_differentiable(out.data)
         return out.data, _geom(out), None, None
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# fine-tuned residual blocks (models.resnet3d.ResNet3D.fine_tune)
+# ---------------------------------------------------------------------------------------------------------------
+class BlockTrainFunction(torch.autograd.Function):
+    """BasicBlock / Bottleneck with a backward (engine.block_backward).  Inputs: the block input matrix and the block's
+    conv weights and BatchNorm gamma / beta (engine.train_params), so autograd routes their gradients.  The forward runs
+    the same kernels as the frozen path and keeps the block input, its post-ReLU intermediates and its output.  Gradients
+    in and out are loss-scaled fp16 matrices already multiplied by the ReLU mask of the tensor they belong to; ``ls`` is
+    the device pair [scale, 1/scale] shared by every fine-tuned block of one forward."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, block, ls, *params):
+        from . import engine
+        keep = []
+        body = engine._bottleneck_body if hasattr(block, "conv3") else engine._basic_body
+        y = body(block, Act(x2d, *geom), keep=keep)
+        ctx.save_for_backward(x2d, y.data)
+        ctx.hs = [h.data for h in keep]
+        ctx.geoms = (geom, _geom(y), [_geom(h) for h in keep])
+        ctx.block, ctx.ls = block, ls
+        return y.data, _geom(y)
+
+    @staticmethod
+    def backward(ctx, gy, _geom_grad):
+        from . import engine
+        x2d, y2d = ctx.saved_tensors
+        gx, gyo, ghs = ctx.geoms
+        hs = [Act(h, *g) for h, g in zip(ctx.hs, ghs)]
+        dx, grads = engine.block_backward(ctx.block, Act(x2d, *gx), hs, Act(gy.contiguous(), *gyo), ctx.ls, ctx.needs_input_grad[0],
+                                          ctx.needs_input_grad[4:])
+        return (dx.data if dx is not None else None, None, None, None) + tuple(grads)
+
+    @classmethod
+    def run(cls, block, a, ls):
+        from . import engine
+        data, geom = cls.apply(a.data, _geom(a), block, ls, *engine.train_params(block))
+        return Act(data, *geom)
+
+
+class FineTunePoolFunction(torch.autograd.Function):
+    """Global average pool of the last fine-tuned block: fp32 [N][C] features out.  The backward picks the loss scale from
+    the incoming fp32 gradient (ops.loss_scale_) and writes the scaled, ReLU-masked fp16 gradient of the block output."""
+
+    @staticmethod
+    def forward(ctx, y2d, geom, ls):
+        a = Act(y2d, *geom)
+        ctx.save_for_backward(y2d)
+        ctx.geom, ctx.ls = geom, ls
+        return ops.avgpool_global(a)[:, :a.C].float()
+
+    @staticmethod
+    def backward(ctx, gf):
+        (y2d,) = ctx.saved_tensors
+        ops.loss_scale_(gf, ctx.ls)
+        return ops.avgpool_global_backward(gf, ctx.ls, Act(y2d, *ctx.geom)).data, None, None
 
 
 # ---------------------------------------------------------------------------------------------------------------

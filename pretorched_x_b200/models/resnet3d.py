@@ -186,14 +186,47 @@ class ResNet3D(engine.CacheOwner, nn.Module):
             if src in state_dict and dst not in state_dict:
                 state_dict[dst] = state_dict.pop(src)
 
+    # -- fine-tuning -----------------------------------------------------------------------------
+    ft_begin_index = None           # set by fine_tune(): first trainable stage (1..5), None = frozen trunk
+
+    def fine_tune(self, ft_begin_index):
+        """Make ``layer{k}..layer4`` and the head trainable (k = ``ft_begin_index``, 1 <= k <= 5) and freeze the stem and
+        ``layer1..layer{k-1}`` (``requires_grad``), the split of the reference's ``get_fine_tuning_parameters``.
+
+        Under grad mode the forward then runs the fine-tuned stages through Functions with a backward on the engine's
+        kernels.  BatchNorm stays in eval mode ("frozen BN", the usual choice at video batch sizes): it normalises with its
+        running statistics, which are not updated, while its gamma / beta are trainable.  The model itself must stay in
+        ``eval()``.  k = 0 (the stem) is not supported, nor are blocks other than the plain BasicBlock / Bottleneck."""
+        k = int(ft_begin_index)
+        if k == 0:
+            raise NotImplementedError("fine-tuning the stem (7x7x7 convolution and max-pool) is not supported: use 1 <= k <= 5")
+        if not 1 <= k <= 5:
+            raise ValueError("ft_begin_index must be in 1..5, got %d" % k)
+        for i in range(k, 5):
+            for blk in getattr(self, 'layer%d' % i):
+                engine.check_trainable_block(blk)
+        trainable = tuple('layer%d.' % i for i in range(k, 5)) + ('%s.' % self.head_name,)
+        for name, p in self.named_parameters():
+            p.requires_grad_(name.startswith(trainable))
+        self.ft_begin_index = k
+        return self
+
+    def _fine_tuning(self):
+        return self.ft_begin_index is not None and self.ft_begin_index <= 4 and torch.is_grad_enabled()
+
     # -- reference API ------------------------------------------------------------------------
     def features_act(self, x):
         """Trunk on the engine's native layout (fp16 NDHWC ``Act``)."""
         if self.training:
             raise RuntimeError("the forward engine is inference-only: call model.eval() first")
+        if self._fine_tuning():
+            return engine.run_trunk_finetune(self, x, self.ft_begin_index)
         return engine.run_trunk(self, x)
 
     def features(self, input):
+        if self._fine_tuning():
+            raise NotImplementedError("in fine-tune mode the gradient enters the trunk through the pooled features: use "
+                                      "model(x) or model.logits(model.features_act(x)), or call features() under torch.no_grad()")
         return ops.to_ncdhw(self.features_act(input))
 
     def logits(self, features):
@@ -202,6 +235,16 @@ class ResNet3D(engine.CacheOwner, nn.Module):
 
     def forward(self, input):
         return self.logits(self.features_act(input))
+
+
+def get_fine_tuning_parameters(model, ft_begin_index):
+    """Parameter groups of the reference's fine-tuning recipe (resnet3D.py:221-239): parameters of ``layer{k}..layer4`` and
+    the head as ``{'params': p}``, every other one as ``{'params': p, 'lr': 0.0}``, in ``named_parameters`` order.  Also
+    switches the model into fine-tune mode (``model.fine_tune(ft_begin_index)``).  The head matches as ``fc`` or
+    ``last_linear`` (the reference only knows ``fc`` and so freezes the renamed head)."""
+    model.fine_tune(ft_begin_index)
+    names = ['layer%d' % i for i in range(ft_begin_index, 5)] + ['fc', 'last_linear']
+    return [{'params': v} if any(n in k for n in names) else {'params': v, 'lr': 0.0} for k, v in model.named_parameters()]
 
 
 def _attach_settings(model, settings):

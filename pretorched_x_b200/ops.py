@@ -248,7 +248,7 @@ def _out_rows(out, M, ld):
 
 @_on_device
 def conv(a, pc, residual=None, relu=False, simt=False, sample_affine=None, residual_up=False, residual_pre=False,
-         next_affine=None, pool_w=False, in_affine=None, out=None):
+         next_affine=None, pool_w=False, in_affine=None, out=None, mask=None):
     """nn.Conv3d -> BatchNorm3d -> (+residual) -> ReLU in one kernel
     (resnet3D.py:91-106, 125-143, 176-185; r2plus1d.py:85-88; torchvision_models.py:449-451).
 
@@ -259,7 +259,8 @@ def conv(a, pc, residual=None, relu=False, simt=False, sample_affine=None, resid
     y = act(scale * (conv + residual) + shift).  ``next_affine=(scale2, shift2)`` (fp32 [N][pitch] views): also return
     relu(y * scale2[n] + shift2[n]) -- the ccbn + ReLU that opens the next GBlock -- as a second Act, written by the same
     kernel.  All three: 1x1 convolutions only.  ``out``: preallocated fp16 [M][round_up(K, 8)] rows to write instead of a
-    fresh tensor (a row range of a larger batch buffer: the depth-first trunk schedule)."""
+    fresh tensor (a row range of a larger batch buffer: the depth-first trunk schedule).  ``mask``: an Act of the output's
+    shape; the result is zeroed where mask <= 0 (the ReLU derivative of the fine-tuning backward, b2_conv_args.mask)."""
     if a.ld != pc.C:
         raise ValueError("activation pitch %d != packed filter pitch %d" % (a.ld, pc.C))
     kt, kh, kw = pc.k
@@ -307,6 +308,10 @@ def conv(a, pc, residual=None, relu=False, simt=False, sample_affine=None, resid
         args.in_scale, args.in_shift, args.in_aff_ld = _ptr(isc), _ptr(ish), isc.stride(0)
     if pc.up and simt:
         raise ValueError("the CUDA-core cross-check has no fused upsampling")
+    if mask is not None:
+        if simt or relu or mask.M != M or mask.C != pc.K:
+            raise ValueError("mask %r does not fit the output (%d rows, %d channels) of a tensor-core call without ReLU" % (mask, M, pc.K))
+        args.mask, args.ldm = _ptr(mask.data), mask.ld
     if sample_affine is not None:
         sc, sh = sample_affine
         if simt or sc.shape != sh.shape or sc.shape[0] != a.N or sc.stride(0) != sh.stride(0) or sc.shape[1] < pc.K:
@@ -329,9 +334,10 @@ def conv(a, pc, residual=None, relu=False, simt=False, sample_affine=None, resid
 
 @_on_device
 def gemm(a2d, b2d, scale, shift, M, N, Kd, residual=None, relu=False, per_row=False, out=None, out_f32=False,
-         accumulate=False, second=None, aff_rows=0, next_affine=None):
+         accumulate=False, second=None, aff_rows=0, next_affine=None, mask=None):
     """D[M][N] = act(scale * A[M][Kd] . B[N][Kd]^T + shift + residual) on wgmma (b2_gemm_f16).
-    ``second=(A2, B2, K2)`` adds A2[M][K2] . B2[N][K2]^T into the same accumulator (b2_gemm2_f16)."""
+    ``second=(A2, B2, K2)`` adds A2[M][K2] . B2[N][K2]^T into the same accumulator (b2_gemm2_f16).  ``mask``: fp16
+    [M][ldm] matrix; D is zeroed where mask <= 0 (b2_gemm_args.mask)."""
     dev = a2d.device
     if out is None:
         ldd = N if out_f32 else _round_up(N, 8)
@@ -344,6 +350,10 @@ def gemm(a2d, b2d, scale, shift, M, N, Kd, residual=None, relu=False, per_row=Fa
     g.lda, g.ldb, g.ldd = a2d.stride(0), b2d.stride(0), out.stride(0)
     g.ldr = residual.stride(0) if residual is not None else 0
     g.per_row, g.relu, g.out_f32, g.accumulate = int(per_row), int(relu), int(out_f32), int(accumulate)
+    if mask is not None:
+        if mask.shape[0] != M or mask.stride(1) != 1 or mask.stride(0) < out.stride(0):
+            raise ValueError("mask must be an fp16 [%d][>= %d] matrix" % (M, out.stride(0)))
+        g.mask, g.ldm = _ptr(mask), mask.stride(0)
     if aff_rows:                      # per-sample affine: scale/shift are fp32 [M / aff_rows][pitch] views
         g.aff_ld, g.aff_rows = scale.stride(0), int(aff_rows)
     if next_affine is not None:       # (scale2, shift2, rows per sample): second output relu(D * scale2 + shift2), returned too
@@ -480,6 +490,76 @@ def gather_frame_tuples(x3d, idx_dev, n_tuples, n_idx):
     _lib.check(_lib.load().b2_gather_frame_tuples(_ptr(x3d), _ptr(y), _ptr(idx_dev), N, T, F, n_idx, n_tuples, _stream()),
                "b2_gather_frame_tuples")
     return y
+
+
+# ---------------------------------------------------------------------------------------------
+# fine-tuning backward (functions.BottleneckTrainFunction / BasicBlockTrainFunction)
+# ---------------------------------------------------------------------------------------------
+@_on_device
+def conv_wgrad(g, x, k, stride, pad, weight=None, scale=None, inv_loss_scale=None):
+    """Weight gradient of a k x k x k convolution (b2_conv_wgrad): g = Act gradient at the convolution output, x = Act input.
+    Returns (dw fp32 in the nn.Conv3d.weight layout, scaled by ``scale[co]`` and ``inv_loss_scale``, and, with ``weight``,
+    wdot[co] = <weight[co], G[co]> * inv_loss_scale)."""
+    Cout, Cin = g.C, x.C
+    dev = g.data.device
+    lib = _lib.load()
+    n = lib.b2_conv_wgrad_workspace_elems(x.N, x.T, x.H, x.W, Cin, Cout, k, stride, pad)
+    ws = torch.empty(max(int(n), 1), dtype=torch.float32, device=dev)
+    dw = torch.empty((Cout, Cin, k, k, k), dtype=torch.float32, device=dev)
+    w = weight.detach().float().contiguous() if weight is not None else None
+    wdot = torch.empty(Cout, dtype=torch.float32, device=dev) if weight is not None else None
+    with _timed("wgrad", "wgrad %dx%dx%d s%d C%d->%d M=%d" % (k, k, k, stride, Cin, Cout, g.M), 2.0 * g.M * Cout * Cin * k ** 3,
+                2.0 * (g.M * Cout + x.M * Cin) + 4.0 * Cout * Cin * k ** 3):
+        _lib.check(lib.b2_conv_wgrad(_ptr(g.data), g.ld, _ptr(x.data), x.ld, _ptr(w), _ptr(scale), _ptr(inv_loss_scale), _ptr(dw),
+                                     _ptr(wdot), _ptr(ws), ws.numel(), x.N, x.T, x.H, x.W, Cin, Cout, k, stride, pad, _stream()),
+                   "b2_conv_wgrad")
+    return dw, wdot
+
+
+@_on_device
+def zero_insert(g, T, H, W, stride, channels=None, ld=None):
+    """Adjoint of ``shortcut_a``: the low-resolution Act ``g`` placed at every ``stride``-th pixel of a [T, H, W] grid (zeros
+    elsewhere), channels [0, channels) kept."""
+    C = g.C if channels is None else channels
+    ldy = _round_up(C, 8) if ld is None else ld
+    y = torch.empty((g.N * T * H * W, ldy), dtype=torch.float16, device=g.data.device)
+    with _timed("zero_insert", "zero_insert C%d s%d M=%d" % (C, stride, y.shape[0]), 0.0, 2.0 * (g.M * C + y.numel())):
+        _lib.check(_lib.load().b2_zero_insert_ndhwc(_ptr(g.data), g.ld, C, _ptr(y), ldy, g.N, T, H, W, stride, _stream()),
+                   "b2_zero_insert_ndhwc")
+    return Act(y, g.N, T, H, W, C)
+
+
+@_on_device
+def colsum(g, inv_loss_scale=None):
+    """fp32 [C]: inv_loss_scale * sum over the rows of the Act ``g`` (the BatchNorm beta gradient)."""
+    lib = _lib.load()
+    dev = g.data.device
+    ws = torch.empty(int(lib.b2_colsum_workspace_elems(g.C)), dtype=torch.float32, device=dev)
+    out = torch.empty(g.C, dtype=torch.float32, device=dev)
+    with _timed("colsum", "colsum C%d M=%d" % (g.C, g.M), 0.0, 2.0 * g.M * g.C):
+        _lib.check(lib.b2_colsum_f16(_ptr(g.data), g.ld, g.M, g.C, _ptr(inv_loss_scale), _ptr(out), _ptr(ws), _stream()),
+                   "b2_colsum_f16")
+    return out
+
+
+@_on_device
+def loss_scale_(gf, scale_pair):
+    """Fill the fp32 device pair ``scale_pair`` = [2^k, 2^-k] from max |gf| (see b2_loss_scale_f32)."""
+    gf = gf.contiguous().float()
+    _lib.check(_lib.load().b2_loss_scale_f32(_ptr(gf), gf.shape[0], gf.shape[1], gf.stride(0), _ptr(scale_pair), _stream()),
+               "b2_loss_scale_f32")
+    return scale_pair
+
+
+@_on_device
+def avgpool_global_backward(gf, scale_pair, out):
+    """Gradient at the input of ``avgpool_global`` (and of the ReLU that produced ``out``): fp16 Act, loss-scaled."""
+    gf = gf.contiguous().float()
+    y = torch.empty_like(out.data)
+    with _timed("pool_bwd", "avgpool backward C%d M=%d" % (out.C, out.M), 0.0, 4.0 * out.M * out.ld):
+        _lib.check(_lib.load().b2_avgpool_global_backward(_ptr(gf), gf.stride(0), _ptr(scale_pair), _ptr(out.data), _ptr(y), out.N,
+                                                         out.positions, out.C, out.ld, _stream()), "b2_avgpool_global_backward")
+    return Act(y, out.N, out.T, out.H, out.W, out.C)
 
 
 # ---------------------------------------------------------------------------------------------

@@ -7,7 +7,7 @@
 O=gpurun_out/sanitizer; mkdir -p $O
 CS="compute-sanitizer --error-exitcode 7 --kernel-name kns=N2b2 --print-limit 40 --report-api-errors no"
 timeout 600 $CS --tool memcheck --log-file $O/memcheck.log python tools/sanitize_run.py > $O/memcheck.out 2>&1; echo "memcheck rc=$?" | tee $O/memcheck.rc
-timeout 420 $CS --tool synccheck --log-file $O/synccheck.log python tools/sanitize_run.py resnet3d50 r2plus1d34 resnet18 nonlocalresnet3d50 biggan > $O/synccheck.out 2>&1; echo "synccheck rc=$?" | tee $O/synccheck.rc
+timeout 420 $CS --tool synccheck --log-file $O/synccheck.log python tools/sanitize_run.py resnet3d50 r2plus1d34 resnet18 nonlocalresnet3d50 biggan finetune > $O/synccheck.out 2>&1; echo "synccheck rc=$?" | tee $O/synccheck.rc
 if [ "$1" = "all" ]; then
   timeout 300 $CS --tool racecheck --log-file $O/racecheck.log python tools/sanitize_run.py resnet3d50 r2plus1d34 resnet18 > $O/racecheck.out 2>&1; echo "racecheck rc=$?" | tee $O/racecheck.rc
 fi

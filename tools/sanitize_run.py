@@ -77,4 +77,17 @@ if not only or "dfs" in only:
     engine.set_dfs("off")
     torch.cuda.synchronize()
     print("%-28s %s" % ("resnet3d50 depth-first", tuple(y.shape)), flush=True)
+if not only or "finetune" in only:
+    # one fine-tuning step through layer3..layer4 (weight-gradient, zero-insert, mask, column-sum, loss-scale, pool backward)
+    for arch in ("resnet3d50", "resnet3d18"):
+        torch.manual_seed(0)
+        m = OF.randomize_bn_(getattr(P, arch)(num_classes=10, pretrained=None), 1).eval().to(dev)
+        groups = P.models.resnet3d.get_fine_tuning_parameters(m, 3)
+        x = torch.randn((2, 3, 8, 64, 64), generator=torch.Generator().manual_seed(5)).to(dev)
+        loss = torch.nn.functional.cross_entropy(m(x), torch.tensor([1, 2], device=dev))
+        loss.backward()
+        torch.optim.SGD(groups, lr=1e-5).step()
+        torch.cuda.synchronize()
+        assert all(torch.isfinite(p.grad).all() for p in m.parameters() if p.grad is not None)
+        print("%-28s loss %.4f" % ("%s fine-tune step" % arch, loss.item()), flush=True)
 print("sanitize_run: done")
