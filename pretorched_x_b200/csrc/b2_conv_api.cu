@@ -553,6 +553,8 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   p.Ho = (a->H + 2 * a->ph - a->kh) / 2 + 1;
   p.Wo = (a->W + 6 - 7) / 2 + 1;
   p.kt = a->kt; p.kh = a->kh; p.pt = a->pt; p.ph = a->ph;
+  // with pt >= kt the first output frames see no input frame at all; the kernel expects every item to have a tap inside the clip
+  if (a->pt >= a->kt) return set_error(B2_ERR_UNSUPPORTED, "stem convolution needs temporal padding < kt (got pt=%d, kt=%d)", a->pt, a->kt);
   p.G = kStemAccCols / BN;
   p.rows = 2 * (p.G - 1) + a->kh;
   if (p.rows > kStemMaxRows) return set_error(B2_ERR_UNSUPPORTED, "stem kernel height %d too large", a->kh);
@@ -567,7 +569,7 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   }
   p.w_bytes = a->kh * BN * 64;
   p.stage_bytes = ((p.rows * kStemPitch + p.w_bytes) + 127) / 128 * 128;
-  const int tail_bytes = 128 + 2048 + 1024 + acc_bytes(2 * kStemAccCols) + 256;   // barriers, scale / shift, W-pool exchange slots, accumulators
+  const int tail_bytes = kStemTailBytes + 128;                  // + alignment of the dynamic shared-memory base
   p.nstages = (227 * 1024 - tail_bytes) / p.stage_bytes;
   if (p.nstages > kStemMaxStages) p.nstages = kStemMaxStages;
   if (p.nstages < 1) return set_error(B2_ERR_UNSUPPORTED, "stem slab does not fit in shared memory (kh=%d)", a->kh);
@@ -593,7 +595,8 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   if (a->pool_w && (!a->relu || p.tiles_w != 1))
     return set_error(B2_ERR_UNSUPPORTED, "fused W pooling needs ReLU and an output row of at most %d columns (got %d)", kStemTileW, p.Wo);
   const int smem_bytes = p.nstages * p.stage_bytes + tail_bytes;
-  B2_OPT_IN_SMEM(stemconv_kernel<BN>, 227 * 1024);
+  B2_OPT_IN_SMEM((stemconv_kernel<BN, false>), 227 * 1024);
+  B2_OPT_IN_SMEM((stemconv_kernel<BN, true>), 227 * 1024);
   // input viewed as 8-byte pixels (W, H, N*T); box (256, rows, 1); no swizzle -> dense 2 KB rows in smem
   CUtensorMap tmX;
   cuuint64_t dims[3] = {(cuuint64_t)a->W, (cuuint64_t)a->H, (cuuint64_t)a->N * a->T};
@@ -610,7 +613,8 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error(B2_ERR_CUDA, "cuTensorMapEncodeTiled(stem) failed (%d)", (int)r);
   const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
-  B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN>, dim3(grid), dim3(kStemThreads), smem_bytes, stream, tmX, p));
+  if (p.nstages == 1) B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, true>, dim3(grid), dim3(kStemThreads), smem_bytes, stream, tmX, p));
+  else B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, false>, dim3(grid), dim3(kStemThreads), smem_bytes, stream, tmX, p));
   B2_CHECK_LAUNCH("stemconv_kernel");
   return B2_OK;
 }

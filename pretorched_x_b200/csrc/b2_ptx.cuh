@@ -192,6 +192,14 @@ __device__ __forceinline__ void acc_zero32(const AccTile& t, int row, int col) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// Register accumulators that wgmma reads and writes asynchronously: keeps the compiler from moving ordinary reads or writes of
+// them across a wgmma.fence / wait_group.
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 template <int TB>
 __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b) {

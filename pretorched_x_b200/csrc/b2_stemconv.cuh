@@ -11,38 +11,49 @@
 // its way to the tensor core.
 //
 // Input-row-stationary schedule.  Slab row i (input row 2*ho0 - ph + i) feeds local output row g through vertical
-// tap dh = i - 2g, i.e. up to G consecutive output rows.  The per-row accumulators sit side by side in the accumulator
-// tile (row g at column BN*g) and the weight image stores the taps of one parity class in *decreasing* dh order, so
-// all of those contributions are ONE MMA: A = the Toeplitz tile of slab row i, B = [W(dh_max); W(dh_max-2); ...]
-// (N = BN x #taps, up to kStemAccCols), D = the accumulator columns of the touched output rows.  Every A tile is read
-// from shared memory once per slab row instead of once per (output row, dh).  Accumulators start from zero (stored
-// by the epilogue warps), so every MMA accumulates.
+// tap dh = i - 2g, i.e. up to G consecutive output rows.  The per-row accumulators sit side by side in each consumer
+// thread's registers (row g at fragment columns [BN*g, BN*g + BN)) and the weight image stores the taps of one parity class
+// in *decreasing* dh order, so all of those contributions are ONE wgmma: A = the Toeplitz tile of slab row i, B =
+// [W(dh_max); W(dh_max-2); ...] (N = BN x #taps <= G * BN), D = the fragments of the touched output rows.  Every A tile is
+// read from shared memory once per slab row instead of once per (output row, dh).
 //
-// Persistent CTAs (one per SM) walk (plane, row-group, column-tile) work items; two accumulator sets in shared memory
-// let the epilogue of item i (BN + ReLU -> fp16 NDHWC) overlap the MMAs of item i+1.
-// Warps 0-7: epilogue (the two warpgroups split the 32-column chunks), 8-11: MMA warpgroup, 12: TMA/bulk-copy producer.
+// Register accumulators.  Two consumer warpgroups own 64 of the 128 tile rows each (pair mode: one plane each) and keep
+// G * BN / 2 fp32 accumulators per thread for a whole work item.  A temporal tap's MMAs are issued back to back and committed
+// as one group; wait_group 1 keeps one tap in flight while the next one is issued, and a ring slot is released once the
+// group that read it has retired.  Each element sees the same sequence of fp32 accumulations as a per-row, per-N-tile
+// schedule would: temporal tap, slab row ascending, K step ascending.
+//
+// Persistent CTAs (one per SM) walk (plane, row-group, column-tile) work items.  At the end of an item the consumers apply
+// the BN affine (+ ReLU) to their fragments and write fp16 into one of two staging tiles ([128 rows][G * BN + 8]); the
+// epilogue warps (one tile row per thread) take the W direction of the max-pool there and do the global stores while the
+// consumers run the next item.
+// Warps 0-7: consumer warpgroups, 8-11: epilogue, 12: TMA/bulk-copy producer.
 #pragma once
 
 #include "b2_ptx.cuh"
 
 namespace b2 {
 
-constexpr int kStemThreads = 416;       // warps 0-7: epilogue (even / odd 32-column chunks), 8-11: MMA warpgroup, 12: producer
-constexpr int kStemMmaWarp0 = 8;
+constexpr int kStemThreads = 416;       // warps 0-7: two consumer warpgroups, 8-11: epilogue, 12: producer
+constexpr int kStemEpiWarp0 = 8;
 constexpr int kStemTmaWarp = 12;
-constexpr int kStemAccCols = 128;       // one accumulator set: G * BN columns
+constexpr int kStemAccCols = 128;       // accumulator columns of one item: G * BN
 constexpr int kStemPitch = 2048;        // bytes per slab row: 256 pixels [2*w0-4, 2*w0+252) of 8 bytes
 constexpr int kStemRowPx = 256;         // TMA box width (the maximum box extent), one 8-byte element per pixel
 constexpr int kStemTileW = 120;         // output columns per item: rows r < 124 of the 128-row MMA tile see complete runs
 constexpr int kStemMaxStages = 4;
-constexpr int kStemMaxRows = 16;        // slab rows = 2*(G-1) + kh <= 2*3 + 9
+constexpr int kStemMaxRows = 16;        // slab rows = 2*(G-1) + kh
+constexpr int kStemStgLd = kStemAccCols + 8;                 // staging tile pitch in halves (272 B: conflict-free both ways)
+constexpr int kStemStgBytes = 128 * kStemStgLd * 2;          // one fp16 staging tile
+// barriers, scale / shift, W-pool exchange slots, two staging tiles
+constexpr int kStemTailBytes = 128 + 2048 + 512 + 2 * kStemStgBytes;
 
 struct StemParams {
   int T, H, W;             // input dims per clip (W even)
   int To, Ho, Wo;
   int kt, kh;              // kw == 7, strides (1, 2, 2)
   int pt, ph;
-  int G;                   // output rows per item (G * BN <= kStemAccCols)
+  int G;                   // output rows per item (G * BN == kStemAccCols)
   int rows;                // slab rows = 2*(G-1) + kh
   int stage_bytes;         // slab + weights of one temporal tap, multiple of 128
   int w_bytes;             // kh * BN * 64: weight image of one temporal tap for one N tile
@@ -100,29 +111,44 @@ __device__ __forceinline__ StemItem stem_item(const StemParams& p, int item) {
   return it;
 }
 
-template <int BN>
+// One slab row's contribution (two K steps of 16) to the N = N_ fragment columns starting at d.  A: SWIZZLE_NONE Toeplitz view,
+// K step 32 B; B: the stacked tap images, K step 256 B.
+template <int N_>
+__device__ __forceinline__ void stem_mma(float* d, uint64_t a, uint64_t b) {
+  static_assert(N_ == 64 || N_ == 128, "stem MMA width");
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    if constexpr (N_ == 64) wgmma_n64<0>(*reinterpret_cast<float(*)[32]>(d), a + 2 * k, b + 16 * k);
+    else wgmma_n128_ss(*reinterpret_cast<float(*)[64]>(d), a + 2 * k, b + 16 * k);
+  }
+}
+
+// kOneSlot: tall filters (BN = 128 with kh >= 8, BN = 64 with kh >= 13) leave room for a single ring slot.  A separate instance,
+// because a wait_group 0 inside the tap loop makes ptxas serialise the wgmma pipeline of the common, multi-slot one.
+template <int BN, bool kOneSlot>
 __global__ void __launch_bounds__(kStemThreads, 1)
 stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pixels (W, H, N*T), box (256, rows, 1), no swizzle
                 const StemParams p) {
+  constexpr int G = kStemAccCols / BN;
+  static_assert(G * BN == kStemAccCols && (G == 1 || G == 2), "stem tile");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align<128>(smem_raw);
   uint8_t* tail = smem + p.nstages * p.stage_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(tail);          // [kStemMaxStages]
   uint64_t* empty = full + kStemMaxStages;
-  uint64_t* acc_full = empty + kStemMaxStages;                 // [2]
-  uint64_t* acc_empty = acc_full + 2;                          // [2]
+  uint64_t* stg_full = empty + kStemMaxStages;                 // [2]
+  uint64_t* stg_empty = stg_full + 2;                          // [2]
   float* s_scale = reinterpret_cast<float*>(tail + 128);       // [256] (ntiles_n * BN <= 256 is enforced by the host)
   float* s_shift = s_scale + 256;
-  uint32_t* s_xchg = reinterpret_cast<uint32_t*>(s_shift + 256);   // [2 groups][2][4][16]: lane 31 of each epilogue warp, for the W pool
-  const AccTile at{reinterpret_cast<float*>(s_xchg + 256), acc_ld(2 * kStemAccCols)};
+  uint32_t* s_xchg = reinterpret_cast<uint32_t*>(s_shift + 256);   // [2][4][16]: lane 31 of each epilogue warp, for the W pool
+  __half* s_stg = reinterpret_cast<__half*>(s_xchg + 128);         // [2][128][kStemStgLd]
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int slab_bytes = p.rows * kStemPitch;
-  constexpr int kAccCols = kStemAccCols;
 
-  if (tid == 128) {
-    for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 256); }
+  if (tid == 0) {
+    for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&stg_full[i], 256); mbar_init(&stg_empty[i], 128); }
     fence_mbar_init();
     tma_prefetch_desc(&tmX);
   }
@@ -154,89 +180,125 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
         __syncwarp();
       }
     }
-  } else if (warp >= kStemMmaWarp0) {
-    // ================================ MMA warpgroup =====================================
-    // SWIZZLE_NONE K-major descriptors: hi = SBO >> 4; lo = addr >> 4 | (LBO >> 4) << 16.  A: SBO 128 B (64 rows = 1 KB),
-    // K step 32 B; B: SBO 512 B (16 rows = 1 KB), LBO 128 B, K step 256 B.
+  } else if (warp < kStemEpiWarp0) {
+    // ================================ consumer warpgroups ===============================
+    // SWIZZLE_NONE K-major descriptors: hi = SBO >> 4; lo = addr >> 4 | (LBO >> 4) << 16.  A: SBO 128 B, LBO 16 B; the
+    // warpgroup's 64 tile rows start 64 x 16 B = 1 KB into the slab row.  B: SBO 512 B (8 rows), LBO 128 B.
     constexpr uint32_t a_hi = 128u >> 4, b_hi = 512u >> 4;
     constexpr uint32_t kTapBytes = BN * 64;            // weight image of one (dt, dh) tap: BN rows x 32 k
-    const uint32_t base = smem_u32(smem);
+    const int wg = warp >> 2;
+    const uint32_t base = smem_u32(smem) + static_cast<uint32_t>(wg) * 1024u;
+    // fragment position: rows r0 and r0 + 8 of the tile, column pairs 8 j + c0
+    const int r0 = wg * 64 + (warp & 3) * 16 + ((tid & 31) >> 2);
+    const int c0 = 2 * (tid & 3);
+    float acc[G * BN / 2];
     int it = 0, lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const StemItem w = stem_item(p, item);
       const int dt_lo = max(0, p.pt - w.to), dt_hi = min(p.kt - 1, p.T - 1 - w.to + p.pt);
-      const int g_valid = min(p.G, p.Ho - w.ho0);
-      const int ab = lt & 1;
-      mbar_wait(&acc_empty[ab], (lt >> 1) & 1);            // the epilogue has drained and re-zeroed this set
-      const int acc = ab * kAccCols;
+#pragma unroll
+      for (int k = 0; k < G * BN / 2; ++k) acc[k] = 0.f;
+      reg_fence(acc);
+      int prev_s = -1;
       for (int dt = dt_lo; dt <= dt_hi; ++dt, ++it) {
         const int s = it % p.nstages;
         mbar_wait(&full[s], (it / p.nstages) & 1);
         const uint32_t slab = base + s * p.stage_bytes;
-        const uint32_t wbase = slab + slab_bytes;
+        const uint32_t wbase = smem_u32(smem) + s * p.stage_bytes + slab_bytes;
+        wgmma_fence();
+#pragma unroll 1
         for (int i = 0; i < p.rows; ++i) {
-          const int g_lo = p.row_glo[i];
-          const int g_hi = min(static_cast<int>(p.row_ghi[i]), g_valid - 1);
+          const int g_lo = p.row_glo[i], g_hi = p.row_ghi[i];
           if (g_lo > g_hi) continue;
           const uint32_t a_lo = ((slab + static_cast<uint32_t>(i) * kStemPitch) >> 4) | ((16u >> 4) << 16);
           const uint32_t b_lo = ((wbase + static_cast<uint32_t>(p.row_slot[i]) * kTapBytes) >> 4) | ((128u >> 4) << 16);
-          const WgOperands ops{desc_from(a_hi, a_lo), desc_from(b_hi, b_lo), 2u, 64u, 16u, 256u, 64u};
-          wg_mma(at, acc + g_lo * BN, (g_hi - g_lo + 1) * BN, ops, 2, true);
+          const uint64_t a = desc_from(a_hi, a_lo), b = desc_from(b_hi, b_lo);
+          if constexpr (G == 1) {
+            stem_mma<BN>(acc, a, b);
+          } else {
+            if (g_lo != g_hi) stem_mma<2 * BN>(acc, a, b);
+            else if (g_lo == 0) stem_mma<BN>(acc, a, b);
+            else stem_mma<BN>(acc + BN / 2, a, b);
+          }
         }
-        wg_sync();
-        wg_arrive(&empty[s]);
-        if (dt == dt_hi) wg_arrive(&acc_full[ab]);
+        wgmma_commit();
+        if constexpr (kOneSlot) {                       // the next tap is loaded into this same slot: release it now
+          wgmma_wait0();
+          mbar_arrive(&empty[s]);
+        } else {
+          wgmma_wait1();                                // the previous tap's group has retired: its ring slot is free
+          if (prev_s >= 0) mbar_arrive(&empty[prev_s]);
+          prev_s = s;
+        }
       }
+      wgmma_wait0();
+      reg_fence(acc);
+      if constexpr (!kOneSlot) mbar_arrive(&empty[prev_s]);   // every item has a tap inside the clip (pt < kt, checked by the host)
+
+      // ---- BN affine (+ ReLU) -> fp16 staging tile ----
+      const int sb = lt & 1;
+      mbar_wait(&stg_empty[sb], ((lt >> 1) & 1) ^ 1);
+      __half* stg = s_stg + sb * (128 * kStemStgLd);
+      const int n0 = w.ntile * BN;
+#pragma unroll
+      for (int g = 0; g < G; ++g) {
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + c0;
+          const float2 sc = *reinterpret_cast<const float2*>(&s_scale[n0 + c]);
+          const float2 sh = *reinterpret_cast<const float2*>(&s_shift[n0 + c]);
+          const float* v = acc + g * (BN / 2) + 4 * j;
+          float a0 = v[0] * sc.x + sh.x, a1 = v[1] * sc.y + sh.y;
+          float b0 = v[2] * sc.x + sh.x, b1 = v[3] * sc.y + sh.y;
+          if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); b0 = fmaxf(b0, 0.f); b1 = fmaxf(b1, 0.f); }
+          *reinterpret_cast<uint32_t*>(stg + r0 * kStemStgLd + g * BN + c) = pack_half2(a0, a1);
+          *reinterpret_cast<uint32_t*>(stg + (r0 + 8) * kStemStgLd + g * BN + c) = pack_half2(b0, b1);
+        }
+      }
+      mbar_arrive(&stg_full[sb]);
     }
   } else {
     // ================================ epilogue ==========================================
-    // pixel (accumulator row) index of this thread, and its warpgroup's column chunks
-    const int ew = warp & 3, egroup = warp >= 4 ? 1 : 0;
-    const int erow = ew * 32 + (tid & 31);
-    for (int c = egroup * 32; c < 2 * kAccCols; c += 64) acc_zero32(at, erow, c);   // both accumulator sets start at zero
-    mbar_arrive(&acc_empty[0]);
-    mbar_arrive(&acc_empty[1]);
-    int lt = 0;
+    // thread = tile row (pixel) erow
+    const int ew = warp - kStemEpiWarp0;
+    const int erow = tid - kStemEpiWarp0 * 32;
+    const int lane = tid & 31;
+    int lt = 0, xit = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const StemItem w = stem_item(p, item);
       const int g_valid = min(p.G, p.Ho - w.ho0);
-      const int ab = lt & 1;
+      const int sb = lt & 1;
       const int n0 = w.ntile * BN;
       const int ncols_here = min(BN, p.ldy - n0);
       const int wo = p.pair ? (erow & 63) : w.w0 + erow;
       const int plane_out = p.pair ? 2 * w.plane_o + (erow >> 6) : w.plane_o;
       const bool col_ok = p.pair ? (wo < p.Wo && plane_out < p.planes_total) : ((erow < kStemTileW) && (wo < p.Wo));
-      mbar_wait(&acc_full[ab], (lt >> 1) & 1);
-      const int acc = ab * kAccCols;
+      mbar_wait(&stg_full[sb], (lt >> 1) & 1);
+      const __half* srow = s_stg + sb * (128 * kStemStgLd) + erow * kStemStgLd;
       if (p.pool_w) {
-        // ---- BN + ReLU, then max over the 3-wide / stride-2 window along W before anything is written ----
-        // thread tid holds output column wo = tid (one column tile per row); even columns 2wp produce pooled column wp from
+        // ---- max over the 3-wide / stride-2 window along W before anything is written ----
+        // thread erow holds output column wo = erow (one column tile per row); even columns 2wp produce pooled column wp from
         // their own value and both neighbours: lanes +-1 by shuffle, the left neighbour of lane 0 through shared memory.
         // Post-ReLU values are >= 0, so a missing neighbour (image border, column >= Wo) contributes 0 without changing the max.
-        const int lane = tid & 31;
-        int xit = 0;
         for (int g = 0; g < g_valid; ++g) {
           const size_t prow = (static_cast<size_t>(w.plane_o) * p.Ho + (w.ho0 + g)) * p.Wp + (erow >> 1);
           __half* yrow = p.y + prow * p.ldy + n0;
 #pragma unroll 1
-          for (int jc = egroup; jc < BN / 32; jc += 2, ++xit) {
-            uint32_t v[32];
-            acc_ld32(at, erow, acc + g * BN + jc * 32, v);
+          for (int jc = 0; jc < BN / 32; ++jc, ++xit) {
             uint32_t h[16];
+            const uint4* src = reinterpret_cast<const uint4*>(srow + g * BN + jc * 32);
 #pragma unroll
-            for (int e = 0; e < 16; ++e) {
-              const int ci = n0 + jc * 32 + e * 2;
-              const float a0 = fmaxf(__uint_as_float(v[e * 2]) * s_scale[ci] + s_shift[ci], 0.f);
-              const float a1 = fmaxf(__uint_as_float(v[e * 2 + 1]) * s_scale[ci + 1] + s_shift[ci + 1], 0.f);
-              h[e] = col_ok ? pack_half2(a0, a1) : 0u;
+            for (int q = 0; q < 4; ++q) {
+              const uint4 u = src[q];
+              h[4 * q] = col_ok ? u.x : 0u; h[4 * q + 1] = col_ok ? u.y : 0u;
+              h[4 * q + 2] = col_ok ? u.z : 0u; h[4 * q + 3] = col_ok ? u.w : 0u;
             }
-            uint32_t* xb = s_xchg + (((egroup * 2 + (xit & 1)) * 4) + ew) * 16;
+            uint32_t* xb = s_xchg + ((xit & 1) * 4 + ew) * 16;
             if (lane == 31) {
 #pragma unroll
               for (int e = 0; e < 16; ++e) xb[e] = h[e];
             }
-            if (egroup) asm volatile("bar.sync 2, 128;" ::: "memory");       // the four warps of this warpgroup (double-buffered slots:
-            else asm volatile("bar.sync 1, 128;" ::: "memory");             // one barrier per chunk)
+            asm volatile("bar.sync 1, 128;" ::: "memory");       // the four epilogue warps (double-buffered slots: one barrier per chunk)
             uint32_t m[16];
 #pragma unroll
             for (int e = 0; e < 16; ++e) {
@@ -257,36 +319,17 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
             }
           }
         }
-      } else
-      for (int g = 0; g < g_valid; ++g) {
-        const size_t row = (static_cast<size_t>(plane_out) * p.Ho + (w.ho0 + g)) * p.Wo + wo;
-        __half* yrow = p.y + row * p.ldy + n0;
-#pragma unroll 1
-        for (int jc = egroup; jc < BN / 32; jc += 2) {
-          uint32_t v[32];
-          acc_ld32(at, erow, acc + g * BN + jc * 32, v);
-          if (col_ok) {
+      } else if (col_ok) {
+        for (int g = 0; g < g_valid; ++g) {
+          const size_t row = (static_cast<size_t>(plane_out) * p.Ho + (w.ho0 + g)) * p.Wo + wo;
+          __half* yrow = p.y + row * p.ldy + n0;
+          const uint4* src = reinterpret_cast<const uint4*>(srow + g * BN);
 #pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8) {
-              const int col = jc * 32 + c8 * 8;
-              if (col < ncols_here) {
-                uint32_t o[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const int ci = n0 + col + e * 2;
-                  float a0 = __uint_as_float(v[c8 * 8 + e * 2]) * s_scale[ci] + s_shift[ci];
-                  float a1 = __uint_as_float(v[c8 * 8 + e * 2 + 1]) * s_scale[ci + 1] + s_shift[ci + 1];
-                  if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
-                  o[e] = pack_half2(a0, a1);
-                }
-                *reinterpret_cast<uint4*>(yrow + col) = make_uint4(o[0], o[1], o[2], o[3]);
-              }
-            }
-          }
+          for (int c8 = 0; c8 < BN / 8; ++c8)
+            if (c8 * 8 < ncols_here) *reinterpret_cast<uint4*>(yrow + c8 * 8) = src[c8];
         }
       }
-      for (int c = egroup * 32; c < kAccCols; c += 64) acc_zero32(at, erow, acc + c);   // hand the set back zeroed (this group's chunks)
-      mbar_arrive(&acc_empty[ab]);
+      mbar_arrive(&stg_empty[sb]);
     }
   }
 }
