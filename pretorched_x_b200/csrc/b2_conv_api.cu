@@ -152,7 +152,8 @@ int make_tmap_ndhwc_5d(CUtensorMap* out, const void* base, uint64_t C, uint64_t 
 // ------------------------------------------------------------------------------------------
 static int g_conv_algo = 0;   // 0 auto, 1 force gather (debug / A-B comparisons)
 static int g_slab_wide = -1;       // 1: request 256-column N tiles for channel counts that are multiples of 256 (tuning; they only run
-                                   // where their accumulator tile fits in shared memory), otherwise the 128-column rule
+                                   // where MT * 256 fits kSlabAccCols, which the current register budget never allows), otherwise the
+                                   // 128-column rule
 static int g_slab_force_mt = -1;   // M tiles per slab work item: -1 read B2_SLAB_MT once, 0 cost model, > 0 forced (tuning)
 
 static int slab_naff(int ldy) { return (ldy + 31) / 32 * 32 + 256; }   // chunk reads may run past ldy inside the last N tile
@@ -258,8 +259,10 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.plane_stride = R * p.PW * 128;
   p.slab_bytes = ((R * p.PW * 128 * (p.mp > 1 ? p.mp : 1)) + 1023) / 1024 * 1024;
   p.MT = MT;
-  const int smem_one = kSlabSStages * p.slab_bytes + kSlabWStages * p.wbytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024;
-  p.nacc = (smem_one + acc_bytes(2 * MT * p.accs) <= 227 * 1024) ? 2 : 1;
+  if (MT * BN > kSlabAccCols)
+    return set_error(B2_ERR_INVALID, "slab plan MT=%d x N=%d exceeds the %d register accumulator columns", MT, BN, kSlabAccCols);
+  if (!BNT && BN != 16 && (BN < 144 || BN > kSlabAccCols || BN % 16 != 0))
+    return set_error(B2_ERR_INVALID, "slab runtime N tile %d is not one of the compiled widths", BN);
   p.Ncols = a->K;
   p.scale = a->scale; p.shift = a->shift;
   p.residual = reinterpret_cast<const __half*>(a->residual);
@@ -279,7 +282,8 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.fd_To = make_fastdiv(p.To); p.fd_PW = make_fastdiv(p.PW);
   if (a->aff_ld && ((a->aff_ld & 3) || (reinterpret_cast<uintptr_t>(a->scale) & 15) || (reinterpret_cast<uintptr_t>(a->shift) & 15)))
     return set_error(B2_ERR_INVALID, "per-sample scale/shift must be 16-byte aligned with a pitch that is a multiple of 4 floats");
-  const int smem_bytes = smem_one + acc_bytes(p.nacc * MT * p.accs);
+  const int smem_bytes = kSlabSStages * p.slab_bytes + kSlabWStages * p.wbytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 +
+                         acc_bytes(MT * p.accs);
   B2_OPT_IN_SMEM(slabconv_kernel<BNT>, 227 * 1024);
   CUtensorMap tmX, tmB;
   int rc;
@@ -307,7 +311,7 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   if (a->ldy > 128) {
     const int tn = (a->ldy + 255) / 256;
     const int bn = (((a->ldy + tn - 1) / tn) + 15) / 16 * 16;
-    if ((long long)bn * tn * 21 <= (long long)ntn * 128 * 20 || (g_slab_wide == 1 && a->ldy % 256 == 0)) {
+    if (bn <= kSlabAccCols && ((long long)bn * tn * 21 <= (long long)ntn * 128 * 20 || (g_slab_wide == 1 && a->ldy % 256 == 0))) {
       flex = true; BN = bn; ntn = tn;
       p.bn = bn; p.wbytes = (bn * 128 + 1023) / 1024 * 1024; p.accs = (bn + 31) / 32 * 32;
     }
@@ -320,8 +324,8 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   const int acc_stride = flex ? p.accs : BN;
   const int w_stage = flex ? p.wbytes : BN * 128;
   // Pick the M tiles per work item from a cycle model of one SM's share: rounds of items x the slower of the MMA
-  // stream and the slab/weight loads, plus the epilogue when shared memory holds a single accumulator set (the rule of
-  // launch_slab) and the epilogue is therefore exposed.  (Model constants:
+  // stream and the slab/weight loads (the epilogue of an item overlaps the next item's MMAs).  MT * N is bounded by the
+  // consumers' register accumulators (kSlabAccCols).  (Model constants:
   // a 128xNx16 MMA retires in ~40 + N/2 cycles, TMA delivers ~48 B/cycle/SM out of L2; not re-fitted on H100.)
   int best_mt = 0, best_R = 0;
   double best_cost = 0.0;
@@ -340,13 +344,13 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   p.mp = 0;
   for (int MT = 4; MT >= 1; --MT) {
     if (force_mt > 0 && MT != force_mt && MT != 1) continue;
+    if (MT * BN > kSlabAccCols) continue;
     // (multi-plane: rows one plane's positions and taps can touch -- slab_rows assumes a full 128-position tile)
     const int R = mp_ok ? (p.P - 1 + p.reach) / p.PW + (p.reach + p.PW - 1) / p.PW + 1 : slab_rows(MT, p.PW, p.reach, p.P);
     if (p.ss * (R - 1) + 1 > 256) continue;
     const long long slab_b = ((long long)R * p.PW * 128 * (mp_ok ? MT : 1) + 1023) / 1024 * 1024;
     const long long smem_one = 2ll * slab_b + kSlabWStages * w_stage + 256 + 2 * slab_naff(a->ldy) * 4 + 1024;
     if (smem_one + acc_bytes(MT * acc_stride) > 227 * 1024) continue;
-    const bool two_sets = smem_one + acc_bytes(2 * MT * acc_stride) <= 227 * 1024;
     const long long tq = mp_ok ? 1 : (p.P + MT * 128 - 1) / (MT * 128);
     const long long items = (long long)ntn * tq * (mp_ok ? (planes + MT - 1) / MT : planes) * p.wchunks * (p.up ? 4 : 1);
     const double rounds = (double)((items + sm_count() - 1) / sm_count());
@@ -356,8 +360,7 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
     // (modelled as 26 B/cycle/SM), not one SM's TMA rate
     const double bpc = mp_ok ? 26.0 : 48.0;
     const double load = (double)p.kt * p.n_sub * p.cchunks * slab_b / bpc + (double)p.kt * taps_hw * p.cchunks * w_stage / bpc;
-    const double epi = two_sets ? 0.0 : tiles_per_item * ((BN + 31) / 32) * 250.0;
-    const double cost = rounds * ((mma > load ? mma : load) + epi + 1500.0);
+    const double cost = rounds * ((mma > load ? mma : load) + 1500.0);
     if (force_mt == -1) {                                   // previous rule (A/B): largest power-of-two MT with >= 2 rounds of items
       if ((MT & (MT - 1)) != 0 && !flex) continue;
       best_mt = MT; best_R = R;
@@ -367,7 +370,7 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
     if (best_mt == 0 || cost < best_cost || (force_mt > 0 && MT == force_mt)) { best_mt = MT; best_R = R; best_cost = cost; }
     if (force_mt > 0 && MT == force_mt) break;
   }
-  if (mp_ok && best_mt >= 2 && best_mt < 4 && force_mt <= 0) {
+  if (mp_ok && best_mt >= 2 && best_mt < 4 && force_mt <= 0 && 4 * BN <= kSlabAccCols) {
     // four planes per item share each weight tile twice as often as two, as long as a full wave of items remains
     const int R4 = (p.P - 1 + p.reach) / p.PW + (p.reach + p.PW - 1) / p.PW + 1;
     const long long slab4 = ((long long)R4 * p.PW * 128 * 4 + 1023) / 1024 * 1024;
@@ -440,20 +443,17 @@ static int try_slabts(const b2_conv_args* a, cudaStream_t stream) {
   if (a->kh * a->kw < 9 || a->residual) return 0;
   SlabParams p;
   if (!slab_geometry(a, &p, 0) || p.n_sub != 1) return 0;
-  int MT = p.P > 128 ? 2 : 1, R = 0;
-  long long smem = 0;
-  for (; MT >= 1; --MT) {
-    R = slab_rows(MT, p.PW, p.reach, p.P);
-    const long long slab_b = ((long long)R * p.PW * 128 + 1023) / 1024 * 1024;
-    smem = kSlabSStages * slab_b + kSlabWStages * kTsWBytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 + acc_bytes(MT * kTsGroup * kTsBN);
-    if (R <= 256 && smem <= 227 * 1024) break;
-  }
-  if (MT < 1) return 0;
+  // one M tile per item: its 3 x 64 accumulator columns are what the consumers' registers hold (kSlabAccCols)
+  const int R = slab_rows(1, p.PW, p.reach, p.P);
+  const long long slab_b = ((long long)R * p.PW * 128 + 1023) / 1024 * 1024;
+  const long long smem = kSlabSStages * slab_b + kSlabWStages * kTsWBytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 +
+                         acc_bytes(kTsGroup * kTsBN);
+  if (R > 256 || smem > 227 * 1024) return 0;
   p.R = R;
   p.planes_total = a->N * p.To;
   p.plane_stride = R * p.PW * 128;
-  p.slab_bytes = ((R * p.PW * 128 * (p.mp > 1 ? p.mp : 1)) + 1023) / 1024 * 1024;
-  p.MT = MT; p.nacc = 1; p.bn = kTsBN; p.wbytes = kTsWBytes; p.accs = kTsBN;
+  p.slab_bytes = (int)slab_b;
+  p.MT = 1; p.bn = kTsBN; p.wbytes = kTsWBytes; p.accs = kTsBN;
   p.Ncols = a->K;
   p.scale = a->scale; p.shift = a->shift;
   p.residual = reinterpret_cast<const __half*>(a->residual);
@@ -463,7 +463,7 @@ static int try_slabts(const b2_conv_args* a, cudaStream_t stream) {
   p.relu = a->relu;
   p.naff = slab_naff(a->ldy);
   p.tiles_n = 1;
-  p.tiles_q = (p.P + MT * 128 - 1) / (MT * 128);
+  p.tiles_q = (p.P + 127) / 128;
   const int groups = (p.To + kTsGroup - 1) / kTsGroup;
   const long long items = (long long)p.tiles_q * p.wchunks * a->N * groups;
   if (items >= (1ll << 31)) return 0;

@@ -20,18 +20,26 @@
 // positions that fall on halo columns are discarded.  Rows longer than a TMA box are cut into W chunks (each with
 // its own halo); a purely temporal (kt,1,1) filter is run as a (1,kt,1) filter over the image "frames x (H*W)",
 // so its slab holds MT+kt-1 frames of one position chunk and every temporal tap is a whole-row shift of it.
-// CTAs are persistent (one per SM): the producer runs ahead
-// into the next item's slabs, and when shared memory has room for two accumulator sets (AccTile, b2_ptx.cuh) the
-// epilogue of item i overlaps the MMAs of item i+1.
+// CTAs are persistent (one per SM): the producer runs ahead into the next item's slabs.  Two consumer warpgroups keep the
+// item's fp32 accumulators in registers (each owns 64 rows of every M tile) from its first K block to its last, then store
+// them once into an accumulator tile in shared memory (AccTile, b2_ptx.cuh) and go on with the next item while the three
+// epilogue warps (one tile row per thread and pass) apply the affine / residual / ReLU and write y.
 #pragma once
 
 #include "b2_ptx.cuh"
 
 namespace b2 {
 
-constexpr int kSlabThreads = 416;   // warps 0-7: epilogue (even / odd 32-column chunks), 8-11: MMA warpgroup, 12: TMA producer
-constexpr int kSlabMmaWarp0 = 8;
-constexpr int kSlabTmaWarp = 12;
+constexpr int kSlabThreads = 384;   // warps 0-7: two consumer (MMA) warpgroups, 8-10: epilogue, 11: TMA producer
+constexpr int kSlabConsumerWarps = 8;
+constexpr int kSlabEpiWarp0 = 8;
+constexpr int kSlabEpiWarps = 3;
+constexpr int kSlabTmaWarp = 11;
+// Accumulator columns of one work item (MT x N tile) held in registers: each consumer thread keeps kSlabAccCols / 2 fp32 for the
+// whole item.  Twelve warps are three per SM sub-partition, whose 64 KB register file then allows 168 registers per thread (a
+// thirteenth warp would cut that to 128).  The tile planner (slab_pick_tiles, try_slabts in b2_conv_api.cu) never picks MT * N
+// above kSlabAccCols; the consumer loops size their register arrays from it.
+constexpr int kSlabAccCols = 192;
 constexpr int kSlabWStages = 4;     // weight-tile ring depth
 constexpr int kSlabSStages = 2;     // slab ring depth
 
@@ -57,8 +65,7 @@ struct SlabParams {
   unsigned char sub_tap[kSlabMaxSub][kSlabMaxTaps];
   int reach;               // max |sub_off|
   int slab_bytes;          // R * PW * 128, rounded up to 1024
-  int MT;                  // M tiles per work item
-  int nacc;                // accumulator sets: 2 when they fit in shared memory (epilogue overlaps the next item)
+  int MT;                  // M tiles per work item (MT * N tile <= kSlabAccCols)
   // runtime N tile (slabconv_kernel<0> only; the <64>/<128> instances use their template value): Cout = 144, 288,
   // 576 ... of the (2+1)D factorisation would waste up to 44% of the MMA columns on 128-wide tiles
   int bn;                  // N per MMA / per tile, multiple of 16, <= 256
@@ -90,7 +97,7 @@ struct SlabParams {
 };
 
 // scale/shift live in smem for all (padded) output channels: SlabParams::naff = round_up(ldy, 32) + 32 entries each; the
-// accumulator tile (nacc * MT * accs columns) follows them
+// accumulator tile (MT * accs columns) through which the consumers hand each item to the epilogue follows them
 
 struct SlabItem {
   int n0, q0, wc, plane_o, plane_i0, r_lo, dt_lo, n_dt, n_slabs, mt_valid;   // plane_i0: input plane of temporal tap 0
@@ -124,6 +131,86 @@ __device__ __forceinline__ SlabItem slab_item(const SlabParams& p, int item, int
   return w;
 }
 
+// eight consecutive accumulator columns of one row of an AccTile (16-byte aligned)
+__device__ __forceinline__ void acc_ld8(const float* src, float (&v)[8]) {
+  const float4 a = reinterpret_cast<const float4*>(src)[0], b = reinterpret_cast<const float4*>(src)[1];
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+
+// K steps of one (tap, 64-channel block) for an N-column tile whose fragments start at d: one wgmma per K step; the last channel
+// chunk of C = 144, 288, 232 ... skips its all-zero K steps
+template <int N>
+__device__ __forceinline__ void slab_mma(float* d, uint64_t a, uint64_t b, int ksteps) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (k < ksteps) wgmma_ss<N>(d, a + 2 * k, b + 2 * k);    // K step: +32 B on both start addresses
+}
+
+// Consumer warpgroups of slabconv_kernel for an N tile of N columns.  Warpgroup wg owns rows [64 wg, 64 wg + 64) of every M tile of
+// an item; tile j sits at fragment columns [j N, j N + N) of each thread's registers from the item's first K block to its last.  The
+// MMAs of one tap form one commit group, one group stays in flight, and a ring slot is released when the group that read it retires.
+template <int N>
+__device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile& at, int accs, uint32_t slab0, uint32_t w0s,
+                                              int w_bytes, uint64_t* slab_full, uint64_t* slab_empty, uint64_t* w_full,
+                                              uint64_t* w_empty, uint64_t* acc_full, uint64_t* acc_empty) {
+  constexpr int kMaxMT = kSlabAccCols / N < 4 ? kSlabAccCols / N : 4;
+  float acc[kMaxMT * N / 2];
+  const int wg = threadIdx.x >> 7;
+  const bool lead = (threadIdx.x & 31) == 0;                 // one arrival per consumer warp on the ring barriers
+  const uint32_t a_wg = static_cast<uint32_t>(wg) * (64u * 128u >> 4);   // this warpgroup's 64 rows, in 16-byte units
+  const uint32_t tile_stride16 = (p.mp > 1 ? static_cast<uint32_t>(p.plane_stride) : 128u * 128u) >> 4;   // A start of tile j
+  int wit = 0, sg = 0, lt = 0;
+  for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
+    const SlabItem w = slab_item(p, item, N);
+#pragma unroll
+    for (int k = 0; k < kMaxMT * N / 2; ++k) acc[k] = 0.f;
+    reg_fence(acc);
+    int prev_ws = -1, prev_s = -1;                           // ring slots read by the group in flight
+    const int mt_valid = warp_uniform(w.mt_valid);
+    for (int si = 0; si < w.n_slabs; ++si, ++sg) {
+      const int sub = p.up ? w.phase : si % p.n_sub;
+      const int ntaps = p.sub_ntaps[sub];
+      const int cc = (si / p.n_sub) / w.n_dt;
+      const int ksteps = warp_uniform(min(4, (p.C - cc * 64 + 15) >> 4));       // 16-channel K steps that hold real channels
+      const int s = sg % kSlabSStages;
+      mbar_wait(&slab_full[s], (sg / kSlabSStages) & 1);
+      const uint32_t slab_addr = slab0 + s * p.slab_bytes;
+      for (int ti = 0; ti < ntaps; ++ti, ++wit) {
+        const int ws = wit % kSlabWStages;
+        mbar_wait(&w_full[ws], (wit / kSlabWStages) & 1);
+        // slab-local pixel index of padded output position q0 under this tap
+        const int pix0 = w.q0 + p.sub_off[sub][ti] - w.r_lo * p.PW;
+        const uint64_t b = desc_from(kSw128DescHi, sw128_desc_lo(w0s + ws * w_bytes));
+        const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u) + a_wg;
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < kMaxMT; ++j)
+          if (j < mt_valid) slab_mma<N>(acc + j * (N / 2), desc_from(kSw128DescHi, a_lo0 + j * tile_stride16), b, ksteps);
+        wgmma_commit();
+        wgmma_wait1();                                       // the previous tap's group has retired: release what it read
+        if (lead && prev_ws >= 0) {
+          mbar_arrive(&w_empty[prev_ws]);
+          if (prev_s >= 0) mbar_arrive(&slab_empty[prev_s]);
+        }
+        prev_ws = ws;
+        prev_s = (ti == ntaps - 1) ? s : -1;
+      }
+    }
+    wgmma_wait0();
+    reg_fence(acc);
+    if (lead) {                                              // every item has a slab and a tap ("same" padding keeps tap 0 inside)
+      mbar_arrive(&w_empty[prev_ws]);
+      mbar_arrive(&slab_empty[prev_s]);
+    }
+    // hand the item to the epilogue: one store of the fragments into the accumulator tile, then straight on to the next item
+    mbar_wait(acc_empty, (lt & 1) ^ 1);
+#pragma unroll
+    for (int j = 0; j < kMaxMT; ++j)
+      if (j < mt_valid) frag_io<N>(at, wg * 64, j * accs, *reinterpret_cast<float(*)[N / 2]>(acc + j * (N / 2)), false, false);
+    mbar_arrive(acc_full);
+  }
+}
+
 template <int BN>   // BN = 0: N tile taken from SlabParams::bn at run time
 __global__ void __launch_bounds__(kSlabThreads, 1)
 slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N*T), box (64, PW, R, 1)
@@ -141,19 +228,19 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
   uint64_t* slab_empty = slab_full + kSlabSStages;
   uint64_t* w_full = slab_empty + kSlabSStages;
   uint64_t* w_empty = w_full + kSlabWStages;
-  uint64_t* acc_full = w_empty + kSlabWStages;      // [2]
-  uint64_t* acc_empty = acc_full + 2;               // [2]
+  uint64_t* acc_full = w_empty + kSlabWStages;
+  uint64_t* acc_empty = acc_full + 1;
   float* s_scale = reinterpret_cast<float*>(tail + 256);     // barriers occupy the first 128 bytes
   float* s_shift = s_scale + p.naff;
 
   const int tid = threadIdx.x, warp = tid >> 5;
-  const int acc_cols = p.MT * accs;
-  const AccTile at{s_shift + p.naff, acc_ld(p.nacc * acc_cols)};
+  const AccTile at{s_shift + p.naff, acc_ld(p.MT * accs)};
 
-  if (tid == 128) {
-    for (int s = 0; s < kSlabSStages; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 1); }
-    for (int s = 0; s < kSlabWStages; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 256); }
+  if (tid == 0) {
+    for (int s = 0; s < kSlabSStages; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], kSlabConsumerWarps); }
+    for (int s = 0; s < kSlabWStages; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], kSlabConsumerWarps); }
+    mbar_init(acc_full, 32 * kSlabConsumerWarps);
+    mbar_init(acc_empty, 32 * kSlabEpiWarps);
     fence_mbar_init();
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmB);
@@ -169,8 +256,9 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
   if (warp == kSlabTmaWarp) {
     // ================================ TMA producer ======================================
     // Walks (item, slab) pairs; the slab after the current one -- possibly the first slab of the NEXT item -- is
-    // requested once the weight ring (kSlabWStages deep) guarantees the MMA warpgroup has retired the slab that
-    // occupied the target slot, so that wait never stalls weight issue.
+    // requested after weight tap min(kSlabWStages, ntaps - 1) of the current slab: from tap kSlabWStages on, the weight ring
+    // guarantees the consumers have retired the slab that occupied the target slot, so that wait never stalls weight issue;
+    // a slab with fewer taps issues all of its weights first (the previous slab is released only once this one's first tap runs).
     int wit = 0, sg = 0;                     // global weight-tile / slab counters (ring phases persist across items)
     int item = blockIdx.x;
     if (item < p.items_total) {
@@ -207,7 +295,6 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
           const int ntaps = p.sub_ntaps[sub];
           const int pf = min(kSlabWStages, ntaps - 1);
           for (int ti = 0; ti < ntaps; ++ti, ++wit) {
-            if (ti == pf && nxt_item < p.items_total) load_next();
             const int ws = wit % kSlabWStages;
             mbar_wait(&w_empty[ws], ((wit / kSlabWStages) & 1) ^ 1);
             const int tap = dt * p.khw + p.sub_tap[sub][ti];
@@ -216,158 +303,136 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
               tma_load_2d(w_base + ws * kWBytes, &tmB, &w_full[ws], tap * p.C + cc * 64, cur.n0);
             }
             __syncwarp();
+            if (ti == pf && nxt_item < p.items_total) load_next();
           }
         }
       }
     }
-  } else if (warp >= kSlabMmaWarp0) {
-    // ================================ MMA warpgroup =====================================
+  } else if (warp < kSlabEpiWarp0) {
+    // ================================ consumer warpgroups ===============================
     const uint32_t slab0 = smem_u32(slab_base), w0s = smem_u32(w_base);
-    const uint32_t tile_stride16 = (p.mp > 1 ? static_cast<uint32_t>(p.plane_stride) : 128u * 128u) >> 4;   // A start of tile j, in 16-byte units
-    int wit = 0, sg = 0, lt = 0;
-    for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
-      const SlabItem w = slab_item(p, item, bn);
-      const int ab = lt % p.nacc;
-      mbar_wait(&acc_empty[ab], (((lt / p.nacc) & 1) ^ 1));      // epilogue drained this accumulator set
-      const int acc = ab * acc_cols;
-      int wl = 0;                                                // weight step within the item
-      for (int si = 0; si < w.n_slabs; ++si, ++sg) {
-        const int sub = p.up ? w.phase : si % p.n_sub;
-        const int ntaps = p.sub_ntaps[sub];
-        const int cc = (si / p.n_sub) / w.n_dt;
-        const int ksteps = min(4, (p.C - cc * 64 + 15) >> 4);       // 16-channel K steps that hold real channels
-        const int s = sg % kSlabSStages;
-        mbar_wait(&slab_full[s], (sg / kSlabSStages) & 1);
-        const uint32_t slab_addr = slab0 + s * p.slab_bytes;
-        for (int ti = 0; ti < ntaps; ++ti, ++wit, ++wl) {
-          const int ws = wit % kSlabWStages;
-          mbar_wait(&w_full[ws], (wit / kSlabWStages) & 1);
-          // slab-local pixel index of padded output position q0 under this tap
-          const int pix0 = w.q0 + p.sub_off[sub][ti] - w.r_lo * p.PW;
-          const uint32_t b_lo = sw128_desc_lo(w0s + ws * kWBytes);
-          const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u);
-          // (the last channel chunk of C = 144, 288, 232 ... skips its all-zero K steps)
-          for (int j = 0; j < w.mt_valid; ++j)
-            wg_mma(at, acc + j * accs, bn, wg_sw128(desc_from(kSw128DescHi, a_lo0 + j * tile_stride16), desc_from(kSw128DescHi, b_lo)),
-                   ksteps, wl != 0);
-          wg_sync();
-          wg_arrive(&w_empty[ws]);
-          if (ti == ntaps - 1) wg_arrive(&slab_empty[s]);
-          if (ti == ntaps - 1 && si == w.n_slabs - 1) wg_arrive(&acc_full[ab]);
-        }
+    if constexpr (BN != 0) {
+      slab_consumer<BN>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty);
+    } else {
+      // runtime N: one compiled main loop per width the tile planner can pick (launch_slab rejects any other)
+      switch (bn) {
+#define B2_SLAB_N(n) case n: slab_consumer<n>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty); break;
+        B2_SLAB_N(16) B2_SLAB_N(144) B2_SLAB_N(160) B2_SLAB_N(176) B2_SLAB_N(192)
+#undef B2_SLAB_N
+        default: __trap();
       }
     }
   } else {
     // ================================ epilogue ==========================================
-    // thread = accumulator row; the two warpgroups split the accumulator columns
-    const int erow = (warp & 3) * 32 + (tid & 31);
-    const int egroup = warp >= 4 ? 1 : 0;
     int lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const SlabItem w = slab_item(p, item, bn);
-      const int ab = lt % p.nacc;
-      mbar_wait(&acc_full[ab], (lt / p.nacc) & 1);
-      const int acc = ab * acc_cols;
+      mbar_wait(acc_full, lt & 1);
       const int ncols_here = min(bn, p.ldy - w.n0);     // columns of this tile that exist in y (incl. zero padding)
-      // output row of this thread in each of the item's M tiles
-      size_t row[4];
-      bool ok[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int q = p.mp > 1 ? erow : w.q0 + j * 128 + erow;          // multi-plane items: tile j is plane plane_o + j
-        const int h = fdiv(q, p.fd_PW), wp = q - h * p.PW;
-        const int wo = w.wc * p.WC + wp - p.halo_l;       // output column
-        ok[j] = (j < w.mt_valid) && (q < p.P) && (wp >= p.halo_l) && (wp < p.halo_l + p.WC) && (wo < p.Wo);
-        const size_t plane = static_cast<size_t>(w.plane_o) + (p.mp > 1 ? j : 0);
-        row[j] = p.up ? (plane * (2 * p.Ho) + 2 * h + (w.phase >> 1)) * (2 * p.Wo) + 2 * wo + (w.phase & 1)
-                      : (plane * p.Ho + h) * p.Wo + wo;
-      }
+      // thread = accumulator row; the 96 epilogue threads cover the 128 tile rows in two passes
 #pragma unroll 1
-      for (int jc = egroup; jc * 32 < ncols_here; jc += 2) {
-        // folded-BN scale/shift of these 32 channels: registers, reused by every M tile of the item
-        float sc[32], sh[32];
-        const int c0 = w.n0 + jc * 32;
-        if (p.aff_ld) {
-          // per-sample affine (class-conditional BN of the consumer): the item lies in one image, every lane reads the
-          // same 32 + 32 floats (L1 broadcast) as 16-byte vectors; launch_slab checks the 16-byte alignment
-          const float* gs = p.scale + static_cast<size_t>(fdiv(w.plane_o, p.fd_To)) * p.aff_ld + c0;
-          const float* gt = p.shift + static_cast<size_t>(fdiv(w.plane_o, p.fd_To)) * p.aff_ld + c0;
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-            if (c0 + 4 * g + 4 <= p.Ncols) {
-              a = __ldg(reinterpret_cast<const float4*>(gs) + g);
-              b = __ldg(reinterpret_cast<const float4*>(gt) + g);
-            } else if (c0 + 4 * g < p.Ncols) {              // ragged tail of a channel count that is not a multiple of 4
-              float* ap = reinterpret_cast<float*>(&a); float* bp = reinterpret_cast<float*>(&b);
-              for (int e = 0; e < 4; ++e)
-                if (c0 + 4 * g + e < p.Ncols) { ap[e] = __ldg(gs + 4 * g + e); bp[e] = __ldg(gt + 4 * g + e); }
-            }
-            sc[4 * g] = a.x; sc[4 * g + 1] = a.y; sc[4 * g + 2] = a.z; sc[4 * g + 3] = a.w;
-            sh[4 * g] = b.x; sh[4 * g + 1] = b.y; sh[4 * g + 2] = b.z; sh[4 * g + 3] = b.w;
-          }
-        } else {
-#pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            sc[c] = s_scale[c0 + c];
-            sh[c] = s_shift[c0 + c];
-          }
-        }
-        // residual rows are requested one M tile AHEAD of their use (two register sets): the loads are independent of the MMAs,
-        // and issued load -> use per tile each would expose the HBM latency to the epilogue warps
-        uint4 rres[2][4];
-        auto load_res = [&](int j) {
-          if (p.residual && j < w.mt_valid && ok[j]) {
-            const __half* rrow = p.residual + row[j] * p.ldr + c0;
-#pragma unroll
-            for (int c8 = 0; c8 < 4; ++c8)
-              if (jc * 32 + c8 * 8 < ncols_here) rres[j & 1][c8] = __ldg(reinterpret_cast<const uint4*>(rrow + c8 * 8));
-          }
-        };
-        load_res(0);
+      for (int erow = tid - kSlabEpiWarp0 * 32; erow < 128; erow += 32 * kSlabEpiWarps) {
+        // output row of this thread in each of the item's M tiles
+        size_t row[4];
+        bool ok[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          if (j < w.mt_valid) {                            // warp-uniform
-            if (j + 1 < 4) load_res(j + 1);
-            uint32_t v[32];
-            acc_ld32(at, erow, acc + j * accs + jc * 32, v);
-            if (ok[j]) {
-              __half* yrow = p.y + row[j] * p.ldy + c0;
-              if (p.residual) {                              // uniform: residual added in fp32 before the single rounding
+          const int q = p.mp > 1 ? erow : w.q0 + j * 128 + erow;          // multi-plane items: tile j is plane plane_o + j
+          const int h = fdiv(q, p.fd_PW), wp = q - h * p.PW;
+          const int wo = w.wc * p.WC + wp - p.halo_l;       // output column
+          ok[j] = (j < w.mt_valid) && (q < p.P) && (wp >= p.halo_l) && (wp < p.halo_l + p.WC) && (wo < p.Wo);
+          const size_t plane = static_cast<size_t>(w.plane_o) + (p.mp > 1 ? j : 0);
+          row[j] = p.up ? (plane * (2 * p.Ho) + 2 * h + (w.phase >> 1)) * (2 * p.Wo) + 2 * wo + (w.phase & 1)
+                        : (plane * p.Ho + h) * p.Wo + wo;
+        }
+#pragma unroll 1
+        for (int jc = 0; jc * 32 < ncols_here; ++jc) {
+          // folded-BN scale/shift of these 32 channels: registers, reused by every M tile of the item
+          float sc[32], sh[32];
+          const int c0 = w.n0 + jc * 32;
+          if (p.aff_ld) {
+            // per-sample affine (class-conditional BN of the consumer): the item lies in one image, every lane reads the
+            // same 32 + 32 floats (L1 broadcast) as 16-byte vectors; launch_slab checks the 16-byte alignment
+            const float* gs = p.scale + static_cast<size_t>(fdiv(w.plane_o, p.fd_To)) * p.aff_ld + c0;
+            const float* gt = p.shift + static_cast<size_t>(fdiv(w.plane_o, p.fd_To)) * p.aff_ld + c0;
 #pragma unroll
-                for (int c8 = 0; c8 < 4; ++c8) {
-                  if (jc * 32 + c8 * 8 < ncols_here) {
-                    const uint4 rv = rres[j & 1][c8];
-                    const uint32_t rr[4] = {rv.x, rv.y, rv.z, rv.w};
-                    uint32_t o[4];
+            for (int g = 0; g < 8; ++g) {
+              float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+              if (c0 + 4 * g + 4 <= p.Ncols) {
+                a = __ldg(reinterpret_cast<const float4*>(gs) + g);
+                b = __ldg(reinterpret_cast<const float4*>(gt) + g);
+              } else if (c0 + 4 * g < p.Ncols) {              // ragged tail of a channel count that is not a multiple of 4
+                float* ap = reinterpret_cast<float*>(&a); float* bp = reinterpret_cast<float*>(&b);
+                for (int e = 0; e < 4; ++e)
+                  if (c0 + 4 * g + e < p.Ncols) { ap[e] = __ldg(gs + 4 * g + e); bp[e] = __ldg(gt + 4 * g + e); }
+              }
+              sc[4 * g] = a.x; sc[4 * g + 1] = a.y; sc[4 * g + 2] = a.z; sc[4 * g + 3] = a.w;
+              sh[4 * g] = b.x; sh[4 * g + 1] = b.y; sh[4 * g + 2] = b.z; sh[4 * g + 3] = b.w;
+            }
+          } else {
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                      const int c = c8 * 8 + e * 2;
-                      const float2 rf = unpack_half2(rr[e]);
-                      float a0 = fmaf(__uint_as_float(v[c]), sc[c], sh[c]) + rf.x;
-                      float a1 = fmaf(__uint_as_float(v[c + 1]), sc[c + 1], sh[c + 1]) + rf.y;
-                      if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
-                      o[e] = pack_half2(a0, a1);
+            for (int c = 0; c < 32; ++c) {
+              sc[c] = s_scale[c0 + c];
+              sh[c] = s_shift[c0 + c];
+            }
+          }
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            if (j < w.mt_valid) {                            // warp-uniform
+              // (the HBM latency of the residual row is hidden behind the consumers' next item, not behind the next M tile: one
+              // register set of residuals is what the budget leaves next to the scale / shift registers)
+              uint4 rres[4];
+              if (p.residual && ok[j]) {
+                const __half* rrow = p.residual + row[j] * p.ldr + c0;
+#pragma unroll
+                for (int c8 = 0; c8 < 4; ++c8)
+                  if (jc * 32 + c8 * 8 < ncols_here) rres[c8] = __ldg(reinterpret_cast<const uint4*>(rrow + c8 * 8));
+              }
+              // accumulators are read 8 columns at a time next to their use: with the scale / shift and residual registers a
+              // whole 32-column row segment would not fit the register budget
+              const float* arow = at.p + static_cast<size_t>(erow) * at.ld + j * accs + jc * 32;
+              if (ok[j]) {
+                __half* yrow = p.y + row[j] * p.ldy + c0;
+                if (p.residual) {                              // uniform: residual added in fp32 before the single rounding
+#pragma unroll
+                  for (int c8 = 0; c8 < 4; ++c8) {
+                    if (jc * 32 + c8 * 8 < ncols_here) {
+                      const uint4 rv = rres[c8];
+                      const uint32_t rr[4] = {rv.x, rv.y, rv.z, rv.w};
+                      float v[8];
+                      acc_ld8(arow + c8 * 8, v);
+                      uint32_t o[4];
+#pragma unroll
+                      for (int e = 0; e < 4; ++e) {
+                        const int c = c8 * 8 + e * 2;
+                        const float2 rf = unpack_half2(rr[e]);
+                        float a0 = fmaf(v[2 * e], sc[c], sh[c]) + rf.x;
+                        float a1 = fmaf(v[2 * e + 1], sc[c + 1], sh[c + 1]) + rf.y;
+                        if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                        o[e] = pack_half2(a0, a1);
+                      }
+                      *reinterpret_cast<uint4*>(yrow + c8 * 8) = make_uint4(o[0], o[1], o[2], o[3]);
                     }
-                    *reinterpret_cast<uint4*>(yrow + c8 * 8) = make_uint4(o[0], o[1], o[2], o[3]);
                   }
-                }
-              } else {                                       // no residual: affine, round, ReLU on the packed pairs
-                const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
+                } else {                                       // no residual: affine, round, ReLU on the packed pairs
+                  const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
 #pragma unroll
-                for (int c8 = 0; c8 < 4; ++c8) {
-                  if (jc * 32 + c8 * 8 < ncols_here) {
-                    uint4 ov;
-                    uint32_t* o = reinterpret_cast<uint32_t*>(&ov);
+                  for (int c8 = 0; c8 < 4; ++c8) {
+                    if (jc * 32 + c8 * 8 < ncols_here) {
+                      float v[8];
+                      acc_ld8(arow + c8 * 8, v);
+                      uint4 ov;
+                      uint32_t* o = reinterpret_cast<uint32_t*>(&ov);
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                      const int c = c8 * 8 + e * 2;
-                      __half2 hv = __floats2half2_rn(fmaf(__uint_as_float(v[c]), sc[c], sh[c]),
-                                                     fmaf(__uint_as_float(v[c + 1]), sc[c + 1], sh[c + 1]));
-                      if (p.relu) hv = __hmax2(hv, zero2);
-                      o[e] = *reinterpret_cast<uint32_t*>(&hv);
+                      for (int e = 0; e < 4; ++e) {
+                        const int c = c8 * 8 + e * 2;
+                        __half2 hv = __floats2half2_rn(fmaf(v[2 * e], sc[c], sh[c]),
+                                                       fmaf(v[2 * e + 1], sc[c + 1], sh[c + 1]));
+                        if (p.relu) hv = __hmax2(hv, zero2);
+                        o[e] = *reinterpret_cast<uint32_t*>(&hv);
+                      }
+                      *reinterpret_cast<uint4*>(yrow + c8 * 8) = ov;
                     }
-                    *reinterpret_cast<uint4*>(yrow + c8 * 8) = ov;
                   }
                 }
               }
@@ -375,7 +440,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
           }
         }
       }
-      mbar_arrive(&acc_empty[ab]);
+      mbar_arrive(acc_empty);
     }
   }
 }

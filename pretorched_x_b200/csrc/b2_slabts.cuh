@@ -9,11 +9,13 @@
 // a CONTIGUOUS row range of that stack and a contiguous column range of the accumulator [tile][slot][64]: one MMA of N = 64, 128 or
 // 192 per (in-plane tap, K step) instead of one N = 64 MMA per (temporal tap, in-plane tap, K step).  Five A tiles are read where the
 // plain form reads nine, and the operand bytes per MMA column drop from 96 to 53 (N = 192): 304 instead of 432 shared-memory cycles
-// per in-plane tap.  Accumulators start from zero (stored by the epilogue, as in the stem kernel), so every MMA accumulates and
-// slots may receive their first contribution from different input frames.
+// per in-plane tap.  Accumulators start from zero, so every MMA accumulates and slots may receive their first contribution from
+// different input frames.
 //
 // Same building blocks as the slab kernel: 4-D TMA halo slabs (SWIZZLE_128B, zero-filled padding), shifted descriptors for the
-// in-plane taps, persistent CTAs, TMA producer warp / MMA warpgroup / 8 epilogue warps.  Stride 1, kt = 3, pt = 1, plain per-channel affine.
+// in-plane taps, persistent CTAs, TMA producer warp / two consumer warpgroups with register accumulators / 3 epilogue warps.  The
+// 3 x 64 accumulator columns of one M tile take 192 of the kSlabAccCols register columns, so an item is a single M tile (MT = 1).
+// Stride 1, kt = 3, pt = 1, plain per-channel affine.
 #pragma once
 
 #include "b2_slabconv.cuh"
@@ -25,13 +27,13 @@ constexpr int kTsBN = 64;            // output-channel tile
 constexpr int kTsWBytes = 3 * kTsBN * 128;   // weight stage: [W(dt=2); W(dt=1); W(dt=0)], 64 rows x 128 B each
 
 struct SlabTsItem {
-  int q0, wc, plane_o0, plane_i0, r_lo, mt_valid;   // plane_o0: first output plane of the group; plane_i0: input plane of relative frame 0
+  int q0, wc, plane_o0, plane_i0, r_lo;             // plane_o0: first output plane of the group; plane_i0: input plane of relative frame 0
   int nf;                                           // valid output frames in the group (1..3)
   int fr_lo, fr_hi;                                 // valid relative input frames (inside the clip)
   int n_slabs;
 };
 
-// SlabParams fields reused: T, C, To, Ho, Wo, khw, cchunks, PW, WC, wchunks, halo_l, R, sub_* [0], reach, slab_bytes, MT, P, Ncols,
+// SlabParams fields reused: T, C, To, Ho, Wo, khw, cchunks, PW, WC, wchunks, halo_l, R, sub_* [0], reach, slab_bytes, P, Ncols,
 // tiles_q, items_total, scale, shift, residual, ldr, y, ldy, relu, naff, fd_tiles_q, fd_wchunks, fd_PW; fd_To divides by the number
 // of frame groups per clip (ceil(To / 3)), tiles_n == 1.
 __device__ __forceinline__ SlabTsItem slabts_item(const SlabParams& p, int item) {
@@ -48,13 +50,13 @@ __device__ __forceinline__ SlabTsItem slabts_item(const SlabParams& p, int item)
   w.fr_lo = max(0, 1 - to0);
   w.fr_hi = min(w.nf + 1, p.T - to0);                // absolute frame to0 - 1 + fr < T
   w.n_slabs = p.cchunks * (w.fr_hi - w.fr_lo + 1);
-  w.q0 = tq * (p.MT * 128);
+  w.q0 = tq * 128;
   const int lo = w.q0 - p.reach;
   w.r_lo = (lo >= 0) ? fdiv(lo, p.fd_PW) : -fdiv(-lo + p.PW - 1, p.fd_PW);
-  const int mv = (p.P - w.q0 + 127) / 128;
-  w.mt_valid = mv > p.MT ? p.MT : mv;
   return w;
 }
+
+static_assert(kTsGroup * kTsBN <= kSlabAccCols, "slabts: one M tile of accumulators per item");
 
 __global__ void __launch_bounds__(kSlabThreads, 1)
 slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N*T), box (64, PW, R, 1)
@@ -69,19 +71,20 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
   uint64_t* slab_empty = slab_full + kSlabSStages;
   uint64_t* w_full = slab_empty + kSlabSStages;
   uint64_t* w_empty = w_full + kSlabWStages;
-  uint64_t* acc_full = w_empty + kSlabWStages;      // [1]
-  uint64_t* acc_empty = acc_full + 2;               // [1]
+  uint64_t* acc_full = w_empty + kSlabWStages;
+  uint64_t* acc_empty = acc_full + 1;
   float* s_scale = reinterpret_cast<float*>(tail + 256);
   float* s_shift = s_scale + p.naff;
 
   const int tid = threadIdx.x, warp = tid >> 5;
-  const int tile_cols = kTsGroup * kTsBN;            // accumulator columns of one M tile: [slot][64]
-  const AccTile at{s_shift + p.naff, acc_ld(p.MT * tile_cols)};
+  constexpr int tile_cols = kTsGroup * kTsBN;        // accumulator columns of the item's M tile: [slot][64]
+  const AccTile at{s_shift + p.naff, acc_ld(tile_cols)};
 
-  if (tid == 128) {
-    for (int s = 0; s < kSlabSStages; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 1); }
-    for (int s = 0; s < kSlabWStages; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], 1); }
-    mbar_init(&acc_full[0], 1); mbar_init(&acc_empty[0], 256);
+  if (tid == 0) {
+    for (int s = 0; s < kSlabSStages; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], kSlabConsumerWarps); }
+    for (int s = 0; s < kSlabWStages; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], kSlabConsumerWarps); }
+    mbar_init(acc_full, 32 * kSlabConsumerWarps);
+    mbar_init(acc_empty, 32 * kSlabEpiWarps);
     fence_mbar_init();
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmB);
@@ -128,7 +131,7 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
         const int nfr = cur.fr_hi - cur.fr_lo + 1;
         for (int si = 0; si < cur.n_slabs; ++si) {
           const int cc = si / nfr;
-          const int pf = min(kSlabWStages, ntaps - 1);
+          const int pf = min(kSlabWStages, ntaps - 1);      // (ntaps >= 9: the previous slab has retired by then, see b2_slabconv.cuh)
           for (int ti = 0; ti < ntaps; ++ti, ++wit) {
             if (ti == pf && nxt_item < p.items_total) load_next();
             const int ws = wit % kSlabWStages;
@@ -145,21 +148,28 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
         }
       }
     }
-  } else if (warp >= kSlabMmaWarp0) {
-    // ================================ MMA warpgroup =====================================
+  } else if (warp < kSlabEpiWarp0) {
+    // ================================ consumer warpgroups ===============================
+    // warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile; slot s of the accumulator sits at fragment columns [64 s, 64 s + 64)
+    float acc[tile_cols / 2];
+    const int wg = tid >> 7;
+    const bool lead = (tid & 31) == 0;
     const uint32_t slab0 = smem_u32(slab_base), w0s = smem_u32(w_base);
+    const uint32_t a_wg = static_cast<uint32_t>(wg) * (64u * 128u >> 4);
     const int ntaps = p.sub_ntaps[0];
     int wit = 0, sg = 0, lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const SlabTsItem w = slabts_item(p, item);
-      mbar_wait(&acc_empty[0], lt & 1);                    // the epilogue has drained AND re-zeroed the accumulators
+#pragma unroll
+      for (int k = 0; k < tile_cols / 2; ++k) acc[k] = 0.f;
+      reg_fence(acc);
+      int prev_ws = -1, prev_s = -1;
       const int nfr = w.fr_hi - w.fr_lo + 1;
       for (int si = 0; si < w.n_slabs; ++si, ++sg) {
         const int cc = si / nfr, fr = w.fr_lo + (si - cc * nfr);
-        const int s_lo = max(0, fr - 2), s_hi = min(w.nf - 1, fr);          // output slots this input frame feeds
-        const int nslots = s_hi - s_lo + 1;                                 // >= 1 for every valid frame
+        const int s_lo = warp_uniform(max(0, fr - 2)), s_hi = warp_uniform(min(w.nf - 1, fr));          // output slots this input frame feeds
         const uint32_t b_row = static_cast<uint32_t>(2 - (fr - s_lo));      // first row block of the stack: dt = fr - s_lo
-        const int ksteps = min(4, (p.C - cc * 64 + 15) >> 4);
+        const int ksteps = warp_uniform(min(4, (p.C - cc * 64 + 15) >> 4));
         const int s = sg % kSlabSStages;
         mbar_wait(&slab_full[s], (sg / kSlabSStages) & 1);
         const uint32_t slab_addr = slab0 + s * p.slab_bytes;
@@ -167,55 +177,62 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
           const int ws = wit % kSlabWStages;
           mbar_wait(&w_full[ws], (wit / kSlabWStages) & 1);
           const int pix0 = w.q0 + p.sub_off[0][ti] - w.r_lo * p.PW;
-          const uint32_t b_lo = sw128_desc_lo(w0s + ws * kTsWBytes + b_row * (kTsBN * 128));
-          const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u);
-          for (int j = 0; j < w.mt_valid; ++j)
-            wg_mma(at, j * tile_cols + s_lo * kTsBN, nslots * kTsBN,
-                   wg_sw128(desc_from(kSw128DescHi, a_lo0 + j * (128u * 128u >> 4)), desc_from(kSw128DescHi, b_lo)), ksteps, true);
-          wg_sync();
-          wg_arrive(&w_empty[ws]);
-          if (ti == ntaps - 1) wg_arrive(&slab_empty[s]);
-          if (ti == ntaps - 1 && si == w.n_slabs - 1) wg_arrive(&acc_full[0]);
+          const uint64_t b = desc_from(kSw128DescHi, sw128_desc_lo(w0s + ws * kTsWBytes + b_row * (kTsBN * 128)));
+          const uint64_t a = desc_from(kSw128DescHi, sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u) + a_wg);
+          wgmma_fence();
+          // one N = 64 MMA per slot the frame feeds, B = the stack row block of its temporal tap.  (A single MMA over the slot range,
+          // N = 64, 128 or 192 on overlapping fragment windows, makes ptxas serialise the kernel's whole wgmma pipeline for want of
+          // registers; with the accumulators in registers the A re-reads cost less than that.)
+          if (s_lo == 0) slab_mma<64>(acc, a, b, ksteps);
+          if (s_lo <= 1 && s_hi >= 1) slab_mma<64>(acc + 32, a, b + (kTsBN * 128 >> 4) * (1 - s_lo), ksteps);
+          if (s_hi == 2) slab_mma<64>(acc + 64, a, b + (kTsBN * 128 >> 4) * (2 - s_lo), ksteps);
+          wgmma_commit();
+          wgmma_wait1();
+          if (lead && prev_ws >= 0) {
+            mbar_arrive(&w_empty[prev_ws]);
+            if (prev_s >= 0) mbar_arrive(&slab_empty[prev_s]);
+          }
+          prev_ws = ws;
+          prev_s = (ti == ntaps - 1) ? s : -1;
         }
       }
+      wgmma_wait0();
+      reg_fence(acc);
+      if (lead) {
+        mbar_arrive(&w_empty[prev_ws]);
+        mbar_arrive(&slab_empty[prev_s]);
+      }
+      mbar_wait(acc_empty, (lt & 1) ^ 1);
+      frag_io<tile_cols>(at, wg * 64, 0, acc, false, false);
+      mbar_arrive(acc_full);
     }
   } else {
     // ================================ epilogue ==========================================
-    const int erow = (warp & 3) * 32 + (tid & 31);
-    const int egroup = warp >= 4 ? 1 : 0;
-    const int used_cols = p.MT * tile_cols;
-    for (int c = egroup * 32; c < used_cols; c += 64) acc_zero32(at, erow, c);     // accumulators start at zero
-    mbar_arrive(&acc_empty[0]);
     const size_t plane_rows = static_cast<size_t>(p.Ho) * p.Wo;
+    const int ncols_here = min(kTsBN, p.ldy);
     int lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const SlabTsItem w = slabts_item(p, item);
-      size_t row[4];
-      bool ok[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int q = w.q0 + j * 128 + erow;
+      mbar_wait(acc_full, lt & 1);
+#pragma unroll 1
+      for (int erow = tid - kSlabEpiWarp0 * 32; erow < 128; erow += 32 * kSlabEpiWarps) {   // two passes over the tile rows
+        const int q = w.q0 + erow;
         const int h = fdiv(q, p.fd_PW), wp = q - h * p.PW;
         const int wo = w.wc * p.WC + wp - p.halo_l;
-        ok[j] = (j < w.mt_valid) && (q < p.P) && (wp >= p.halo_l) && (wp < p.halo_l + p.WC) && (wo < p.Wo);
-        row[j] = (static_cast<size_t>(w.plane_o0) * p.Ho + h) * p.Wo + wo;
-      }
-      const int jc = egroup;                               // 64 channels = two 32-column chunks, one per warpgroup
-      const int c0 = jc * 32;
-      float sc[32], sh[32];
-#pragma unroll
-      for (int c = 0; c < 32; ++c) { sc[c] = s_scale[c0 + c]; sh[c] = s_shift[c0 + c]; }
-      const int ncols_here = min(kTsBN, p.ldy);
-      mbar_wait(&acc_full[0], lt & 1);
+        const bool ok = (q < p.P) && (wp >= p.halo_l) && (wp < p.halo_l + p.WC) && (wo < p.Wo);
+        const size_t row = (static_cast<size_t>(w.plane_o0) * p.Ho + h) * p.Wo + wo;
 #pragma unroll 1
-      for (int s = 0; s < w.nf; ++s) {
+        for (int jc = 0; jc < 2; ++jc) {                     // 64 channels = two 32-column chunks
+          const int c0 = jc * 32;
+          float sc[32], sh[32];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (j < w.mt_valid) {                            // warp-uniform
+          for (int c = 0; c < 32; ++c) { sc[c] = s_scale[c0 + c]; sh[c] = s_shift[c0 + c]; }
+#pragma unroll 1
+          for (int s = 0; s < w.nf; ++s) {
             uint32_t v[32];
-            acc_ld32(at, erow, j * tile_cols + s * kTsBN + c0, v);
-            if (ok[j]) {
-              const size_t r = row[j] + s * plane_rows;
+            acc_ld32(at, erow, s * kTsBN + c0, v);
+            if (ok) {
+              const size_t r = row + s * plane_rows;
               __half* yrow = p.y + r * p.ldy + c0;
               const __half* rrow = p.residual ? p.residual + r * p.ldr + c0 : nullptr;
 #pragma unroll
@@ -243,8 +260,7 @@ slabts_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N
           }
         }
       }
-      for (int c = egroup * 32; c < used_cols; c += 64) acc_zero32(at, erow, c);   // hand the accumulators back zeroed (this group's chunks)
-      mbar_arrive(&acc_empty[0]);
+      mbar_arrive(acc_empty);
     }
   }
 }
