@@ -776,14 +776,15 @@ static int g_gemm_algo = 0;   // 0 auto (persistent kernel where it applies), 1 
 
 template <int BN, int GAN, int MASK = 0>
 static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
-  using S = PgemmSmem<BN>;
+  using S = PgemmSmem<BN, GAN>;
   B2_OPT_IN_SMEM((pgemm_kernel<BN, GAN, MASK>), S::kTotal);
   const IgemmParams& ip = L.p;
   CUtensorMap tmA, tmB, tmC, tmR;
   int rc;
   if ((rc = make_tmap_2d_f16(&tmA, L.a_mat, (uint64_t)L.a_cols, (uint64_t)ip.M_total, (uint64_t)L.lda, 64, 128, true)) != B2_OK) return rc;
   if ((rc = make_tmap_2d_f16(&tmB, L.w, (uint64_t)L.b_cols, (uint64_t)ip.Ncols, (uint64_t)L.ldb, 64, BN, true)) != B2_OK) return rc;
-  if ((rc = make_tmap_2d_f16(&tmC, ip.y, (uint64_t)ip.ldy, (uint64_t)ip.M_total, (uint64_t)ip.ldy, 64, 128, true)) != B2_OK) return rc;
+  // outputs are stored per consumer warpgroup: boxes of 64 rows
+  if ((rc = make_tmap_2d_f16(&tmC, ip.y, (uint64_t)ip.ldy, (uint64_t)ip.M_total, (uint64_t)ip.ldy, 64, 64, true)) != B2_OK) return rc;
   const int up_W = ip.up_W > 0 ? ip.up_W : 2;
   const int res_rows = up_W >= 128 ? 64 : 32;
   if (ip.residual && ip.res_up) {
@@ -797,7 +798,7 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
     tmR = tmC;
   }
   CUtensorMap tmC2 = tmC;
-  if (ip.y2 && (rc = make_tmap_2d_f16(&tmC2, ip.y2, (uint64_t)ip.ldy, (uint64_t)ip.M_total, (uint64_t)ip.ldy, 64, 128, true)) != B2_OK) return rc;
+  if (ip.y2 && (rc = make_tmap_2d_f16(&tmC2, ip.y2, (uint64_t)ip.ldy, (uint64_t)ip.M_total, (uint64_t)ip.ldy, 64, 64, true)) != B2_OK) return rc;
   CUtensorMap tmA2 = tmA, tmB2 = tmB;
   if (L.k2 > 0) {
     if ((rc = make_tmap_2d_f16(&tmA2, L.a2, (uint64_t)L.k2, (uint64_t)ip.M_total, (uint64_t)L.lda2, 64, 128, true)) != B2_OK) return rc;
@@ -840,10 +841,11 @@ static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   }
   if (g_gemm_algo == 0 && densem_applies(L.p, L.k2)) { g_last_gemm_path = 1; return launch_densem(L, stream); }
   if (g_gemm_algo == 0 && L.p.amode == AMODE_TMA && L.p.epi == EPI_TMA_F16 && !L.p.per_row) {
-    // 64-wide N tiles only (see b2_pgemm.cuh: the accumulator tiles of a 128-wide instance do not fit in shared memory)
+    // 64-wide N tiles for narrow outputs, 128 otherwise
     g_last_gemm_path = 2;
-    if (L.p.y2 || L.p.res_up || L.p.res_pre || L.p.in_scale) return launch_pgemm<64, 1>(L, stream);
-    return launch_pgemm<64, 0>(L, stream);
+    const bool gan = L.p.y2 || L.p.res_up || L.p.res_pre || L.p.in_scale;
+    if (L.p.ldy <= 64) return gan ? launch_pgemm<64, 1>(L, stream) : launch_pgemm<64, 0>(L, stream);
+    return gan ? launch_pgemm<128, 1>(L, stream) : launch_pgemm<128, 0>(L, stream);
   }
   if (L.p.aff_ld)
     return set_error(B2_ERR_UNSUPPORTED, "per-sample affine is implemented by the slab convolution and the persistent GEMM only");
