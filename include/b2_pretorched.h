@@ -207,6 +207,22 @@ int b2_gather_frame_tuples(const void* x, void* y, const int32_t* idx_dev, int N
                            void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * MobileNetV2 (mobilenet.py:38-126)
+ * ------------------------------------------------------------------------------------------- */
+/* Depthwise 3x3 convolution (nn.Conv2d(C, C, 3, stride, 1, groups=C), mobilenet.py:50,64) -> BatchNorm -> ReLU6:
+ *     y[n, ho, wo, c] = act( scale[c] * sum_{kh,kw} in(x[n, ho*s + kh - 1, wo*s + kw - 1, c]) * w[kh*3 + kw][c] + shift[c] )
+ * with zero padding 1, in(v) = clamp_in ? min(v, 6) : v (the ReLU6 of the producer, which stored ReLU(v)) and
+ * act = relu6 ? clamp to [0, 6] : identity.  fp32 accumulation in the fixed tap order (kh, kw), the affine in fp32, one fp16
+ * rounding.  x: fp16 [N*H*W][ld] (N counts images: a clip's frames fold into it); y: fp16 [N*Ho*Wo][ld] with
+ * Ho = (H - 1) / stride + 1 (same for W), channels [C, ld) written as zero; w: fp32 [9][C] (tap-major); scale, shift: fp32 [C].
+ * C % 8 == 0, ld % 8 == 0, ld >= C, stride 1 or 2, every pointer 16-byte aligned. */
+int b2_dwconv3x3_ndhwc(const void* x, const float* w, const float* scale, const float* shift, void* y, int N, int H, int W, int C,
+                       int ld, int stride, int clamp_in, int relu6, void* stream);
+/* x = min(max(x, 0), 6) in place over an fp16 [rows][ld] matrix: the ReLU6 of the last 1x1 convolution (mobilenet.py:30-35),
+ * whose epilogue stored ReLU(x), ahead of the global average. */
+int b2_relu6_inplace_ndhwc(void* x, long long rows, int ld, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Fine-tuning backward of the residual blocks (the backward of resnet3D.py:91-143 with eval-mode BatchNorm).  Gradients
  * travel between kernels as fp16 NDHWC matrices multiplied by a device-resident power-of-two loss scale; the fp32 results
  * (weight, gamma and beta gradients) divide it out.  `inv_loss_scale` / `scale_pair` are DEVICE pointers.

@@ -94,6 +94,8 @@ SYMBOLS = {
     "b2_colsum_f16": (c_int, [c_void_p, c_int, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_loss_scale_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "b2_avgpool_global_backward": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
+    "b2_dwconv3x3_ndhwc": (c_int, [c_void_p] * 5 + [c_int] * 8 + [c_void_p]),
+    "b2_relu6_inplace_ndhwc": (c_int, [c_void_p, ctypes.c_longlong, c_int, c_void_p]),
 }
 
 

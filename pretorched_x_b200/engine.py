@@ -413,6 +413,71 @@ def _nonlocal_body(nl, a, simt=False, out=None):
 
 
 # ---------------------------------------------------------------------------------------------
+# MobileNetV2 (mobilenet.py:22-126)
+# ---------------------------------------------------------------------------------------------
+# Every ReLU6 of the network except the last feeds a depthwise convolution: the producers (the stem conv_bn, the expansion
+# 1x1 convolutions) store ReLU(x) with their ordinary epilogue and the depthwise kernel reads min(x, 6).  That is exact:
+# fp16 rounding is monotone and 6 is representable, so round(min(v, 6)) == min(round(v), 6).  The last ReLU6 (the 1x1
+# convolution that feeds the global average) is one in-place clamp pass.
+def depthwise_bn_relu6(conv, bn, a, clamp_in=True, out=None):
+    """Depthwise 3x3 conv (groups = channels, padding 1, stride 1 or 2) -> eval-mode BN -> ReLU6 on the CUDA-core kernel."""
+    C = conv.weight.shape[0]
+    stride, padding = _conv_geometry(conv)
+    if (conv.groups != C or tuple(conv.weight.shape[1:]) != (1, 3, 3) or padding[1:] != (1, 1) or stride[1] != stride[2]
+            or stride[1] not in (1, 2) or any(d != 1 for d in conv.dilation)):
+        raise NotImplementedError("the depthwise kernel covers 3x3 convolutions with groups = channels, padding 1, stride 1 or 2")
+    if a.C != C:
+        raise ValueError("depthwise convolution over %d channels got %r" % (C, a))
+    dev = a.data.device
+
+    def build():
+        w9 = conv.weight.detach().reshape(C, 9).t().float().contiguous()
+        return (w9,) + ops.fold_affine(C, conv.bias, bn, dev)
+
+    w9, scale, shift = _cached(conv, "dw", _sig(conv.weight, conv.bias, *_bn_tensors(bn)), build)
+    return ops.dwconv3x3(a, w9, scale, shift, stride[1], clamp_in=clamp_in, out=out)
+
+
+def _conv_bn_relu6_body(seq, a, clamp_out=True):
+    """conv_bn / conv_1x1_bn (mobilenet.py:22-35): conv -> BN -> ReLU(6).  ``clamp_out=False`` when the only consumer is a
+    depthwise convolution, which applies the upper clamp as it loads."""
+    y = conv_bn_act(seq[0], seq[1], a, relu=True)
+    return ops.relu6_(y) if clamp_out else y
+
+
+def _inverted_residual_body(block, a, out=None):
+    """[1x1 expand -> BN -> ReLU6] -> depthwise 3x3 -> BN -> ReLU6 -> 1x1 project -> BN (+ x) (mobilenet.py:38-76).  The
+    residual joins in the projection GEMM's epilogue."""
+    layers = list(block.conv)
+    if len(layers) == 8:
+        h = conv_bn_act(layers[0], layers[1], a, relu=True)
+        dw, dbn, pw, pbn = layers[3], layers[4], layers[6], layers[7]
+    elif len(layers) == 5:
+        h = a
+        dw, dbn, pw, pbn = layers[0], layers[1], layers[3], layers[4]
+    else:
+        raise NotImplementedError("unsupported inverted residual layout %r" % (block,))
+    h = depthwise_bn_relu6(dw, dbn, h, clamp_in=True)
+    return conv_bn_act(pw, pbn, h, residual=a if block.use_res_connect else None, relu=False, out=out)
+
+
+def run_mobilenet_features(features, x):
+    """``MobileNetV2.features`` (mobilenet.py:100-113) on the engine: fp32 NCHW (or an Act with channel pitch 8) in, Act out.
+    The stem's 3 input channels are stored with pitch 8: its 3x3 stride-2 convolution runs on the generic convolution path."""
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
+    mods = list(features)
+    for i, m in enumerate(mods):
+        if hasattr(m, "use_res_connect"):
+            a = Fn.InvertedResidualFunction.run(m, a)
+            continue
+        nxt = mods[i + 1] if i + 1 < len(mods) else None
+        # the output may skip the upper clamp only when a depthwise convolution is its sole reader
+        feeds_dw = hasattr(nxt, "use_res_connect") and not nxt.use_res_connect and nxt.conv[0].groups > 1
+        a = Fn.ConvBNReLU6Function.run(m, a, not feeds_dw)
+    return a
+
+
+# ---------------------------------------------------------------------------------------------
 # stem / trunk / head
 # ---------------------------------------------------------------------------------------------
 def _pool_args(mp):

@@ -98,6 +98,24 @@ class NonLocalFunction(_FrozenFunction):
         return NonLocalFunction._finish(ctx, engine._nonlocal_body(nl, Act(x2d, *geom), simt, out))
 
 
+class ConvBNReLU6Function(_FrozenFunction):
+    """MobileNetV2 conv_bn / conv_1x1_bn: conv -> BN -> ReLU6 (mobilenet.py:22-35)."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, seq, clamp_out=True):
+        from . import engine
+        return ConvBNReLU6Function._finish(ctx, engine._conv_bn_relu6_body(seq, Act(x2d, *geom), clamp_out))
+
+
+class InvertedResidualFunction(_FrozenFunction):
+    """MobileNetV2 inverted residual: expand -> depthwise -> project (+ x) (mobilenet.py:38-76)."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, block, out=None):
+        from . import engine
+        return InvertedResidualFunction._finish(ctx, engine._inverted_residual_body(block, Act(x2d, *geom), out))
+
+
 class GBlockFunction(_FrozenFunction):
     """BigGAN-deep GBlock: ccbn-ReLU-1x1 -> ccbn-ReLU-[up]-3x3 -> ccbn-ReLU-3x3 -> ccbn-ReLU-1x1 (+ skip)."""
 

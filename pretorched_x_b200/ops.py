@@ -429,6 +429,32 @@ def avgpool_global(a):
 
 
 @_on_device
+def dwconv3x3(a, w9, scale, shift, stride, clamp_in=False, relu6=True, out=None):
+    """Depthwise 3x3 convolution, padding 1 (nn.Conv2d(C, C, 3, stride, 1, groups=C), mobilenet.py:50,64) -> folded BatchNorm
+    ``scale``/``shift`` (fp32 [C]) -> ReLU6, on CUDA cores (b2_dwconv3x3_ndhwc).  ``w9``: fp32 [9][C] taps (kh * 3 + kw).
+    ``clamp_in``: the kernel reads min(x, 6) -- the ReLU6 of a producer that stored ReLU(x).  A clip's frames fold into the
+    batch.  ``out``: see ``conv``."""
+    if a.C % 8 or stride not in (1, 2):
+        raise ValueError("depthwise convolution needs C %% 8 == 0 and stride 1 or 2 (got C %d, stride %d)" % (a.C, stride))
+    Ho, Wo = (a.H - 1) // stride + 1, (a.W - 1) // stride + 1
+    M = a.N * a.T * Ho * Wo
+    y = _out_rows(out, M, a.ld) if out is not None else torch.empty((M, a.ld), dtype=torch.float16, device=a.data.device)
+    with _timed("dwconv", "dwconv 3x3 s%d C%d M=%d%s" % (stride, a.C, M, " clamp_in" if clamp_in else ""), 18.0 * M * a.C,
+                2.0 * a.C * (a.M + M)):
+        _lib.check(_lib.load().b2_dwconv3x3_ndhwc(_ptr(a.data), _ptr(w9), _ptr(scale), _ptr(shift), _ptr(y), a.N * a.T, a.H, a.W, a.C,
+                                                 a.ld, stride, int(clamp_in), int(relu6), _stream()), "b2_dwconv3x3_ndhwc")
+    return Act(y, a.N, a.T, Ho, Wo, a.C)
+
+
+@_on_device
+def relu6_(a):
+    """In-place min(max(x, 0), 6) over an Act (nn.ReLU6 after a producer that stored ReLU(x), mobilenet.py:30-35)."""
+    with _timed("relu6", "relu6 C%d M=%d" % (a.C, a.M), 0.0, 4.0 * a.M * a.ld):
+        _lib.check(_lib.load().b2_relu6_inplace_ndhwc(_ptr(a.data), a.M, a.ld, _stream()), "b2_relu6_inplace_ndhwc")
+    return a
+
+
+@_on_device
 def shortcut_a(a, stride, out_channels):
     """Type-A shortcut: F.avg_pool3d(k=1, stride) + zero channel padding (resnet3D.py:65-74)."""
     To, Ho, Wo = (a.T - 1) // stride + 1, (a.H - 1) // stride + 1, (a.W - 1) // stride + 1
