@@ -542,6 +542,43 @@ static int try_tstack(const b2_conv_args* a, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------
 // stem convolution launcher (Toeplitz-descriptor kernel)
 // ------------------------------------------------------------------------------------------
+// Output rows per item of the BN = 64 stem: -2 = not read yet, -1 = the rule, 2 / 4 = forced (4 only where eligible).
+// B2_STEM_ROWS=2 / 4 in the environment (read once) or b2_debug_set_stem_rows() force an instance, for A/B comparisons.
+static int g_stem_rows = -2;
+static int g_last_stem_rows = 0;
+template <int BN, int G>
+static int launch_stem_g(cudaStream_t stream, const StemParams& p, const CUtensorMap& tmX, int smem_bytes) {
+  B2_OPT_IN_SMEM((stemconv_kernel<BN, G, false>), 227 * 1024);
+  if constexpr (G != 4) B2_OPT_IN_SMEM((stemconv_kernel<BN, G, true>), 227 * 1024);
+  const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
+  if constexpr (G != 4)
+    if (p.nstages == 1) {
+      B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, G, true>, dim3(grid), dim3(stem_threads(G)), smem_bytes, stream, tmX, p));
+      B2_CHECK_LAUNCH("stemconv_kernel");
+      return B2_OK;
+    }
+  B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, G, false>, dim3(grid), dim3(stem_threads(G)), smem_bytes, stream, tmX, p));
+  B2_CHECK_LAUNCH("stemconv_kernel");
+  return B2_OK;
+}
+
+// Which G a BN = 64 stem runs with.  G = 4 is eligible outside pair mode when its slab (2 * 3 + kh rows) and weight image leave
+// room for three ring stages next to its staging tile, i.e. kh <= 7; taller filters keep G = 2 and its deeper ring.  The rule
+// takes it for temporal filters (kt > 1): on an H100 the 7x7x7 stems of resnet3d50 / nonlocal50 run 15-17 % faster.  A 2-D
+// stem (kt == 1, resnet18) has one tap per item, so the item-end drain and the single staging tile are exposed: G = 4 measured
+// 16 % slower there and it keeps G = 2.
+static int stem_rows_for(int BN, int kt, int kh, bool pair) {
+  if (BN != 64) return 1;
+  if (g_stem_rows == -2) {
+    const char* e = getenv("B2_STEM_ROWS");
+    g_stem_rows = (e && (e[0] == '2' || e[0] == '4')) ? e[0] - '0' : -1;
+  }
+  const int stage4 = ((2 * 3 + kh) * kStemPitch + kh * 64 * 64 + 127) / 128 * 128;
+  const bool eligible = !pair && (227 * 1024 - stem_tail_bytes(4, 64) - 128) / stage4 >= 3;
+  if (!eligible || g_stem_rows == 2) return 2;
+  return (g_stem_rows == 4 || kt > 1) ? 4 : 2;
+}
+
 template <int BN>
 static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   PFN_encodeTiled enc = get_encode_tiled();
@@ -555,21 +592,22 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   p.kt = a->kt; p.kh = a->kh; p.pt = a->pt; p.ph = a->ph;
   // with pt >= kt the first output frames see no input frame at all; the kernel expects every item to have a tap inside the clip
   if (a->pt >= a->kt) return set_error(B2_ERR_UNSUPPORTED, "stem convolution needs temporal padding < kt (got pt=%d, kt=%d)", a->pt, a->kt);
-  p.G = kStemAccCols / BN;
+  static int pair_env = -1;
+  if (pair_env < 0) { const char* e = getenv("B2_STEM_PAIR"); pair_env = (e && e[0] == '0') ? 0 : 1; }
+  p.pair = (pair_env && a->kt == 1 && a->pt == 0 && p.Wo <= 60 && !a->pool_w && a->W <= 120) ? 1 : 0;
+  p.G = stem_rows_for(BN, a->kt, a->kh, p.pair != 0);
   p.rows = 2 * (p.G - 1) + a->kh;
   if (p.rows > kStemMaxRows) return set_error(B2_ERR_UNSUPPORTED, "stem kernel height %d too large", a->kh);
   for (int i = 0; i < p.rows; ++i) {
-    int g_lo = i - (a->kh - 1);
-    g_lo = g_lo > 0 ? (g_lo + 1) / 2 : 0;
-    int g_hi = i / 2;
-    if (g_hi > p.G - 1) g_hi = p.G - 1;
+    int g_lo, g_hi, slot;
+    stem_row_plan(p.G, a->kh, i, &g_lo, &g_hi, &slot);
     p.row_glo[i] = (signed char)g_lo;
     p.row_ghi[i] = (signed char)g_hi;
-    p.row_slot[i] = (signed char)(g_lo <= g_hi ? stem_slot(i - 2 * g_lo, a->kh) : 0);
+    p.row_slot[i] = (signed char)slot;
   }
   p.w_bytes = a->kh * BN * 64;
   p.stage_bytes = ((p.rows * kStemPitch + p.w_bytes) + 127) / 128 * 128;
-  const int tail_bytes = kStemTailBytes + 128;                  // + alignment of the dynamic shared-memory base
+  const int tail_bytes = stem_tail_bytes(p.G, BN) + 128;        // + alignment of the dynamic shared-memory base
   p.nstages = (227 * 1024 - tail_bytes) / p.stage_bytes;
   if (p.nstages > kStemMaxStages) p.nstages = kStemMaxStages;
   if (p.nstages < 1) return set_error(B2_ERR_UNSUPPORTED, "stem slab does not fit in shared memory (kh=%d)", a->kh);
@@ -578,10 +616,7 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   if (p.ntiles_n * BN > 256) return set_error(B2_ERR_UNSUPPORTED, "stem convolution supports at most 256 output channels");
   p.tiles_w = (p.Wo + kStemTileW - 1) / kStemTileW;
   p.tiles_h = (p.Ho + p.G - 1) / p.G;
-  static int pair_env = -1;
-  if (pair_env < 0) { const char* e = getenv("B2_STEM_PAIR"); pair_env = (e && e[0] == '0') ? 0 : 1; }
   p.planes_total = a->N * p.To;
-  p.pair = (pair_env && a->kt == 1 && a->pt == 0 && p.Wo <= 60 && !a->pool_w && a->W <= 120) ? 1 : 0;
   const long long plane_items = p.pair ? (p.planes_total + 1) / 2 : p.planes_total;
   const long long items = (long long)p.tiles_w * p.tiles_h * p.ntiles_n * plane_items;
   if (items >= (1ll << 31)) return set_error(B2_ERR_INVALID, "stem problem too large");
@@ -595,8 +630,6 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   if (a->pool_w && (!a->relu || p.tiles_w != 1))
     return set_error(B2_ERR_UNSUPPORTED, "fused W pooling needs ReLU and an output row of at most %d columns (got %d)", kStemTileW, p.Wo);
   const int smem_bytes = p.nstages * p.stage_bytes + tail_bytes;
-  B2_OPT_IN_SMEM((stemconv_kernel<BN, false>), 227 * 1024);
-  B2_OPT_IN_SMEM((stemconv_kernel<BN, true>), 227 * 1024);
   // input viewed as 8-byte pixels (W, H, N*T); box (256, rows, 1); no swizzle -> dense 2 KB rows in smem
   CUtensorMap tmX;
   cuuint64_t dims[3] = {(cuuint64_t)a->W, (cuuint64_t)a->H, (cuuint64_t)a->N * a->T};
@@ -612,11 +645,9 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error(B2_ERR_CUDA, "cuTensorMapEncodeTiled(stem) failed (%d)", (int)r);
-  const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
-  if (p.nstages == 1) B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, true>, dim3(grid), dim3(kStemThreads), smem_bytes, stream, tmX, p));
-  else B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, false>, dim3(grid), dim3(kStemThreads), smem_bytes, stream, tmX, p));
-  B2_CHECK_LAUNCH("stemconv_kernel");
-  return B2_OK;
+  g_last_stem_rows = p.G;
+  if constexpr (BN == 128) return launch_stem_g<128, 1>(stream, p, tmX, smem_bytes);
+  else return p.G == 4 ? launch_stem_g<64, 4>(stream, p, tmX, smem_bytes) : launch_stem_g<64, 2>(stream, p, tmX, smem_bytes);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -918,6 +949,16 @@ int b2_debug_tstack_plan(const b2_conv_args* a, int* out) {
   return B2_OK;
 }
 int b2_debug_last_conv_path(void) { return g_last_conv_path; }
+/* stem convolution: output rows per work item of the last launch (1, 2 or 4); rows = 2 / 4 forces the two- / four-row BN = 64
+   instance (four only where eligible), -1 the rule.  The row plan of (G, kh): out[3 i .. 3 i + 2] = {g_lo, g_hi, first weight slot} of slab row i, returns the slab row count. */
+int b2_debug_last_stem_rows(void) { return g_last_stem_rows; }
+int b2_debug_set_stem_rows(int rows) { g_stem_rows = (rows == 2 || rows == 4) ? rows : -1; return B2_OK; }
+int b2_debug_stem_row_plan(int G, int kh, int* out) {
+  const int rows = 2 * (G - 1) + kh;
+  if (G < 1 || kh < 1 || rows > kStemMaxRows) return -1;
+  for (int i = 0; i < rows; ++i) stem_row_plan(G, kh, i, &out[3 * i], &out[3 * i + 1], &out[3 * i + 2]);
+  return rows;
+}
 int b2_debug_last_gemm_path(void) { return g_last_gemm_path; }   /* 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (last GEMM-family launch) */   /* 1: the temporal stack kernel took the last convolution */
 int b2_debug_set_tstack(int mode) { g_tstack = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }   /* temporal stack kernel: -1 rule, 0 never, 1 whenever eligible */
 int b2_debug_set_slab_mt(int mt) { g_slab_force_mt = mt < 0 ? 0 : mt; return B2_OK; }

@@ -193,6 +193,12 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// Warp-specialised kernels: hand registers from the producer / epilogue warpgroups to the MMA warpgroups.  Executed by every warp
+// of a warpgroup; the per-thread budget of the launch (65536 / threads) is the starting point of both.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 // Register accumulators that wgmma reads and writes asynchronously: keeps the compiler from moving ordinary reads or writes of
 // them across a wgmma.fence / wait_group.
 template <int N>

@@ -18,42 +18,52 @@
 // read from shared memory once per slab row instead of once per (output row, dh).
 //
 // Register accumulators.  Two consumer warpgroups own 64 of the 128 tile rows each (pair mode: one plane each) and keep
-// G * BN / 2 fp32 accumulators per thread for a whole work item.  A temporal tap's MMAs are issued back to back and committed
+// G * BN / 2 fp32 accumulators per thread for a whole work item.  Instances: BN = 128 with G = 1, BN = 64 with G = 2 or G = 4
+// (128 accumulators per thread).  A temporal tap's MMAs are issued back to back and committed
 // as one group; wait_group 1 keeps one tap in flight while the next one is issued, and a ring slot is released once the
 // group that read it has retired.  Each element sees the same sequence of fp32 accumulations as a per-row, per-N-tile
 // schedule would: temporal tap, slab row ascending, K step ascending.
 //
 // Persistent CTAs (one per SM) walk (plane, row-group, column-tile) work items.  At the end of an item the consumers apply
-// the BN affine (+ ReLU) to their fragments and write fp16 into one of two staging tiles ([128 rows][G * BN + 8]); the
-// epilogue warps (one tile row per thread) take the W direction of the max-pool there and do the global stores while the
-// consumers run the next item.
+// the BN affine (+ ReLU) to their fragments and write fp16 into a staging tile ([rows][G * BN + 8]); the epilogue warps (one
+// tile row per thread) take the W direction of the max-pool there and do the global stores while the consumers run the next item.
 // Warps 0-7: consumer warpgroups, 8-11: epilogue, 12: TMA/bulk-copy producer.
+//
+// G = 4 (BN = 64, never pair mode; N = 64 MMAs, see stem_row_mma): 128 accumulators per consumer thread do not fit the 152
+// registers a 416-thread CTA leaves, so the CTA has 512 threads (warps 13-15 complete the producer warpgroup and exit) and
+// setmaxnreg moves registers from the producer (40) and epilogue (56) warpgroups to the consumers (208).  Its shared memory holds three 54 KB ring stages (13 slab rows + the 28 KB weight
+// image of a 7-tall filter) and ONE staging tile of the 120 tile rows that carry output columns: the epilogue drains an item in
+// a small fraction of the next item's main loop.
 #pragma once
 
 #include "b2_ptx.cuh"
 
 namespace b2 {
 
-constexpr int kStemThreads = 416;       // warps 0-7: two consumer warpgroups, 8-11: epilogue, 12: producer
 constexpr int kStemEpiWarp0 = 8;
 constexpr int kStemTmaWarp = 12;
-constexpr int kStemAccCols = 128;       // accumulator columns of one item: G * BN
 constexpr int kStemPitch = 2048;        // bytes per slab row: 256 pixels [2*w0-4, 2*w0+252) of 8 bytes
 constexpr int kStemRowPx = 256;         // TMA box width (the maximum box extent), one 8-byte element per pixel
 constexpr int kStemTileW = 120;         // output columns per item: rows r < 124 of the 128-row MMA tile see complete runs
 constexpr int kStemMaxStages = 4;
 constexpr int kStemMaxRows = 16;        // slab rows = 2*(G-1) + kh
-constexpr int kStemStgLd = kStemAccCols + 8;                 // staging tile pitch in halves (272 B: conflict-free both ways)
-constexpr int kStemStgBytes = 128 * kStemStgLd * 2;          // one fp16 staging tile
-// barriers, scale / shift, W-pool exchange slots, two staging tiles
-constexpr int kStemTailBytes = 128 + 2048 + 512 + 2 * kStemStgBytes;
+// per instance (G output rows per item, BN output channels per N tile)
+__host__ __device__ constexpr int stem_threads(int G) { return G == 4 ? 512 : 416; }
+__host__ __device__ constexpr int stem_stg_ld(int G, int BN) { return G * BN + 8; }   // pitch in halves: 16 B past a multiple of
+                                                                                       // 128 B, conflict-free both ways
+__host__ __device__ constexpr int stem_stg_rows(int G) { return G == 4 ? kStemTileW : 128; }
+__host__ __device__ constexpr int stem_stg_bufs(int G) { return G == 4 ? 1 : 2; }
+// barriers, scale / shift, W-pool exchange slots, staging tiles
+__host__ __device__ constexpr int stem_tail_bytes(int G, int BN) {
+  return 128 + 2048 + 512 + stem_stg_bufs(G) * stem_stg_rows(G) * stem_stg_ld(G, BN) * 2;
+}
 
 struct StemParams {
   int T, H, W;             // input dims per clip (W even)
   int To, Ho, Wo;
   int kt, kh;              // kw == 7, strides (1, 2, 2)
   int pt, ph;
-  int G;                   // output rows per item (G * BN == kStemAccCols)
+  int G;                   // output rows per item: 1 (BN = 128), 2 or 4 (BN = 64)
   int rows;                // slab rows = 2*(G-1) + kh
   int stage_bytes;         // slab + weights of one temporal tap, multiple of 128
   int w_bytes;             // kh * BN * 64: weight image of one temporal tap for one N tile
@@ -87,6 +97,17 @@ __host__ __device__ inline int stem_slot(int dh, int kh) {
   return (dh % 2 == 0) ? (emax - dh) / 2 : n_even + (omax - dh) / 2;
 }
 
+// Row plan: slab row i feeds local output rows g_lo..g_hi (dh = i - 2g, 0 <= dh < kh); the taps it uses for them are dh(g_lo),
+// dh(g_lo) - 2, ..., consecutive slots of the weight image starting at slot_lo.  g_lo > g_hi: the row feeds nothing.
+__host__ inline void stem_row_plan(int G, int kh, int i, int* g_lo, int* g_hi, int* slot_lo) {
+  int lo = i - (kh - 1);
+  lo = lo > 0 ? (lo + 1) / 2 : 0;
+  int hi = i / 2;
+  if (hi > G - 1) hi = G - 1;
+  *g_lo = lo; *g_hi = hi;
+  *slot_lo = lo <= hi ? stem_slot(i - 2 * lo, kh) : 0;
+}
+
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                    smem_u32(smem_dst)),
@@ -117,42 +138,62 @@ template <int N_>
 __device__ __forceinline__ void stem_mma(float* d, uint64_t a, uint64_t b) {
   static_assert(N_ == 64 || N_ == 128, "stem MMA width");
 #pragma unroll
-  for (int k = 0; k < 2; ++k) {
-    if constexpr (N_ == 64) wgmma_n64<0>(*reinterpret_cast<float(*)[32]>(d), a + 2 * k, b + 16 * k);
-    else wgmma_n128_ss(*reinterpret_cast<float(*)[64]>(d), a + 2 * k, b + 16 * k);
+  for (int k = 0; k < 2; ++k) wgmma_ss<N_>(d, a + 2 * k, b + 16 * k);
+}
+
+// Slab row feeding local output rows g_lo..g_hi (row g's fragments at acc + g * BN / 2).  G <= 2: one MMA over all of them; the
+// register offset and width must be compile-time constants, hence one case per (g_lo, g_hi).  G = 4: one N = 64 MMA per output
+// row.  Wider windows (N = 256 / 192 over the touched rows, or N = 128 pairs at fragment offsets 0 and 64 next to N = 64 ones)
+// make ptxas serialise the wgmma pipeline (C7511) or, for N > 128, need more registers than a 512-thread launch allows at
+// compile time; four equal, disjoint windows do neither.
+template <int BN, int G>
+__device__ __forceinline__ void stem_row_mma(float* acc, int g_lo, int g_hi, uint64_t a, uint64_t b) {
+  if constexpr (G == 1) {
+    stem_mma<BN>(acc, a, b);
+  } else if constexpr (G == 2) {
+    if (g_lo != g_hi) stem_mma<2 * BN>(acc, a, b);
+    else if (g_lo == 0) stem_mma<BN>(acc, a, b);
+    else stem_mma<BN>(acc + BN / 2, a, b);
+  } else {
+    static_assert(G == 4 && BN == 64, "stem tile");
+    const uint64_t bs = BN * 64 / 16;                 // one tap image (BN rows x 64 B) in descriptor units
+#pragma unroll
+    for (int g = 0; g < 4; ++g)
+      if (g >= g_lo && g <= g_hi) stem_mma<64>(acc + 32 * g, a, b + (g - g_lo) * bs);
   }
 }
 
 // kOneSlot: tall filters (BN = 128 with kh >= 8, BN = 64 with kh >= 13) leave room for a single ring slot.  A separate instance,
 // because a wait_group 0 inside the tap loop makes ptxas serialise the wgmma pipeline of the common, multi-slot one.
-template <int BN, bool kOneSlot>
-__global__ void __launch_bounds__(kStemThreads, 1)
+template <int BN, int G, bool kOneSlot>
+__global__ void __launch_bounds__(stem_threads(G), 1)
 stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pixels (W, H, N*T), box (256, rows, 1), no swizzle
                 const StemParams p) {
-  constexpr int G = kStemAccCols / BN;
-  static_assert(G * BN == kStemAccCols && (G == 1 || G == 2), "stem tile");
+  static_assert((BN == 128 && G == 1) || (BN == 64 && (G == 2 || G == 4)), "stem tile");
+  constexpr int kThreads = stem_threads(G);
+  constexpr int kStgLd = stem_stg_ld(G, BN), kStgRows = stem_stg_rows(G), kStgBufs = stem_stg_bufs(G);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align<128>(smem_raw);
   uint8_t* tail = smem + p.nstages * p.stage_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(tail);          // [kStemMaxStages]
   uint64_t* empty = full + kStemMaxStages;
-  uint64_t* stg_full = empty + kStemMaxStages;                 // [2]
-  uint64_t* stg_empty = stg_full + 2;                          // [2]
+  uint64_t* stg_full = empty + kStemMaxStages;                 // [kStgBufs]
+  uint64_t* stg_empty = stg_full + 2;                          // [kStgBufs]
   float* s_scale = reinterpret_cast<float*>(tail + 128);       // [256] (ntiles_n * BN <= 256 is enforced by the host)
   float* s_shift = s_scale + 256;
   uint32_t* s_xchg = reinterpret_cast<uint32_t*>(s_shift + 256);   // [2][4][16]: lane 31 of each epilogue warp, for the W pool
-  __half* s_stg = reinterpret_cast<__half*>(s_xchg + 128);         // [2][128][kStemStgLd]
+  __half* s_stg = reinterpret_cast<__half*>(s_xchg + 128);         // [kStgBufs][kStgRows][kStgLd]
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int slab_bytes = p.rows * kStemPitch;
 
   if (tid == 0) {
     for (int s = 0; s < p.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&stg_full[i], 256); mbar_init(&stg_empty[i], 128); }
+    for (int i = 0; i < kStgBufs; ++i) { mbar_init(&stg_full[i], 256); mbar_init(&stg_empty[i], 128); }
     fence_mbar_init();
     tma_prefetch_desc(&tmX);
   }
-  for (int i = tid; i < 256; i += kStemThreads) {
+  for (int i = tid; i < 256; i += kThreads) {
     s_scale[i] = (i < p.Ncols) ? __ldg(&p.scale[i]) : 0.f;
     s_shift[i] = (i < p.Ncols) ? __ldg(&p.shift[i]) : 0.f;
   }
@@ -160,8 +201,10 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
   pdl_launch_dependents();
   pdl_wait();                       // everything above touched only weights / on-chip state
 
-  if (warp == kStemTmaWarp) {
+  if (G == 4 ? warp >= kStemTmaWarp : warp == kStemTmaWarp) {   // G = 4: the whole producer warpgroup runs setmaxnreg
     // ================================ producer ==========================================
+    if constexpr (G == 4) setmaxnreg_dec<40>();
+    if (warp != kStemTmaWarp) return;
     int it = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x) {
       const StemItem w = stem_item(p, item);
@@ -182,6 +225,7 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
     }
   } else if (warp < kStemEpiWarp0) {
     // ================================ consumer warpgroups ===============================
+    if constexpr (G == 4) setmaxnreg_inc<208>();
     // SWIZZLE_NONE K-major descriptors: hi = SBO >> 4; lo = addr >> 4 | (LBO >> 4) << 16.  A: SBO 128 B, LBO 16 B; the
     // warpgroup's 64 tile rows start 64 x 16 B = 1 KB into the slab row.  B: SBO 512 B (8 rows), LBO 128 B.
     constexpr uint32_t a_hi = 128u >> 4, b_hi = 512u >> 4;
@@ -212,14 +256,7 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
           if (g_lo > g_hi) continue;
           const uint32_t a_lo = ((slab + static_cast<uint32_t>(i) * kStemPitch) >> 4) | ((16u >> 4) << 16);
           const uint32_t b_lo = ((wbase + static_cast<uint32_t>(p.row_slot[i]) * kTapBytes) >> 4) | ((128u >> 4) << 16);
-          const uint64_t a = desc_from(a_hi, a_lo), b = desc_from(b_hi, b_lo);
-          if constexpr (G == 1) {
-            stem_mma<BN>(acc, a, b);
-          } else {
-            if (g_lo != g_hi) stem_mma<2 * BN>(acc, a, b);
-            else if (g_lo == 0) stem_mma<BN>(acc, a, b);
-            else stem_mma<BN>(acc + BN / 2, a, b);
-          }
+          stem_row_mma<BN, G>(acc, g_lo, g_hi, desc_from(a_hi, a_lo), desc_from(b_hi, b_lo));
         }
         wgmma_commit();
         if constexpr (kOneSlot) {                       // the next tap is loaded into this same slot: release it now
@@ -236,9 +273,9 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
       if constexpr (!kOneSlot) mbar_arrive(&empty[prev_s]);   // every item has a tap inside the clip (pt < kt, checked by the host)
 
       // ---- BN affine (+ ReLU) -> fp16 staging tile ----
-      const int sb = lt & 1;
-      mbar_wait(&stg_empty[sb], ((lt >> 1) & 1) ^ 1);
-      __half* stg = s_stg + sb * (128 * kStemStgLd);
+      const int sb = lt % kStgBufs;
+      mbar_wait(&stg_empty[sb], ((lt / kStgBufs) & 1) ^ 1);
+      __half* stg = s_stg + sb * (kStgRows * kStgLd);
       const int n0 = w.ntile * BN;
 #pragma unroll
       for (int g = 0; g < G; ++g) {
@@ -251,8 +288,9 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
           float a0 = v[0] * sc.x + sh.x, a1 = v[1] * sc.y + sh.y;
           float b0 = v[2] * sc.x + sh.x, b1 = v[3] * sc.y + sh.y;
           if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); b0 = fmaxf(b0, 0.f); b1 = fmaxf(b1, 0.f); }
-          *reinterpret_cast<uint32_t*>(stg + r0 * kStemStgLd + g * BN + c) = pack_half2(a0, a1);
-          *reinterpret_cast<uint32_t*>(stg + (r0 + 8) * kStemStgLd + g * BN + c) = pack_half2(b0, b1);
+          *reinterpret_cast<uint32_t*>(stg + r0 * kStgLd + g * BN + c) = pack_half2(a0, a1);
+          if (kStgRows == 128 || r0 + 8 < kStgRows)         // tile rows >= kStemTileW carry no output column
+            *reinterpret_cast<uint32_t*>(stg + (r0 + 8) * kStgLd + g * BN + c) = pack_half2(b0, b1);
         }
       }
       mbar_arrive(&stg_full[sb]);
@@ -260,6 +298,7 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
   } else {
     // ================================ epilogue ==========================================
     // thread = tile row (pixel) erow
+    if constexpr (G == 4) setmaxnreg_dec<56>();
     const int ew = warp - kStemEpiWarp0;
     const int erow = tid - kStemEpiWarp0 * 32;
     const int lane = tid & 31;
@@ -267,14 +306,16 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const StemItem w = stem_item(p, item);
       const int g_valid = min(p.G, p.Ho - w.ho0);
-      const int sb = lt & 1;
+      const int sb = lt % kStgBufs;
       const int n0 = w.ntile * BN;
       const int ncols_here = min(BN, p.ldy - n0);
       const int wo = p.pair ? (erow & 63) : w.w0 + erow;
       const int plane_out = p.pair ? 2 * w.plane_o + (erow >> 6) : w.plane_o;
       const bool col_ok = p.pair ? (wo < p.Wo && plane_out < p.planes_total) : ((erow < kStemTileW) && (wo < p.Wo));
-      mbar_wait(&stg_full[sb], (lt >> 1) & 1);
-      const __half* srow = s_stg + sb * (128 * kStemStgLd) + erow * kStemStgLd;
+      mbar_wait(&stg_full[sb], (lt / kStgBufs) & 1);
+      // rows past a shorter staging tile have col_ok == false: they read (and then ignore) its last row
+      const int srow_i = (kStgRows < 128 && erow >= kStgRows) ? kStgRows - 1 : erow;
+      const __half* srow = s_stg + sb * (kStgRows * kStgLd) + srow_i * kStgLd;
       if (p.pool_w) {
         // ---- max over the 3-wide / stride-2 window along W before anything is written ----
         // thread erow holds output column wo = erow (one column tile per row); even columns 2wp produce pooled column wp from

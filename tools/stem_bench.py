@@ -2,10 +2,11 @@
 the Toeplitz stem kernel with BN + ReLU (and, where the network's max-pool follows, the W direction of that pool) in its
 epilogue, then the remaining (T, H) pool pass.  Each is timed as CUDA-graph replays between CUDA events after a warm-up.
 
-Per shape: conv ms and stem ms (conv + pool pass), the conv's algorithmic TFLOP/s (3 input channels, every tap) and executed
+Per shape: the output rows per work item the kernel ran with (G), conv ms and stem ms (conv + pool pass), the conv's algorithmic TFLOP/s (3 input channels, every tap) and executed
 TFLOP/s (what the kernel issues: K padded from 21 to 32 per (dt, dh), 128-row M tiles, output channels rounded up to the N tile,
 temporal taps outside the clip skipped), and the card's name and power limit.
-usage: stem_bench.py [shape ...]   (default: all shapes below)"""
+usage: stem_bench.py [--rows 2|4] [shape ...]   (default: all shapes below; --rows forces the two- or four-row instance of the
+BN = 64 stems where it applies, as B2_STEM_ROWS does)"""
 import os
 import subprocess
 import sys
@@ -15,7 +16,7 @@ import torch.nn as nn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from pretorched_x_b200 import engine, ops  # noqa: E402
+from pretorched_x_b200 import _lib, engine, ops  # noqa: E402
 
 # name: clips N, T, H, W, output channels, conv kernel, conv padding, max-pool (kernel, stride, padding) of the (T, H) pass or None
 SHAPES = {
@@ -69,6 +70,12 @@ def time_graph(fn):
 
 def main(names):
     dev = torch.device("cuda:0")
+    lib = _lib.load()
+    if "--rows" in names:
+        i = names.index("--rows")
+        lib.b2_debug_set_stem_rows(int(names[i + 1]))
+        names = names[:i] + names[i + 2:]
+    names = names or list(SHAPES)
     print("card: %s" % card(), flush=True)
     for name in names:
         N, T, H, W, K, k, p, pool = SHAPES[name]
@@ -83,11 +90,14 @@ def main(names):
             stem_fn = (lambda: ops.maxpool3d(conv_fn(), *pool)) if pool is not None else conv_fn
             ms_conv = time_graph(conv_fn)
             ms_stem = time_graph(stem_fn) if pool is not None else ms_conv
+            conv_fn()
+            torch.cuda.synchronize()
+            G = lib.b2_debug_last_stem_rows()
         alg = 2.0 * N * To * Ho * Wo * K * 3 * k[0] * k[1] * 7
         exe = executed_flops(N, T, Ho, Wo, K, k[0], k[1], p[0])
-        print("%-11s N=%-3d T=%-2d %dx%d %s->%d  conv %7.3f ms  stem %7.3f ms  algorithmic %6.1f TFLOP/s  executed %6.1f TFLOP/s"
-              % (name, N, T, H, W, "x".join(map(str, k)), K, ms_conv, ms_stem, alg / ms_conv / 1e9, exe / ms_conv / 1e9), flush=True)
+        print("%-11s N=%-3d T=%-2d %dx%d %s->%d  G=%d  conv %7.3f ms  stem %7.3f ms  algorithmic %6.1f TFLOP/s  executed %6.1f TFLOP/s"
+              % (name, N, T, H, W, "x".join(map(str, k)), K, G, ms_conv, ms_stem, alg / ms_conv / 1e9, exe / ms_conv / 1e9), flush=True)
 
 
 if __name__ == "__main__":
-    main(sys.argv[1:] or list(SHAPES))
+    main(sys.argv[1:])
