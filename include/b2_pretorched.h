@@ -238,6 +238,16 @@ size_t b2_conv_wgrad_workspace_elems(int N, int T, int H, int W, int Cin, int Co
 int b2_conv_wgrad(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
                   float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int Cin, int Cout, int k,
                   int stride, int pad, void* stream);
+/* The same for a kt x kh x kw filter with separate temporal and in-plane geometry (kt, kh = kw in {1, 3}; padding pt = kt / 2,
+ * p = kh / 2; strides st, s in {1, 2}):
+ *     G[co][ci][dt][dh][dw] = sum over output positions (n, t, h, w) of g[n, t, h, w][co] * x[n, st*t+dt-pt, s*h+dh-p, s*w+dw-p][ci]
+ * dw is fp32 [Cout][Cin][kt][kh][kw]; a 2-D filter is the (1, kh, kw) case with T = 1, whose dw is nn.Conv2d.weight's layout.
+ * b2_conv_wgrad(..., k, stride, pad) computes bitwise the same as this entry with (k, k, k, stride, stride, pad, pad). */
+size_t b2_conv_wgrad_thw_workspace_elems(int N, int T, int H, int W, int Cin, int Cout, int kt, int kh, int kw, int st, int s,
+                                         int pt, int p);
+int b2_conv_wgrad_thw(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
+                      float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int Cin, int Cout, int kt,
+                      int kh, int kw, int st, int s, int pt, int p, void* stream);
 /* Adjoint of b2_shortcut_a_ndhwc: y[n, s*to, s*ho, s*wo, 0:C] = g[n, to, ho, wo, 0:C] for the low-resolution extent
  * To = (T-1)/s + 1 (etc.), every other pixel and channels [C, ldy) zero; y is [N*T*H*W][ldy].  The backward of the type-A
  * shortcut, the placement of the type-B projection gradient, and the zero-insertion that turns the input gradient of a

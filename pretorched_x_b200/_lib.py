@@ -89,6 +89,8 @@ SYMBOLS = {
     "b2_tanh_nhwc_to_nchw": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, ctypes.c_longlong, c_int, c_void_p]),
     "b2_conv_wgrad_workspace_elems": (ctypes.c_size_t, [c_int] * 9),
     "b2_conv_wgrad": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 6 + [ctypes.c_size_t] + [c_int] * 9 + [c_void_p]),
+    "b2_conv_wgrad_thw_workspace_elems": (ctypes.c_size_t, [c_int] * 13),
+    "b2_conv_wgrad_thw": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 6 + [ctypes.c_size_t] + [c_int] * 13 + [c_void_p]),
     "b2_zero_insert_ndhwc": (c_int, [c_void_p, c_int, c_int, c_void_p] + [c_int] * 6 + [c_void_p]),
     "b2_colsum_workspace_elems": (ctypes.c_size_t, [c_int]),
     "b2_colsum_f16": (c_int, [c_void_p, c_int, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -1,6 +1,8 @@
-// b2_wgrad.cu -- weight gradient of a convolution (the backward of nn.Conv3d's weight, resnet3D.py:91-143) on wgmma:
-//     G[co][ci][tap] = sum_{n, p} g[n, p][co] * x[n, s * p + tap - pad][ci]
-// for 1x1x1 and 3x3x3 filters at stride 1 or 2, fp16 operands, fp32 accumulation.
+// b2_wgrad.cu -- weight gradient of a convolution (the backward of nn.Conv3d's / nn.Conv2d's weight, resnet3D.py:91-143 and
+// torchvision's BasicBlock / Bottleneck) on wgmma:
+//     G[co][ci][dt, dh, dw] = sum_{n, t, h, w} g[n, t, h, w][co] * x[n, st * t + dt - pt, s * h + dh - p, s * w + dw - p][ci]
+// for kt x kh x kw filters with kt, kh = kw in {1, 3} (1x1x1, 1x3x3 -- a 2-D filter as a clip with T = 1 --, 3x3x3), temporal
+// stride st and in-plane stride s in {1, 2}, fp16 operands, fp32 accumulation.
 //
 // Both operands are read in their natural channels-last layout [positions][channels]: a block of 64 output positions of g
 // and the matching (shifted, strided) 64 input positions of x arrive as two SWIZZLE_128B TMA boxes and feed the MMA as
@@ -30,7 +32,7 @@ struct WgradParams {
   int Cout, Cin, taps, kh, kw;
   int To, Ho, Wo, hb, wb;      // output extent, 8 x 8 blocks per frame
   int nbox, splits;
-  int stride, pad;
+  int st, s, pt, p;            // temporal / in-plane stride and padding
   float* ws;                   // [splits][taps][Cout][Cin]
 };
 
@@ -74,7 +76,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
         const int t = q % p.To;
         const int n = q / p.To;
         const int h0 = hbi * 8, w0 = wbi * 8;
-        const int xt = t * p.stride + dt - p.pad, xh = h0 * p.stride + dh - p.pad, xw = w0 * p.stride + dw - p.pad;
+        const int xt = t * p.st + dt - p.pt, xh = h0 * p.s + dh - p.p, xw = w0 * p.s + dw - p.p;
         uint8_t* st = smem + s * kWgStageBytes;
         mbar_expect_tx(&full[s], kWgStageBytes);
         tma_load_5d(st, &tmG, &full[s], co0, w0, h0, t, n);
@@ -156,13 +158,14 @@ struct WgradPlan {
   int To, Ho, Wo, nbox, tiles, splits;
 };
 
-static WgradPlan wgrad_plan(int N, int T, int H, int W, int Cin, int Cout, int k, int stride, int pad) {
+static WgradPlan wgrad_plan(int N, int T, int H, int W, int Cin, int Cout, int kt, int kh, int kw, int st, int s_hw, int pt,
+                            int p_hw) {
   WgradPlan q;
-  q.To = (T + 2 * pad - k) / stride + 1;
-  q.Ho = (H + 2 * pad - k) / stride + 1;
-  q.Wo = (W + 2 * pad - k) / stride + 1;
+  q.To = (T + 2 * pt - kt) / st + 1;
+  q.Ho = (H + 2 * p_hw - kh) / s_hw + 1;
+  q.Wo = (W + 2 * p_hw - kw) / s_hw + 1;
   q.nbox = N * q.To * ((q.Ho + 7) / 8) * ((q.Wo + 7) / 8);
-  q.tiles = ((Cin + 127) / 128) * ((Cout + 127) / 128) * k * k * k;
+  q.tiles = ((Cin + 127) / 128) * ((Cout + 127) / 128) * kt * kh * kw;
   // enough CTAs for two waves over the SMs, at least 4 position blocks per split (pipeline fill), at most 64 slices
   int s = (2 * sm_count() + q.tiles - 1) / q.tiles;
   s = s < q.nbox / 4 ? s : q.nbox / 4;
@@ -177,45 +180,62 @@ using namespace b2;
 
 extern "C" {
 
-size_t b2_conv_wgrad_workspace_elems(int N, int T, int H, int W, int Cin, int Cout, int k, int stride, int pad) {
-  if (N <= 0 || T <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || k <= 0 || stride <= 0) return 0;
-  const WgradPlan q = wgrad_plan(N, T, H, W, Cin, Cout, k, stride, pad);
-  return static_cast<size_t>(q.splits) * k * k * k * Cout * Cin;
+size_t b2_conv_wgrad_thw_workspace_elems(int N, int T, int H, int W, int Cin, int Cout, int kt, int kh, int kw, int st, int s,
+                                         int pt, int p) {
+  if (N <= 0 || T <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || kt <= 0 || kh <= 0 || kw <= 0 || st <= 0 || s <= 0) return 0;
+  const WgradPlan q = wgrad_plan(N, T, H, W, Cin, Cout, kt, kh, kw, st, s, pt, p);
+  return static_cast<size_t>(q.splits) * kt * kh * kw * Cout * Cin;
 }
 
-int b2_conv_wgrad(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
-                  float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int Cin, int Cout, int k,
-                  int stride, int pad, void* stream) {
+int b2_conv_wgrad_thw(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
+                      float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int Cin, int Cout, int kt,
+                      int kh, int kw, int st, int s, int pt, int p, void* stream) {
   B2_CHECK_ARG(g && x && dw && ws, "null pointer");
   B2_CHECK_ARG(!wdot || w, "wdot needs the weight");
   B2_CHECK_ARG(N > 0 && T > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0, "non-positive dimension");
-  B2_CHECK_ARG((k == 1 && pad == 0) || (k == 3 && pad == 1), "filters are 1x1x1 (padding 0) or 3x3x3 (padding 1), got k=%d pad=%d", k, pad);
-  B2_CHECK_ARG(stride == 1 || stride == 2, "stride %d is not 1 or 2", stride);
+  B2_CHECK_ARG((kt == 1 || kt == 3) && (kh == 1 || kh == 3) && kw == kh && pt == kt / 2 && p == kh / 2,
+               "filters are kt x k x k with kt, k in {1, 3} and padding (kt / 2, k / 2, k / 2), got %dx%dx%d padding (%d, %d)", kt, kh,
+               kw, pt, p);
+  B2_CHECK_ARG((st == 1 || st == 2) && (s == 1 || s == 2), "strides (%d, %d) are not 1 or 2", st, s);
   B2_CHECK_ARG(Cin % 8 == 0 && Cout % 8 == 0 && ldg >= Cout && ldx >= Cin, "channel counts must be multiples of 8 within their pitches");
-  const WgradPlan q = wgrad_plan(N, T, H, W, Cin, Cout, k, stride, pad);
+  const WgradPlan q = wgrad_plan(N, T, H, W, Cin, Cout, kt, kh, kw, st, s, pt, p);
+  const int taps = kt * kh * kw;
   B2_CHECK_ARG(q.To > 0 && q.Ho > 0 && q.Wo > 0, "empty output");
-  B2_CHECK_ARG(ws_elems >= static_cast<size_t>(q.splits) * k * k * k * Cout * Cin, "workspace too small (see b2_conv_wgrad_workspace_elems)");
+  B2_CHECK_ARG(ws_elems >= static_cast<size_t>(q.splits) * taps * Cout * Cin, "workspace too small (see b2_conv_wgrad_thw_workspace_elems)");
   int rc;
   if ((rc = require_sm90()) != B2_OK) return rc;
   CUtensorMap tmG, tmX;
   if ((rc = make_tmap_ndhwc_5d(&tmG, g, (uint64_t)Cout, (uint64_t)ldg, (uint64_t)q.Wo, (uint64_t)q.Ho, (uint64_t)q.To, (uint64_t)N,
                                8, 8, 1)) != B2_OK)
     return rc;
+  // the temporal stride needs no element stride: the x box is one frame deep and its frame index is computed per box
   if ((rc = make_tmap_ndhwc_5d(&tmX, x, (uint64_t)Cin, (uint64_t)ldx, (uint64_t)W, (uint64_t)H, (uint64_t)T, (uint64_t)N, 8, 8,
-                               (uint32_t)stride)) != B2_OK)
+                               (uint32_t)s)) != B2_OK)
     return rc;
-  WgradParams p;
-  p.Cout = Cout; p.Cin = Cin; p.taps = k * k * k; p.kh = k; p.kw = k;
-  p.To = q.To; p.Ho = q.Ho; p.Wo = q.Wo; p.hb = (q.Ho + 7) / 8; p.wb = (q.Wo + 7) / 8;
-  p.nbox = q.nbox; p.splits = q.splits; p.stride = stride; p.pad = pad; p.ws = ws;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  WgradParams prm;
+  prm.Cout = Cout; prm.Cin = Cin; prm.taps = taps; prm.kh = kh; prm.kw = kw;
+  prm.To = q.To; prm.Ho = q.Ho; prm.Wo = q.Wo; prm.hb = (q.Ho + 7) / 8; prm.wb = (q.Wo + 7) / 8;
+  prm.nbox = q.nbox; prm.splits = q.splits; prm.st = st; prm.s = s; prm.pt = pt; prm.p = p; prm.ws = ws;
+  cudaStream_t stm = reinterpret_cast<cudaStream_t>(stream);
   B2_OPT_IN_SMEM(wgrad_kernel, kWgSmem);
-  dim3 grid((Cin + 127) / 128, (Cout + 127) / 128, p.taps * q.splits);
-  wgrad_kernel<<<grid, kWgThreads, kWgSmem, st>>>(tmG, tmX, p);
+  dim3 grid((Cin + 127) / 128, (Cout + 127) / 128, taps * q.splits);
+  wgrad_kernel<<<grid, kWgThreads, kWgSmem, stm>>>(tmG, tmX, prm);
   B2_CHECK_LAUNCH("wgrad");
-  wgrad_reduce_kernel<<<Cout, kWgReduceThreads, 0, st>>>(ws, q.splits, Cout, Cin, p.taps, w, scale, inv_loss_scale, dw, wdot);
+  wgrad_reduce_kernel<<<Cout, kWgReduceThreads, 0, stm>>>(ws, q.splits, Cout, Cin, taps, w, scale, inv_loss_scale, dw, wdot);
   B2_CHECK_LAUNCH("wgrad_reduce");
   return B2_OK;
+}
+
+size_t b2_conv_wgrad_workspace_elems(int N, int T, int H, int W, int Cin, int Cout, int k, int stride, int pad) {
+  return b2_conv_wgrad_thw_workspace_elems(N, T, H, W, Cin, Cout, k, k, k, stride, stride, pad, pad);
+}
+
+int b2_conv_wgrad(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
+                  float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int Cin, int Cout, int k,
+                  int stride, int pad, void* stream) {
+  B2_CHECK_ARG((k == 1 && pad == 0) || (k == 3 && pad == 1), "filters are 1x1x1 (padding 0) or 3x3x3 (padding 1), got k=%d pad=%d", k, pad);
+  return b2_conv_wgrad_thw(g, ldg, x, ldx, w, scale, inv_loss_scale, dw, wdot, ws, ws_elems, N, T, H, W, Cin, Cout, k, k, k, stride,
+                           stride, pad, pad, stream);
 }
 
 }  // extern "C"

@@ -20,7 +20,7 @@ NOT seen: ``model.invalidate()`` / ``engine.invalidate(model)`` drops every pack
 
 Every block body is entered through a ``torch.autograd.Function`` (``functions.py``, SURVEY.md section 8b-ii): the
 Function's ``forward`` is the ctypes call sequence, its outputs are marked non-differentiable (frozen-backbone
-semantics), except for the stages a ``ResNet3D.fine_tune(k)`` call made trainable (``block_backward``), and the dense heads (``last_linear``, the TRN
+semantics), except for the stages a ``fine_tune(k)`` call (``ResNet3D``, ``ResNet2D``, ``TRN``) made trainable (``block_backward``), and the dense heads (``last_linear``, the TRN
 relation MLPs) have a real backward on the same wgmma GEMM so that a head can be trained on engine features.
 """
 import os
@@ -606,9 +606,35 @@ class TrainAct(Act):
     __slots__ = ("loss_scale",)
 
 
+def _check_trainable_2d(block):
+    """torchvision BasicBlock / Bottleneck (the 2-D ResNets): Conv2d 1x1 / 3x3 with padding k // 2, stride 1 or 2, no groups,
+    bias or dilation, BatchNorm2d, identity or (Conv2d 1x1, BatchNorm2d) shortcut."""
+    convs = [(block.conv1, block.bn1), (block.conv2, block.bn2)] + ([(block.conv3, block.bn3)] if hasattr(block, "conv3") else [])
+    ds = block.downsample
+    ok = True
+    if isinstance(ds, nn.Sequential):
+        ok = len(ds) == 2 and type(ds[0]) is nn.Conv2d and tuple(ds[0].weight.shape[2:]) == (1, 1)
+        convs.append((ds[0], ds[1]) if ok else (None, None))
+    elif ds is not None:
+        ok = False
+    for conv, bn in convs if ok else ():
+        k = tuple(conv.weight.shape[2:])
+        ok = ok and type(conv) is nn.Conv2d and conv.groups == 1 and conv.bias is None and all(d == 1 for d in conv.dilation)
+        ok = ok and k in ((1, 1), (3, 3)) and tuple(conv.padding) == (k[0] // 2,) * 2
+        ok = ok and len(set(conv.stride)) == 1 and conv.stride[0] in (1, 2)
+        ok = ok and isinstance(bn, nn.BatchNorm2d) and bn.affine and bn.running_var is not None
+    if not ok:
+        raise NotImplementedError("fine-tuning backward covers torchvision's BasicBlock / Bottleneck with 1x1 / 3x3 Conv2d filters "
+                                  "and an identity or 1x1 projection shortcut; got a %s that is not of that form" % type(block).__name__)
+
+
 def check_trainable_block(block):
-    """Raise NotImplementedError unless ``block`` is a plain 3-D ResNet BasicBlock / Bottleneck the backward covers."""
+    """Raise NotImplementedError unless ``block`` is a plain 3-D ResNet BasicBlock / Bottleneck or a torchvision (2-D)
+    BasicBlock / Bottleneck the backward covers."""
+    import torchvision.models.resnet as tvresnet
     from .models.resnet3d import BasicBlock, Bottleneck, ShortcutA
+    if type(block) in (tvresnet.BasicBlock, tvresnet.Bottleneck):
+        return _check_trainable_2d(block)
     name = type(block).__name__
     ok = type(block) in (BasicBlock, Bottleneck) and getattr(block, "nonlocalblock", None) is None
     convs = [(block.conv1, block.bn1), (block.conv2, block.bn2)] + ([(block.conv3, block.bn3)] if ok and hasattr(block, "conv3") else [])
@@ -653,10 +679,27 @@ def _dgrad_1x1(conv, s):
     return w.t().contiguous().to(torch.float16)
 
 
+def _kernel_thw(conv):
+    """(kt, kh, kw) of a Conv3d / Conv2d filter (a 2-D filter is (1, kh, kw))."""
+    k = tuple(conv.weight.shape[2:])
+    return (1,) + k if len(k) == 2 else k
+
+
 def _dgrad_3x3(conv, s, g_pitch):
-    """The input gradient of a 3x3x3 convolution as a stride-1, padding-1 convolution with the transposed, flipped, s-folded filter."""
-    w = conv.weight.detach().float() * s[:, None, None, None, None]
-    return ops.PackedConv(w.flip(2, 3, 4).transpose(0, 1).contiguous(), None, None, (1, 1, 1), (1, 1, 1), in_pitch=g_pitch)
+    """The input gradient of a 3x3x3 (or 2-D 3x3) convolution as a stride-1 convolution with the transposed, flipped,
+    s-folded filter and padding (1, 1, 1) (or (0, 1, 1))."""
+    w = conv.weight.detach().float()
+    w = w * s.view((-1,) + (1,) * (w.dim() - 1))
+    if w.dim() == 4:                                   # Conv2d: a (1, 3, 3) filter at T = 1
+        w = w.unsqueeze(2)
+    pad = tuple(k // 2 for k in w.shape[2:])
+    return ops.PackedConv(w.flip(2, 3, 4).transpose(0, 1).contiguous(), None, None, (1, 1, 1), pad, in_pitch=g_pitch)
+
+
+def _inplane_stride(conv):
+    """The stride b2_zero_insert_ndhwc applies.  It takes one stride for all three axes: the 3-D blocks have cubic strides,
+    and a 2-D convolution runs at T = 1, where inserting zeros along T is the identity."""
+    return _conv_geometry(conv)[0][1]
 
 
 def _gemm_dgrad(g, wt, residual=None, second=None, mask=None):
@@ -671,7 +714,7 @@ def _gemm_dgrad(g, wt, residual=None, second=None, mask=None):
 
 def _conv_dgrad(conv, s, g, x):
     """Gradient at the input ``x`` of a 3x3x3 convolution for the gradient ``g`` at its (BN-scaled) output, before any residual."""
-    stride = conv.stride[0]
+    stride = _inplane_stride(conv)
     z = g if stride == 1 else ops.zero_insert(g, x.T, x.H, x.W, stride)
     return z, _dgrad_3x3(conv, s, z.ld)
 
@@ -682,9 +725,10 @@ def _param_grads(conv, bn, g, x, ls, needs):
     dw = wdot = dbeta = dgamma = None
     inv = ls[1:]
     if need_w or need_g:
-        k = conv.weight.shape[2]
-        dw, wdot = ops.conv_wgrad(g, x, k, conv.stride[0], k // 2, weight=conv.weight if need_g else None, scale=_bn_scale(bn),
+        stride, pad = _conv_geometry(conv)
+        dw, wdot = ops.conv_wgrad(g, x, _kernel_thw(conv), stride, pad, weight=conv.weight if need_g else None, scale=_bn_scale(bn),
                                   inv_loss_scale=inv)
+        dw = dw.view(conv.weight.shape)
     if need_b or need_g:
         dbeta = ops.colsum(g, inv)
     if need_g:
@@ -698,7 +742,7 @@ def _shortcut_grad(block, g, x):
     if ds is None:
         return g
     if isinstance(ds, nn.Sequential):
-        stride = ds[0].stride[0]
+        stride = _inplane_stride(ds[0])
         pg = _gemm_dgrad(g, _dgrad_1x1(ds[0], _bn_scale(ds[1])))
         return pg if stride == 1 else ops.zero_insert(pg, x.T, x.H, x.W, stride, ld=x.ld)
     return ops.zero_insert(g, x.T, x.H, x.W, ds.stride, channels=x.C, ld=x.ld)       # type A: subsample + zero channels
@@ -731,7 +775,7 @@ def block_backward(block, x, hs, gy, ls, need_x, needs):
     ds = block.downsample
     if hasattr(block, "conv3"):
         w1 = _dgrad_1x1(block.conv1, s1)
-        if isinstance(ds, nn.Sequential) and ds[0].stride[0] == 1:     # both 1x1 products in one two-operand GEMM
+        if isinstance(ds, nn.Sequential) and _inplane_stride(ds[0]) == 1:     # both 1x1 products in one two-operand GEMM
             dx = _gemm_dgrad(g1, w1, second=(gy.data, _dgrad_1x1(ds[0], _bn_scale(ds[1])), gy.C), mask=x)
         else:
             dx = _gemm_dgrad(g1, w1, residual=_shortcut_grad(block, gy, x), mask=x)

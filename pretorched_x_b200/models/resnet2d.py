@@ -11,7 +11,7 @@ import torchvision.models.resnet as tvresnet
 
 from .. import engine, ops
 from ..ops import Act
-from .resnet3d import _attach_settings
+from .resnet3d import FineTunable, _attach_settings
 
 __all__ = ['ResNet2D', 'resnet18', 'resnet34', 'resnet50', 'resnet101', 'resnet152']
 
@@ -35,8 +35,13 @@ pretrained_settings['resnet18']['places365'] = _row('http://pretorched-x.csail.m
 pretrained_settings['resnet50']['places365'] = _row('http://pretorched-x.csail.mit.edu/models/resnet50_places365-a570fcfc.pth', 365)
 
 
-class ResNet2D(engine.CacheOwner, tvresnet.ResNet):
-    """torchvision ResNet parameters + engine forward; ``last_linear`` replaces ``fc``."""
+class ResNet2D(engine.CacheOwner, FineTunable, tvresnet.ResNet):
+    """torchvision ResNet parameters + engine forward; ``last_linear`` replaces ``fc``.
+
+    ``fine_tune(k)`` trains ``layer{k}..layer4`` and ``last_linear`` on the engine, with the contract of
+    ``ResNet3D.fine_tune`` (frozen BatchNorm, model in ``eval()``, 1 <= k <= 5)."""
+
+    stem_desc = '7x7 convolution'
 
     def __init__(self, block, layers, num_classes=1000):
         super().__init__(block, layers, num_classes=num_classes)
@@ -51,12 +56,8 @@ class ResNet2D(engine.CacheOwner, tvresnet.ResNet):
             if src in state_dict and dst not in state_dict:
                 state_dict[dst] = state_dict.pop(src)
 
-    def features_act(self, x):
-        if self.training:
-            raise RuntimeError("the forward engine is inference-only: call model.eval() first")
-        return engine.run_trunk(self, x)
-
     def features(self, input):
+        self._refuse_features_in_fine_tune_mode()
         return ops.to_ncdhw(self.features_act(input)).squeeze(2)
 
     def logits(self, features):

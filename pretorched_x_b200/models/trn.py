@@ -29,8 +29,11 @@ def _packed(linear):
                           lambda: ops.PackedLinear(linear.weight, linear.bias))
 
 
-def _wants_grad(module):
-    return torch.is_grad_enabled() and any(p.requires_grad for p in module.parameters())
+def _wants_grad(module, input=None):
+    """Take the differentiable path: under grad mode, when the module has a trainable parameter or its input needs a
+    gradient (a fine-tuned backbone underneath)."""
+    return torch.is_grad_enabled() and (any(p.requires_grad for p in module.parameters()) or
+                                        (input is not None and input.requires_grad))
 
 
 class Relation(engine.CacheOwner, nn.Module):
@@ -60,7 +63,7 @@ class Relation(engine.CacheOwner, nn.Module):
 
     def forward(self, input):
         flat = input.contiguous().view(-1, self.num_inputs * self.in_features)
-        if _wants_grad(self):
+        if _wants_grad(self, input):
             return self.mlp_grad(flat.float()).view(input.size(0), -1, self.out_features)
         x16 = ops.cast_rows(flat, relu=True)          # leading nn.ReLU fused into the fp16 cast
         return self.mlp_f16(x16).view(input.size(0), -1, self.out_features)
@@ -138,7 +141,7 @@ class MultiScaleRelation(engine.CacheOwner, nn.Module):
         feats = input.contiguous().view(-1, self.num_input, self.in_features)
         rows = feats.shape[0]
         picks = self.sample_tuples()
-        if _wants_grad(self):
+        if _wants_grad(self, input):
             # differentiable path: per tuple, through LinearFunction (indexing and the sum are torch autograd ops)
             total = None
             for si, tuples in enumerate(picks):
@@ -188,7 +191,13 @@ class TRN(engine.CacheOwner, nn.Module):
     argument (trn.py:230-233), which for the default ``consensus='HTRN'`` is ``relation_size`` -- the module degenerates to
     one 8-frame ``Relation`` with a 512-wide bottleneck; 'MSHTRN' and HTRN with depth > 0 raise upstream and raise here.
     Upstream defect NOT kept (section 0.8): ``TRN(pretrained=None)`` crashes on ``base_model.std`` because preprocessing
-    attributes are only attached by ``load_pretrained``; here they fall back to the backbone's ImageNet registry row."""
+    attributes are only attached by ``load_pretrained``; here they fall back to the backbone's ImageNet registry row.
+
+    Training: ``fine_tune(k)`` trains the backbone's ``layer{k}..layer4``, the relation and the final Linear on the engine, and
+    ``get_optim_policies()`` gives the reference's parameter groups (trn.py:287-330).  Deviation: the reference's ``train()``
+    (trn.py:265-282) leaves the first BatchNorm in batch-statistics mode ("partial BN"); here every BatchNorm stays frozen (eval
+    mode, running statistics) and the model must stay in ``eval()`` -- after ``train()`` the forward raises, as for every engine
+    model.  ``partialBN(enable)`` still selects which BatchNorm parameters ``get_optim_policies`` lists."""
 
     def __init__(self, num_classes, num_segments=8, arch='resnet50', frame_bottleneck_dim=1024, video_feature_dim=1024,
                  consensus='HTRN', pretrained='moments', dropout=0.5, partial_bn=True):
@@ -240,6 +249,51 @@ class TRN(engine.CacheOwner, nn.Module):
 
     def partialBN(self, enable):
         self._enable_pbn = enable
+
+    def fine_tune(self, ft_begin_index):
+        """Train ``base_model.layer{k}..layer4`` (k = ``ft_begin_index``, see ``ResNet2D.fine_tune``), ``temporal_relation``
+        and ``last_linear``; freeze everything else.  The gradient reaches the backbone through the relation's
+        differentiable path and the backbone's fp32 pooled features."""
+        if not hasattr(self.base_model, 'fine_tune'):
+            raise NotImplementedError("fine-tuning a TRN needs a backbone with fine_tune(); the %s backbone has none" % self.arch)
+        self.base_model.fine_tune(ft_begin_index)
+        for m in (self.temporal_relation, self.last_linear):
+            for p in m.parameters():
+                p.requires_grad_(True)
+        return self
+
+    def get_optim_policies(self):
+        """The reference's parameter groups (trn.py:287-330), in module order: the first Conv weight / bias, the other
+        Conv1d / Conv2d / Linear weights / biases, and BatchNorm gamma / beta -- every BatchNorm1d, and of the BatchNorm2d
+        only the first when partial BN is on (``partialBN(True)``, the default) or all of them when it is off.  A leaf module
+        of any other type that has parameters raises ValueError."""
+        first_w, first_b, weights, biases, bn = [], [], [], [], []
+        n_conv = n_bn2d = 0
+        for m in self.modules():
+            ps = list(m.parameters())
+            if isinstance(m, (nn.Conv1d, nn.Conv2d)):
+                n_conv += 1
+                w, b = (first_w, first_b) if n_conv == 1 else (weights, biases)
+                w.append(ps[0])
+                b.extend(ps[1:2] if len(ps) == 2 else [])
+            elif isinstance(m, nn.Linear):
+                weights.append(ps[0])
+                biases.extend(ps[1:2] if len(ps) == 2 else [])
+            elif isinstance(m, nn.BatchNorm1d):
+                bn.extend(ps)
+            elif isinstance(m, nn.BatchNorm2d):
+                n_bn2d += 1
+                if n_bn2d == 1 or not self._enable_pbn:
+                    bn.extend(ps)
+            elif not m._modules and ps:
+                raise ValueError("no learning policy for a leaf module of type %s" % type(m).__name__)
+        return [
+            {'params': first_w, 'lr_mult': 1, 'decay_mult': 1, 'name': "first_conv_weight"},
+            {'params': first_b, 'lr_mult': 2, 'decay_mult': 0, 'name': "first_conv_bias"},
+            {'params': weights, 'lr_mult': 1, 'decay_mult': 1, 'name': "normal_weight"},
+            {'params': biases, 'lr_mult': 2, 'decay_mult': 0, 'name': "normal_bias"},
+            {'params': bn, 'lr_mult': 1, 'decay_mult': 0, 'name': "BN scale/shift"},
+        ]
 
     @property
     def crop_size(self):

@@ -521,24 +521,35 @@ def gather_frame_tuples(x3d, idx_dev, n_tuples, n_idx):
 # ---------------------------------------------------------------------------------------------
 # fine-tuning backward (functions.BottleneckTrainFunction / BasicBlockTrainFunction)
 # ---------------------------------------------------------------------------------------------
+def _thw(v):
+    return tuple(int(i) for i in v) if isinstance(v, (tuple, list)) else (int(v),) * 3
+
+
 @_on_device
 def conv_wgrad(g, x, k, stride, pad, weight=None, scale=None, inv_loss_scale=None):
-    """Weight gradient of a k x k x k convolution (b2_conv_wgrad): g = Act gradient at the convolution output, x = Act input.
-    Returns (dw fp32 in the nn.Conv3d.weight layout, scaled by ``scale[co]`` and ``inv_loss_scale``, and, with ``weight``,
-    wdot[co] = <weight[co], G[co]> * inv_loss_scale)."""
+    """Weight gradient of a convolution (b2_conv_wgrad_thw): g = Act gradient at the convolution output, x = Act input.
+    ``k``, ``stride`` and ``pad`` are ints (cubic filter, one geometry for all axes) or (t, h, w) triples whose h and w entries
+    agree, e.g. (1, 3, 3), (1, 2, 2), (0, 1, 1) for a 2-D 3x3 stride-2 filter run as a clip with T = 1.
+    Returns (dw fp32 [Cout][Cin][kt][kh][kw], scaled by ``scale[co]`` and ``inv_loss_scale``, and, with ``weight``,
+    wdot[co] = <weight[co], G[co]> * inv_loss_scale; ``weight`` may be 4-D or 5-D)."""
+    (kt, kh, kw), (st, sh, sw), (pt, ph, pw) = _thw(k), _thw(stride), _thw(pad)
+    if sh != sw or ph != pw:
+        raise ValueError("the weight gradient takes one in-plane stride and padding, got stride %r padding %r" % (stride, pad))
     Cout, Cin = g.C, x.C
     dev = g.data.device
     lib = _lib.load()
-    n = lib.b2_conv_wgrad_workspace_elems(x.N, x.T, x.H, x.W, Cin, Cout, k, stride, pad)
+    n = lib.b2_conv_wgrad_thw_workspace_elems(x.N, x.T, x.H, x.W, Cin, Cout, kt, kh, kw, st, sh, pt, ph)
     ws = torch.empty(max(int(n), 1), dtype=torch.float32, device=dev)
-    dw = torch.empty((Cout, Cin, k, k, k), dtype=torch.float32, device=dev)
+    dw = torch.empty((Cout, Cin, kt, kh, kw), dtype=torch.float32, device=dev)
     w = weight.detach().float().contiguous() if weight is not None else None
     wdot = torch.empty(Cout, dtype=torch.float32, device=dev) if weight is not None else None
-    with _timed("wgrad", "wgrad %dx%dx%d s%d C%d->%d M=%d" % (k, k, k, stride, Cin, Cout, g.M), 2.0 * g.M * Cout * Cin * k ** 3,
-                2.0 * (g.M * Cout + x.M * Cin) + 4.0 * Cout * Cin * k ** 3):
-        _lib.check(lib.b2_conv_wgrad(_ptr(g.data), g.ld, _ptr(x.data), x.ld, _ptr(w), _ptr(scale), _ptr(inv_loss_scale), _ptr(dw),
-                                     _ptr(wdot), _ptr(ws), ws.numel(), x.N, x.T, x.H, x.W, Cin, Cout, k, stride, pad, _stream()),
-                   "b2_conv_wgrad")
+    taps = kt * kh * kw
+    with _timed("wgrad", "wgrad %dx%dx%d s%d,%d C%d->%d M=%d" % (kt, kh, kw, st, sh, Cin, Cout, g.M), 2.0 * g.M * Cout * Cin * taps,
+                2.0 * (g.M * Cout + x.M * Cin) + 4.0 * Cout * Cin * taps):
+        _lib.check(lib.b2_conv_wgrad_thw(_ptr(g.data), g.ld, _ptr(x.data), x.ld, _ptr(w), _ptr(scale), _ptr(inv_loss_scale), _ptr(dw),
+                                         _ptr(wdot), _ptr(ws), ws.numel(), x.N, x.T, x.H, x.W, Cin, Cout, kt, kh, kw, st, sh, pt, ph,
+                                         _stream()),
+                   "b2_conv_wgrad_thw")
     return dw, wdot
 
 

@@ -91,4 +91,24 @@ if not only or "finetune" in only:
         torch.cuda.synchronize()
         assert all(torch.isfinite(p.grad).all() for p in m.parameters() if p.grad is not None)
         print("%-28s loss %.4f" % ("%s fine-tune step" % arch, loss.item()), flush=True)
+if not only or "finetune2d" in only:
+    # the 2-D / TRN fine-tuning step: (1, 3, 3) and (1, 1, 1) weight gradients, stride-2 zero insertion at T = 1, the relation's
+    # differentiable path into the backbone
+    torch.manual_seed(0)
+    m = OF.randomize_bn_(P.resnet50(num_classes=10, pretrained=None), 1).eval().to(dev)
+    groups = P.models.resnet3d.get_fine_tuning_parameters(m, 3)
+    x = torch.randn((2, 3, 64, 64), generator=torch.Generator().manual_seed(6)).to(dev)
+    loss = torch.nn.functional.cross_entropy(m(x), torch.tensor([1, 2], device=dev))
+    loss.backward()
+    torch.optim.SGD(groups, lr=1e-5).step()
+    torch.manual_seed(0)
+    t = OF.randomize_bn_(P.TRN(num_classes=10, num_segments=8, arch="resnet18", pretrained=None, consensus="MSTRN"), 1).eval().to(dev)
+    t.fine_tune(3)
+    x = torch.randn((2, 8, 3, 64, 64), generator=torch.Generator().manual_seed(7)).to(dev)
+    tloss = torch.nn.functional.cross_entropy(t(x), torch.tensor([1, 2], device=dev))
+    tloss.backward()
+    torch.cuda.synchronize()
+    for mod in (m, t):
+        assert all(torch.isfinite(p.grad).all() for p in mod.parameters() if p.grad is not None)
+    print("%-28s loss %.4f, TRN(resnet18, MSTRN) k=3 loss %.4f" % ("resnet50 2-D fine-tune step", loss.item(), tloss.item()), flush=True)
 print("sanitize_run: done")
