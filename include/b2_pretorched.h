@@ -57,7 +57,8 @@ typedef struct b2_conv_args {
   const void* residual; /* nullable; fp16 [M][ldr], M = N*To*Ho*Wo                                 */
   void* y;              /* fp16 [M][ldy]  (fp32 when out_f32)                                      */
   int32_t N, T, H, W, C;
-  int32_t K;            /* logical output channels; columns [K, ldy) of y are written as zero      */
+  int32_t K;            /* logical output channels; columns [K, ldy) of an fp16 y are written as zero, those of an fp32 y
+                           (out_f32) are left untouched                                            */
   int32_t ldy, ldr;
   int32_t kt, kh, kw;
   int32_t st, sh, sw;
@@ -256,7 +257,7 @@ int b2_zero_insert_ndhwc(const void* g, int ldg, int C, void* y, int ldy, int N,
 /* out[c] = inv_loss_scale * sum_r g[r][c] (fp32, fixed-order two-pass reduction; ws: b2_colsum_workspace_elems(C) floats). */
 size_t b2_colsum_workspace_elems(int C);
 int b2_colsum_f16(const void* g, int ldg, long long rows, int C, const float* inv_loss_scale, float* out, float* ws, void* stream);
-/* scale_pair = [2^k, 2^-k] with max |g| * 2^k in [2^7, 2^8) (k = 0 when g is all zero or has a non-finite entry). */
+/* scale_pair = [2^k, 2^-k] with max |g| * 2^k in [2^7, 2^8), |k| <= 126 (k = 0 when g is all zero or has a non-finite entry). */
 int b2_loss_scale_f32(const float* g, int rows, int cols, int ldg, float* scale_pair, void* stream);
 /* Backward of b2_avgpool_global_ndhwc followed by the block's closing ReLU: y[n*S + p][c] = fp16(gf[n][c] * scale_pair[0] / S)
  * where out[n*S + p][c] > 0, else 0 (channels [C, ld) zero).  gf fp32 [N][ldf]; out, y fp16 [N*S][ld]. */

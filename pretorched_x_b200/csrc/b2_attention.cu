@@ -497,6 +497,7 @@ static int launch_attention(const void* q, int ldq, const void* k, int ldk, cons
   dim3 grid((Nq + kAttBM - 1) / kAttBM, B, dv / DVT);
   B2_CHECK_CUDA(launch_pdl(nonlocal_attention_kernel<DVT>, grid, dim3(kAttThreads), S::kTotal, stream, tmQ, tmK, tmV, p));
   B2_CHECK_LAUNCH("nonlocal_attention_kernel");
+  set_last_kernel(KID_ATTENTION, 0, DVT);
   return B2_OK;
 }
 
@@ -518,6 +519,7 @@ static int launch_attention_online(const void* q, int ldq, const void* k, int ld
   dim3 grid((Nq + kAttBM - 1) / kAttBM, B, dv / DVT);
   B2_CHECK_CUDA(launch_pdl(nonlocal_attention_online_kernel<DVT>, grid, dim3(kOnThreads), S::kTotal, stream, tmQ, tmK, tmV, p));
   B2_CHECK_LAUNCH("nonlocal_attention_online_kernel");
+  set_last_kernel(KID_ATTENTION, 1, DVT);
   return B2_OK;
 }
 
@@ -530,6 +532,7 @@ extern "C" int b2_debug_set_attention_algo(int algo) { g_att_algo = algo; return
 
 extern "C" int b2_nonlocal_attention(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* o,
                                      int ldo, int B, int Nq, int Nk, int d, int dv, int mode, void* stream) {
+  set_last_kernel(KID_NONE);
   B2_CHECK_ARG(q && k && v && o, "null pointer");
   B2_CHECK_ARG(B > 0 && Nq > 0 && Nk > 0 && d > 0 && dv > 0, "non-positive dimension");
   B2_CHECK_ARG(mode >= 0 && mode <= 2, "unknown attention mode %d", mode);

@@ -489,7 +489,8 @@ __global__ void __launch_bounds__(1024) loss_scale_kernel(const float* __restric
     int e = 0;
     if (m > 0.f && !bad_any) frexpf(m, &e);              // m = f * 2^e, f in [0.5, 1)
     int k = (m > 0.f && !bad_any) ? 8 - e : 0;
-    k = k > 100 ? 100 : (k < -100 ? -100 : k);
+    // |k| <= 126 keeps both 2^k and 2^-k finite and normal in fp32; any finite max |g| >= 2^-118 then lands in [2^7, 2^8)
+    k = k > 126 ? 126 : (k < -126 ? -126 : k);
     sc[0] = ldexpf(1.f, k);
     sc[1] = ldexpf(1.f, -k);
   }
@@ -555,6 +556,7 @@ int b2_pack_conv_weight(const float* w, void* out, int K, int Cin, int kt, int k
 }
 
 int b2_conv_ndhwc_fprop_simt(const b2_conv_args* a, void* stream) {
+  set_last_kernel(KID_NONE);
   B2_CHECK_ARG(a && a->x && a->w && a->scale && a->shift && a->y, "null pointer");
   SimtConvParams p;
   p.x = (const __half*)a->x; p.w = (const __half*)a->w; p.scale = a->scale; p.shift = a->shift;
@@ -569,6 +571,7 @@ int b2_conv_ndhwc_fprop_simt(const b2_conv_args* a, void* stream) {
   const long long total = (long long)a->N * p.To * p.Ho * p.Wo * a->ldy;
   conv_simt_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, total);
   B2_CHECK_LAUNCH("conv_simt");
+  set_last_kernel(KID_SIMT);
   return B2_OK;
 }
 

@@ -31,6 +31,13 @@ int set_error(int code, const char* fmt, ...) {
 }
 void count_launch(int n) { g_launches.fetch_add(static_cast<uint64_t>(n), std::memory_order_relaxed); }
 
+static int g_last_kernel = KID_NONE;
+static int g_last_info[5] = {0, 0, 0, 0, 0};
+void set_last_kernel(int id, int i0, int i1, int i2, int i3, int i4) {
+  g_last_kernel = id;
+  g_last_info[0] = i0; g_last_info[1] = i1; g_last_info[2] = i2; g_last_info[3] = i3; g_last_info[4] = i4;
+}
+
 int require_sm90() {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
@@ -424,6 +431,7 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream) {
   if (best_mt == 0) return 0;
   int rc = flex ? launch_slab<0>(a, p, best_mt, best_R, stream)
                 : (BN == 64) ? launch_slab<64>(a, p, best_mt, best_R, stream) : launch_slab<128>(a, p, best_mt, best_R, stream);
+  if (rc == B2_OK) set_last_kernel(KID_SLAB, BN, best_mt, flex, p.wchunks, a != a_in);
   return rc == B2_OK ? 1 : rc;
 }
 
@@ -431,7 +439,7 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------
 // temporal-group slab kernel (b2_slabts.cuh): 3 x kh x kw stride-1 "same" convolutions with <= 64 output channels
 // ------------------------------------------------------------------------------------------
-static int g_slabts = -1;     // B2_SLABTS=0 disables (A/B measurements)
+static int g_slabts = -1;     // -1: read B2_SLABTS (0 disables, for A/B measurements) on the next call; 0 never; 1 when eligible
 static int try_slabts(const b2_conv_args* a, cudaStream_t stream) {
   if (g_slabts < 0) { const char* e = getenv("B2_SLABTS"); g_slabts = (e && e[0] == '0') ? 0 : 1; }
   if (!g_slabts || g_conv_algo != 0) return 0;
@@ -480,6 +488,7 @@ static int try_slabts(const b2_conv_args* a, cudaStream_t stream) {
   const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
   B2_CHECK_CUDA(launch_pdl(slabts_kernel, dim3(grid), dim3(kSlabThreads), (size_t)smem, stream, tmX, tmB, p));
   B2_CHECK_LAUNCH("slabts_kernel");
+  set_last_kernel(KID_SLABTS);
   return 1;
 }
 
@@ -536,6 +545,7 @@ static int try_tstack(const b2_conv_args* a, cudaStream_t stream) {
   B2_CHECK_CUDA(launch_pdl(tstack_kernel, dim3(grid), dim3(kTkThreads), smem, stream, tmX, tmB, p));
   B2_CHECK_LAUNCH("tstack_kernel");
   g_last_conv_path = 1;
+  set_last_kernel(KID_TSTACK);
   return 1;
 }
 
@@ -646,6 +656,7 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error(B2_ERR_CUDA, "cuTensorMapEncodeTiled(stem) failed (%d)", (int)r);
   g_last_stem_rows = p.G;
+  set_last_kernel(KID_STEM, p.G);
   if constexpr (BN == 128) return launch_stem_g<128, 1>(stream, p, tmX, smem_bytes);
   else return p.G == 4 ? launch_stem_g<64, 4>(stream, p, tmX, smem_bytes) : launch_stem_g<64, 2>(stream, p, tmX, smem_bytes);
 }
@@ -696,6 +707,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   dim3 grid((p.epi == EPI_TMA_F16 ? (p.ldy + BN - 1) / BN : (p.Ncols + BN - 1) / BN), (p.M_total + kBM - 1) / kBM, 1);
   B2_CHECK_CUDA(launch_pdl(igemm_kernel<BN, MASK>, grid, dim3(kThreads), S::kTotalBytes, stream, tmA, tmB, tmC, tmR, p));
   B2_CHECK_LAUNCH("igemm_kernel");
+  set_last_kernel(KID_IGEMM, BN, MASK);
   return B2_OK;
 }
 
@@ -790,6 +802,7 @@ static int launch_densem(const IgemmLaunch& L, cudaStream_t stream) {
   cfg.attrs = attr; cfg.numAttrs = 2;
   B2_CHECK_CUDA(cudaLaunchKernelEx(&cfg, densem_kernel, tmA, tmB, dp));
   B2_CHECK_LAUNCH("densem_kernel");
+  set_last_kernel(KID_DENSEM, bn, S);
   return B2_OK;
 }
 
@@ -854,6 +867,7 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
   const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
   B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, GAN, MASK>, dim3(grid), dim3(GAN ? kPgThreadsGan : kPgThreads), S::kTotal, stream, tmA, tmB, tmA2, tmB2, tmC, tmR, tmC2, p));
   B2_CHECK_LAUNCH("pgemm_kernel");
+  set_last_kernel(KID_PGEMM, BN, MASK);
   return B2_OK;
 }
 
@@ -963,6 +977,15 @@ int b2_debug_last_gemm_path(void) { return g_last_gemm_path; }   /* 1 dense-M, 2
 int b2_debug_set_tstack(int mode) { g_tstack = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }   /* temporal stack kernel: -1 rule, 0 never, 1 whenever eligible */
 int b2_debug_set_slab_mt(int mt) { g_slab_force_mt = mt < 0 ? 0 : mt; return B2_OK; }
 int b2_debug_set_densem(int maxm, int force_s) { g_densem_maxm = maxm < 0 ? -2 : maxm; g_densem_force_s = force_s; return B2_OK; }
+/* temporal-group slab kernel: -1 the rule (B2_SLABTS, read on the next call), 0 never, 1 whenever the shape is eligible */
+int b2_debug_set_slabts(int mode) { g_slabts = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }
+/* kernel of the last convolution / GEMM / attention call (a KID_* id of b2_host.h, 0 when the call launched nothing) and its
+   tile parameters in info[0..4]: slab {BN, MT, flex, wchunks, remapped}, densem {bn, S}, pgemm / igemm {BN, masked}, stem {G},
+   attention {online, DVT}; unused entries are 0 */
+int b2_debug_last_kernel(int* info) {
+  if (info) memcpy(info, g_last_info, sizeof(g_last_info));
+  return g_last_kernel;
+}
 const char* b2_last_error(void) { return g_err; }
 uint64_t b2_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
@@ -1010,6 +1033,7 @@ static int validate_conv(const b2_conv_args* a) {
 }
 
 int b2_conv_ndhwc_fprop(const b2_conv_args* a, void* stream) {
+  set_last_kernel(KID_NONE);
   int rc = validate_conv(a);
   if (rc != B2_OK) return rc;
   if ((rc = require_sm90()) != B2_OK) return rc;
@@ -1111,6 +1135,7 @@ int b2_gemm2_f16(const b2_gemm_args* g, const void* a2, int lda2, const void* b2
 }
 
 static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream) {
+  set_last_kernel(KID_NONE);
   B2_CHECK_ARG(g != nullptr, "null args");
   B2_CHECK_ARG(g->a && g->b && g->scale && g->shift && g->d, "null tensor pointer");
   B2_CHECK_ARG(g->M > 0 && g->N > 0 && g->Kd > 0, "non-positive dimension");

@@ -72,6 +72,14 @@ int make_tmap_ndhwc_5d(CUtensorMap* out, const void* base, uint64_t C, uint64_t 
 
 int require_sm90();
 
+// Which kernel the last b2_conv_ndhwc_fprop(_simt), GEMM or attention call launched, with that launch's tile parameters
+// (b2_debug_last_kernel: tests pin the variant a case exercised, so a dispatch change cannot silently move its coverage).
+enum LastKernel : int {
+  KID_NONE = 0, KID_STEM = 1, KID_SLAB = 2, KID_SLABTS = 3, KID_TSTACK = 4, KID_DENSEM = 5, KID_PGEMM = 6, KID_IGEMM = 7,
+  KID_SIMT = 8, KID_ATTENTION = 9
+};
+void set_last_kernel(int id, int i0 = 0, int i1 = 0, int i2 = 0, int i3 = 0, int i4 = 0);
+
 // Launch with programmatic stream serialization (see pdl_wait() in b2_ptx.cuh).  B2_PDL=0 in the environment turns
 // the attribute off (A/B measurements).
 bool pdl_enabled();
