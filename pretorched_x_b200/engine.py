@@ -46,13 +46,61 @@ def _bn_tensors(bn):
     return (bn.weight, bn.bias, bn.running_mean, bn.running_var)
 
 
-def _cached(owner, slot, sig, build):
+def _reads_trainable(owner, reads):
+    """True when a pack built on ``owner`` reads a tensor with ``requires_grad``: a parameter of the owner (itself or its
+    children) or one of ``reads`` (e.g. the BatchNorm a convolution's pack folds)."""
+    return (any(t is not None and t.requires_grad for t in reads)
+            or (isinstance(owner, nn.Module) and any(p.requires_grad for p in owner.parameters())))
+
+
+# A CUDA-graph replay of an optimizer step (graph.GraphedFineTuneStep) changes the trainable parameters on the device
+# without advancing their host-side ``_version``, so the cache key alone cannot see it.  Two rules cover it:
+# * while a step is captured (``repack_trainable``), every pack that reads a trainable tensor is rebuilt on each call -- the
+#   build becomes part of the graph and reads the live parameters at every replay -- and is not stored (it lives in the
+#   graph's memory pool);
+# * a pack that reads a trainable tensor is stored with the current parameter epoch and only reused within it;
+#   ``parameters_changed()`` (called after every replay) starts a new epoch.
+# Packs of frozen tensors ignore both: they are built once and kept.
+_REPACK_TRAINABLE = False
+_EPOCH = 0
+
+
+class repack_trainable:
+    """``with engine.repack_trainable(): ...`` -- packs that read a trainable tensor bypass the packed-parameter cache."""
+
+    def __enter__(self):
+        global _REPACK_TRAINABLE
+        self.prev, _REPACK_TRAINABLE = _REPACK_TRAINABLE, True
+        return self
+
+    def __exit__(self, *exc):
+        global _REPACK_TRAINABLE
+        _REPACK_TRAINABLE = self.prev
+        return False
+
+
+def repacking_trainable():
+    return _REPACK_TRAINABLE
+
+
+def parameters_changed():
+    """Trainable parameters changed without a host-side version bump: every cached pack that reads a trainable tensor is
+    rebuilt at its next use; packs of frozen tensors stay."""
+    global _EPOCH
+    _EPOCH += 1
+
+
+def _cached(owner, slot, sig, build, reads=()):
+    """Cached ``build()`` on ``owner`` under key ``sig``.  ``reads``: tensors the pack folds that are not parameters of
+    ``owner`` (they decide, with the owner's own parameters, whether the pack follows trainable tensors)."""
+    if _REPACK_TRAINABLE and _reads_trainable(owner, reads):
+        return build()
     cache = owner.__dict__.setdefault("_b2_cache", {})
     hit = cache.get(slot)
-    if hit is not None and hit[0] == sig:
+    if hit is not None and hit[0] == sig and hit[2] in (None, _EPOCH):
         return hit[1]
     val = build()
-    cache[slot] = (sig, val)
+    cache[slot] = (sig, val, _EPOCH if _reads_trainable(owner, reads) else None)
     return val
 
 
@@ -107,7 +155,7 @@ def packed_conv(conv, bn, in_pitch, stem=False, stride=None):
     # grouped convolution (ResNeXt-3D, resnext3D.py:86-93): packed as the block-diagonal dense filter, see ops.dense_from_grouped
     return _cached(conv, "pc", sig,
                    lambda: ops.PackedConv(ops.dense_from_grouped(conv.weight.detach(), conv.groups), conv.bias, bn, stride, padding,
-                                          in_pitch=in_pitch, stem=stem))
+                                          in_pitch=in_pitch, stem=stem), reads=_bn_tensors(bn))
 
 
 def _is_stem_shape(conv):
@@ -434,7 +482,7 @@ def depthwise_bn_relu6(conv, bn, a, clamp_in=True, out=None):
         w9 = conv.weight.detach().reshape(C, 9).t().float().contiguous()
         return (w9,) + ops.fold_affine(C, conv.bias, bn, dev)
 
-    w9, scale, shift = _cached(conv, "dw", _sig(conv.weight, conv.bias, *_bn_tensors(bn)), build)
+    w9, scale, shift = _cached(conv, "dw", _sig(conv.weight, conv.bias, *_bn_tensors(bn)), build, reads=_bn_tensors(bn))
     return ops.dwconv3x3(a, w9, scale, shift, stride[1], clamp_in=clamp_in, out=out)
 
 

@@ -4,8 +4,13 @@ A forward of resnet3d50 is ~75 kernel launches, each preceded by a Python -> cty
 CUtensorMap encode; at H100 speeds that host work is comparable to the device time.  Capturing the launch
 sequence once (static shapes, buffers from the graph's private pool) removes it: the timed step is one
 ``cudaGraphLaunch``.  All C-ABI entry points are capture-safe (no syncs, no allocations).
+
+``GraphedFineTuneStep`` does the same for a whole fine-tuning step: forward, loss, backward and optimizer update.
 """
+import numpy as np
 import torch
+
+from . import engine, ops
 
 
 class GraphedForward:
@@ -90,3 +95,140 @@ class PipelinedForward:
     def drain(self):
         self.compute_stream.synchronize()
         self.copy_stream.synchronize()
+
+
+def _check_optimizer(optimizer):
+    """Refuse optimizers whose step keeps host-side state a graph would freeze."""
+    if isinstance(optimizer, (torch.optim.Adam, torch.optim.AdamW)):
+        if not all(g.get("capturable", False) for g in optimizer.param_groups):
+            raise ValueError("GraphedFineTuneStep: %s must be built with capturable=True (its step count then lives on the "
+                             "device)" % type(optimizer).__name__)
+    elif not isinstance(optimizer, torch.optim.SGD):
+        raise TypeError("GraphedFineTuneStep supports torch.optim.SGD and Adam / AdamW(capturable=True), got %s"
+                        % type(optimizer).__name__)
+
+
+def _snapshot(trainable, optimizer):
+    return ([p.detach().clone() for p in trainable],
+            {p: {k: v.clone() if torch.is_tensor(v) else v for k, v in st.items()} for p, st in optimizer.state.items()})
+
+
+def _restore(trainable, optimizer, saved):
+    """Put the parameters and the optimizer state back as ``_snapshot`` found them, in place (the graph keeps the addresses).
+    State the warm-up created is zeroed: zero momentum / moment buffers and a zero step count are the fresh state."""
+    params, state = saved
+    with torch.no_grad():
+        for p, v in zip(trainable, params):
+            p.copy_(v)
+        for p, st in optimizer.state.items():
+            old = state.get(p, {})
+            for k, v in st.items():
+                if torch.is_tensor(v):
+                    v.copy_(old[k]) if k in old else v.zero_()
+                elif k in old:
+                    st[k] = old[k]
+            if isinstance(optimizer, torch.optim.SGD) and "momentum_buffer" in st and "momentum_buffer" not in old:
+                group = next(g for g in optimizer.param_groups if any(q is p for q in g["params"]))
+                if group["dampening"] != 0:
+                    raise ValueError("GraphedFineTuneStep: SGD with dampening starts its momentum buffer from the first gradient, "
+                                     "which a graph cannot do: take one eager step before capturing")
+
+
+class GraphedFineTuneStep:
+    """One fine-tuning step -- forward, ``loss_fn``, backward and ``optimizer.step()`` -- captured once and replayed.
+
+    ``s = GraphedFineTuneStep(model, optimizer, loss_fn, example_input, example_target); loss = s(x, target)``: each call
+    copies ``x`` / ``target`` (same shapes and dtypes as the examples; device or pinned host) into the static buffers, replays
+    the step and returns the static fp32 loss tensor, overwritten by the next call.
+
+    Models: those with ``fine_tune(k)`` (``ResNet3D``, ``ResNet2D``, ``TRN``) and frozen-trunk models with a trainable
+    ``nn.Linear`` head.  The model stays in ``eval()`` (frozen BatchNorm); a model in ``train()`` mode is refused.
+
+    Capture follows torch's whole-network recipe: ``warmup`` eager steps on a side stream, then the capture with the gradients
+    allocated in the graph's pool -- after construction ``p.grad`` of every trainable parameter is a static tensor the
+    replays rewrite.  The warm-up steps do not count: the parameters, the optimizer state and NumPy's global RNG are put
+    back as they were, so the first replay is the first step.  While the step is captured every module that owns a trainable
+    parameter, and every convolution whose folded BatchNorm is trainable, rebuilds its packed filter / folded affine on each
+    call (``engine.repack_trainable``), so each replay packs the live parameters; packs of frozen tensors stay cached.  Every
+    replay starts a new parameter epoch (``engine.parameters_changed``), so an eager forward never reuses a pack of trainable
+    tensors made before the replay.  In-place edits of a trainable parameter (``with torch.no_grad(): p.mul_(0.5)``) reach
+    the next replay; an edit of a frozen one does not (its pack is part of the graph).  The trainable set is fixed at capture:
+    a call after ``requires_grad`` of a parameter changed raises.
+
+    Optimizers: ``torch.optim.SGD`` (with or without momentum, Nesterov, weight decay; with dampening only when the momentum
+    buffers already exist) and ``Adam`` / ``AdamW`` built with ``capturable=True``; anything else raises.  A Python-float
+    learning rate is baked into the graph: changing ``param_groups[i]['lr']`` afterwards has no effect -- capture again, or
+    give the optimizer a tensor ``lr``.  Learning-rate schedules are not captured.
+
+    TRN's ``MultiScaleRelation`` draws its frame tuples on the host (``np.random``, as the reference does); each call draws
+    them for that step and writes them into the relation's persistent tuple table before the replay, so seeding NumPy the
+    same way before an eager step and before a call gives both the same tuples.
+
+    The capture runs eager steps and synchronises: it cannot run inside ``ops.profile()``.
+    """
+
+    def __init__(self, model, optimizer, loss_fn, example_input, example_target, warmup=2):
+        if model.training:
+            raise RuntimeError("GraphedFineTuneStep: the engine trains with frozen BatchNorm -- call model.eval() first")
+        if ops._PROFILE is not None:
+            raise RuntimeError("GraphedFineTuneStep cannot capture inside ops.profile(): its per-launch events would be "
+                               "captured and its exit synchronises")
+        if not (example_input.is_cuda and example_target.is_cuda):
+            raise RuntimeError("GraphedFineTuneStep needs CUDA example tensors: the engine has no CPU path")
+        _check_optimizer(optimizer)
+        self.model, self.optimizer = model, optimizer
+        self.trainable = [p for p in model.parameters() if p.requires_grad]
+        if not self.trainable:
+            raise ValueError("GraphedFineTuneStep: the model has no trainable parameter (call fine_tune(k) or unfreeze a head)")
+        self._params = list(model.parameters())
+        self._trainable_mask = [p.requires_grad for p in self._params]
+        self.relations = [m for m in model.modules() if hasattr(m, "sample_tuples") and hasattr(m, "upload_tuples")]
+        self.static_input = example_input.detach().clone()
+        self.static_target = example_target.detach().clone()
+
+        def step():
+            optimizer.zero_grad(set_to_none=True)
+            loss = loss_fn(model(self.static_input), self.static_target)
+            loss.backward()
+            optimizer.step()
+            return loss
+
+        np_state = np.random.get_state()
+        saved = _snapshot(self.trainable, optimizer)
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(max(1, warmup)):      # packs frozen weights, creates the optimizer state, warms the allocator
+                step()
+        torch.cuda.current_stream().wait_stream(side)
+        _restore(self.trainable, optimizer, saved)
+        del saved
+        optimizer.zero_grad(set_to_none=True)    # the captured backward allocates the gradients in the graph's pool
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        with engine.repack_trainable(), torch.cuda.graph(self.graph):
+            self.static_loss = step().detach()   # keeps no autograd node of the captured step alive
+        engine.parameters_changed()
+        np.random.set_state(np_state)
+
+    @staticmethod
+    def _load(dst, src, what):
+        if tuple(src.shape) != tuple(dst.shape) or src.dtype != dst.dtype:
+            raise ValueError("GraphedFineTuneStep was captured for a %s of %s %s, got %s %s" % (what, tuple(dst.shape), dst.dtype,
+                                                                                             tuple(src.shape), src.dtype))
+        if src.data_ptr() != dst.data_ptr():
+            dst.copy_(src, non_blocking=True)
+
+    def __call__(self, x=None, target=None):
+        if [p.requires_grad for p in self._params] != self._trainable_mask:
+            raise RuntimeError("GraphedFineTuneStep: requires_grad of a parameter changed since the capture; the graph still "
+                               "trains the parameters that were trainable then -- build a new GraphedFineTuneStep")
+        if x is not None:
+            self._load(self.static_input, x, "input")
+        if target is not None:
+            self._load(self.static_target, target, "target")
+        for rel in self.relations:
+            rel.upload_tuples(rel.sample_tuples(), self.static_input.device)
+        self.graph.replay()
+        engine.parameters_changed()
+        return self.static_loss

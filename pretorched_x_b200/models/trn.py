@@ -84,6 +84,7 @@ class MultiScaleRelation(engine.CacheOwner, nn.Module):
         self._offsets = np.cumsum([0] + [n * s for n, s in zip(self.subsample_scales, self.scales)]).tolist()
         self._host_table = None
         self._dev_table = None
+        self._copied = None             # CUDA event after the last copy out of the pinned table
 
     def return_relationset(self, num_input, num_input_relation):
         return list(itertools.combinations(range(num_input), num_input_relation))
@@ -99,15 +100,35 @@ class MultiScaleRelation(engine.CacheOwner, nn.Module):
 
     def upload_tuples(self, picks, device):
         """Writes ``picks`` into the persistent device table with ONE asynchronous copy from pinned host memory.  The table
-        keeps its address, so a CUDA graph captured over ``forward_tuples`` is replayable: draw new tuples, call this, replay."""
+        keeps its address, so a CUDA graph captured over ``forward_tuples`` is replayable: draw new tuples, call this, replay.
+        Outside a capture the host waits until the previous copy out of the pinned table has run before rewriting it (normally
+        long finished: it was enqueued one forward earlier); without that wait a host running ahead of the device could
+        overwrite tuples another forward has not copied yet.  The pinned table keeps one address because a graph captured
+        over a whole forward copies from it at every replay."""
         flat = [f for tuples in picks for tup in tuples for f in tup]
         if self._host_table is None or self._dev_table is None or self._dev_table.device != device:
             self._host_table = torch.empty(self._offsets[-1], dtype=torch.int32).pin_memory() if device.type == "cuda" \
                 else torch.empty(self._offsets[-1], dtype=torch.int32)
             self._dev_table = torch.empty(self._offsets[-1], dtype=torch.int32, device=device)
+            self._copied = None
+        capturing = device.type == "cuda" and torch.cuda.is_current_stream_capturing()
+        if self._copied is not None and not capturing:
+            self._copied.synchronize()
         self._host_table.copy_(torch.tensor(flat, dtype=torch.int32))
         self._dev_table.copy_(self._host_table, non_blocking=True)
+        if device.type == "cuda" and not capturing:
+            self._copied = torch.cuda.Event()
+            self._copied.record()
         return self._dev_table
+
+    def _tuple_table(self, picks, device):
+        """The device table for this forward.  While a training step is captured (graph.GraphedFineTuneStep) the table is
+        used as it stands: the step runner uploads freshly drawn tuples before every replay."""
+        if engine.repacking_trainable() and device.type == "cuda" and torch.cuda.is_current_stream_capturing():
+            if self._dev_table is None or self._dev_table.device != device:
+                raise RuntimeError("MultiScaleRelation: run the step once eagerly before capturing it (no tuple table yet)")
+            return self._dev_table
+        return self.upload_tuples(picks, device)
 
     def _stacked_w2(self, rel, n):
         """Second Linear of a scale's MLP tiled ``n`` times along K, bias scaled by ``n``: sum_t (W2 h_t + b2) in one GEMM."""
@@ -142,17 +163,24 @@ class MultiScaleRelation(engine.CacheOwner, nn.Module):
         rows = feats.shape[0]
         picks = self.sample_tuples()
         if _wants_grad(self, input):
-            # differentiable path: per tuple, through LinearFunction (indexing and the sum are torch autograd ops)
+            # differentiable path: per tuple, through LinearFunction (the frame gather and the sum are torch autograd ops).
+            # The frames are picked by index views of the device table, so a captured step reads each replay's tuples.
+            # Autograd keeps those views for the backward: an eager forward takes a private copy, so that later forwards
+            # (gradient accumulation, an evaluation pass) may rewrite the persistent table before this backward runs.
+            table = self._tuple_table(picks, input.device)
+            if not (input.is_cuda and torch.cuda.is_current_stream_capturing()):
+                table = table.clone()
             total = None
-            for si, tuples in enumerate(picks):
-                for tup in tuples:
-                    y = self.relations[si].mlp_grad(feats[:, list(tup), :].reshape(rows, -1).float())
+            for si, s in enumerate(self.scales):
+                for j in range(self.subsample_scales[si]):
+                    idx = table[self._offsets[si] + j * s:self._offsets[si] + (j + 1) * s]
+                    y = self.relations[si].mlp_grad(feats.index_select(1, idx).reshape(rows, -1).float())
                     total = y if total is None else total + y
             return total.view(input.size(0), -1, self.out_features)
         x16 = ops.cast_rows(feats.view(rows, -1), relu=True).view(rows, self.num_input, -1)
         if x16.shape[2] != self.in_features:
             raise ValueError("in_features must be a multiple of 8 for the fp16 frame gather")
-        table = self.upload_tuples(picks, input.device)
+        table = self._tuple_table(picks, input.device)
         total = torch.empty((rows, self.out_features), dtype=torch.float32, device=input.device)
         return self.forward_tuples(x16, table, total).view(input.size(0), -1, self.out_features)
 

@@ -2,14 +2,18 @@
 """Time one fine-tuning step (forward + backward + SGD step) of resnet3d50 on the engine and on torch's own fp16 cuDNN
 autograd, in the same process on the same card.
 
-    python tools/bench_finetune.py [--batch 32] [--frames 16] [--size 224] [--ks 4,3] [--steps 10] [--warmup 3]
+    python tools/bench_finetune.py [--batch 32] [--frames 16] [--size 224] [--ks 4,3] [--steps 10] [--warmup 3] [--graph]
 
 Engine: ``get_fine_tuning_parameters(model, k)`` + SGD, eval-mode (frozen) BatchNorm.  Baseline: ``oracle.functional.forward``
 on fp16 CUDA copies of the same parameters (the same ones trainable), input and filters in ``channels_last_3d``,
 ``cudnn.benchmark`` on, SGD on the fp16 trainable parameters.  Both timed with CUDA events over ``--steps`` steps after
 ``--warmup`` steps.  A separate profiled engine step reports the share of the backward time spent in the weight-gradient
 kernel (CUDA events around every library launch, ``ops.profile``).  The card name and power limit are read in the same run.
-Prints one JSON line.  Needs an H100; there is no CPU fallback."""
+Prints one JSON line.  Needs an H100; there is no CPU fallback.
+
+``--graph``: instead, the same engine step run eagerly and as a replay of one CUDA graph (``graph.GraphedFineTuneStep``) on
+the same model and optimizer, timed alternately (``--rounds`` rounds of ``--steps`` steps each, median reported), and the
+device time the replayed step spends re-packing the trainable filters (``repack_cost``)."""
 import argparse
 import json
 import os
@@ -23,7 +27,8 @@ import torch  # noqa: E402
 import torch.nn.functional as F  # noqa: E402
 
 import pretorched_x_b200 as P  # noqa: E402
-from pretorched_x_b200 import ops  # noqa: E402
+from pretorched_x_b200 import engine, ops  # noqa: E402
+from pretorched_x_b200.graph import GraphedFineTuneStep, GraphedForward  # noqa: E402
 from oracle import functional as OF  # noqa: E402
 
 
@@ -101,6 +106,46 @@ def torch_case(model, x, target, k, steps, warmup):
     return timed(step, steps, warmup)
 
 
+def alternate(eager_step, graphed, steps, warmup, rounds):
+    """Median ms per step of ``eager_step`` and of graph replays, timed in alternating rounds, and the per-round lists."""
+    eager_ms, graph_ms = [], []
+    for _ in range(rounds):
+        eager_ms.append(timed(eager_step, steps, warmup))
+        graph_ms.append(timed(graphed, steps, warmup))
+    med = lambda v: sorted(v)[len(v) // 2]
+    return dict(eager_ms_per_step=round(med(eager_ms), 3), graph_ms_per_step=round(med(graph_ms), 3),
+                graph_speedup=round(med(eager_ms) / med(graph_ms), 3),
+                eager_ms_rounds=[round(v, 3) for v in eager_ms], graph_ms_rounds=[round(v, 3) for v in graph_ms])
+
+
+def repack_cost(model, x, steps, warmup):
+    """Device cost of re-packing the trainable modules' filters and BatchNorm affines, as the captured step does at every
+    replay: a no-grad forward replayed from a graph with cached packs against one captured under ``engine.repack_trainable``."""
+    cached = GraphedForward(model, x)
+    with engine.repack_trainable():
+        repacked = GraphedForward(model, x)
+    a, b = timed(cached, steps, warmup), timed(repacked, steps, warmup)
+    del cached, repacked
+    return dict(forward_graph_ms=round(a, 3), forward_graph_repacking_ms=round(b, 3), repack_ms=round(b - a, 3))
+
+
+def graph_case(x, target, k, steps, warmup, rounds):
+    torch.manual_seed(0)
+    model = OF.randomize_bn_(P.resnet3d50(num_classes=400, pretrained=None), 1).eval().cuda()
+    opt = torch.optim.SGD(P.models.resnet3d.get_fine_tuning_parameters(model, k), lr=1e-5, momentum=0.9)
+
+    def step():
+        opt.zero_grad(set_to_none=True)
+        F.cross_entropy(model(x), target).backward()
+        opt.step()
+
+    graphed = GraphedFineTuneStep(model, opt, F.cross_entropy, x, target)
+    row = dict(k=k, **alternate(step, graphed, steps, warmup, rounds))
+    row.update(repack_cost(model, x, steps, warmup))
+    row["repack_share_of_replayed_step"] = round(row["repack_ms"] / row["graph_ms_per_step"], 4)
+    return row
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=32)
@@ -110,12 +155,23 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--no-torch", action="store_true", help="skip the cuDNN baseline")
+    ap.add_argument("--graph", action="store_true", help="eager steps against CUDA-graph replays of the step")
+    ap.add_argument("--rounds", type=int, default=5, help="--graph: alternating rounds")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_finetune needs an H100 (no GPU found)")
     name, power = card()
     x = torch.randn((args.batch, 3, args.frames, args.size, args.size), generator=torch.Generator().manual_seed(1)).cuda()
     target = torch.randint(0, 400, (args.batch,), generator=torch.Generator().manual_seed(2)).cuda()
+    if args.graph:
+        rows = []
+        for k in [int(v) for v in args.ks.split(",")]:
+            rows.append(graph_case(x, target, k, args.steps, args.warmup, args.rounds))
+            torch.cuda.empty_cache()
+        print(json.dumps(dict(metric="ms per fine-tuning step (forward + backward + SGD step), eager vs CUDA-graph replay",
+                              model="resnet3d50", input=[args.batch, 3, args.frames, args.size, args.size], steps=args.steps,
+                              warmup=args.warmup, rounds=args.rounds, gpu=name, power_limit=power, results=rows)))
+        return
     rows = []
     for k in [int(v) for v in args.ks.split(",")]:
         ms, bwd_ms, wgrad_ms, by_kind, model = engine_case(x, target, k, args.steps, args.warmup)

@@ -2,7 +2,7 @@
 """Time one fine-tuning step (forward + backward + SGD step) of TRN-MSTRN on a resnet50 backbone on the engine and on torch's
 own fp16 cuDNN autograd, in the same process on the same card.
 
-    python tools/bench_finetune_trn.py [--batch 16] [--segments 8] [--size 224] [--ks 4,3] [--steps 10] [--warmup 3]
+    python tools/bench_finetune_trn.py [--batch 16] [--segments 8] [--size 224] [--ks 4,3] [--steps 10] [--warmup 3] [--graph]
 
 Engine: ``TRN(339, arch='resnet50', consensus='MSTRN').fine_tune(k)`` + SGD on the trainable parameters (the backbone's
 ``layer{k}..layer4``, the relation and the final Linear), eval-mode (frozen) BatchNorm.  Baseline:
@@ -11,7 +11,12 @@ Engine: ``TRN(339, arch='resnet50', consensus='MSTRN').fine_tune(k)`` + SGD on t
 NumPy's global RNG the same way.  Both timed with CUDA events over ``--steps`` steps after ``--warmup`` steps.  A separate
 profiled engine step reports the share of the backward time spent in the weight-gradient kernel (CUDA events around every
 library launch, ``ops.profile``).  The card name and power limit are read in the same run.  Prints one JSON line.  Needs an
-H100; there is no CPU fallback."""
+H100; there is no CPU fallback.
+
+``--graph``: instead, the same engine step run eagerly and as a replay of one CUDA graph (``graph.GraphedFineTuneStep``, which
+draws the frame tuples of every replay on the host like the eager forward) on the same model and optimizer, timed alternately
+(``--rounds`` rounds of ``--steps`` steps each, median reported), and the device time the replayed step spends re-packing the
+trainable filters (``bench_finetune.repack_cost``)."""
 import argparse
 import json
 import os
@@ -28,7 +33,8 @@ import torch.nn.functional as F  # noqa: E402
 import pretorched_x_b200 as P  # noqa: E402
 from pretorched_x_b200 import ops  # noqa: E402
 from oracle import functional as OF  # noqa: E402
-from bench_finetune import card, timed  # noqa: E402
+from pretorched_x_b200.graph import GraphedFineTuneStep  # noqa: E402
+from bench_finetune import alternate, card, repack_cost, timed  # noqa: E402
 
 NUM_CLASSES = 339
 
@@ -60,6 +66,25 @@ def engine_case(x, target, k, segments, steps, warmup):
     for r in prof.rows:
         by_kind[r["kind"]] = by_kind.get(r["kind"], 0.0) + r["ms"]
     return ms, bwd_ms, wgrad_ms, by_kind, model
+
+
+def graph_case(x, target, k, segments, steps, warmup, rounds):
+    torch.manual_seed(0)
+    model = P.TRN(NUM_CLASSES, num_segments=segments, arch="resnet50", consensus="MSTRN", pretrained=None)
+    model = OF.randomize_bn_(model, 1).eval().cuda().fine_tune(k)
+    opt = torch.optim.SGD([p for p in model.parameters() if p.requires_grad], lr=1e-5, momentum=0.9)
+    np.random.seed(0)
+
+    def step():
+        opt.zero_grad(set_to_none=True)
+        F.cross_entropy(model(x), target).backward()
+        opt.step()
+
+    graphed = GraphedFineTuneStep(model, opt, F.cross_entropy, x, target)
+    row = dict(k=k, **alternate(step, graphed, steps, warmup, rounds))
+    row.update(repack_cost(model, x, steps, warmup))
+    row["repack_share_of_replayed_step"] = round(row["repack_ms"] / row["graph_ms_per_step"], 4)
+    return row
 
 
 def torch_case(model, x, target, segments, steps, warmup):
@@ -94,6 +119,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--no-torch", action="store_true", help="skip the cuDNN baseline")
+    ap.add_argument("--graph", action="store_true", help="eager steps against CUDA-graph replays of the step")
+    ap.add_argument("--rounds", type=int, default=5, help="--graph: alternating rounds")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_finetune_trn needs an H100 (no GPU found)")
@@ -101,6 +128,15 @@ def main():
     shape = (args.batch, args.segments, 3, args.size, args.size)
     x = torch.randn(shape, generator=torch.Generator().manual_seed(1)).cuda()
     target = torch.randint(0, NUM_CLASSES, (args.batch,), generator=torch.Generator().manual_seed(2)).cuda()
+    if args.graph:
+        rows = []
+        for k in [int(v) for v in args.ks.split(",")]:
+            rows.append(graph_case(x, target, k, args.segments, args.steps, args.warmup, args.rounds))
+            torch.cuda.empty_cache()
+        print(json.dumps(dict(metric="ms per fine-tuning step (forward + backward + SGD step), eager vs CUDA-graph replay",
+                              model="TRN-MSTRN resnet50", input=list(shape), steps=args.steps, warmup=args.warmup,
+                              rounds=args.rounds, gpu=name, power_limit=power, results=rows)))
+        return
     rows = []
     for k in [int(v) for v in args.ks.split(",")]:
         ms, bwd_ms, wgrad_ms, by_kind, model = engine_case(x, target, k, args.segments, args.steps, args.warmup)
