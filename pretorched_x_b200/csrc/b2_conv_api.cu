@@ -10,7 +10,6 @@
 #include "b2_densem.cuh"
 #include "b2_pgemm.cuh"
 #include "b2_slabconv.cuh"
-#include "b2_slabts.cuh"
 #include "b2_tstack.cuh"
 #include "b2_stemconv.cuh"
 
@@ -257,6 +256,15 @@ static bool slab_geometry(const b2_conv_args* a, SlabParams* p, int wc_hint) {
   return p->n_sub > 0 && p->PW <= 256;
 }
 
+template <int BNT, int TMT>
+static int run_slab(int grid, int smem_bytes, const CUtensorMap& tmX, const CUtensorMap& tmB, const SlabParams& p, cudaStream_t stream) {
+  auto kernel = slabconv_kernel<BNT, TMT>;
+  B2_OPT_IN_SMEM(kernel, 227 * 1024);
+  B2_CHECK_CUDA(launch_pdl(kernel, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
+  B2_CHECK_LAUNCH("slabconv_kernel");
+  return B2_OK;
+}
+
 template <int BNT>   // BNT = 0: runtime N tile p.bn (set by the caller)
 static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cudaStream_t stream) {
   if (BNT) { p.bn = BNT; p.wbytes = BNT * 128; p.accs = BNT; }
@@ -291,7 +299,6 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
     return set_error(B2_ERR_INVALID, "per-sample scale/shift must be 16-byte aligned with a pitch that is a multiple of 4 floats");
   const int smem_bytes = kSlabSStages * p.slab_bytes + kSlabWStages * p.wbytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 +
                          acc_bytes(MT * p.accs);
-  B2_OPT_IN_SMEM(slabconv_kernel<BNT>, 227 * 1024);
   CUtensorMap tmX, tmB;
   int rc;
   const int taps = p.up ? 16 : a->kt * a->kh * a->kw;
@@ -301,9 +308,12 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   if ((rc = make_tmap_2d_f16(&tmB, a->w, (uint64_t)taps * a->C, (uint64_t)a->K, (uint64_t)taps * a->C, 64, BN, true)) != B2_OK)
     return rc;
   const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
-  B2_CHECK_CUDA(launch_pdl(slabconv_kernel<BNT>, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
-  B2_CHECK_LAUNCH("slabconv_kernel");
-  return B2_OK;
+  // the 64-wide tile's MMA form (b2_slabconv.cuh): one N = 128 MMA over a warpgroup's two chunks, otherwise one per chunk.  (MT = 3
+  // is never planned outside multi-plane items: its 192-column accumulator tile and two slabs of 384 positions plus halo exceed
+  // 227 KB.)
+  if constexpr (BNT == 64)
+    if (p.mp <= 1 && MT == 2) return run_slab<64, 2>(grid, smem_bytes, tmX, tmB, p, stream);
+  return run_slab<BNT, 0>(grid, smem_bytes, tmX, tmB, p, stream);
 }
 
 // Picks the N tile (fixed 64 / 128 or runtime), the M tiles per work item and the slab rows for a geometry; *best_mt == 0
@@ -435,62 +445,6 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream) {
   return rc == B2_OK ? 1 : rc;
 }
 
-
-// ------------------------------------------------------------------------------------------
-// temporal-group slab kernel (b2_slabts.cuh): 3 x kh x kw stride-1 "same" convolutions with <= 64 output channels
-// ------------------------------------------------------------------------------------------
-static int g_slabts = -1;     // -1: read B2_SLABTS (0 disables, for A/B measurements) on the next call; 0 never; 1 when eligible
-static int try_slabts(const b2_conv_args* a, cudaStream_t stream) {
-  if (g_slabts < 0) { const char* e = getenv("B2_SLABTS"); g_slabts = (e && e[0] == '0') ? 0 : 1; }
-  if (!g_slabts || g_conv_algo != 0) return 0;
-  if (a->mode != B2_CONV_AUTO || a->out_f32 || a->upsample || a->aff_ld || a->y2 || a->residual_up || a->residual_pre || a->in_scale) return 0;
-  if (a->kt != 3 || a->st != 1 || a->pt != 1 || a->sh != 1 || a->sw != 1 || a->ldy > 64 || a->T < 3) return 0;
-  // The operand traffic it saves in shared memory comes back as 2.5x more weight bytes per output tile from L2 (one 24 KB stack per
-  // tap and input frame), the single accumulator set exposes a residual read, and with a 1x1 in-plane filter the frames-as-rows remap
-  // of the slab kernel has less to gain from.  So: true 3-D filters without a residual only.
-  if (a->kh * a->kw < 9 || a->residual) return 0;
-  SlabParams p;
-  if (!slab_geometry(a, &p, 0) || p.n_sub != 1) return 0;
-  // one M tile per item: its 3 x 64 accumulator columns are what the consumers' registers hold (kSlabAccCols)
-  const int R = slab_rows(1, p.PW, p.reach, p.P);
-  const long long slab_b = ((long long)R * p.PW * 128 + 1023) / 1024 * 1024;
-  const long long smem = kSlabSStages * slab_b + kSlabWStages * kTsWBytes + 256 + 2 * slab_naff(a->ldy) * 4 + 1024 +
-                         acc_bytes(kTsGroup * kTsBN);
-  if (R > 256 || smem > 227 * 1024) return 0;
-  p.R = R;
-  p.planes_total = a->N * p.To;
-  p.plane_stride = R * p.PW * 128;
-  p.slab_bytes = (int)slab_b;
-  p.MT = 1; p.bn = kTsBN; p.wbytes = kTsWBytes; p.accs = kTsBN;
-  p.Ncols = a->K;
-  p.scale = a->scale; p.shift = a->shift;
-  p.residual = reinterpret_cast<const __half*>(a->residual);
-  p.ldr = a->ldr;
-  p.y = reinterpret_cast<__half*>(a->y);
-  p.ldy = a->ldy;
-  p.relu = a->relu;
-  p.naff = slab_naff(a->ldy);
-  p.tiles_n = 1;
-  p.tiles_q = (p.P + 127) / 128;
-  const int groups = (p.To + kTsGroup - 1) / kTsGroup;
-  const long long items = (long long)p.tiles_q * p.wchunks * a->N * groups;
-  if (items >= (1ll << 31)) return 0;
-  p.items_total = (int)items;
-  p.fd_tiles_n = make_fastdiv(1); p.fd_tiles_q = make_fastdiv(p.tiles_q); p.fd_wchunks = make_fastdiv(p.wchunks);
-  p.fd_To = make_fastdiv(groups); p.fd_PW = make_fastdiv(p.PW);
-  B2_OPT_IN_SMEM(slabts_kernel, 227 * 1024);
-  CUtensorMap tmX, tmB;
-  int rc;
-  const int taps = a->kt * a->kh * a->kw;
-  if ((rc = make_tmap_ndhwc_slab(&tmX, a->x, (uint64_t)a->C, (uint64_t)a->W, (uint64_t)a->H, (uint64_t)a->N * a->T, (uint32_t)p.PW,
-                                 (uint32_t)R, 1u)) != B2_OK) return rc;
-  if ((rc = make_tmap_2d_f16(&tmB, a->w, (uint64_t)taps * a->C, (uint64_t)a->K, (uint64_t)taps * a->C, 64, kTsBN, true)) != B2_OK) return rc;
-  const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
-  B2_CHECK_CUDA(launch_pdl(slabts_kernel, dim3(grid), dim3(kSlabThreads), (size_t)smem, stream, tmX, tmB, p));
-  B2_CHECK_LAUNCH("slabts_kernel");
-  set_last_kernel(KID_SLABTS);
-  return 1;
-}
 
 // ------------------------------------------------------------------------------------------
 // temporal stack kernel (b2_tstack.cuh): (kt,1,1) stride-1 "same" convolutions with <= 64 output channels, resident filter
@@ -977,8 +931,9 @@ int b2_debug_last_gemm_path(void) { return g_last_gemm_path; }   /* 1 dense-M, 2
 int b2_debug_set_tstack(int mode) { g_tstack = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }   /* temporal stack kernel: -1 rule, 0 never, 1 whenever eligible */
 int b2_debug_set_slab_mt(int mt) { g_slab_force_mt = mt < 0 ? 0 : mt; return B2_OK; }
 int b2_debug_set_densem(int maxm, int force_s) { g_densem_maxm = maxm < 0 ? -2 : maxm; g_densem_force_s = force_s; return B2_OK; }
-/* temporal-group slab kernel: -1 the rule (B2_SLABTS, read on the next call), 0 never, 1 whenever the shape is eligible */
-int b2_debug_set_slabts(int mode) { g_slabts = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }
+/* The temporal-group slab kernel this selected is gone (the slab kernel's 64-wide tile does what it was for); the entry point
+   stays for the ABI and accepts its argument with no effect. */
+int b2_debug_set_slabts(int mode) { (void)mode; return B2_OK; }
 /* kernel of the last convolution / GEMM / attention call (a KID_* id of b2_host.h, 0 when the call launched nothing) and its
    tile parameters in info[0..4]: slab {BN, MT, flex, wchunks, remapped}, densem {bn, S}, pgemm / igemm {BN, masked}, stem {G},
    attention {online, DVT}; unused entries are 0 */
@@ -1046,8 +1001,6 @@ int b2_conv_ndhwc_fprop(const b2_conv_args* a, void* stream) {
   g_last_gemm_path = 0;
   const bool skip_slab = small_m || a->mask != nullptr;     // the slab / temporal kernels have no masked epilogue
   rc = skip_slab ? 0 : try_tstack(a, reinterpret_cast<cudaStream_t>(stream));
-  if (rc != 0) return rc < 0 ? rc : B2_OK;
-  rc = skip_slab ? 0 : try_slabts(a, reinterpret_cast<cudaStream_t>(stream));
   if (rc != 0) return rc < 0 ? rc : B2_OK;
   rc = skip_slab ? 0 : try_slab(a, reinterpret_cast<cudaStream_t>(stream));
   if (rc != 0) return rc < 0 ? rc : B2_OK;

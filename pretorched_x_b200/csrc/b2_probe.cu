@@ -11,12 +11,41 @@
 //   mode 1: K-major SWIZZLE_NONE A operand built as an overlapping (Toeplitz) view of a linear buffer:
 //           row r starts at byte 16*r, K = 32 elements: LBO = 16 B, SBO = 128 B.
 //           Expected: D[r][n] = sum_{k<32} buf[8*r + k] * B[n][k].
+//   mode 3: the mode 0 question for the B operand (the slab kernel's 64-wide tile reads its slab as B): K-major SWIZZLE_128B
+//           B of N = `base_off` (64, 128 or 192) rows whose start address is shifted by `shift` rows from a 1024-byte aligned
+//           tile; A is the 64 x 64 K-major tile given as `b`, the 256 x 64 tile given as `a` holds the B rows.  Expected:
+//           D[m][n] = sum_k b[m][k] * a[shift + n][k], written to out as [64][N].
 #include "b2_host.h"
 #include "b2_ptx.cuh"
 
 #include <string.h>
 
 namespace b2 {
+
+// mode 3: one m64nNk16 chain with the accumulators in registers, fragments written straight to out[64][N]
+template <int N>
+__device__ void probe_shifted_b(uint32_t a_addr, uint32_t b_addr, float* __restrict__ out) {
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  reg_fence(d);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    wgmma_ss<N>(d, make_desc_sw128_kmajor(a_addr) + 2 * k, make_desc_sw128_kmajor(b_addr) + 2 * k);
+  wgmma_commit();
+  wgmma_wait0();
+  reg_fence(d);
+  const int t = threadIdx.x & 127;
+  const int r = (t >> 5) * 16 + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    out[r * N + 8 * j + c] = d[4 * j];
+    out[r * N + 8 * j + c + 1] = d[4 * j + 1];
+    out[(r + 8) * N + 8 * j + c] = d[4 * j + 2];
+    out[(r + 8) * N + 8 * j + c + 1] = d[4 * j + 3];
+  }
+}
 
 __global__ void __launch_bounds__(128, 1)
 mma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -34,6 +63,20 @@ mma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   __syncthreads();
 
   const int ncol = (mode == 2) ? 128 : 64;
+  if (mode == 3) {
+    if (tid == 0) {
+      mbar_expect_tx(bar, 32768 + 8192);
+      tma_load_2d(sA, &tmA, bar, 0, 0);
+      tma_load_2d(sA + 16384, &tmA, bar, 0, 128);
+      tma_load_2d(sB, &tmB, bar, 0, 0);
+    }
+    mbar_wait(bar, 0);
+    const uint32_t b_addr = smem_u32(sA) + shift * 128;
+    if (base_off == 64) probe_shifted_b<64>(smem_u32(sB), b_addr, out);
+    else if (base_off == 128) probe_shifted_b<128>(smem_u32(sB), b_addr, out);
+    else probe_shifted_b<192>(smem_u32(sB), b_addr, out);
+    return;
+  }
   if (mode == 0) {
     if (tid == 0) {
       mbar_expect_tx(bar, 32768 + 8192);
@@ -88,17 +131,20 @@ mma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
 using namespace b2;
 
-// a: mode 0 -> fp16 [256][64]; mode 1 -> fp16 [2048] linear.  b: mode 0 -> fp16 [64][64]; mode 1 -> fp16 [64][32].
+// a: mode 0 / 3 -> fp16 [256][64]; mode 1 -> fp16 [2048] linear.  b: mode 0 / 3 -> fp16 [64][64]; mode 1 -> fp16 [64][32].
+// out: mode 3 -> fp32 [64][base_off], otherwise [128][64] ([128][128] for mode 2).
 extern "C" int b2_debug_umma_probe(const void* a, const void* b, float* out, int mode, int shift, int base_off,
                                    void* stream) {
   B2_CHECK_ARG(a && b && out, "null pointer");
+  B2_CHECK_ARG(mode != 3 || ((base_off == 64 || base_off == 128 || base_off == 192) && shift >= 0 && shift + base_off <= 256),
+               "mode 3 takes N = 64, 128 or 192 rows of B inside the 256-row tile");
   int rc;
   if ((rc = require_sm90()) != B2_OK) return rc;
   const int smem_bytes = 32768 + 8192 + 64 + acc_bytes(128) + 1024;
   B2_OPT_IN_SMEM(mma_probe_kernel, smem_bytes);
   CUtensorMap tmA, tmB;
   memset(&tmA, 0, sizeof(tmA)); memset(&tmB, 0, sizeof(tmB));
-  if (mode == 0) {
+  if (mode == 0 || mode == 3) {
     if ((rc = make_tmap_2d_f16(&tmA, a, 64, 256, 64, 64, 128, true)) != B2_OK) return rc;
     if ((rc = make_tmap_2d_f16(&tmB, b, 64, 64, 64, 64, 64, true)) != B2_OK) return rc;
   } else if (mode == 2) {

@@ -183,6 +183,9 @@ __device__ __forceinline__ void acc_st32(const AccTile& t, int row, int col, con
     s[q] = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
                        __uint_as_float(v[4 * q + 3]));
 }
+__device__ __forceinline__ void st_shared_f32(uint32_t addr, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
 __device__ __forceinline__ void acc_zero32(const AccTile& t, int row, int col) {
   float4* s = reinterpret_cast<float4*>(t.p + static_cast<size_t>(row) * t.ld + col);
 #pragma unroll

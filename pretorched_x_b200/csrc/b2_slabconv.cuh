@@ -37,7 +37,7 @@ constexpr int kSlabEpiWarps = 3;
 constexpr int kSlabTmaWarp = 11;
 // Accumulator columns of one work item (MT x N tile) held in registers: each consumer thread keeps kSlabAccCols / 2 fp32 for the
 // whole item.  Twelve warps are three per SM sub-partition, whose 64 KB register file then allows 168 registers per thread (a
-// thirteenth warp would cut that to 128).  The tile planner (slab_pick_tiles, try_slabts in b2_conv_api.cu) never picks MT * N
+// thirteenth warp would cut that to 128).  The tile planner (slab_pick_tiles in b2_conv_api.cu) never picks MT * N
 // above kSlabAccCols; the consumer loops size their register arrays from it.
 constexpr int kSlabAccCols = 192;
 constexpr int kSlabWStages = 4;     // weight-tile ring depth
@@ -146,19 +146,38 @@ __device__ __forceinline__ void slab_mma(float* d, uint64_t a, uint64_t b, int k
     if (k < ksteps) wgmma_ss<N>(d, a + 2 * k, b + 2 * k);    // K step: +32 B on both start addresses
 }
 
+// 64-wide tile, transposed product.  With at most 64 output channels the weight stage is exactly one m64 A operand, so each
+// warpgroup computes D^T[64 channels][positions] = W[64][K] . X^T with the slab rows as a K-major B operand.  One m64n(64 c)k16
+// per K step reads 2 KB of A and c 2 KB of B from shared memory where c m64n64k16 read c (2 KB + 2 KB): at c = 2, 96 instead of
+// 128 bytes per tensor cycle, so the SM's 128 B/cycle shared-memory port no longer bounds the MMAs.  The item's MT * 128 positions
+// v = 128 j + r (tile j, row r) are split into two contiguous halves: warpgroup wg owns v in [wg MT 64, wg MT 64 + MT 64), its
+// 64-position chunk c at fragment columns [64 c, 64 c + 64).
+//   TMT = MT = 2: one m64n128k16 per K step over the whole half.
+//   TMT = 0 (MT = 1, and multi-plane items, whose tiles lie plane_stride apart in the slab): one m64n64k16 per chunk.
+// Every chunk is issued, also where a ragged item (mt_valid < MT) has no valid position in it: slab_rows sizes the slab for
+// MT * 128 positions from every item start, so those rows are inside it (multi-plane items read the same rows the M-tile
+// orientation did), their columns of D are discarded by the epilogue, and skipping them -- or issuing narrower forms on the
+// same accumulators -- makes ptxas serialise the wgmma pipeline (C7515).
+__device__ __forceinline__ int slab_t64_v0(int wg, int MT, int c) { return (wg * MT + c) * 64; }
+__device__ __forceinline__ uint32_t slab_t64_off16(int v0, uint32_t tile_stride16) {   // slab start of position v0, 16-byte units
+  return static_cast<uint32_t>(v0 >> 7) * tile_stride16 + static_cast<uint32_t>(v0 & 127) * 8u;
+}
+
 // Consumer warpgroups of slabconv_kernel for an N tile of N columns.  Warpgroup wg owns rows [64 wg, 64 wg + 64) of every M tile of
-// an item; tile j sits at fragment columns [j N, j N + N) of each thread's registers from the item's first K block to its last.  The
-// MMAs of one tap form one commit group, one group stays in flight, and a ring slot is released when the group that read it retires.
-template <int N>
+// an item; tile j sits at fragment columns [j N, j N + N) of each thread's registers from the item's first K block to its last
+// (N = 64: the transposed product above).  The MMAs of one tap form one commit group, one group stays in flight, and a ring slot is
+// released when the group that read it retires.
+template <int N, int TMT>
 __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile& at, int accs, uint32_t slab0, uint32_t w0s,
                                               int w_bytes, uint64_t* slab_full, uint64_t* slab_empty, uint64_t* w_full,
                                               uint64_t* w_empty, uint64_t* acc_full, uint64_t* acc_empty) {
   constexpr int kMaxMT = kSlabAccCols / N < 4 ? kSlabAccCols / N : 4;
   float acc[kMaxMT * N / 2];
-  const int wg = threadIdx.x >> 7;
+  const int wg = warp_uniform(threadIdx.x >> 7);
   const bool lead = (threadIdx.x & 31) == 0;                 // one arrival per consumer warp on the ring barriers
   const uint32_t a_wg = static_cast<uint32_t>(wg) * (64u * 128u >> 4);   // this warpgroup's 64 rows, in 16-byte units
   const uint32_t tile_stride16 = (p.mp > 1 ? static_cast<uint32_t>(p.plane_stride) : 128u * 128u) >> 4;   // A start of tile j
+  const int MT = TMT ? TMT : p.MT;
   int wit = 0, sg = 0, lt = 0;
   for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
     const SlabItem w = slab_item(p, item, N);
@@ -181,11 +200,26 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
         // slab-local pixel index of padded output position q0 under this tap
         const int pix0 = w.q0 + p.sub_off[sub][ti] - w.r_lo * p.PW;
         const uint64_t b = desc_from(kSw128DescHi, sw128_desc_lo(w0s + ws * w_bytes));
-        const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u) + a_wg;
+        const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u);
         wgmma_fence();
+        if constexpr (N == 64) {
+          // the weight stage is A, slab rows are B (the descriptor formats are the same K-major SWIZZLE_128B)
+          if constexpr (TMT == 0) {
 #pragma unroll
-        for (int j = 0; j < kMaxMT; ++j)
-          if (j < mt_valid) slab_mma<N>(acc + j * (N / 2), desc_from(kSw128DescHi, a_lo0 + j * tile_stride16), b, ksteps);
+            for (int c = 0; c < kMaxMT; ++c)
+              if (c < MT)
+                slab_mma<64>(acc + c * 32, b, desc_from(kSw128DescHi, a_lo0 + slab_t64_off16(slab_t64_v0(wg, MT, c), tile_stride16)),
+                             ksteps);
+          } else {
+            static_assert(TMT * 64 <= kSlabAccCols, "one warpgroup's half of the item in registers");
+            slab_mma<TMT * 64>(acc, b, desc_from(kSw128DescHi, a_lo0 + slab_t64_off16(slab_t64_v0(wg, MT, 0), tile_stride16)),
+                               ksteps);
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < kMaxMT; ++j)
+            if (j < mt_valid) slab_mma<N>(acc + j * (N / 2), desc_from(kSw128DescHi, a_lo0 + a_wg + j * tile_stride16), b, ksteps);
+        }
         wgmma_commit();
         wgmma_wait1();                                       // the previous tap's group has retired: release what it read
         if (lead && prev_ws >= 0) {
@@ -204,14 +238,39 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
     }
     // hand the item to the epilogue: one store of the fragments into the accumulator tile, then straight on to the next item
     mbar_wait(acc_empty, (lt & 1) ^ 1);
+    if constexpr (N == 64) {
+      // transposed into the [position][channel] tile: fragment (channel ch (+8), positions v, v + 1) goes to row v & 127 of tile
+      // v >> 7.  A pitch of 4 (mod 32) floats puts the 8 channels x 4 even positions of one store in 32 distinct banks.
+      // (32-bit shared addresses stepped from one base: the 96 accumulators leave no room for a 64-bit pointer per store)
+      const int t = threadIdx.x & 127;
+      const uint32_t ld4 = static_cast<uint32_t>(at.ld) * 4u;
+      const uint32_t base = smem_u32(at.p) + static_cast<uint32_t>((t >> 5) * 16 + ((t & 31) >> 2) + 2 * (t & 3) * at.ld) * 4u;
 #pragma unroll
-    for (int j = 0; j < kMaxMT; ++j)
-      if (j < mt_valid) frag_io<N>(at, wg * 64, j * accs, *reinterpret_cast<float(*)[N / 2]>(acc + j * (N / 2)), false, false);
+      for (int c = 0; c < kMaxMT; ++c) {
+        if (c < MT) {
+          const int v0 = slab_t64_v0(wg, MT, c);
+          uint32_t a = base + static_cast<uint32_t>((v0 & 127) * at.ld + (v0 >> 7) * accs) * 4u;
+#pragma unroll
+          for (int jb = 0; jb < 8; ++jb, a += 8u * ld4) {
+            const float* f = acc + c * 32 + 4 * jb;
+            st_shared_f32(a, f[0]);
+            st_shared_f32(a + 32u, f[2]);
+            st_shared_f32(a + ld4, f[1]);
+            st_shared_f32(a + ld4 + 32u, f[3]);
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < kMaxMT; ++j)
+        if (j < mt_valid) frag_io<N>(at, wg * 64, j * accs, *reinterpret_cast<float(*)[N / 2]>(acc + j * (N / 2)), false, false);
+    }
     mbar_arrive(acc_full);
   }
 }
 
-template <int BN>   // BN = 0: N tile taken from SlabParams::bn at run time
+// BN = 0: N tile taken from SlabParams::bn at run time.  TMT: the 64-wide tile's MMA form (slab_consumer; 0 for the other tiles)
+template <int BN, int TMT = 0>
 __global__ void __launch_bounds__(kSlabThreads, 1)
 slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N*T), box (64, PW, R, 1)
                 const __grid_constant__ CUtensorMap tmB,   // weights [Ncols][taps*C], box (64, BN)
@@ -312,11 +371,11 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
     // ================================ consumer warpgroups ===============================
     const uint32_t slab0 = smem_u32(slab_base), w0s = smem_u32(w_base);
     if constexpr (BN != 0) {
-      slab_consumer<BN>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty);
+      slab_consumer<BN, TMT>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty);
     } else {
       // runtime N: one compiled main loop per width the tile planner can pick (launch_slab rejects any other)
       switch (bn) {
-#define B2_SLAB_N(n) case n: slab_consumer<n>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty); break;
+#define B2_SLAB_N(n) case n: slab_consumer<n, 0>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty); break;
         B2_SLAB_N(16) B2_SLAB_N(144) B2_SLAB_N(160) B2_SLAB_N(176) B2_SLAB_N(192)
 #undef B2_SLAB_N
         default: __trap();

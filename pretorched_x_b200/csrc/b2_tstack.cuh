@@ -8,8 +8,8 @@
 // output frames sit side by side in the accumulator tile ([slot][64 columns]) and the weights are stacked [W(dt=kt-1); ...; W(dt=0)]
 // (64 rows each): the slots an input frame feeds are a CONTIGUOUS row range of that stack and a contiguous column range of the
 // accumulator tile, and one MMA of N = 64 x (slots fed) <= 128 replaces up to two N = 64 MMAs on the same A tile.
-// b2_slabts.cuh does the same for 3 x kh x kw filters but streams a 24 KB weight stack per (tap, input frame) from L2, which is what
-// made it lose on 1x1 in-plane filters.  Here the in-plane filter is 1x1: the whole filter is
+// (The slab kernel's 64-wide tile attacks the same feed for 3 x kh x kw filters the other way round: the weight stage becomes the
+// A operand and up to 192 slab positions the B operand.)  Here the in-plane filter is 1x1: the whole filter is
 // kt x ceil(C/64) blocks of 8 KB (72 KB for C144, 112 KB for C110 x 7 taps) and stays RESIDENT in shared memory, loaded once per CTA
 // before griddepcontrol.wait (weights do not depend on the previous kernel); A tiles are plain [128 positions][64 channels] TMA boxes
 // (no halo, rows past the end of a frame zero-filled).  The accumulator tile (128 x 128 fp32, 66 KB) shares the 227 KB of shared

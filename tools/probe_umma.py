@@ -18,7 +18,8 @@ g = torch.Generator().manual_seed(0)
 
 
 def run(a, b, mode, shift, base_off):
-    out = torch.zeros(128, 128 if mode == 2 else 64, dtype=torch.float32, device=dev)
+    shape = (64, base_off) if mode == 3 else (128, 128 if mode == 2 else 64)
+    out = torch.full(shape, float("nan"), dtype=torch.float32, device=dev)
     rc = fn(a.data_ptr(), b.data_ptr(), out.data_ptr(), mode, shift, base_off, None)
     assert rc == 0, _lib.last_error()
     torch.cuda.synchronize()
@@ -50,3 +51,16 @@ want = A2.float() @ V2.float()
 got = run(A2.to(dev), V2.to(dev), 2, 0, 0)
 err = (got - want).abs().max().item() / want.abs().max().item()
 print("mode 2: MN-major SW128 B (LBO=8192, SBO=1024, K step 2048 B): rel err %.3e %s" % (err, "EXACT" if err < 1e-5 else "wrong"))
+
+print("mode 3: SW128 K-major B (N rows) with start address shifted by s rows (128 B each), A = 64 x 64 K-major tile")
+bad = 0
+for n in (64, 128, 192):
+    for s in (0, 1, 3, 5, 7, 8, 9, 13, 37, 256 - n):
+        want = B.float() @ A[s:s + n].float().t()
+        got = run(Ad, Bd, 3, s, n)
+        err = ((got - want).abs().max() / want.abs().max()).item()
+        ok = err < 1e-5
+        bad += not ok
+        print("  N %3d shift %3d: rel err %.3e %s" % (n, s, err, "EXACT" if ok else "wrong"))
+print("mode 3: %s" % ("all EXACT" if bad == 0 else "%d WRONG" % bad))
+sys.exit(1 if bad else 0)
