@@ -506,41 +506,48 @@ static int try_tstack(const b2_conv_args* a, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------
 // stem convolution launcher (Toeplitz-descriptor kernel)
 // ------------------------------------------------------------------------------------------
-// Output rows per item of the BN = 64 stem: -2 = not read yet, -1 = the rule, 2 / 4 = forced (4 only where eligible).
-// B2_STEM_ROWS=2 / 4 in the environment (read once) or b2_debug_set_stem_rows() force an instance, for A/B comparisons.
+// Instance of the BN = 64 stem: -2 = not read yet, -1 = the rule; 2 / 4 = forced two- / four-row instance with positions along
+// M, kStemForceT = the transposed four-row instance (each only where eligible).  B2_STEM_ROWS=2 / 4 / 4t in the environment (read
+// once) or b2_debug_set_stem_rows() force an instance, for A/B comparisons.
+constexpr int kStemForceT = 4 | 16;
 static int g_stem_rows = -2;
 static int g_last_stem_rows = 0;
-template <int BN, int G>
+template <int BN, int G, bool kT>
 static int launch_stem_g(cudaStream_t stream, const StemParams& p, const CUtensorMap& tmX, int smem_bytes) {
-  B2_OPT_IN_SMEM((stemconv_kernel<BN, G, false>), 227 * 1024);
-  if constexpr (G != 4) B2_OPT_IN_SMEM((stemconv_kernel<BN, G, true>), 227 * 1024);
+  B2_OPT_IN_SMEM((stemconv_kernel<BN, G, false, kT>), 227 * 1024);
+  if constexpr (G != 4) B2_OPT_IN_SMEM((stemconv_kernel<BN, G, true, false>), 227 * 1024);
   const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
   if constexpr (G != 4)
     if (p.nstages == 1) {
-      B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, G, true>, dim3(grid), dim3(stem_threads(G)), smem_bytes, stream, tmX, p));
+      B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, G, true, false>, dim3(grid), dim3(stem_threads(G)), smem_bytes, stream, tmX, p));
       B2_CHECK_LAUNCH("stemconv_kernel");
       return B2_OK;
     }
-  B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, G, false>, dim3(grid), dim3(stem_threads(G)), smem_bytes, stream, tmX, p));
+  B2_CHECK_CUDA(launch_pdl(stemconv_kernel<BN, G, false, kT>, dim3(grid), dim3(stem_threads(G)), smem_bytes, stream, tmX, p));
   B2_CHECK_LAUNCH("stemconv_kernel");
   return B2_OK;
 }
 
-// Which G a BN = 64 stem runs with.  G = 4 is eligible outside pair mode when its slab (2 * 3 + kh rows) and weight image leave
-// room for three ring stages next to its staging tile, i.e. kh <= 7; taller filters keep G = 2 and its deeper ring.  The rule
-// takes it for temporal filters (kt > 1): on an H100 the 7x7x7 stems of resnet3d50 / nonlocal50 run 15-17 % faster.  A 2-D
-// stem (kt == 1, resnet18) has one tap per item, so the item-end drain and the single staging tile are exposed: G = 4 measured
-// 16 % slower there and it keeps G = 2.
-static int stem_rows_for(int BN, int kt, int kh, bool pair) {
+// Which instance a stem runs with: returns G, *transposed for the transposed four-row one.  G = 4 is eligible at BN = 64 outside
+// pair mode when its slab (2 * 3 + kh rows) and weight image leave room for three ring stages next to its staging tile, i.e.
+// kh <= 7; taller filters keep G = 2 and its deeper ring.  The rule takes it for temporal filters (kt > 1): on an H100 the 7x7x7
+// stems of resnet3d50 / nonlocal50 run 15-17 % faster than with G = 2.  A 2-D stem (kt == 1, resnet18) has one tap per item, so the
+// item-end drain and the single staging tile are exposed: G = 4 measured 16 % slower there and it keeps G = 2.  Where G = 4 runs
+// and a row has at most kStemTileT = 112 output columns, the transposed instance computes it (one N = 112 MMA per output row
+// instead of two 64-row halves of a 128-row tile; 112 / Wo columns of waste instead of 128 / Wo).
+static int stem_rows_for(int BN, int kt, int kh, int Wo, bool pair, bool* transposed) {
+  *transposed = false;
   if (BN != 64) return 1;
   if (g_stem_rows == -2) {
     const char* e = getenv("B2_STEM_ROWS");
-    g_stem_rows = (e && (e[0] == '2' || e[0] == '4')) ? e[0] - '0' : -1;
+    g_stem_rows = (e && e[0] == '2') ? 2 : (e && e[0] == '4') ? ((e[1] == 't' || e[1] == 'T') ? kStemForceT : 4) : -1;
   }
   const int stage4 = ((2 * 3 + kh) * kStemPitch + kh * 64 * 64 + 127) / 128 * 128;
   const bool eligible = !pair && (227 * 1024 - stem_tail_bytes(4, 64) - 128) / stage4 >= 3;
   if (!eligible || g_stem_rows == 2) return 2;
-  return (g_stem_rows == 4 || kt > 1) ? 4 : 2;
+  if (g_stem_rows == -1 && kt == 1) return 2;
+  *transposed = Wo <= kStemTileT && g_stem_rows != 4;
+  return 4;
 }
 
 template <int BN>
@@ -559,7 +566,8 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
   static int pair_env = -1;
   if (pair_env < 0) { const char* e = getenv("B2_STEM_PAIR"); pair_env = (e && e[0] == '0') ? 0 : 1; }
   p.pair = (pair_env && a->kt == 1 && a->pt == 0 && p.Wo <= 60 && !a->pool_w && a->W <= 120) ? 1 : 0;
-  p.G = stem_rows_for(BN, a->kt, a->kh, p.pair != 0);
+  bool transposed = false;
+  p.G = stem_rows_for(BN, a->kt, a->kh, p.Wo, p.pair != 0, &transposed);
   p.rows = 2 * (p.G - 1) + a->kh;
   if (p.rows > kStemMaxRows) return set_error(B2_ERR_UNSUPPORTED, "stem kernel height %d too large", a->kh);
   for (int i = 0; i < p.rows; ++i) {
@@ -610,9 +618,10 @@ static int launch_stem(const b2_conv_args* a, cudaStream_t stream) {
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_error(B2_ERR_CUDA, "cuTensorMapEncodeTiled(stem) failed (%d)", (int)r);
   g_last_stem_rows = p.G;
-  set_last_kernel(KID_STEM, p.G);
-  if constexpr (BN == 128) return launch_stem_g<128, 1>(stream, p, tmX, smem_bytes);
-  else return p.G == 4 ? launch_stem_g<64, 4>(stream, p, tmX, smem_bytes) : launch_stem_g<64, 2>(stream, p, tmX, smem_bytes);
+  set_last_kernel(KID_STEM, p.G, transposed);
+  if constexpr (BN == 128) return launch_stem_g<128, 1, false>(stream, p, tmX, smem_bytes);
+  else if (p.G == 2) return launch_stem_g<64, 2, false>(stream, p, tmX, smem_bytes);
+  else return transposed ? launch_stem_g<64, 4, true>(stream, p, tmX, smem_bytes) : launch_stem_g<64, 4, false>(stream, p, tmX, smem_bytes);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -917,10 +926,20 @@ int b2_debug_tstack_plan(const b2_conv_args* a, int* out) {
   return B2_OK;
 }
 int b2_debug_last_conv_path(void) { return g_last_conv_path; }
-/* stem convolution: output rows per work item of the last launch (1, 2 or 4); rows = 2 / 4 forces the two- / four-row BN = 64
-   instance (four only where eligible), -1 the rule.  The row plan of (G, kh): out[3 i .. 3 i + 2] = {g_lo, g_hi, first weight slot} of slab row i, returns the slab row count. */
+/* stem convolution: output rows per work item of the last launch (1, 2 or 4; b2_debug_last_kernel's info[1] tells whether the
+   four-row instance was the transposed one); rows = 2 / 4 forces the two- / four-row BN = 64 instance with positions along M,
+   rows = 20 (4 | 16) the transposed four-row instance (each only where eligible), -1 the rule.  The row plan of (G, kh):
+   out[3 i .. 3 i + 2] = {g_lo, g_hi, first weight slot} of slab row i, returns the slab row count. */
 int b2_debug_last_stem_rows(void) { return g_last_stem_rows; }
-int b2_debug_set_stem_rows(int rows) { g_stem_rows = (rows == 2 || rows == 4) ? rows : -1; return B2_OK; }
+int b2_debug_set_stem_rows(int rows) { g_stem_rows = (rows == 2 || rows == 4 || rows == kStemForceT) ? rows : -1; return B2_OK; }
+/* host-only view of the stem's instance choice (no launch, no GPU needed) for K output channels, a kt x kh x 7 filter, Wo output
+   columns and pair mode on / off, under the current force knob: out = {G, transposed} */
+int b2_debug_stem_plan(int K, int kt, int kh, int Wo, int pair, int* out) {
+  bool transposed = false;
+  out[0] = stem_rows_for(K <= 64 ? 64 : 128, kt, kh, Wo, pair != 0, &transposed);
+  out[1] = transposed;
+  return B2_OK;
+}
 int b2_debug_stem_row_plan(int G, int kh, int* out) {
   const int rows = 2 * (G - 1) + kh;
   if (G < 1 || kh < 1 || rows > kStemMaxRows) return -1;
@@ -935,7 +954,7 @@ int b2_debug_set_densem(int maxm, int force_s) { g_densem_maxm = maxm < 0 ? -2 :
    stays for the ABI and accepts its argument with no effect. */
 int b2_debug_set_slabts(int mode) { (void)mode; return B2_OK; }
 /* kernel of the last convolution / GEMM / attention call (a KID_* id of b2_host.h, 0 when the call launched nothing) and its
-   tile parameters in info[0..4]: slab {BN, MT, flex, wchunks, remapped}, densem {bn, S}, pgemm / igemm {BN, masked}, stem {G},
+   tile parameters in info[0..4]: slab {BN, MT, flex, wchunks, remapped}, densem {bn, S}, pgemm / igemm {BN, masked}, stem {G, transposed},
    attention {online, DVT}; unused entries are 0 */
 int b2_debug_last_kernel(int* info) {
   if (info) memcpy(info, g_last_info, sizeof(g_last_info));

@@ -15,6 +15,9 @@
 //           B of N = `base_off` (64, 128 or 192) rows whose start address is shifted by `shift` rows from a 1024-byte aligned
 //           tile; A is the 64 x 64 K-major tile given as `b`, the 256 x 64 tile given as `a` holds the B rows.  Expected:
 //           D[m][n] = sum_k b[m][k] * a[shift + n][k], written to out as [64][N].
+//   mode 4: the mode 1 Toeplitz view as the B operand at N = 112 (the transposed stem reads a slab row so): A is the 64 x 32
+//           no-swizzle K-major tile of mode 1's B (LBO = 128 B, SBO = 512 B), B row n starts at byte 16*n of the linear buffer
+//           (LBO = 16 B, SBO = 128 B).  Expected: D[m][n] = sum_{k<32} b[m][k] * buf[8*n + k], written to out as [64][112].
 #include "b2_host.h"
 #include "b2_ptx.cuh"
 
@@ -22,7 +25,21 @@
 
 namespace b2 {
 
-// mode 3: one m64nNk16 chain with the accumulators in registers, fragments written straight to out[64][N]
+// modes 3 and 4: accumulator fragments of an m64nN tile written straight to out[64][N]
+template <int N>
+__device__ void probe_store_frag(const float (&d)[N / 2], float* __restrict__ out) {
+  const int t = threadIdx.x & 127;
+  const int r = (t >> 5) * 16 + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    out[r * N + 8 * j + c] = d[4 * j];
+    out[r * N + 8 * j + c + 1] = d[4 * j + 1];
+    out[(r + 8) * N + 8 * j + c] = d[4 * j + 2];
+    out[(r + 8) * N + 8 * j + c + 1] = d[4 * j + 3];
+  }
+}
+
+// mode 3: one m64nNk16 chain with the accumulators in registers
 template <int N>
 __device__ void probe_shifted_b(uint32_t a_addr, uint32_t b_addr, float* __restrict__ out) {
   float d[N / 2];
@@ -36,15 +53,23 @@ __device__ void probe_shifted_b(uint32_t a_addr, uint32_t b_addr, float* __restr
   wgmma_commit();
   wgmma_wait0();
   reg_fence(d);
-  const int t = threadIdx.x & 127;
-  const int r = (t >> 5) * 16 + ((t & 31) >> 2), c = 2 * (t & 3);
+  probe_store_frag<N>(d, out);
+}
+
+// mode 4: two K steps of 16 (A +256 B, B +32 B), as the transposed stem issues them
+__device__ void probe_toeplitz_b(uint32_t a_addr, uint32_t b_addr, float* __restrict__ out) {
+  float d[56];
 #pragma unroll
-  for (int j = 0; j < N / 8; ++j) {
-    out[r * N + 8 * j + c] = d[4 * j];
-    out[r * N + 8 * j + c + 1] = d[4 * j + 1];
-    out[(r + 8) * N + 8 * j + c] = d[4 * j + 2];
-    out[(r + 8) * N + 8 * j + c + 1] = d[4 * j + 3];
-  }
+  for (int i = 0; i < 56; ++i) d[i] = 0.f;
+  reg_fence(d);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 2; ++k)
+    wgmma_ss<112>(d, make_desc_noswz_kmajor(a_addr, 128, 512) + 16 * k, make_desc_noswz_kmajor(b_addr, 16, 128) + 2 * k);
+  wgmma_commit();
+  wgmma_wait0();
+  reg_fence(d);
+  probe_store_frag<112>(d, out);
 }
 
 __global__ void __launch_bounds__(128, 1)
@@ -114,6 +139,10 @@ mma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
     fence_proxy_async();
     __syncthreads();
+    if (mode == 4) {
+      probe_toeplitz_b(smem_u32(sB), smem_u32(sA), out);
+      return;
+    }
     // K = 32 -> two K=16 steps; A advances two 16-byte chunks (32 B), B two 128-byte chunk columns (256 B)
     const WgOperands ops{make_desc_noswz_kmajor(smem_u32(sA), /*LBO*/ 16, /*SBO*/ 128),
                          make_desc_noswz_kmajor(smem_u32(sB), /*LBO*/ 128, /*SBO*/ 512), 2u, 64u, 16u, 256u, 64u};
@@ -131,8 +160,8 @@ mma_probe_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
 using namespace b2;
 
-// a: mode 0 / 3 -> fp16 [256][64]; mode 1 -> fp16 [2048] linear.  b: mode 0 / 3 -> fp16 [64][64]; mode 1 -> fp16 [64][32].
-// out: mode 3 -> fp32 [64][base_off], otherwise [128][64] ([128][128] for mode 2).
+// a: mode 0 / 3 -> fp16 [256][64]; mode 1 / 4 -> fp16 [2048] linear.  b: mode 0 / 3 -> fp16 [64][64]; mode 1 / 4 -> fp16 [64][32].
+// out: mode 3 -> fp32 [64][base_off], mode 4 -> [64][112], otherwise [128][64] ([128][128] for mode 2).
 extern "C" int b2_debug_umma_probe(const void* a, const void* b, float* out, int mode, int shift, int base_off,
                                    void* stream) {
   B2_CHECK_ARG(a && b && out, "null pointer");

@@ -270,6 +270,17 @@ template <>
 __device__ __forceinline__ void wgmma_ss<16>(float* d, uint64_t a, uint64_t b) { wgmma_n16<0>(*reinterpret_cast<float(*)[8]>(d), a, b); }
 template <>
 __device__ __forceinline__ void wgmma_ss<64>(float* d, uint64_t a, uint64_t b) { wgmma_n64<0>(*reinterpret_cast<float(*)[32]>(d), a, b); }
+// N = 112: one whole 112-column output row of the transposed stem (positions along N)
+template <>
+__device__ __forceinline__ void wgmma_ss<112>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n112k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, 1, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+      : "l"(a), "l"(b));
+}
 template <>
 __device__ __forceinline__ void wgmma_ss<128>(float* d, uint64_t a, uint64_t b) { wgmma_n128_ss(*reinterpret_cast<float(*)[64]>(d), a, b); }
 template <>
@@ -467,6 +478,14 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
+}
+// Four 8 x 8 fp16 matrices, each held in the accumulator-fragment layout (lane l: row l / 4, columns 2 (l % 4) and 2 (l % 4) + 1,
+// one fp16 pair per register), stored TRANSPOSED: lanes 8 k .. 8 k + 7 give the addresses of the 8 memory rows of matrix k (16 B
+// each), and memory row c of matrix k receives its fragment column c.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t smem_addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(smem_addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
 }
 __device__ __forceinline__ float2 unpack_half2(uint32_t u) {
   __half2 h = *reinterpret_cast<__half2*>(&u);

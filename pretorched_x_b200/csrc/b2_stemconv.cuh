@@ -34,6 +34,14 @@
 // setmaxnreg moves registers from the producer (40) and epilogue (56) warpgroups to the consumers (208).  Its shared memory holds three 54 KB ring stages (13 slab rows + the 28 KB weight
 // image of a 7-tall filter) and ONE staging tile of the 120 tile rows that carry output columns: the epilogue drains an item in
 // a small fraction of the next item's main loop.
+//
+// Transposed G = 4 (kT; rows of at most 112 output columns): the same CTA, ring, producer and epilogue warps compute
+// D^T[64 channels][112 positions] = W . X^T per output row.  A (m64) is the tap image of (dt, dh), read with the descriptor the
+// other instances use for B; B is the Toeplitz view of one slab row at N = 112 (tools/probe_umma.py, mode 4), so a whole output
+// row is one MMA and no tile row is padding.  Consumer warpgroup wg owns output rows 2 wg and 2 wg + 1 (56 fp32 each per thread)
+// and issues one N = 112 MMA pair per (slab row, owned row): 2 KB of A + 3.5 KB of B per 56 tensor cycles, against 2 KB + 2 KB per
+// 32 for a 64-row N = 64 piece.  The fragments are stored transposed (stmatrix .trans) into the [position][channel] staging
+// tile, so the epilogue is shared.  Every element keeps the accumulation order of the other instances.
 #pragma once
 
 #include "b2_ptx.cuh"
@@ -45,6 +53,8 @@ constexpr int kStemTmaWarp = 12;
 constexpr int kStemPitch = 2048;        // bytes per slab row: 256 pixels [2*w0-4, 2*w0+252) of 8 bytes
 constexpr int kStemRowPx = 256;         // TMA box width (the maximum box extent), one 8-byte element per pixel
 constexpr int kStemTileW = 120;         // output columns per item: rows r < 124 of the 128-row MMA tile see complete runs
+constexpr int kStemTileT = 112;         // output columns of the transposed instance, the N of its MMAs: position n reads the bytes
+                                        // [16 n, 16 n + 64) of a 2 KB slab row
 constexpr int kStemMaxStages = 4;
 constexpr int kStemMaxRows = 16;        // slab rows = 2*(G-1) + kh
 // per instance (G output rows per item, BN output channels per N tile)
@@ -140,6 +150,11 @@ __device__ __forceinline__ void stem_mma(float* d, uint64_t a, uint64_t b) {
 #pragma unroll
   for (int k = 0; k < 2; ++k) wgmma_ss<N_>(d, a + 2 * k, b + 16 * k);
 }
+// The transposed form: A = one tap image (K step 256 B), B = the Toeplitz view of a slab row at N = 112 (K step 32 B).
+__device__ __forceinline__ void stem_mma_t(float* d, uint64_t w, uint64_t x) {
+#pragma unroll
+  for (int k = 0; k < 2; ++k) wgmma_ss<kStemTileT>(d, w + 16 * k, x + 2 * k);
+}
 
 // Slab row feeding local output rows g_lo..g_hi (row g's fragments at acc + g * BN / 2).  G <= 2: one MMA over all of them; the
 // register offset and width must be compile-time constants, hence one case per (g_lo, g_hi).  G = 4: one N = 64 MMA per output
@@ -165,11 +180,13 @@ __device__ __forceinline__ void stem_row_mma(float* acc, int g_lo, int g_hi, uin
 
 // kOneSlot: tall filters (BN = 128 with kh >= 8, BN = 64 with kh >= 13) leave room for a single ring slot.  A separate instance,
 // because a wait_group 0 inside the tap loop makes ptxas serialise the wgmma pipeline of the common, multi-slot one.
-template <int BN, int G, bool kOneSlot>
+// kT: the transposed four-row instance (G = 4, Wo <= kStemTileT).
+template <int BN, int G, bool kOneSlot, bool kT>
 __global__ void __launch_bounds__(stem_threads(G), 1)
 stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pixels (W, H, N*T), box (256, rows, 1), no swizzle
                 const StemParams p) {
   static_assert((BN == 128 && G == 1) || (BN == 64 && (G == 2 || G == 4)), "stem tile");
+  static_assert(!kT || (BN == 64 && G == 4 && !kOneSlot), "transposed stem tile");
   constexpr int kThreads = stem_threads(G);
   constexpr int kStgLd = stem_stg_ld(G, BN), kStgRows = stem_stg_rows(G), kStgBufs = stem_stg_bufs(G);
   extern __shared__ uint8_t smem_raw[];
@@ -226,22 +243,24 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
   } else if (warp < kStemEpiWarp0) {
     // ================================ consumer warpgroups ===============================
     if constexpr (G == 4) setmaxnreg_inc<208>();
-    // SWIZZLE_NONE K-major descriptors: hi = SBO >> 4; lo = addr >> 4 | (LBO >> 4) << 16.  A: SBO 128 B, LBO 16 B; the
-    // warpgroup's 64 tile rows start 64 x 16 B = 1 KB into the slab row.  B: SBO 512 B (8 rows), LBO 128 B.
-    constexpr uint32_t a_hi = 128u >> 4, b_hi = 512u >> 4;
+    // SWIZZLE_NONE K-major descriptors: hi = SBO >> 4; lo = addr >> 4 | (LBO >> 4) << 16.  Toeplitz view of a slab row (A; kT: B):
+    // SBO 128 B, LBO 16 B; outside kT the warpgroup's 64 tile rows start 64 x 16 B = 1 KB into the slab row.  Weight image (B;
+    // kT: A): SBO 512 B (8 rows), LBO 128 B.
+    constexpr uint32_t x_hi = 128u >> 4, w_hi = 512u >> 4;
     constexpr uint32_t kTapBytes = BN * 64;            // weight image of one (dt, dh) tap: BN rows x 32 k
     const int wg = warp >> 2;
-    const uint32_t base = smem_u32(smem) + static_cast<uint32_t>(wg) * 1024u;
+    const uint32_t base = smem_u32(smem) + (kT ? 0u : static_cast<uint32_t>(wg) * 1024u);
     // fragment position: rows r0 and r0 + 8 of the tile, column pairs 8 j + c0
     const int r0 = wg * 64 + (warp & 3) * 16 + ((tid & 31) >> 2);
     const int c0 = 2 * (tid & 3);
-    float acc[G * BN / 2];
+    constexpr int kAcc = kT ? kStemTileT : G * BN / 2;   // kT: output rows 2 wg and 2 wg + 1, kStemTileT / 2 fp32 each
+    float acc[kAcc];
     int it = 0, lt = 0;
     for (int item = blockIdx.x; item < p.items_total; item += gridDim.x, ++lt) {
       const StemItem w = stem_item(p, item);
       const int dt_lo = max(0, p.pt - w.to), dt_hi = min(p.kt - 1, p.T - 1 - w.to + p.pt);
 #pragma unroll
-      for (int k = 0; k < G * BN / 2; ++k) acc[k] = 0.f;
+      for (int k = 0; k < kAcc; ++k) acc[k] = 0.f;
       reg_fence(acc);
       int prev_s = -1;
       for (int dt = dt_lo; dt <= dt_hi; ++dt, ++it) {
@@ -250,13 +269,32 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
         const uint32_t slab = base + s * p.stage_bytes;
         const uint32_t wbase = smem_u32(smem) + s * p.stage_bytes + slab_bytes;
         wgmma_fence();
+        if constexpr (kT) {
+          // slab row i feeds the owned row g = 2 wg + gg through dh = i - 2 g, the slot row_slot[i] + g - g_lo: i in [4 wg, 4 wg + kh + 1]
+          const int wgu = warp_uniform(wg);
+          const int i_end = min(p.rows, 4 * wgu + p.kh + 2);
 #pragma unroll 1
-        for (int i = 0; i < p.rows; ++i) {
-          const int g_lo = p.row_glo[i], g_hi = p.row_ghi[i];
-          if (g_lo > g_hi) continue;
-          const uint32_t a_lo = ((slab + static_cast<uint32_t>(i) * kStemPitch) >> 4) | ((16u >> 4) << 16);
-          const uint32_t b_lo = ((wbase + static_cast<uint32_t>(p.row_slot[i]) * kTapBytes) >> 4) | ((128u >> 4) << 16);
-          stem_row_mma<BN, G>(acc, g_lo, g_hi, desc_from(a_hi, a_lo), desc_from(b_hi, b_lo));
+          for (int i = 4 * wgu; i < i_end; ++i) {
+            const int g_lo = p.row_glo[i], g_hi = p.row_ghi[i];
+            const uint32_t x_lo = ((slab + static_cast<uint32_t>(i) * kStemPitch) >> 4) | ((16u >> 4) << 16);
+#pragma unroll
+            for (int gg = 0; gg < 2; ++gg) {
+              const int g = 2 * wgu + gg;
+              if (g >= g_lo && g <= g_hi) {
+                const uint32_t w_lo = ((wbase + static_cast<uint32_t>(p.row_slot[i] + g - g_lo) * kTapBytes) >> 4) | ((128u >> 4) << 16);
+                stem_mma_t(acc + gg * (kStemTileT / 2), desc_from(w_hi, w_lo), desc_from(x_hi, x_lo));
+              }
+            }
+          }
+        } else {
+#pragma unroll 1
+          for (int i = 0; i < p.rows; ++i) {
+            const int g_lo = p.row_glo[i], g_hi = p.row_ghi[i];
+            if (g_lo > g_hi) continue;
+            const uint32_t a_lo = ((slab + static_cast<uint32_t>(i) * kStemPitch) >> 4) | ((16u >> 4) << 16);
+            const uint32_t b_lo = ((wbase + static_cast<uint32_t>(p.row_slot[i]) * kTapBytes) >> 4) | ((128u >> 4) << 16);
+            stem_row_mma<BN, G>(acc, g_lo, g_hi, desc_from(x_hi, a_lo), desc_from(w_hi, b_lo));
+          }
         }
         wgmma_commit();
         if constexpr (kOneSlot) {                       // the next tap is loaded into this same slot: release it now
@@ -277,20 +315,48 @@ stemconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as 8-byte pi
       mbar_wait(&stg_empty[sb], ((lt / kStgBufs) & 1) ^ 1);
       __half* stg = s_stg + sb * (kStgRows * kStgLd);
       const int n0 = w.ntile * BN;
+      if constexpr (kT) {
+        // fragment of row g = 2 wg + gg: channels m (d[4 j], d[4 j + 1]) and m + 8 (d[4 j + 2], d[4 j + 3]), positions 8 j + c0, +1.
+        // stmatrix k = 2 q + h of step jp holds positions 16 jp + 8 q + [0, 8) x channels 16 (warp % 4) + 8 h + [0, 8); lane l
+        // addresses its memory row l % 8, one position.  A 528-byte pitch puts those 8 rows x 16 B in 32 different banks.  Staging
+        // rows 112..119 are not written: with Wo <= 112 the epilogue's col_ok is false there.
+        const int lane = tid & 31, k = lane >> 3;
+        const int m = n0 + 16 * (warp & 3) + (lane >> 2);
+        const float sc0 = s_scale[m], sh0 = s_shift[m], sc1 = s_scale[m + 8], sh1 = s_shift[m + 8];
+        const uint32_t st0 = smem_u32(stg + (8 * (k >> 1) + (lane & 7)) * kStgLd + 16 * (warp & 3) + 8 * (k & 1));
 #pragma unroll
-      for (int g = 0; g < G; ++g) {
+        for (int gg = 0; gg < 2; ++gg) {
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int c = 8 * j + c0;
-          const float2 sc = *reinterpret_cast<const float2*>(&s_scale[n0 + c]);
-          const float2 sh = *reinterpret_cast<const float2*>(&s_shift[n0 + c]);
-          const float* v = acc + g * (BN / 2) + 4 * j;
-          float a0 = v[0] * sc.x + sh.x, a1 = v[1] * sc.y + sh.y;
-          float b0 = v[2] * sc.x + sh.x, b1 = v[3] * sc.y + sh.y;
-          if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); b0 = fmaxf(b0, 0.f); b1 = fmaxf(b1, 0.f); }
-          *reinterpret_cast<uint32_t*>(stg + r0 * kStgLd + g * BN + c) = pack_half2(a0, a1);
-          if (kStgRows == 128 || r0 + 8 < kStgRows)         // tile rows >= kStemTileW carry no output column
-            *reinterpret_cast<uint32_t*>(stg + (r0 + 8) * kStgLd + g * BN + c) = pack_half2(b0, b1);
+          for (int jp = 0; jp < kStemTileT / 16; ++jp) {
+            uint32_t r[4];
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+              const float* v = acc + gg * (kStemTileT / 2) + 4 * (2 * jp + q);
+              float a0 = v[0] * sc0 + sh0, a1 = v[1] * sc0 + sh0;
+              float b0 = v[2] * sc1 + sh1, b1 = v[3] * sc1 + sh1;
+              if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); b0 = fmaxf(b0, 0.f); b1 = fmaxf(b1, 0.f); }
+              r[2 * q] = pack_half2(a0, a1);
+              r[2 * q + 1] = pack_half2(b0, b1);
+            }
+            stmatrix_x4_trans(st0 + 2u * static_cast<uint32_t>(16 * jp * kStgLd + (2 * wg + gg) * BN), r);
+          }
+        }
+      } else {
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int c = 8 * j + c0;
+            const float2 sc = *reinterpret_cast<const float2*>(&s_scale[n0 + c]);
+            const float2 sh = *reinterpret_cast<const float2*>(&s_shift[n0 + c]);
+            const float* v = acc + g * (BN / 2) + 4 * j;
+            float a0 = v[0] * sc.x + sh.x, a1 = v[1] * sc.y + sh.y;
+            float b0 = v[2] * sc.x + sh.x, b1 = v[3] * sc.y + sh.y;
+            if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); b0 = fmaxf(b0, 0.f); b1 = fmaxf(b1, 0.f); }
+            *reinterpret_cast<uint32_t*>(stg + r0 * kStgLd + g * BN + c) = pack_half2(a0, a1);
+            if (kStgRows == 128 || r0 + 8 < kStgRows)         // tile rows >= kStemTileW carry no output column
+              *reinterpret_cast<uint32_t*>(stg + (r0 + 8) * kStgLd + g * BN + c) = pack_half2(b0, b1);
+          }
         }
       }
       mbar_arrive(&stg_full[sb]);

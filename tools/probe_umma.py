@@ -18,7 +18,7 @@ g = torch.Generator().manual_seed(0)
 
 
 def run(a, b, mode, shift, base_off):
-    shape = (64, base_off) if mode == 3 else (128, 128 if mode == 2 else 64)
+    shape = (64, base_off) if mode == 3 else (64, 112) if mode == 4 else (128, 128 if mode == 2 else 64)
     out = torch.full(shape, float("nan"), dtype=torch.float32, device=dev)
     rc = fn(a.data_ptr(), b.data_ptr(), out.data_ptr(), mode, shift, base_off, None)
     assert rc == 0, _lib.last_error()
@@ -45,6 +45,12 @@ got = run(buf.to(dev), B1.to(dev), 1, 0, 0)
 err = (got - want).abs().max().item() / want.abs().max().item()
 print("mode 1: no-swizzle Toeplitz A (LBO=16, SBO=128): rel err %.3e %s" % (err, "EXACT" if err < 1e-5 else "wrong"))
 
+want = B1.float() @ buf.float()[idx[:112]].t()
+got = run(buf.to(dev), B1.to(dev), 4, 0, 0)
+err4 = (got - want).abs().max().item() / want.abs().max().item()
+print("mode 4: no-swizzle Toeplitz B at N = 112 (LBO=16, SBO=128), A = 64 x 32 no-swizzle: rel err %.3e %s"
+      % (err4, "EXACT" if err4 < 1e-5 else "wrong"))
+
 A2 = torch.randn(128, 64, generator=g).half()
 V2 = (torch.randn(64, 128, generator=g) / 8).half()
 want = A2.float() @ V2.float()
@@ -63,4 +69,5 @@ for n in (64, 128, 192):
         bad += not ok
         print("  N %3d shift %3d: rel err %.3e %s" % (n, s, err, "EXACT" if ok else "wrong"))
 print("mode 3: %s" % ("all EXACT" if bad == 0 else "%d WRONG" % bad))
+bad += err4 >= 1e-5
 sys.exit(1 if bad else 0)

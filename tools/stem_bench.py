@@ -2,11 +2,13 @@
 the Toeplitz stem kernel with BN + ReLU (and, where the network's max-pool follows, the W direction of that pool) in its
 epilogue, then the remaining (T, H) pool pass.  Each is timed as CUDA-graph replays between CUDA events after a warm-up.
 
-Per shape: the output rows per work item the kernel ran with (G), conv ms and stem ms (conv + pool pass), the conv's algorithmic TFLOP/s (3 input channels, every tap) and executed
-TFLOP/s (what the kernel issues: K padded from 21 to 32 per (dt, dh), 128-row M tiles, output channels rounded up to the N tile,
-temporal taps outside the clip skipped), and the card's name and power limit.
-usage: stem_bench.py [--rows 2|4] [shape ...]   (default: all shapes below; --rows forces the two- or four-row instance of the
-BN = 64 stems where it applies, as B2_STEM_ROWS does)"""
+Per shape: the instance the kernel ran with (G output rows per work item, "G=4t" for the transposed four-row one), conv ms and
+stem ms (conv + pool pass), the conv's algorithmic TFLOP/s (3 input channels, every tap) and executed TFLOP/s (what the kernel
+issues: K padded from 21 to 32 per (dt, dh), 128-row M tiles or 112-wide N tiles for the transposed instance, output channels
+rounded up to the N tile, temporal taps outside the clip skipped), and the card's name and power limit.
+usage: stem_bench.py [--rows 2|4|4t] [shape ...]   (default: all shapes below; --rows forces the two-row, the four-row or the
+transposed four-row instance of the BN = 64 stems where it applies, as B2_STEM_ROWS does)"""
+import ctypes
 import os
 import subprocess
 import sys
@@ -39,13 +41,13 @@ def card():
     return "%s (%s)" % (name, q)
 
 
-def executed_flops(N, T, Ho, Wo, K, kt, kh, pt):
+def executed_flops(N, T, Ho, Wo, K, kt, kh, pt, transposed):
     bn = 64 if K <= 64 else 128
     ncols = -(-((K + 7) // 8 * 8) // bn) * bn
     pair = kt == 1 and pt == 0 and Wo <= 60
     taps = sum(min(kt - 1, T - 1 - t + pt) - max(0, pt - t) + 1 for t in range(T + 2 * pt - kt + 1))
     tiles = Ho * -(-Wo // 120) * (N * taps if not pair else -(-N * T // 2) * kt)   # (plane, temporal tap) pairs x row x column tiles
-    return 2.0 * tiles * 128 * ncols * kh * 32
+    return 2.0 * tiles * (112 if transposed else 128) * ncols * kh * 32
 
 
 def time_graph(fn):
@@ -73,7 +75,7 @@ def main(names):
     lib = _lib.load()
     if "--rows" in names:
         i = names.index("--rows")
-        lib.b2_debug_set_stem_rows(int(names[i + 1]))
+        lib.b2_debug_set_stem_rows({"2": 2, "4": 4, "4t": 4 | 16}[names[i + 1]])
         names = names[:i] + names[i + 2:]
     names = names or list(SHAPES)
     print("card: %s" % card(), flush=True)
@@ -93,10 +95,14 @@ def main(names):
             conv_fn()
             torch.cuda.synchronize()
             G = lib.b2_debug_last_stem_rows()
+            info = (ctypes.c_int * 5)()
+            lib.b2_debug_last_kernel(info)
+            transposed = bool(info[1]) and G == 4
         alg = 2.0 * N * To * Ho * Wo * K * 3 * k[0] * k[1] * 7
-        exe = executed_flops(N, T, Ho, Wo, K, k[0], k[1], p[0])
-        print("%-11s N=%-3d T=%-2d %dx%d %s->%d  G=%d  conv %7.3f ms  stem %7.3f ms  algorithmic %6.1f TFLOP/s  executed %6.1f TFLOP/s"
-              % (name, N, T, H, W, "x".join(map(str, k)), K, G, ms_conv, ms_stem, alg / ms_conv / 1e9, exe / ms_conv / 1e9), flush=True)
+        exe = executed_flops(N, T, Ho, Wo, K, k[0], k[1], p[0], transposed)
+        print("%-11s N=%-3d T=%-2d %dx%d %s->%d  G=%-2s  conv %7.3f ms  stem %7.3f ms  algorithmic %6.1f TFLOP/s  executed %6.1f TFLOP/s"
+              % (name, N, T, H, W, "x".join(map(str, k)), K, "%d%s" % (G, "t" if transposed else ""), ms_conv, ms_stem,
+                 alg / ms_conv / 1e9, exe / ms_conv / 1e9), flush=True)
 
 
 if __name__ == "__main__":
