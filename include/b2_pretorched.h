@@ -224,6 +224,30 @@ int b2_dwconv3x3_ndhwc(const void* x, const float* w, const float* scale, const 
 int b2_relu6_inplace_ndhwc(void* x, long long rows, int ld, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * ResNeXt-3D (resnext3D.py:76-121)
+ * ------------------------------------------------------------------------------------------- */
+/* Grouped convolution (nn.Conv3d(C, C, 3, stride, 1, groups=32), conv2 of ResNeXtBottleneck, resnext3D.py:86-93) -> BatchNorm
+ * -> (+residual) -> ReLU on wgmma at the grouped cost:
+ *     y[m, k] = act( scale[k] * sum_{tap, c in group(k)} x[m @ tap, c] * w[k, c - first(group(k)), tap] + shift[k] + residual[m, k] )
+ * Reads b2_conv_args as b2_conv_ndhwc_fprop does, with `w` the packed grouped filter below.  Contract: C == K (C is also the
+ * channel pitch of x), C % 64 == 0, C / groups in {4, 8, 16, 32}, a 3x3x3 or 1x3x3 filter with padding (kt / 2, 1, 1), sh == sw
+ * in {1, 2}, st in {1, 2}; anything else returns B2_ERR_UNSUPPORTED.  mode, out_f32, accumulate, aff_ld, upsample, residual_up,
+ * residual_pre, y2 / scale2 / shift2 / aff2_ld, pool_w, in_scale / in_shift / in_aff_ld and mask / ldm must be zero / NULL
+ * (B2_ERR_INVALID).  Columns [K, ldy) of y are left untouched.  fp32 accumulation in a fixed order, no atomics.
+ * Executed multiply-accumulates over the algorithmic count: 4x for 4 channels per group, 2x for 8, 1x for 16 and 32 (the
+ * block-diagonal dense filter through b2_conv_ndhwc_fprop: `groups` x).
+ *
+ * Packed filter: fp32 [K][Cin_per_group][kt][kh][kw] (nn.Conv3d.weight of the grouped layer) -> fp16 [K / 64][taps][G][64] with
+ * G = 16 (G = 32 for 32 channels per group), K * G * taps elements: row r, 16-element segment j of a (64-channel slice, tap)
+ * tile is output channel 16 j + r (G = 32: 32 (j / 2) + r) of the slice against its input channels [16 j, 16 j + 16), zero where
+ * the two channels belong to different groups.  b2_pack_grouped_conv_weight_elems is host arithmetic and returns 0 for a filter
+ * outside the contract. */
+size_t b2_pack_grouped_conv_weight_elems(int K, int Cin_per_group, int groups, int kt, int kh, int kw);
+int b2_pack_grouped_conv_weight(const float* w, void* w_packed, int K, int Cin_per_group, int groups, int kt, int kh, int kw,
+                                void* stream);
+int b2_conv_grouped_ndhwc_fprop(const b2_conv_args* a, int groups, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Fine-tuning backward of the residual blocks (the backward of resnet3D.py:91-143 with eval-mode BatchNorm).  Gradients
  * travel between kernels as fp16 NDHWC matrices multiplied by a device-resident power-of-two loss scale; the fp32 results
  * (weight, gamma and beta gradients) divide it out.  `inv_loss_scale` / `scale_pair` are DEVICE pointers.

@@ -256,18 +256,21 @@ static bool slab_geometry(const b2_conv_args* a, SlabParams* p, int wc_hint) {
   return p->n_sub > 0 && p->PW <= 256;
 }
 
-template <int BNT, int TMT>
+template <int BNT, int TMT, int G = 0>
 static int run_slab(int grid, int smem_bytes, const CUtensorMap& tmX, const CUtensorMap& tmB, const SlabParams& p, cudaStream_t stream) {
-  auto kernel = slabconv_kernel<BNT, TMT>;
+  auto kernel = slabconv_kernel<BNT, TMT, G>;
   B2_OPT_IN_SMEM(kernel, 227 * 1024);
   B2_CHECK_CUDA(launch_pdl(kernel, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
   B2_CHECK_LAUNCH("slabconv_kernel");
   return B2_OK;
 }
 
-template <int BNT>   // BNT = 0: runtime N tile p.bn (set by the caller)
+// BNT = 0: runtime N tile p.bn (set by the caller).  G != 0: grouped convolution (b2_groupconv.cuh) -- N tiles are the K / 64
+// channel slices, a.w is the packed grouped filter
+template <int BNT, int G = 0>
 static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cudaStream_t stream) {
   if (BNT) { p.bn = BNT; p.wbytes = BNT * 128; p.accs = BNT; }
+  if (G) { p.wbytes = G * 128; p.cchunks = 1; }
   const int BN = p.bn;
   p.R = R;
   p.planes_total = a->N * p.To;
@@ -287,7 +290,7 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.relu = a->relu;
   p.aff_ld = a->aff_ld;
   p.naff = slab_naff(a->ldy);
-  p.tiles_n = (a->ldy + BN - 1) / BN;
+  p.tiles_n = G ? a->K / 64 : (a->ldy + BN - 1) / BN;
   p.tiles_q = p.mp > 1 ? 1 : (p.P + MT * 128 - 1) / (MT * 128);
   const long long plane_items = p.mp > 1 ? ((long long)a->N * p.To + p.mp - 1) / p.mp : (long long)a->N * p.To;
   const long long items = (long long)p.tiles_n * p.tiles_q * p.wchunks * plane_items * (p.up ? 4 : 1);
@@ -305,9 +308,11 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   if ((rc = make_tmap_ndhwc_slab(&tmX, a->x, (uint64_t)a->C, (uint64_t)a->W, (uint64_t)a->H, (uint64_t)a->N * a->T,
                                  (uint32_t)p.PW, (uint32_t)R, (uint32_t)p.ss, (uint32_t)(p.mp > 1 ? p.mp : 1))) != B2_OK)
     return rc;
-  if ((rc = make_tmap_2d_f16(&tmB, a->w, (uint64_t)taps * a->C, (uint64_t)a->K, (uint64_t)taps * a->C, 64, BN, true)) != B2_OK)
+  if ((rc = G ? make_tmap_2d_f16(&tmB, a->w, 64, (uint64_t)(a->K / 64) * taps * G, 64, 64, G, true)
+              : make_tmap_2d_f16(&tmB, a->w, (uint64_t)taps * a->C, (uint64_t)a->K, (uint64_t)taps * a->C, 64, BN, true)) != B2_OK)
     return rc;
   const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
+  if constexpr (G != 0) return run_slab<64, 0, G>(grid, smem_bytes, tmX, tmB, p, stream);
   // the 64-wide tile's MMA form (b2_slabconv.cuh): one N = 128 MMA over a warpgroup's two chunks, otherwise one per chunk.  (MT = 3
   // is never planned outside multi-plane items: its 192-column accumulator tile and two slabs of 384 positions plus halo exceed
   // 227 KB.)
@@ -318,14 +323,17 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
 
 // Picks the N tile (fixed 64 / 128 or runtime), the M tiles per work item and the slab rows for a geometry; *best_mt == 0
 // when no configuration fits in shared memory.
-static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out, bool* flex_out, int* best_mt_out, int* best_R_out) {
-  int BN = (a->ldy <= 64) ? 64 : 128;
+// G != 0 (grouped convolution): the N tiles are the K / 64 channel slices, each with a G-row weight stage per tap.
+static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out, bool* flex_out, int* best_mt_out, int* best_R_out,
+                              int G = 0) {
+  int BN = (G || a->ldy <= 64) ? 64 : 128;
   const int planes = a->N * p.To;
-  int ntn = (a->ldy + BN - 1) / BN;
+  int ntn = G ? a->K / 64 : (a->ldy + BN - 1) / BN;
   // Channel counts that tile badly by 128 (144, 288, 576 ... of R(2+1)D) take the runtime-N instance: the fewest
   // tiles of <= 256 columns, each a multiple of 16 wide.
   bool flex = false;
-  if (a->ldy > 128) {
+  if (G) {
+  } else if (a->ldy > 128) {
     const int tn = (a->ldy + 255) / 256;
     const int bn = (((a->ldy + tn - 1) / tn) + 15) / 16 * 16;
     if (bn <= kSlabAccCols && ((long long)bn * tn * 21 <= (long long)ntn * 128 * 20 || (g_slab_wide == 1 && a->ldy % 256 == 0))) {
@@ -339,7 +347,7 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
     p.bn = 16; p.wbytes = 2048; p.accs = 32;
   }
   const int acc_stride = flex ? p.accs : BN;
-  const int w_stage = flex ? p.wbytes : BN * 128;
+  const int w_stage = G ? G * 128 : flex ? p.wbytes : BN * 128;
   // Pick the M tiles per work item from a cycle model of one SM's share: rounds of items x the slower of the MMA
   // stream and the slab/weight loads (the epilogue of an item overlaps the next item's MMAs).  MT * N is bounded by the
   // consumers' register accumulators (kSlabAccCols).  (Model constants:
@@ -401,8 +409,9 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
 }
 
 // returns 1 when the slab kernel took the convolution, 0 when it does not apply, <0 on error
-static int try_slab(const b2_conv_args* a_in, cudaStream_t stream) {
-  if (g_conv_algo == 1) return 0;
+// G != 0: grouped convolution inside the contract of b2_conv_grouped_ndhwc_fprop (3x3 in plane, so never the temporal remap)
+static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0) {
+  if (g_conv_algo == 1 && !G) return 0;
   SlabParams p;
   b2_conv_args remap = *a_in;
   const b2_conv_args* a = a_in;
@@ -430,18 +439,22 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream) {
     SlabParams q;
     if (!slab_geometry(a, &q, wc_try[attempt])) { if (attempt == 0) return 0; else continue; }
     if (attempt > 0 && q.wchunks == 1) continue;              // same geometry as the default
-    if (g_conv_algo == 2 && q.ss != 1) return 0;              // debug: strided convs through the gather kernel
+    if (g_conv_algo == 2 && q.ss != 1 && !G) return 0;        // debug: strided convs through the gather kernel
+    if (G) q.cchunks = 1;                                     // an item reads its own 64-channel slice only
     int bn_c = 0, mt_c = 0, r_c = 0;
     bool flex_c = false;
-    const double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c);
+    const double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G);
     if (mt_c == 0) continue;
     if (best_mt == 0 || cost < best_cost) { best_p = q; BN = bn_c; flex = flex_c; best_mt = mt_c; best_R = r_c; best_cost = cost; }
   }
   if (best_mt != 0) p = best_p;
   if (best_mt == 0) return 0;
-  int rc = flex ? launch_slab<0>(a, p, best_mt, best_R, stream)
-                : (BN == 64) ? launch_slab<64>(a, p, best_mt, best_R, stream) : launch_slab<128>(a, p, best_mt, best_R, stream);
-  if (rc == B2_OK) set_last_kernel(KID_SLAB, BN, best_mt, flex, p.wchunks, a != a_in);
+  int rc = G == 16 ? launch_slab<64, 16>(a, p, best_mt, best_R, stream)
+           : G == 32 ? launch_slab<64, 32>(a, p, best_mt, best_R, stream)
+           : flex ? launch_slab<0>(a, p, best_mt, best_R, stream)
+                  : (BN == 64) ? launch_slab<64>(a, p, best_mt, best_R, stream) : launch_slab<128>(a, p, best_mt, best_R, stream);
+  if (rc == B2_OK && G) set_last_kernel(KID_GROUPCONV, G, best_mt, p.mp, p.wchunks);
+  else if (rc == B2_OK) set_last_kernel(KID_SLAB, BN, best_mt, flex, p.wchunks, a != a_in);
   return rc == B2_OK ? 1 : rc;
 }
 
@@ -955,7 +968,7 @@ int b2_debug_set_densem(int maxm, int force_s) { g_densem_maxm = maxm < 0 ? -2 :
 int b2_debug_set_slabts(int mode) { (void)mode; return B2_OK; }
 /* kernel of the last convolution / GEMM / attention call (a KID_* id of b2_host.h, 0 when the call launched nothing) and its
    tile parameters in info[0..4]: slab {BN, MT, flex, wchunks, remapped}, densem {bn, S}, pgemm / igemm {BN, masked}, stem {G, transposed},
-   attention {online, DVT}; unused entries are 0 */
+   attention {online, DVT}, grouped convolution {G, MT, planes per item, wchunks}; unused entries are 0 */
 int b2_debug_last_kernel(int* info) {
   if (info) memcpy(info, g_last_info, sizeof(g_last_info));
   return g_last_kernel;
@@ -1093,6 +1106,52 @@ int b2_conv_ndhwc_fprop(const b2_conv_args* a, void* stream) {
     // weights; the activation side zero-fills channels >= C, so those products vanish.
   }
   return dispatch_igemm(L, reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ------------------------------------------------------------------------------------------
+// grouped convolution (b2_groupconv.cuh)
+// ------------------------------------------------------------------------------------------
+static bool grouped_filter_ok(int K, int cg, int groups, int kt, int kh, int kw) {
+  return K > 0 && groups > 0 && K % 64 == 0 && (cg == 4 || cg == 8 || cg == 16 || cg == 32) && (long long)cg * groups == K &&
+         kh == 3 && kw == 3 && (kt == 1 || kt == 3);
+}
+
+size_t b2_pack_grouped_conv_weight_elems(int K, int Cin_per_group, int groups, int kt, int kh, int kw) {
+  if (!grouped_filter_ok(K, Cin_per_group, groups, kt, kh, kw)) return 0;
+  return (size_t)K * group_block(Cin_per_group) * kt * kh * kw;
+}
+
+int b2_pack_grouped_conv_weight(const float* w, void* out, int K, int Cin_per_group, int groups, int kt, int kh, int kw, void* stream) {
+  B2_CHECK_ARG(w && out, "null pointer");
+  const long long total = (long long)b2_pack_grouped_conv_weight_elems(K, Cin_per_group, groups, kt, kh, kw);
+  if (total == 0)
+    return set_error(B2_ERR_UNSUPPORTED, "grouped packing needs K == C, K %% 64 == 0, 4 / 8 / 16 / 32 channels per group and a 3x3x3 or "
+                                         "1x3x3 filter (got K=%d, %d per group, %d groups, %dx%dx%d)", K, Cin_per_group, groups, kt, kh, kw);
+  pack_grouped_weight_kernel<<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      w, reinterpret_cast<__half*>(out), Cin_per_group, kt * kh * kw, group_block(Cin_per_group), total);
+  B2_CHECK_LAUNCH("pack_grouped_weight_kernel");
+  return B2_OK;
+}
+
+int b2_conv_grouped_ndhwc_fprop(const b2_conv_args* a, int groups, void* stream) {
+  set_last_kernel(KID_NONE);
+  int rc = validate_conv(a);
+  if (rc != B2_OK) return rc;
+  B2_CHECK_ARG(a->mode == B2_CONV_AUTO && !a->out_f32 && !a->accumulate && !a->aff_ld && !a->upsample && !a->residual_up &&
+                   !a->residual_pre && !a->y2 && !a->scale2 && !a->shift2 && !a->aff2_ld && !a->pool_w && !a->in_scale && !a->in_shift &&
+                   !a->in_aff_ld && !a->mask && !a->ldm,
+               "the grouped convolution takes a plain fp16 call: mode, fp32 output, per-sample affines, generator and fine-tuning fields must be zero");
+  B2_CHECK_ARG(groups > 0, "groups must be positive");
+  const int cg = a->C / groups;
+  if (a->C != a->K || a->C % groups || !grouped_filter_ok(a->K, cg, groups, a->kt, a->kh, a->kw) || a->pt != a->kt / 2 || a->ph != 1 ||
+      a->pw != 1 || a->sh != a->sw || (a->sh != 1 && a->sh != 2) || (a->st != 1 && a->st != 2))
+    return set_error(B2_ERR_UNSUPPORTED, "grouped convolution needs C == K, C %% 64 == 0, 4 / 8 / 16 / 32 channels per group, a 3x3x3 or 1x3x3 "
+                                         "'same' filter and strides 1 or 2 (got C=%d K=%d groups=%d, %dx%dx%d, stride %d%d%d, padding %d%d%d)",
+                     a->C, a->K, groups, a->kt, a->kh, a->kw, a->st, a->sh, a->sw, a->pt, a->ph, a->pw);
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  rc = try_slab(a, reinterpret_cast<cudaStream_t>(stream), group_block(cg));
+  if (rc == 0) return set_error(B2_ERR_UNSUPPORTED, "no slab tiling of this image fits in shared memory (H=%d W=%d)", a->H, a->W);
+  return rc < 0 ? rc : B2_OK;
 }
 
 static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream);

@@ -27,6 +27,7 @@
 #pragma once
 
 #include "b2_ptx.cuh"
+#include "b2_groupconv.cuh"
 
 namespace b2 {
 
@@ -166,8 +167,9 @@ __device__ __forceinline__ uint32_t slab_t64_off16(int v0, uint32_t tile_stride1
 // Consumer warpgroups of slabconv_kernel for an N tile of N columns.  Warpgroup wg owns rows [64 wg, 64 wg + 64) of every M tile of
 // an item; tile j sits at fragment columns [j N, j N + N) of each thread's registers from the item's first K block to its last
 // (N = 64: the transposed product above).  The MMAs of one tap form one commit group, one group stays in flight, and a ring slot is
-// released when the group that read it retires.
-template <int N, int TMT>
+// released when the group that read it retires.  G != 0 (N = 64): the grouped convolution of b2_groupconv.cuh -- positions stay
+// along M and each K step of a tap goes into its own G-column range of the fragment.
+template <int N, int TMT, int G = 0>
 __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile& at, int accs, uint32_t slab0, uint32_t w0s,
                                               int w_bytes, uint64_t* slab_full, uint64_t* slab_empty, uint64_t* w_full,
                                               uint64_t* w_empty, uint64_t* acc_full, uint64_t* acc_empty) {
@@ -202,7 +204,7 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
         const uint64_t b = desc_from(kSw128DescHi, sw128_desc_lo(w0s + ws * w_bytes));
         const uint32_t a_lo0 = sw128_desc_lo(slab_addr + static_cast<uint32_t>(pix0) * 128u);
         wgmma_fence();
-        if constexpr (N == 64) {
+        if constexpr (N == 64 && G == 0) {
           // the weight stage is A, slab rows are B (the descriptor formats are the same K-major SWIZZLE_128B)
           if constexpr (TMT == 0) {
 #pragma unroll
@@ -217,8 +219,13 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
           }
         } else {
 #pragma unroll
-          for (int j = 0; j < kMaxMT; ++j)
-            if (j < mt_valid) slab_mma<N>(acc + j * (N / 2), desc_from(kSw128DescHi, a_lo0 + a_wg + j * tile_stride16), b, ksteps);
+          for (int j = 0; j < kMaxMT; ++j) {
+            if (j < mt_valid) {
+              const uint64_t a = desc_from(kSw128DescHi, a_lo0 + a_wg + j * tile_stride16);
+              if constexpr (G != 0) group_mma<G>(acc + j * (N / 2), a, b);
+              else slab_mma<N>(acc + j * (N / 2), a, b, ksteps);
+            }
+          }
         }
         wgmma_commit();
         wgmma_wait1();                                       // the previous tap's group has retired: release what it read
@@ -238,7 +245,7 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
     }
     // hand the item to the epilogue: one store of the fragments into the accumulator tile, then straight on to the next item
     mbar_wait(acc_empty, (lt & 1) ^ 1);
-    if constexpr (N == 64) {
+    if constexpr (N == 64 && G == 0) {
       // transposed into the [position][channel] tile: fragment (channel ch (+8), positions v, v + 1) goes to row v & 127 of tile
       // v >> 7.  A pitch of 4 (mod 32) floats puts the 8 channels x 4 even positions of one store in 32 distinct banks.
       // (32-bit shared addresses stepped from one base: the 96 accumulators leave no room for a 64-bit pointer per store)
@@ -269,16 +276,20 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
   }
 }
 
-// BN = 0: N tile taken from SlabParams::bn at run time.  TMT: the 64-wide tile's MMA form (slab_consumer; 0 for the other tiles)
-template <int BN, int TMT = 0>
+// BN = 0: N tile taken from SlabParams::bn at run time.  TMT: the 64-wide tile's MMA form (slab_consumer; 0 for the other tiles).
+// G = 16 / 32 (BN = 64): grouped convolution with C == K (b2_groupconv.cuh).  N tile tn is the 64-channel slice tn of input AND
+// output, the item has one channel chunk (SlabParams::cchunks = 1) whose TMA channel coordinate is the slice's, and a weight stage
+// is the G-row tile of (slice, tap).
+template <int BN, int TMT = 0, int G = 0>
 __global__ void __launch_bounds__(kSlabThreads, 1)
 slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N*T), box (64, PW, R, 1)
-                const __grid_constant__ CUtensorMap tmB,   // weights [Ncols][taps*C], box (64, BN)
+                const __grid_constant__ CUtensorMap tmB,   // weights [Ncols][taps*C], box (64, BN); G: [slices*taps*G][64], box (64, G)
                 const SlabParams p) {
+  static_assert(G == 0 || (BN == 64 && TMT == 0), "the grouped form runs on the 64-wide tile with positions along M");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align<1024>(smem_raw);
   const int bn = BN ? BN : p.bn;
-  const int kWBytes = BN ? BN * 128 : p.wbytes;      // stage stride; a stage receives bn * 128 bytes
+  const int kWBytes = G ? G * 128 : BN ? BN * 128 : p.wbytes;      // stage stride; a stage receives bn * 128 (G * 128) bytes
   const int accs = BN ? BN : p.accs;
   uint8_t* slab_base = smem;
   uint8_t* w_base = smem + kSlabSStages * p.slab_bytes;
@@ -333,7 +344,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
         mbar_wait(&slab_empty[s], ((sg / kSlabSStages) & 1) ^ 1);
         if (elect_one()) {
           mbar_expect_tx(&slab_full[s], static_cast<uint32_t>(p.R * p.PW * 128 * (p.mp > 1 ? p.mp : 1)));
-          tma_load_4d(slab_base + s * p.slab_bytes, &tmX, &slab_full[s], cc * 64,
+          tma_load_4d(slab_base + s * p.slab_bytes, &tmX, &slab_full[s], G ? nxt.n0 : cc * 64,
                       p.sub_w0[sub] + p.ss * nxt.wc * p.WC, p.ss * nxt.r_lo + p.sub_h0[sub], nxt.plane_i0 + dt);
         }
         __syncwarp();
@@ -358,8 +369,9 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
             mbar_wait(&w_empty[ws], ((wit / kSlabWStages) & 1) ^ 1);
             const int tap = dt * p.khw + p.sub_tap[sub][ti];
             if (elect_one()) {
-              mbar_expect_tx(&w_full[ws], static_cast<uint32_t>(bn * 128));
-              tma_load_2d(w_base + ws * kWBytes, &tmB, &w_full[ws], tap * p.C + cc * 64, cur.n0);
+              mbar_expect_tx(&w_full[ws], static_cast<uint32_t>(G ? G * 128 : bn * 128));
+              if constexpr (G != 0) tma_load_2d(w_base + ws * kWBytes, &tmB, &w_full[ws], 0, ((cur.n0 >> 6) * p.kt * p.khw + tap) * G);
+              else tma_load_2d(w_base + ws * kWBytes, &tmB, &w_full[ws], tap * p.C + cc * 64, cur.n0);
             }
             __syncwarp();
             if (ti == pf && nxt_item < p.items_total) load_next();
@@ -371,7 +383,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
     // ================================ consumer warpgroups ===============================
     const uint32_t slab0 = smem_u32(slab_base), w0s = smem_u32(w_base);
     if constexpr (BN != 0) {
-      slab_consumer<BN, TMT>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty);
+      slab_consumer<BN, TMT, G>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty);
     } else {
       // runtime N: one compiled main loop per width the tile planner can pick (launch_slab rejects any other)
       switch (bn) {

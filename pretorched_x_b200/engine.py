@@ -142,8 +142,18 @@ def _conv_geometry(conv):
     return _triple(conv.stride), _triple(conv.padding)
 
 
-def packed_conv(conv, bn, in_pitch, stem=False, stride=None):
-    """PackedConv for a plain nn.Conv3d / nn.Conv2d followed (optionally) by BatchNorm ``bn``."""
+def grouped_route(conv, stride=None):
+    """True when ``packed_conv`` packs ``conv`` for the group-aware kernel (ops.PackedGroupedConv), from its shape alone."""
+    cstride, padding = _conv_geometry(conv)
+    w = conv.weight
+    kernel = (1,) + tuple(w.shape[2:]) if w.dim() == 4 else tuple(w.shape[2:])
+    return ops.grouped_pack_applies(w.shape[0], w.shape[1] * conv.groups, conv.groups, kernel, stride or cstride, padding)
+
+
+def packed_conv(conv, bn, in_pitch, stem=False, stride=None, dense=False):
+    """PackedConv for a plain nn.Conv3d / nn.Conv2d followed (optionally) by BatchNorm ``bn``; ops.PackedGroupedConv for a
+    grouped convolution inside the group-aware kernel's contract (``grouped_route``) unless ``dense`` asks for the dense
+    layout (the CUDA-core cross-check reads no other)."""
     if any(d != 1 for d in conv.dilation):
         raise NotImplementedError("dilated convolutions are outside the engine's scope")
     if conv.groups != 1 and stem:
@@ -152,8 +162,13 @@ def packed_conv(conv, bn, in_pitch, stem=False, stride=None):
     cstride, padding = _conv_geometry(conv)
     if stride is None:
         stride = cstride
-    # grouped convolution (ResNeXt-3D, resnext3D.py:86-93): packed as the block-diagonal dense filter, see ops.dense_from_grouped
-    return _cached(conv, "pc", sig,
+    if not stem and not dense and grouped_route(conv, stride):
+        # conv2 of ResNeXtBottleneck (resnext3D.py:86-93) and its 2-D counterpart: in_pitch is the channel count (C % 64 == 0)
+        return _cached(conv, "pc", sig,
+                       lambda: ops.PackedGroupedConv(conv.weight.detach(), conv.groups, conv.bias, bn, stride, padding),
+                       reads=_bn_tensors(bn))
+    # any other grouped convolution: the block-diagonal dense filter, see ops.dense_from_grouped
+    return _cached(conv, "pc_dense" if dense else "pc", sig,
                    lambda: ops.PackedConv(ops.dense_from_grouped(conv.weight.detach(), conv.groups), conv.bias, bn, stride, padding,
                                           in_pitch=in_pitch, stem=stem), reads=_bn_tensors(bn))
 
@@ -190,7 +205,7 @@ def conv_bn_act(conv, bn, a, residual=None, relu=False, simt=False, pool_w=False
         sub = ops.shortcut_a(a, stride[0], a.C)
         pc = packed_conv(conv, bn, sub.ld, stride=(1, 1, 1))
         return ops.conv(sub, pc, residual=residual, relu=relu, out=out)
-    pc = packed_conv(conv, bn, a.ld, stem=stem)
+    pc = packed_conv(conv, bn, a.ld, stem=stem, dense=simt)
     return ops.conv(a, pc, residual=residual, relu=relu, simt=simt, pool_w=pool_w, out=out)
 
 

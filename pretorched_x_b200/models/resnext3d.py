@@ -7,10 +7,12 @@ runs ``modify_resnets`` on this family, so there is no ``last_linear`` in its ``
 the reference's tensors in the reference's order (seeded init is bit-identical, checkpoints such as
 ``resnext3d101_kinetics-8e57b772.pth`` load unchanged); the block body is ``engine.run_bottleneck``.
 
-Grouped convolution on the tensor cores: a group of resnext3d50 is 4..32 channels wide -- far below one MMA tile -- so the
-engine packs the grouped filter as the block-diagonal DENSE filter ``[K][taps][C]`` (zeros off the diagonal, built once when
-weights are packed) and runs the ordinary slab convolution: same result, every kernel already verified, at the cost of
-multiplying by zeros (the dense 3x3x3 layers run at ~1 PFLOP/s; a 128-wide grouped layer costs what a 128-wide dense one does).
+Grouped convolution on the tensor cores: a group is 4..32 channels wide -- far below one MMA tile -- but a 64-channel slice
+holds whole groups and reads only its own 64 input channels.  ``conv2`` runs the slab convolution per slice with the filter
+packed as its diagonal 16 x 16 (32 x 32) blocks, each K step of a tap accumulating into its own 16 (32) output columns
+(``ops.PackedGroupedConv``, csrc/b2_groupconv.cuh): 4x / 2x / 1x / 1x the grouped multiply-accumulates for 4 / 8 / 16 / 32
+channels per group, and ``C * 16 * 27`` (``C * 32 * 27``) filter elements.  A grouped convolution outside that kernel's
+contract is packed as the block-diagonal DENSE filter (``ops.dense_from_grouped``): same result at ``groups`` times the work.
 Like R(2+1)D the class additionally offers ``features / logits / last_linear`` (alias of ``fc``).  Upstream quirk kept: ``fc``
 is sized ``cardinality * 32 * expansion`` (resnext3D.py:139) while the trunk always ends with 2048 channels, so only the
 default ``cardinality=32`` yields a network whose forward works -- here as there.

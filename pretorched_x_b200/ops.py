@@ -195,11 +195,49 @@ class PackedConv:
         self.scale, self.shift = fold_affine(K, bias, bn, weight.device)
 
 
+def grouped_pack_applies(K, C, groups, kernel, stride, padding):
+    """Does the group-aware kernel (b2_conv_grouped_ndhwc_fprop) take a grouped convolution C -> K?  Its contract, from the shape
+    alone: C == K, C % 64 == 0, 4 / 8 / 16 / 32 channels per group, a 3x3x3 or 1x3x3 filter with 'same' padding, in-plane
+    stride 1 or 2 (equal in H and W), temporal stride 1 or 2.  Everything else runs the dense filter of ``dense_from_grouped``."""
+    kt, kh, kw = kernel
+    return (groups > 1 and C == K and C % 64 == 0 and C % groups == 0 and C // groups in (4, 8, 16, 32) and (kh, kw) == (3, 3)
+            and kt in (1, 3) and tuple(padding) == (kt // 2, 1, 1) and stride[1] == stride[2] and stride[1] in (1, 2)
+            and stride[0] in (1, 2))
+
+
+class PackedGroupedConv:
+    """Grouped filter (nn.Conv3d / nn.Conv2d weight [K][C / groups][...], C == K) in the group-aware kernel's layout -- fp16
+    [K / 64][taps][G][64], G = 16 (32 for 32 channels per group), see include/b2_pretorched.h -- + the folded per-channel affine.
+    ``ops.conv`` runs it with b2_conv_grouped_ndhwc_fprop (conv2 of ResNeXtBottleneck, resnext3D.py:86-93)."""
+    __slots__ = ("w", "scale", "shift", "K", "Cin", "C", "k", "s", "p", "groups")
+
+    @_on_device
+    def __init__(self, weight, groups, bias=None, bn=None, stride=(1, 1, 1), padding=(0, 0, 0)):
+        _require_cuda(weight, "conv weight")
+        if weight.dim() == 4:       # Conv2d weight -> T = 1
+            weight = weight.unsqueeze(2)
+        K, cg, kt, kh, kw = weight.shape
+        self.K, self.Cin, self.C, self.groups = K, cg, cg * groups, int(groups)
+        self.k = (kt, kh, kw)
+        self.s = tuple(int(v) for v in stride)
+        self.p = tuple(int(v) for v in padding)
+        if not grouped_pack_applies(K, self.C, self.groups, self.k, self.s, self.p):
+            raise ValueError("grouped convolution %d -> %d, groups %d, kernel %s, stride %s, padding %s is outside the group-aware "
+                             "kernel's contract" % (self.C, K, groups, self.k, self.s, self.p))
+        lib = _lib.load()
+        n = lib.b2_pack_grouped_conv_weight_elems(K, cg, self.groups, kt, kh, kw)
+        self.w = torch.empty(n, dtype=torch.float16, device=weight.device)
+        _lib.check(lib.b2_pack_grouped_conv_weight(_ptr(weight.detach().contiguous().float()), _ptr(self.w), K, cg, self.groups, kt, kh,
+                                                   kw, _stream()), "b2_pack_grouped_conv_weight")
+        self.scale, self.shift = fold_affine(K, bias, bn, weight.device)
+
+
 def dense_from_grouped(weight, groups):
     """Grouped-convolution filter [K][C/groups][...] -> the block-diagonal dense filter [K][C][...] (zeros off the diagonal).
     Output channel k belongs to group k // (K / groups) and reads input channels [g * C/groups, (g + 1) * C/groups)
-    (nn.Conv3d semantics, resnext3D.py:86-93).  Groups of the ResNeXt-3D nets are 4..32 channels wide -- far below an MMA
-    tile -- so the tensor-core path runs the dense filter; the product with the zero blocks is exact."""
+    (nn.Conv3d semantics, resnext3D.py:86-93).  The product with the zero blocks is exact, at ``groups`` times the
+    multiply-accumulates and filter memory: the route of grouped shapes outside ``grouped_pack_applies`` (and of the CUDA-core
+    cross-check), and the reference the group-aware kernel is tested against."""
     K, cg = weight.shape[0], weight.shape[1]
     if groups == 1:
         return weight
@@ -263,6 +301,11 @@ def conv(a, pc, residual=None, relu=False, simt=False, sample_affine=None, resid
     shape; the result is zeroed where mask <= 0 (the ReLU derivative of the fine-tuning backward, b2_conv_args.mask)."""
     if a.ld != pc.C:
         raise ValueError("activation pitch %d != packed filter pitch %d" % (a.ld, pc.C))
+    if isinstance(pc, PackedGroupedConv):
+        if simt or sample_affine is not None or residual_up or residual_pre or next_affine is not None or pool_w \
+                or in_affine is not None or mask is not None:
+            raise ValueError("a grouped pack runs the plain tensor-core call only (residual, relu, out=)")
+        return _conv_grouped(a, pc, residual, relu, out)
     kt, kh, kw = pc.k
     To, Ho, Wo = (_out_dim(a.T, kt, pc.s[0], pc.p[0]), _out_dim(a.H, kh, pc.s[1], pc.p[1]),
                   _out_dim(a.W, kw, pc.s[2], pc.p[2]))
@@ -330,6 +373,34 @@ def conv(a, pc, residual=None, relu=False, simt=False, sample_affine=None, resid
         _lib.check(fn(ctypes.byref(args), _stream()), "b2_conv_ndhwc_fprop")
     out = Act(y, a.N, To, Ho, Wo, pc.K)
     return (out, Act(y2, a.N, To, Ho, Wo, pc.K)) if y2 is not None else out
+
+
+def _conv_grouped(a, pc, residual, relu, out):
+    """``conv`` for a PackedGroupedConv: b2_conv_grouped_ndhwc_fprop."""
+    kt, kh, kw = pc.k
+    To, Ho, Wo = (_out_dim(a.T, kt, pc.s[0], pc.p[0]), _out_dim(a.H, kh, pc.s[1], pc.p[1]), _out_dim(a.W, kw, pc.s[2], pc.p[2]))
+    M = a.N * To * Ho * Wo
+    y = _out_rows(out, M, pc.K) if out is not None else torch.empty((M, pc.K), dtype=torch.float16, device=a.data.device)
+    if residual is not None and residual.M != M:
+        raise ValueError("residual rows %d do not match output rows %d" % (residual.M, M))
+    args = ConvArgs()
+    args.x, args.w, args.scale, args.shift = _ptr(a.data), _ptr(pc.w), _ptr(pc.scale), _ptr(pc.shift)
+    args.residual = _ptr(residual.data if residual is not None else None)
+    args.y = _ptr(y)
+    args.N, args.T, args.H, args.W, args.C = a.N, a.T, a.H, a.W, a.ld
+    args.K, args.ldy = pc.K, pc.K
+    args.ldr = residual.ld if residual is not None else 0
+    args.kt, args.kh, args.kw = kt, kh, kw
+    args.st, args.sh, args.sw = pc.s
+    args.pt, args.ph, args.pw = pc.p
+    args.relu, args.mode = int(relu), B2_CONV_AUTO
+    taps = kt * kh * kw
+    flops = 2.0 * M * pc.K * pc.Cin * taps                                # algorithmic (padding taps included)
+    nbytes = 2.0 * (a.M * a.C + M * pc.K * (2 if residual is not None else 1) + pc.K * pc.Cin * taps)
+    desc = "gconv %dx%dx%d s%s C%d g%d M=%d" % (kt, kh, kw, "".join(map(str, pc.s)), pc.K, pc.groups, M)
+    with _timed("conv", desc, flops, nbytes):
+        _lib.check(_lib.load().b2_conv_grouped_ndhwc_fprop(ctypes.byref(args), pc.groups, _stream()), "b2_conv_grouped_ndhwc_fprop")
+    return Act(y, a.N, To, Ho, Wo, pc.K)
 
 
 @_on_device
