@@ -54,7 +54,8 @@ typedef struct b2_conv_args {
   const void* w;        /* fp16 packed [K][taps][C] (b2_pack_conv_weight), taps = kt*kh*kw        */
   const float* scale;   /* fp32 [K]                                                                */
   const float* shift;   /* fp32 [K]                                                                */
-  const void* residual; /* nullable; fp16 [M][ldr], M = N*To*Ho*Wo                                 */
+  const void* residual; /* nullable; fp16 [M][ldr], M = N*To*Ho*Wo.  Only columns [0, K) are read: whatever columns
+                           [K, ldr) hold (a wider skip tensor's dropped channels) never reaches y, and ldr < ldy is fine */
   void* y;              /* fp16 [M][ldy]  (fp32 when out_f32)                                      */
   int32_t N, T, H, W, C;
   int32_t K;            /* logical output channels; columns [K, ldy) of an fp16 y are written as zero, those of an fp32 y
@@ -134,7 +135,7 @@ typedef struct b2_gemm_args {
   const void* b; /* fp16 [N][ldb] */
   const float* scale;
   const float* shift;
-  const void* residual; /* nullable fp16 [M][ldr] */
+  const void* residual; /* nullable fp16 [M][ldr]; only columns [0, N) are read */
   void* d;              /* fp16 [M][ldd] or fp32 when out_f32 */
   int32_t M, N, Kd;
   int32_t lda, ldb, ldd, ldr;

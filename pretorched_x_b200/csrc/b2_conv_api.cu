@@ -672,7 +672,8 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     if ((rc = make_tmap_2d_f16(&tmC, p.y, (uint64_t)p.ldy, (uint64_t)p.M_total, (uint64_t)p.ldy, 64, kBM, true)) != B2_OK)
       return rc;
     if (p.residual) {
-      if ((rc = make_tmap_2d_f16(&tmR, p.residual, (uint64_t)p.ldr, (uint64_t)p.M_total, (uint64_t)p.ldr, 64, kBM, true)) != B2_OK)
+      // column extent Ncols, not ldr: residual columns >= K are never read (TMA zero-fills them), so y's padding stays zero
+      if ((rc = make_tmap_2d_f16(&tmR, p.residual, (uint64_t)p.Ncols, (uint64_t)p.M_total, (uint64_t)p.ldr, 64, kBM, true)) != B2_OK)
         return rc;
     } else {
       tmR = tmC;
@@ -807,13 +808,15 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
   if ((rc = make_tmap_2d_f16(&tmC, ip.y, (uint64_t)ip.ldy, (uint64_t)ip.M_total, (uint64_t)ip.ldy, 64, 64, true)) != B2_OK) return rc;
   const int up_W = ip.up_W > 0 ? ip.up_W : 2;
   const int res_rows = up_W >= 128 ? 64 : 32;
+  // residual maps span Ncols columns, not ldr: columns >= K (a skip tensor's dropped channels, whatever lies in the pitch gap) are
+  // never read -- TMA zero-fills them -- so the output's padding columns stay zero
   if (ip.residual && ip.res_up) {
     // low-res skip tensor: a tile's 128 output rows read res_rows consecutive rows of it (see PgemmParams::res_up)
     if (!(up_W % 128 == 0 || (up_W <= 64 && 64 % up_W == 0)))
       return set_error(B2_ERR_UNSUPPORTED, "residual_up needs an output width that is a multiple of 128 or divides 64 (got %d)", up_W);
-    if ((rc = make_tmap_2d_f16(&tmR, ip.residual, (uint64_t)ip.ldr, (uint64_t)ip.M_total / 4, (uint64_t)ip.ldr, 64, res_rows, true)) != B2_OK) return rc;
+    if ((rc = make_tmap_2d_f16(&tmR, ip.residual, (uint64_t)ip.Ncols, (uint64_t)ip.M_total / 4, (uint64_t)ip.ldr, 64, res_rows, true)) != B2_OK) return rc;
   } else if (ip.residual) {
-    if ((rc = make_tmap_2d_f16(&tmR, ip.residual, (uint64_t)ip.ldr, (uint64_t)ip.M_total, (uint64_t)ip.ldr, 64, 128, true)) != B2_OK) return rc;
+    if ((rc = make_tmap_2d_f16(&tmR, ip.residual, (uint64_t)ip.Ncols, (uint64_t)ip.M_total, (uint64_t)ip.ldr, 64, 128, true)) != B2_OK) return rc;
   } else {
     tmR = tmC;
   }
@@ -843,7 +846,7 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
   const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
   B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, GAN, MASK>, dim3(grid), dim3(GAN ? kPgThreadsGan : kPgThreads), S::kTotal, stream, tmA, tmB, tmA2, tmB2, tmC, tmR, tmC2, p));
   B2_CHECK_LAUNCH("pgemm_kernel");
-  set_last_kernel(KID_PGEMM, BN, MASK);
+  set_last_kernel(KID_PGEMM, BN, MASK, GAN);
   return B2_OK;
 }
 
@@ -967,7 +970,8 @@ int b2_debug_set_densem(int maxm, int force_s) { g_densem_maxm = maxm < 0 ? -2 :
    stays for the ABI and accepts its argument with no effect. */
 int b2_debug_set_slabts(int mode) { (void)mode; return B2_OK; }
 /* kernel of the last convolution / GEMM / attention call (a KID_* id of b2_host.h, 0 when the call launched nothing) and its
-   tile parameters in info[0..4]: slab {BN, MT, flex, wchunks, remapped}, densem {bn, S}, pgemm / igemm {BN, masked}, stem {G, transposed},
+   tile parameters in info[0..4]: slab {BN, MT, flex, wchunks, remapped}, densem {bn, S}, pgemm {BN, masked, generator instance},
+   igemm {BN, masked}, stem {G, transposed},
    attention {online, DVT}, grouped convolution {G, MT, planes per item, wchunks}; unused entries are 0 */
 int b2_debug_last_kernel(int* info) {
   if (info) memcpy(info, g_last_info, sizeof(g_last_info));

@@ -492,6 +492,22 @@ __device__ __forceinline__ float2 unpack_half2(uint32_t u) {
   return __half22float2(h);
 }
 
+// Residual chunk of 8 fp16 channels [c, c + 8) of a row whose logical width is ncols: loaded only when c < ncols, lanes >= ncols
+// zeroed -- the residual's columns past K (a skip tensor's dropped channels, its pitch gap) never reach the output's zero padding,
+// and a pitch narrower than the output's never reads the next row.
+__device__ __forceinline__ uint4 ld_res8(const __half* src, int c, int ncols) {
+  if (c >= ncols) return make_uint4(0u, 0u, 0u, 0u);
+  uint4 v = __ldg(reinterpret_cast<const uint4*>(src));
+  const int n = ncols - c;                       // valid lanes (>= 8: all)
+  if (n < 8) {
+    uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) w[e] = 2 * e + 1 < n ? w[e] : 2 * e < n ? (w[e] & 0xFFFFu) : 0u;
+    v = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+  return v;
+}
+
 // Division by a run-time constant as a 64-bit multiply + shift (exact for 0 <= n < 2^31): the work-item decode and the
 // epilogue's position -> (row, column) split run once per item in every warp; with few-tap 2-D filters an item is short
 // enough that the ~25-instruction integer division sequences show up in the issue-slot budget.

@@ -77,7 +77,7 @@ struct SlabParams {
   int tiles_n, tiles_q, items_total;
   const float* scale;
   const float* shift;
-  const __half* residual;  // nullable, dense [M][ldr]
+  const __half* residual;  // nullable, dense [M][ldr]; only columns < Ncols are read
   int ldr;
   __half* y;               // dense [M][ldy]
   int ldy;
@@ -457,7 +457,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
                 const __half* rrow = p.residual + row[j] * p.ldr + c0;
 #pragma unroll
                 for (int c8 = 0; c8 < 4; ++c8)
-                  if (jc * 32 + c8 * 8 < ncols_here) rres[c8] = __ldg(reinterpret_cast<const uint4*>(rrow + c8 * 8));
+                  if (jc * 32 + c8 * 8 < ncols_here) rres[c8] = ld_res8(rrow + c8 * 8, c0 + c8 * 8, p.Ncols);   // columns >= K: zero
               }
               // accumulators are read 8 columns at a time next to their use: with the scale / shift and residual registers a
               // whole 32-column row segment would not fit the register budget

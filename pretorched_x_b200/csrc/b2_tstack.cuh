@@ -44,7 +44,7 @@ struct TstackParams {
   int Ncols, ldy, ldr, relu;
   const float* scale;
   const float* shift;
-  const __half* residual;  // nullable, dense [M][ldr]
+  const __half* residual;  // nullable, dense [M][ldr]; only columns < Ncols are read
   __half* y;               // dense [M][ldy]
   FastDiv fd_tiles_q, fd_groups;
 };
@@ -185,7 +185,7 @@ tstack_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, HW, 1, 
           const __half* rrow = p.residual + (row0 + static_cast<size_t>(s) * p.HW) * p.ldr + c0;
 #pragma unroll
           for (int c8 = 0; c8 < 4; ++c8)
-            if (c0 + c8 * 8 < ncols_here) rres[s][c8] = __ldg(reinterpret_cast<const uint4*>(rrow + c8 * 8));
+            if (c0 + c8 * 8 < ncols_here) rres[s][c8] = ld_res8(rrow + c8 * 8, c0 + c8 * 8, p.Ncols);   // columns >= K: zero
         }
       };
       load_res(0);

@@ -7,6 +7,8 @@ Bound, per output element:  |got - ref| <= a * 2^-11 * |ref| + b * A + 2^-24, wi
   a = 1 for fp16 output (one rounding to fp16), 0 for fp32 output,
   b = 2^-14: the fp32 accumulation inside wgmma is neither IEEE-sequential nor documented, so this allows 2^10 fp32 units
       of roundoff on the sum of magnitudes -- far below what one dropped tap, channel chunk or output row costs.
+The generator epilogues (per-sample affine, fused upsample, upsampled / pre-affine residual, second output, input affine) use
+the same bound with the magnitude of each epilogue's own terms; see ``epilogue`` below.
 """
 import torch
 import torch.nn.functional as F
@@ -61,3 +63,137 @@ def where_worst(got, ref, A, f16):
     i = int(torch.argmax(r))
     m, c = divmod(i, ref.shape[1])
     return "row %d col %d: got %r ref %r A %r" % (m, c, float(got.reshape(ref.shape)[m, c]), float(ref[m, c]), float(A[m, c]))
+
+
+# ---------------------------------------------------------------------------------------------
+# generator epilogues (tests/test_gpu_epilogue_matrix.py, tests/test_epilogue_matrix_cpu.py): the accumulator and its magnitude
+# come from one of the *_acc functions, the epilogue from ``epilogue`` -- all in fp64 from exactly the operands the kernel reads,
+# every element held to the same bound as above.
+# ---------------------------------------------------------------------------------------------
+def conv_acc(x, w, k, s, p):
+    """sum_{tap,c} x * w and sum |x * w| of a convolution (x [N, T, H, W, C], w [K, taps, C]): fp64 [M, K] each."""
+    x, w = x.double().cpu(), w.double().cpu()
+    K, C = w.shape[0], x.shape[-1]
+    wt = w.reshape(K, k[0], k[1], k[2], C).permute(0, 4, 1, 2, 3)
+    xt = x.permute(0, 4, 1, 2, 3)
+    acc = F.conv3d(xt, wt, stride=s, padding=p).permute(0, 2, 3, 4, 1).reshape(-1, K)
+    mag = F.conv3d(xt.abs(), wt.abs(), stride=s, padding=p).permute(0, 2, 3, 4, 1).reshape(-1, K)
+    return acc, mag
+
+
+def gemm_acc(a, b):
+    """A[M][Kd] . B[N][Kd]^T and its magnitude, fp64."""
+    a, b = a.double().cpu(), b.double().cpu()
+    return a @ b.t(), a.abs() @ b.abs().t()
+
+
+def upconv_acc(x, wph):
+    """conv3x3(nearest_up2(x)) as the kernel computes it: four 2x2 phase convolutions of the LOW-res image x [N, H, W, C]
+    (or [N, 1, H, W, C]) with the packed phase filter wph [K, 16, C] read back from the pack.  Output pixel (2h + py, 2w + px)
+    reads low-res pixel (h - 1 + py + a, w - 1 + px + b) with tap (2 py + px) * 4 + 2 a + b.  fp64 [N * 2H * 2W, K] each."""
+    x = x.double().cpu()
+    if x.dim() == 5:
+        x = x[:, 0]
+    N, H, W, C = x.shape
+    wph = wph.double().cpu()
+    K = wph.shape[0]
+    xp = F.pad(x.permute(0, 3, 1, 2), (1, 1, 1, 1))
+    acc = torch.zeros(N, K, 2 * H, 2 * W, dtype=torch.float64)
+    mag = torch.zeros_like(acc)
+    for py in (0, 1):
+        for px in (0, 1):
+            ph = 2 * py + px
+            f = wph[:, ph * 4:ph * 4 + 4].reshape(K, 2, 2, C).permute(0, 3, 1, 2)
+            src = xp[:, :, py:py + H + 1, px:px + W + 1]
+            acc[:, :, py::2, px::2] = F.conv2d(src, f)
+            mag[:, :, py::2, px::2] = F.conv2d(src.abs(), f.abs())
+    return acc.permute(0, 2, 3, 1).reshape(-1, K), mag.permute(0, 2, 3, 1).reshape(-1, K)
+
+
+# low-res 3x3 rows (or columns) that fold into tap a of output phase p: p = 0 -> {0}, {1, 2}; p = 1 -> {0, 1}, {2}
+UP_FOLD = {(0, 0): (0,), (0, 1): (1, 2), (1, 0): (0, 1), (1, 1): (2,)}
+
+
+def upconv_fold(w):
+    """fp64 fold of a 3x3 filter w [K, Cin, 3, 3] into the phase filter [K, 16, Cin] of b2_pack_upconv3x3_weight, and the sum of
+    |w| over the taps each folded weight adds (its rounding scale)."""
+    w = w.double().cpu()
+    K, Cin = w.shape[:2]
+    fold = torch.zeros(K, 16, Cin, dtype=torch.float64)
+    mag = torch.zeros_like(fold)
+    for py in (0, 1):
+        for px in (0, 1):
+            for a in (0, 1):
+                for b in (0, 1):
+                    t = (2 * py + px) * 4 + 2 * a + b
+                    for r in UP_FOLD[(py, a)]:
+                        for c in UP_FOLD[(px, b)]:
+                            fold[:, t] += w[:, :, r, c]
+                            mag[:, t] += w[:, :, r, c].abs()
+    return fold, mag
+
+
+def nearest_up2(skip, N, H, W, K):
+    """The first K channels of a low-res skip tensor [N * (H/2) * (W/2)][>= K], nearest-2x upsampled to [N * H * W][K] (fp64)."""
+    s = skip[:, :K].double().cpu().reshape(N, H // 2, W // 2, K)
+    return s.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2).reshape(-1, K)
+
+
+def per_row(v, rows, M, K):
+    """Per-sample rows [N][>= K] -> the [M][K] rows the elements use (row m takes sample m // rows); [K] stays [K]."""
+    v = v.double().cpu()
+    if v.dim() == 1:
+        return v[:K]
+    return v[:, :K].repeat_interleave(rows, dim=0)[:M]
+
+
+def epilogue(acc, mag, scale, shift, residual=None, pre=False, relu=False):
+    """Value of an output element before its fp16 rounding, and its magnitude A.  scale / shift: [K] or per-row [M][K] (see
+    ``per_row``); residual: fp64 [M][K].  pre: the residual joins before the affine, v = s * (acc + r) + t with
+    A = |s| * (sum |xw| + |r|) + |t|; otherwise v = s * acc + t + r with A = |s| * sum |xw| + |t| + |r|."""
+    s, t = scale.double().cpu(), shift.double().cpu()
+    if residual is not None and pre:
+        r = residual.double().cpu()
+        v, A = s * (acc + r) + t, s.abs() * (mag + r.abs()) + t.abs()
+    else:
+        v, A = s * acc + t, s.abs() * mag + t.abs()
+        if residual is not None:
+            r = residual.double().cpu()
+            v, A = v + r, A + r.abs()
+    if relu:
+        v = v.clamp_min(0.0)
+    return v, A
+
+
+def second_output(v, A, scale2, shift2):
+    """y2 = relu(s2 * v + t2) from the first output's value v BEFORE its fp16 rounding: (ref2, A2 = |s2| A + |t2|)."""
+    s2, t2 = scale2.double().cpu(), shift2.double().cpu()
+    return (s2 * v + t2).clamp_min(0.0), s2.abs() * A + t2.abs()
+
+
+# relative distance to an fp16 rounding midpoint inside which an fp32 FMA followed by a rounding to fp16 may round the other way
+MIDPOINT_REL = 2.0 ** -23
+
+
+def in_affine_operand(x, scale, shift, rows):
+    """The A operand of a convolution with an input affine: x' = fp16(relu(x * s_n + t_n)), x fp16 [M][C], scale / shift fp32
+    [N][>= C].  Returns (x', other): x' the fp16 rounding of the fp64 value, ``other`` the magnitude of the neighbouring fp16
+    value where the fp64 value lies within MIDPOINT_REL of a rounding midpoint (the kernel's fp32 FMA may land on either side;
+    0 elsewhere)."""
+    x = x.double().cpu()
+    M, C = x.shape
+    v = (x * per_row(scale, rows, M, C) + per_row(shift, rows, M, C)).clamp_min(0.0)
+    lo = (v * (1 - MIDPOINT_REL)).half().double()
+    hi = (v * (1 + MIDPOINT_REL)).half().double()
+    amb = lo != hi
+    return v.half().double(), torch.where(amb, torch.maximum(lo.abs(), hi.abs()), torch.zeros_like(v))
+
+
+def in_affine_acc(x, w, scale, shift, rows):
+    """acc / magnitude of relu(x * s_n + t_n) . w^T (w [K][C]).  An operand that may round either way moves by at most one
+    fp16 unit, 2^-10 |x'|: its products enter A with the weight 2^-10 / B_ACC, so the bound B_ACC * A covers the flip."""
+    xq, other = in_affine_operand(x, scale, shift, rows)
+    acc, mag = gemm_acc(xq, w)
+    if bool((other > 0).any()):
+        mag = mag + (2.0 ** -10 / B_ACC) * (other @ w.double().cpu().abs().t())
+    return acc, mag
