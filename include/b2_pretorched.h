@@ -159,6 +159,15 @@ int b2_gemm_f16(const b2_gemm_args* a, void* stream);
  * (resnet3D.py:136-143) with the two BatchNorm scales folded into B and B2: the shortcut never touches HBM.
  * fp16 output, per-column affine only. */
 int b2_gemm2_f16(const b2_gemm_args* a, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream);
+/* A bottleneck's closing 1x1x1 convolution chained into the next block's conv1 in one kernel:
+ *     d  = act(scale * (A.B^T [+ A2.B2^T]) + shift + residual)        (as b2_gemm_f16 / b2_gemm2_f16; k2 = 0: no second pair)
+ *     d1 = relu(scale1[n] * (d . W1^T) + shift1[n])                   W1 fp16 [n1][ldw1 >= N], d1 fp16 [M][ldd1]
+ * d1 is computed from the fp16 d tile while it is still on chip, so d is written once and not read back.  Both results are
+ * bit-identical to the two stand-alone calls.  Contract: fp16 output, per-column affine, no per-sample affine, mask or second
+ * output, N % 64 == 0, N <= 256, ldd == N, ldd1 <= 128 (columns [n1, ldd1) of d1 are written as zero); anything else returns
+ * B2_ERR_UNSUPPORTED and the caller runs the two calls. */
+int b2_gemm_chain_f16(const b2_gemm_args* a, const void* a2, int lda2, const void* b2, int ldb2, int k2, const void* w1, int ldw1, int n1,
+                      const float* scale1, const float* shift1, void* d1, int ldd1, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Non-local block core (nonlocalnet.py:143-211):

@@ -68,6 +68,8 @@ SYMBOLS = {
     "b2_pack_upconv3x3_weight": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "b2_gemm_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p]),
     "b2_gemm2_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "b2_gemm_chain_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_int,
+                                  c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "b2_nonlocal_attention": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int,
                                       c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "b2_maxpool3d_ndhwc": (c_int, [c_void_p, c_void_p] + [c_int] * 14 + [c_void_p]),

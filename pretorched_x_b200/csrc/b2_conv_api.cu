@@ -850,6 +850,43 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
   return B2_OK;
 }
 
+// The chained instance (b2_gemm_chain_f16): closing GEMM of width N = ldd, then h1 = relu(scale1 * (y . W1^T) + shift1).  Its
+// N tile and the chained MMA width are the ones the two stand-alone launches pick (64 for a pitch <= 64, else 128).
+template <int BN, int BN1>
+static int launch_pgemm_chain(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, const void* w1, int ldw1,
+                              int n1, const float* scale1, const float* shift1, void* d1, int ldd1, cudaStream_t stream) {
+  using S = PgemmChainSmem<BN, BN1>;
+  B2_OPT_IN_SMEM((pgemm_chain_kernel<BN, BN1>), S::kTotal);
+  CUtensorMap tmA, tmB, tmA2, tmB2, tmC, tmR, tmW1, tmH;
+  int rc;
+  if ((rc = make_tmap_2d_f16(&tmA, g->a, (uint64_t)g->Kd, (uint64_t)g->M, (uint64_t)g->lda, 64, 128, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmB, g->b, (uint64_t)g->Kd, (uint64_t)g->N, (uint64_t)g->ldb, 64, BN, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmC, g->d, (uint64_t)g->ldd, (uint64_t)g->M, (uint64_t)g->ldd, 64, 64, true)) != B2_OK) return rc;
+  tmA2 = tmA; tmB2 = tmB; tmR = tmC;
+  if (k2 > 0) {
+    if ((rc = make_tmap_2d_f16(&tmA2, a2, (uint64_t)k2, (uint64_t)g->M, (uint64_t)lda2, 64, 128, true)) != B2_OK) return rc;
+    if ((rc = make_tmap_2d_f16(&tmB2, b2, (uint64_t)k2, (uint64_t)g->N, (uint64_t)ldb2, 64, BN, true)) != B2_OK) return rc;
+  }
+  if (g->residual && (rc = make_tmap_2d_f16(&tmR, g->residual, (uint64_t)g->N, (uint64_t)g->M, (uint64_t)g->ldr, 64, 128, true)) != B2_OK)
+    return rc;
+  if ((rc = make_tmap_2d_f16(&tmW1, w1, (uint64_t)g->N, (uint64_t)n1, (uint64_t)ldw1, 64, BN1, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmH, d1, (uint64_t)ldd1, (uint64_t)g->M, (uint64_t)ldd1, 64, 64, true)) != B2_OK) return rc;
+  PgemmChainParams p;
+  p.M = g->M; p.Ncols = g->N;
+  p.nkb = (g->Kd + 63) / 64; p.nkb2 = (k2 + 63) / 64;
+  p.npass = (g->N + BN - 1) / BN;
+  p.tiles_total = (g->M + 127) / 128;
+  p.scale = g->scale; p.shift = g->shift;
+  p.has_residual = g->residual != nullptr; p.relu = g->relu;
+  p.N1 = n1; p.ld1 = ldd1; p.scale1 = scale1; p.shift1 = shift1;
+  const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
+  B2_CHECK_CUDA(launch_pdl(pgemm_chain_kernel<BN, BN1>, dim3(grid), dim3(kPgThreads), S::kTotal, stream, tmA, tmB, tmA2, tmB2, tmC, tmR,
+                           tmW1, tmH, p));
+  B2_CHECK_LAUNCH("pgemm_chain_kernel");
+  set_last_kernel(KID_PGEMM_CHAIN, BN, BN1);
+  return B2_OK;
+}
+
 static int g_last_gemm_path = 0;   // kernel of the last GEMM-family launch: 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (tests pin it)
 
 static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
@@ -1167,6 +1204,32 @@ int b2_gemm2_f16(const b2_gemm_args* g, const void* a2, int lda2, const void* b2
   B2_CHECK_ARG(lda2 % 8 == 0 && ldb2 % 8 == 0 && lda2 >= k2 && ldb2 >= k2, "bad second operand pitch");
   B2_CHECK_ARG(!g->out_f32 && !g->per_row, "the fused two-operand GEMM produces fp16 output with per-column affine");
   return gemm_common(g, a2, lda2, b2, ldb2, k2, stream);
+}
+
+int b2_gemm_chain_f16(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, const void* w1, int ldw1, int n1,
+                      const float* scale1, const float* shift1, void* d1, int ldd1, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(g != nullptr && g->a && g->b && g->scale && g->shift && g->d, "null tensor pointer");
+  B2_CHECK_ARG(w1 && scale1 && shift1 && d1, "null chained-GEMM pointer");
+  B2_CHECK_ARG(g->M > 0 && g->N > 0 && g->Kd > 0 && n1 > 0, "non-positive dimension");
+  B2_CHECK_ARG(g->lda % 8 == 0 && g->ldb % 8 == 0 && g->lda >= g->Kd && g->ldb >= g->Kd, "bad operand pitch");
+  B2_CHECK_ARG(g->ldd >= g->N && (g->residual == nullptr || (g->ldr % 8 == 0 && g->ldr >= g->N)), "bad output / residual pitch");
+  B2_CHECK_ARG(k2 >= 0 && (k2 == 0 || (a2 && b2 && lda2 % 8 == 0 && ldb2 % 8 == 0 && lda2 >= k2 && ldb2 >= k2)), "bad second operand pair");
+  B2_CHECK_ARG(ldw1 % 8 == 0 && ldw1 >= g->N && ldd1 % 8 == 0 && ldd1 >= n1, "bad chained-GEMM pitch");
+  if (g->out_f32 || g->per_row || g->accumulate || g->aff_ld || g->d2 || g->mask)
+    return set_error(B2_ERR_UNSUPPORTED, "the chained GEMM takes fp16 output with a per-column affine, no mask and no second output");
+  if (g->N % 64 || g->N > 256 || g->ldd != g->N || ldd1 > 128)
+    return set_error(B2_ERR_UNSUPPORTED, "the chained GEMM needs N %% 64 == 0, N <= 256, ldd == N and a chained pitch <= 128 (got %d, %d, %d)",
+                     g->N, g->ldd, ldd1);
+  if (g_gemm_algo != 0) return set_error(B2_ERR_UNSUPPORTED, "the chained GEMM needs the persistent kernel");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (g->N <= 64)
+    return ldd1 <= 64 ? launch_pgemm_chain<64, 64>(g, a2, lda2, b2, ldb2, k2, w1, ldw1, n1, scale1, shift1, d1, ldd1, st)
+                      : launch_pgemm_chain<64, 128>(g, a2, lda2, b2, ldb2, k2, w1, ldw1, n1, scale1, shift1, d1, ldd1, st);
+  return ldd1 <= 64 ? launch_pgemm_chain<128, 64>(g, a2, lda2, b2, ldb2, k2, w1, ldw1, n1, scale1, shift1, d1, ldd1, st)
+                    : launch_pgemm_chain<128, 128>(g, a2, lda2, b2, ldb2, k2, w1, ldw1, n1, scale1, shift1, d1, ldd1, st);
 }
 
 static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream) {

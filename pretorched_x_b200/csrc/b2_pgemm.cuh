@@ -359,4 +359,246 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   }
 }
 
+// ==================================================================================================================================
+// Chained instance: a bottleneck's closing 1x1x1 GEMM and the NEXT block's conv1 in one pass over the block output
+//
+//     y  = relu( scale[n] * (A . B^T [+ A2 . B2^T]) + shift[n] [+ residual] )          [M][N],  N <= 256, N % 64 == 0, ldy == N
+//     h1 = relu( scale1[n] * (y . W1^T) + shift1[n] )                                   [M][N1], ld1 <= 128
+//
+// A CTA owns a 128-row M block across all N columns.  The closing GEMM runs as N / BN passes of the pgemm_kernel<BN, 0> main
+// loop and epilogue; each pass leaves its fp16 y columns in the 128B-swizzled [128 rows][64 columns] boxes of a full-width tile
+// (which held the residual) and TMA-stores them.  Those boxes are exactly the K-major A operand layout a TMA load of y would
+// produce, so the second GEMM reads them in place: K blocks of 64 columns in order, the W1 boxes streamed through the operand
+// ring.  Its MMA width is the one the stand-alone conv1 launch picks (BN1 = 64 for ld1 <= 64, else 128), and both epilogues keep
+// pgemm_kernel's arithmetic: the result is bit-identical to the two launches, without y's re-read from HBM.  h1 is staged in the
+// first boxes of the same tile once the y stores have read them.
+struct PgemmChainParams {
+  int M, Ncols;             // rows, closing-GEMM columns (== output pitch)
+  int nkb, nkb2;            // K blocks of the closing GEMM's two operand pairs (nkb2 = 0: none)
+  int npass;                // closing-GEMM passes of BN columns
+  int tiles_total;          // 128-row M blocks
+  const float* scale;
+  const float* shift;
+  int has_residual, relu;
+  int N1, ld1;              // chained GEMM: logical columns, output pitch (columns [N1, ld1) are written as zero)
+  const float* scale1;
+  const float* shift1;
+};
+
+template <int BN, int BN1>
+struct PgemmChainSmem {
+  static constexpr int kStages = 3;
+  static constexpr int kABytes = 128 * 128;
+  static constexpr int kStage = kABytes + 128 * 128;         // A box + B box of up to 128 rows (closing B, or a W1 K block)
+  static constexpr int kFull = 128 * 256 * 2;                // full-width fp16 tile: residual, y staging, A of the chained GEMM, h1 staging
+  static constexpr int kFullOff = kStages * kStage;          // 2 full-width tiles: the next tile's residual lands during this one
+  static constexpr int kBarOff = kFullOff + 2 * kFull;
+  static constexpr int kTotal = kBarOff + 256 + 1024;        // + barriers, + alignment slack
+  // 3 x 32 KB ring + 2 x 64 KB tiles + 256 B barriers + 1 KB slack = 225.25 KB
+  static_assert(kTotal <= 227 * 1024, "shared memory budget");
+  static_assert(BN * 128 <= kStage - kABytes && BN1 * 128 <= kStage - kABytes, "B box exceeds the ring slot");
+};
+
+template <int BN, int BN1>
+__global__ void __launch_bounds__(kPgThreads, 1)
+pgemm_chain_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
+                   const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmH,
+                   const PgemmChainParams p) {
+  using S = PgemmChainSmem<BN, BN1>;
+  constexpr int kSt = S::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_align<1024>(smem_raw);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::kBarOff);   // [kSt]
+  uint64_t* empty = full + kSt;                                      // [kSt]
+  uint64_t* res_full = empty + kSt;                                  // [2]
+  uint64_t* res_empty = res_full + 2;                                // [2]
+  const int tid = threadIdx.x, warp = tid >> 5;
+  const int nkc = p.Ncols / 64;                                      // K blocks of the chained GEMM
+
+  if (tid == 0) {
+    for (int s = 0; s < kSt; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&res_full[i], 1); mbar_init(&res_empty[i], 2); }
+    fence_mbar_init();
+    tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); tma_prefetch_desc(&tmC); tma_prefetch_desc(&tmW1);
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+  pdl_wait();
+
+  if (warp == kPgProdWarp) {
+    // ================================ producer ==========================================
+    // per tile: the closing K blocks of each pass (the residual after the first pass's), then the W1 K blocks
+    int it = 0, lt = 0;
+    for (int tile = blockIdx.x; tile < p.tiles_total; tile += gridDim.x, ++lt) {
+      const int m0 = tile * 128;
+      for (int pass = 0; pass < p.npass; ++pass) {
+        const int n0 = pass * BN;
+        for (int kb = 0; kb < p.nkb + p.nkb2; ++kb, ++it) {
+          const int s = it % kSt;
+          mbar_wait(&empty[s], ((it / kSt) & 1) ^ 1);
+          if (elect_one()) {
+            mbar_expect_tx(&full[s], S::kABytes + BN * 128);
+            uint8_t* dst = smem + s * S::kStage;
+            if (kb < p.nkb) {
+              tma_load_2d(dst, &tmA, &full[s], kb * 64, m0);
+              tma_load_2d(dst + S::kABytes, &tmB, &full[s], kb * 64, n0);
+            } else {
+              tma_load_2d(dst, &tmA2, &full[s], (kb - p.nkb) * 64, m0);
+              tma_load_2d(dst + S::kABytes, &tmB2, &full[s], (kb - p.nkb) * 64, n0);
+            }
+          }
+          __syncwarp();
+        }
+        if (pass == 0) {
+          const int rb = lt & 1;
+          mbar_wait(&res_empty[rb], ((lt >> 1) & 1) ^ 1);
+          if (elect_one()) {
+            if (p.has_residual) {
+              mbar_expect_tx(&res_full[rb], static_cast<uint32_t>(nkc) * (128 * 128));
+              for (int b = 0; b < nkc; ++b) tma_load_2d(smem + S::kFullOff + rb * S::kFull + b * (128 * 128), &tmR, &res_full[rb], b * 64, m0);
+            } else {
+              mbar_arrive(&res_full[rb]);
+            }
+          }
+          __syncwarp();
+        }
+      }
+      for (int kb = 0; kb < nkc; ++kb, ++it) {
+        const int s = it % kSt;
+        mbar_wait(&empty[s], ((it / kSt) & 1) ^ 1);
+        if (elect_one()) {
+          mbar_expect_tx(&full[s], BN1 * 128);
+          tma_load_2d(smem + s * S::kStage + S::kABytes, &tmW1, &full[s], kb * 64, 0);
+        }
+        __syncwarp();
+      }
+    }
+  } else {
+    // ================================ consumer warpgroups ===============================
+    // Fragment layout, ring protocol and epilogue as in pgemm_kernel; the affines are read from global memory (L1) instead of a
+    // shared-memory copy, which the full-width tiles leave no room for.
+    const int wg = warp >> 2, wt = tid & 127;
+    const bool leader = wt == 0;
+    const int bar_wg = 1 + wg;
+    const int fr = wg * 64 + (warp & 3) * 16 + ((tid & 31) >> 2);
+    const int fc = 2 * (tid & 3);
+    const uint32_t ring = smem_u32(smem);
+    const uint32_t a_wg = static_cast<uint32_t>(wg) * (64u * 128u >> 4);
+    const int nkb_all = warp_uniform(p.nkb + p.nkb2), npass = warp_uniform(p.npass);
+    float acc[(BN > BN1 ? BN : BN1) / 2];
+    int it = 0, lt = 0;
+    for (int tile = blockIdx.x; tile < p.tiles_total; tile += gridDim.x, ++lt) {
+      const int m0 = tile * 128;
+      const int rb = lt & 1;
+      uint8_t* tile_s = smem + S::kFullOff + rb * S::kFull;
+      for (int pass = 0; pass < npass; ++pass) {
+        const int n0 = pass * BN;
+#pragma unroll
+        for (int k = 0; k < BN / 2; ++k) acc[k] = 0.f;
+        reg_fence(acc);
+        int prev_s = -1;
+        for (int kb = 0; kb < nkb_all; ++kb, ++it) {
+          const int s = it % kSt;
+          mbar_wait(&full[s], (it / kSt) & 1);
+          const uint64_t a = desc_from(kSw128DescHi, sw128_desc_lo(ring + s * S::kStage) + a_wg);
+          const uint64_t b = desc_from(kSw128DescHi, sw128_desc_lo(ring + s * S::kStage + S::kABytes));
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) wgmma_ss<BN>(acc, a + 2 * k, b + 2 * k);
+          wgmma_commit();
+          wgmma_wait1();
+          if (leader && prev_s >= 0) mbar_arrive(&empty[prev_s]);
+          prev_s = s;
+        }
+        wgmma_wait0();
+        reg_fence(acc);
+        if (leader) {
+          mbar_arrive(&empty[prev_s]);
+          // the h1 stores of the previous tile had this main loop to read their staging boxes: hand that tile back
+          if (pass == 0 && lt > 0) { tma_store_wait_read0(); mbar_arrive(&res_empty[(lt - 1) & 1]); }
+        }
+        if (pass == 0) mbar_wait(&res_full[rb], (lt >> 1) & 1);
+        uint8_t* stage = tile_s + n0 * (128 * 2);          // boxes n0 / 64 .. of the full-width tile
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = n0 + 8 * j + fc;
+          float2 sc = make_float2(0.f, 0.f), sh = make_float2(0.f, 0.f);
+          if (c < p.Ncols) { sc = make_float2(__ldg(p.scale + c), __ldg(p.scale + c + 1)); sh = make_float2(__ldg(p.shift + c), __ldg(p.shift + c + 1)); }
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            float2 rf = make_float2(0.f, 0.f);
+            if (p.has_residual) rf = unpack_half2(*reinterpret_cast<const uint32_t*>(stage + pg_sw_off(fr + 8 * i, j, fc)));
+            float a0 = acc[4 * j + 2 * i], a1 = acc[4 * j + 2 * i + 1];
+            a0 = a0 * sc.x + sh.x + rf.x;
+            a1 = a1 * sc.y + sh.y + rf.y;
+            if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+            *reinterpret_cast<uint32_t*>(stage + pg_sw_off(fr + 8 * i, j, fc)) = pack_half2(a0, a1);
+          }
+        }
+        fence_proxy_async();                               // y: generic-proxy writes -> the bulk store and the chained wgmma
+        pg_bar(bar_wg, 128);
+        if (leader && m0 + wg * 64 < p.M) {
+#pragma unroll
+          for (int b = 0; b < BN / 64; ++b)
+            if (n0 + b * 64 < p.Ncols) tma_store_2d(&tmC, stage + b * (128 * 128) + wg * (64 * 128), n0 + b * 64, m0 + wg * 64);
+          tma_store_commit();
+        }
+      }
+
+      // ---- chained GEMM: this warpgroup's 64 rows of y (in the tile) times W1^T ----
+#pragma unroll
+      for (int k = 0; k < BN1 / 2; ++k) acc[k] = 0.f;
+      reg_fence(acc);
+      int prev_s = -1;
+      const uint32_t ya = smem_u32(tile_s);
+      for (int kb = 0; kb < nkc; ++kb, ++it) {
+        const int s = it % kSt;
+        mbar_wait(&full[s], (it / kSt) & 1);
+        const uint64_t a = desc_from(kSw128DescHi, sw128_desc_lo(ya + kb * (128 * 128)) + a_wg);
+        const uint64_t b = desc_from(kSw128DescHi, sw128_desc_lo(ring + s * S::kStage + S::kABytes));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss<BN1>(acc, a + 2 * k, b + 2 * k);
+        wgmma_commit();
+        wgmma_wait1();
+        if (leader && prev_s >= 0) mbar_arrive(&empty[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait0();
+      reg_fence(acc);
+      if (leader) {
+        mbar_arrive(&empty[prev_s]);
+        tma_store_wait_read0();                            // the y stores have read the boxes h1 is staged in
+      }
+      pg_bar(bar_wg, 128);
+#pragma unroll
+      for (int j = 0; j < BN1 / 8; ++j) {
+        const int c = 8 * j + fc;
+        float2 sc = make_float2(0.f, 0.f), sh = make_float2(0.f, 0.f);
+        if (c < p.N1) { sc.x = __ldg(p.scale1 + c); sh.x = __ldg(p.shift1 + c); }
+        if (c + 1 < p.N1) { sc.y = __ldg(p.scale1 + c + 1); sh.y = __ldg(p.shift1 + c + 1); }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float2 rf = make_float2(0.f, 0.f);         // the stand-alone conv1 epilogue adds its (absent) residual as zero
+          float a0 = acc[4 * j + 2 * i], a1 = acc[4 * j + 2 * i + 1];
+          a0 = fmaxf(a0 * sc.x + sh.x + rf.x, 0.f);
+          a1 = fmaxf(a1 * sc.y + sh.y + rf.y, 0.f);
+          *reinterpret_cast<uint32_t*>(tile_s + pg_sw_off(fr + 8 * i, j, fc)) = pack_half2(a0, a1);
+        }
+      }
+      fence_proxy_async();
+      pg_bar(bar_wg, 128);
+      if (leader && m0 + wg * 64 < p.M) {
+#pragma unroll
+        for (int b = 0; b < BN1 / 64; ++b)
+          if (b * 64 < p.ld1) tma_store_2d(&tmH, tile_s + b * (128 * 128) + wg * (64 * 128), b * 64, m0 + wg * 64);
+        tma_store_commit();
+      }
+    }
+    if (leader) tma_store_wait_read0();
+  }
+}
+
 }  // namespace b2

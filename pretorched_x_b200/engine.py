@@ -242,10 +242,47 @@ def _plain_1x1(conv):
             and all(p == 0 for p in _conv_geometry(conv)[1]))
 
 
-def _fused_close_with_projection(block, a, h, out=None):
+def _active_nonlocal(block):
+    nl = getattr(block, "nonlocalblock", None)
+    return nl if nl is not None and getattr(block, "nonlocal_layer", True) else None
+
+
+def _chains(block, nxt, simt=False):
+    """Does ``block``'s closing kernel also compute ``nxt``'s conv1 (ops.gemm_chain), so that the block output is not read
+    back from HBM?  Decided from the model alone: two plain (not pre-activation) bottlenecks, no non-local block after
+    ``block``, ``nxt.conv1`` a bias-free stride-1 1x1(x1) convolution, a closing width N % 64 == 0 with N <= 256 (layer1)
+    and a conv1 of at most 128 output channels; never under ``simt``."""
+    import torchvision.models.resnet as tvresnet
+    from .models.resnet3d import Bottleneck
+    from .models.nonlocalnet import NonLocalBottleneck
+    kinds = (Bottleneck, NonLocalBottleneck, tvresnet.Bottleneck)
+    if simt or type(block) not in kinds or type(nxt) not in kinds or _active_nonlocal(block) is not None:
+        return False
+    c3, c1 = block.conv3, nxt.conv1
+    if not (_plain_1x1(c3) and _plain_1x1(c1)) or c1.bias is not None:
+        return False
+    if any(s != 1 for s in _conv_geometry(c3)[0] + _conv_geometry(c1)[0]):
+        return False
+    N = c3.weight.shape[0]
+    return N % 64 == 0 and N <= 256 and c1.weight.shape[1] == N and ops._round_up(c1.weight.shape[0], 8) <= 128
+
+
+def _chained_close(block, nxt, h, w3, scale, shift, residual=None, second=None, out=None):
+    """The closing 1x1x1 GEMM of ``block`` (weights ``w3`` over ``h``) with ``nxt``'s conv1 chained on: (y, nxt's h1).  conv1 uses
+    the packed fp16 filter and fp32 affine of its stand-alone launch, so h1 is bit-identical to it."""
+    K = w3.shape[0]
+    pc1 = packed_conv(nxt.conv1, nxt.bn1, ops._round_up(K, 8))
+    w1 = pc1.w.view(pc1.K, pc1.C)
+    y, h1 = ops.gemm_chain(h.data, w3, scale, shift, h.M, K, h.ld, w1, pc1.scale, pc1.shift, pc1.K,
+                           residual=residual.data if residual is not None else None, relu=True, second=second, out=out)
+    return Act(y, h.N, h.T, h.H, h.W, K), Act(h1, h.N, h.T, h.H, h.W, pc1.K)
+
+
+def _fused_close_with_projection(block, a, h, out=None, nxt=None):
     """conv3 + bn3 + (downsample conv + bn)(x) + ReLU as ONE two-operand GEMM (resnet3D.py:136-143 with the type-B
     shortcut of resnet3D.py:176-185): both BatchNorm scales are folded into the fp16 weight matrices, both products
-    accumulate in the same accumulator tile, and the projected shortcut never goes through HBM."""
+    accumulate in the same accumulator tile, and the projected shortcut never goes through HBM.  ``nxt``: chain the next
+    block's conv1 on (``_chained_close``)."""
     ds_conv, ds_bn = block.downsample[0], block.downsample[1]
     stride = _conv_geometry(ds_conv)[0]
     xs = a if stride == (1, 1, 1) else ops.shortcut_a(a, stride[0], a.C)
@@ -267,30 +304,39 @@ def _fused_close_with_projection(block, a, h, out=None):
                *_bn_tensors(ds_bn)) + (h.ld, xs.ld)
     w3, wd, ones, shift = _cached(block, "close2", sig, build)
     K = w3.shape[0]
+    if nxt is not None:
+        return _chained_close(block, nxt, h, w3, ones, shift, second=(xs.data, wd, xs.ld), out=out)
     if out is not None:
         ops._out_rows(out, h.M, ops._round_up(K, 8))
     y = ops.gemm(h.data, w3, ones, shift, h.M, K, h.ld, relu=True, second=(xs.data, wd, xs.ld), out=out)
     return Act(y, h.N, h.T, h.H, h.W, K)
 
 
-def run_bottleneck(block, a, simt=False, out=None):
-    """1x1x1-BN-ReLU, 3x3x3(stride)-BN-ReLU, 1x1x1-BN-(+shortcut)-ReLU (resnet3D.py:125-143)."""
-    return Fn.BottleneckFunction.run(block, a, simt, out)
+def run_bottleneck(block, a, simt=False, out=None, h1=None, nxt=None):
+    """1x1x1-BN-ReLU, 3x3x3(stride)-BN-ReLU, 1x1x1-BN-(+shortcut)-ReLU (resnet3D.py:125-143).  ``h1`` / ``nxt``: see
+    ``_bottleneck_body``."""
+    return Fn.BottleneckFunction.run(block, a, simt, out, h1, nxt)
 
 
-def _bottleneck_body(block, a, simt=False, out=None, keep=None):
-    """``keep``: a list that receives the two post-ReLU intermediates (the fine-tuning backward reads them)."""
+def _bottleneck_body(block, a, simt=False, out=None, keep=None, h1=None, nxt=None):
+    """``keep``: a list that receives the two post-ReLU intermediates (the fine-tuning backward reads them).  ``h1``: this
+    block's conv1 output, already computed by the previous block's closing kernel (conv1 is skipped).  ``nxt``: the next
+    block (``_chains(block, nxt)`` holds): the closing kernel also computes its conv1 and the body returns (y, nxt's h1)."""
     keep = [] if keep is None else keep
     ds = block.downsample
     if (not simt and isinstance(ds, nn.Sequential) and len(ds) == 2 and _plain_1x1(ds[0]) and _plain_1x1(block.conv3)
             and not ds[1].training and len(set(_conv_geometry(ds[0])[0])) == 1 and (a.T > 1 or _conv_geometry(ds[0])[0][0] == 1)
             and isinstance(ds[0], nn.Conv3d)):
-        keep.append(conv_bn_act(block.conv1, block.bn1, a, relu=True))
+        keep.append(h1 if h1 is not None else conv_bn_act(block.conv1, block.bn1, a, relu=True))
         keep.append(conv_bn_act(block.conv2, block.bn2, keep[-1], relu=True))
-        return _fused_close_with_projection(block, a, keep[-1], out)
+        return _fused_close_with_projection(block, a, keep[-1], out, nxt)
     res = _shortcut(block, a, simt)
-    keep.append(conv_bn_act(block.conv1, block.bn1, a, relu=True, simt=simt))
+    keep.append(h1 if h1 is not None else conv_bn_act(block.conv1, block.bn1, a, relu=True, simt=simt))
     keep.append(conv_bn_act(block.conv2, block.bn2, keep[-1], relu=True, simt=simt))
+    if nxt is not None:
+        h = keep[-1]
+        pc3 = packed_conv(block.conv3, block.bn3, h.ld)
+        return _chained_close(block, nxt, h, pc3.w.view(pc3.K, pc3.C), pc3.scale, pc3.shift, residual=res, out=out)
     return conv_bn_act(block.conv3, block.bn3, keep[-1], residual=res, relu=True, simt=simt, out=out)
 
 
@@ -317,13 +363,14 @@ def _preact_body(block, a, simt=False, out=None):
     return conv_bn_act(block.conv2, None, h, residual=res, relu=False, simt=simt, out=out)
 
 
-def run_block(block, a, simt=False, out=None):
-    """One residual block (+ its non-local block).  ``out``: preallocated rows for the block's result (the last kernel writes there)."""
-    nl = getattr(block, "nonlocalblock", None)
-    if nl is not None and not getattr(block, "nonlocal_layer", True):
-        nl = None
+def run_block(block, a, simt=False, out=None, h1=None, nxt=None):
+    """One residual block (+ its non-local block).  ``out``: preallocated rows for the block's result (the last kernel writes there).
+    ``h1`` / ``nxt`` (bottlenecks paired by ``_chains``): see ``_bottleneck_body``; with ``nxt`` the result is (y, nxt's h1)."""
+    nl = _active_nonlocal(block)
     bout = out if nl is None else None
-    if getattr(block, "preactivation", False):
+    if h1 is not None or nxt is not None:
+        y = run_bottleneck(block, a, simt, bout, h1, nxt)
+    elif getattr(block, "preactivation", False):
         y = Fn.PreActBlockFunction.run(block, a, simt, bout)
     else:
         y = run_bottleneck(block, a, simt, bout) if hasattr(block, "conv3") else run_basic(block, a, simt, bout)
@@ -617,10 +664,25 @@ def _slice_clips(x, n0, n1):
     return x[n0:n1]
 
 
+def _chained_pairs(units, simt):
+    """Indices j of the units whose closing kernel computes unit j + 1's conv1 (``_chains``)."""
+    return {j for j in range(len(units) - 1)
+            if units[j][0] == units[j + 1][0] == "block" and _chains(units[j][1], units[j + 1][1], simt)}
+
+
 def _run_units(units, a, simt, out=None):
+    chained = _chained_pairs(units, simt)
+    h1 = None
     for j, (kind, m) in enumerate(units):
         o = out if j == len(units) - 1 else None
-        a = run_stem(m, a, simt=simt, out=o) if kind == "stem" else run_block(m, a, simt=simt, out=o)
+        if kind == "stem":
+            a = run_stem(m, a, simt=simt, out=o)
+        elif j in chained:
+            a, h1 = run_block(m, a, simt=simt, out=o, h1=h1, nxt=units[j + 1][1])
+        elif h1 is not None:
+            a, h1 = run_block(m, a, simt=simt, out=o, h1=h1), None
+        else:
+            a = run_block(m, a, simt=simt, out=o)
     return a
 
 

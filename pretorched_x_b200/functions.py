@@ -60,10 +60,23 @@ class StemFunction(_FrozenFunction):
 
 
 class BottleneckFunction(_FrozenFunction):
+    """``h1``: the block's conv1 output, computed by the previous block's closing kernel.  ``nxt``: the next block, whose conv1
+    the closing kernel computes too (engine._chains); then the result is (block output, next block's h1), as in GBlockFunction."""
+
     @staticmethod
-    def forward(ctx, x2d, geom, block, simt=False, out=None):
+    def forward(ctx, x2d, geom, block, simt=False, out=None, h1=None, nxt=None):
         from . import engine
-        return BottleneckFunction._finish(ctx, engine._bottleneck_body(block, Act(x2d, *geom), simt, out))
+        out = engine._bottleneck_body(block, Act(x2d, *geom), simt, out, h1=h1, nxt=nxt)
+        if isinstance(out, tuple):
+            ctx.mark_non_differentiable(out[0].data, out[1].data)
+            return out[0].data, _geom(out[0]), out[1].data, _geom(out[1])
+        ctx.mark_non_differentiable(out.data)
+        return out.data, _geom(out), None, None
+
+    @classmethod
+    def run(cls, block, a, simt=False, out=None, h1=None, nxt=None):
+        y2d, geom, h2d, hgeom = cls.apply(a.data, _geom(a), block, simt, out, h1, nxt)
+        return (Act(y2d, *geom), Act(h2d, *hgeom)) if nxt is not None else Act(y2d, *geom)
 
 
 class BasicBlockFunction(_FrozenFunction):

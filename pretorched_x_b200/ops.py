@@ -448,6 +448,33 @@ def gemm(a2d, b2d, scale, shift, M, N, Kd, residual=None, relu=False, per_row=Fa
     return out
 
 
+@_on_device
+def gemm_chain(a2d, b2d, scale, shift, M, N, Kd, w1, scale1, shift1, n1, residual=None, relu=False, second=None, out=None):
+    """``gemm`` (fp16 output, per-column affine, N % 64 == 0, N <= 256) whose kernel also returns
+    h1 = relu(scale1 * (D . W1[n1][N]^T) + shift1), computed from D while it is on chip (b2_gemm_chain_f16): a bottleneck's
+    closing 1x1x1 convolution and the next block's conv1.  Returns (D, h1); both equal the two separate calls bit for bit."""
+    dev = a2d.device
+    ldd = _round_up(N, 8)
+    out = torch.empty((M, ldd), dtype=torch.float16, device=dev) if out is None else _out_rows(out, M, ldd)
+    h1 = torch.empty((M, _round_up(n1, 8)), dtype=torch.float16, device=dev)
+    g = GemmArgs()
+    g.a, g.b, g.scale, g.shift = _ptr(a2d), _ptr(b2d), _ptr(scale), _ptr(shift)
+    g.residual = _ptr(residual)
+    g.d = _ptr(out)
+    g.M, g.N, g.Kd = M, N, Kd
+    g.lda, g.ldb, g.ldd = a2d.stride(0), b2d.stride(0), ldd
+    g.ldr = residual.stride(0) if residual is not None else 0
+    g.relu = int(relu)
+    a2, b2, k2 = second if second is not None else (None, None, 0)
+    with _timed("gemm", "gemm chain M=%d N=%d K=%d%s -> %d" % (M, N, Kd, "+%d" % k2 if k2 else "", n1),
+                2.0 * M * (N * (Kd + k2) + n1 * N),
+                2.0 * (M * (Kd + k2) + N * (Kd + k2) + n1 * N + M * ldd + M * h1.shape[1] + (M * N if residual is not None else 0))):
+        _lib.check(_lib.load().b2_gemm_chain_f16(ctypes.byref(g), _ptr(a2), a2.stride(0) if a2 is not None else 0, _ptr(b2),
+                                                b2.stride(0) if b2 is not None else 0, k2, _ptr(w1), w1.stride(0), n1, _ptr(scale1),
+                                                _ptr(shift1), _ptr(h1), h1.shape[1], _stream()), "b2_gemm_chain_f16")
+    return out, h1
+
+
 class PackedLinear:
     """nn.Linear weights as an fp16 [out][in_pitch] matrix + fp32 bias (resnet3D.py:162, trn.py:42-44)."""
     __slots__ = ("w", "scale", "shift", "out_features", "in_features", "in_pitch")

@@ -107,5 +107,58 @@ def main(names):
           flush=True)
 
 
+# --chain: the three layer1 pairs the engine chains (ops.gemm_chain): closing GEMM K -> 256 (+ K2 projection, + residual) and the
+# next block's conv1 256 -> N1.  name: K2, residual, N1
+CHAIN_PAIRS = {
+    "l1.0->l1.1 (proj)": (64, False, 64),
+    "l1.1->l1.2 (+res)": (0, True, 64),
+    "l1.2->l2.0 (+res)": (0, True, 128),
+}
+
+
+def main_chain():
+    """Per layer1 pair: the chained launch against its two separate launches, each the median of 5 CUDA-graph timings, alternated
+    in one process."""
+    dev = torch.device("cuda:0")
+    print("card: %s (power limit, max SM clock: %s)" % (torch.cuda.get_device_name(0), smi("power.limit,clocks.max.sm")), flush=True)
+    M, N, K = M1, 256, 64
+    total = 0.0
+    for name, (K2, res, N1) in CHAIN_PAIRS.items():
+        g = torch.Generator(device=dev).manual_seed(0)
+        with torch.no_grad():
+            A = torch.randn(M, K, device=dev, generator=g).half()
+            B = (torch.randn(N, K, device=dev, generator=g) / K ** 0.5).half()
+            sc, sh = torch.rand(N, device=dev, generator=g) + 0.5, torch.randn(N, device=dev, generator=g)
+            W1 = (torch.randn(N1, N, device=dev, generator=g) / N ** 0.5).half()
+            sc1, sh1 = torch.rand(N1, device=dev, generator=g) + 0.5, torch.randn(N1, device=dev, generator=g)
+            R = torch.randn(M, N, device=dev, generator=g).half() if res else None
+            second = None
+            if K2:
+                second = (torch.randn(M, K2, device=dev, generator=g).half(),
+                          (torch.randn(N, K2, device=dev, generator=g) / K2 ** 0.5).half(), K2)
+            y = torch.empty(M, N, device=dev, dtype=torch.float16)
+
+            def separate():
+                ops.gemm(A, B, sc, sh, M, N, K, residual=R, relu=True, out=y, second=second)
+                ops.gemm(y, W1, sc1, sh1, M, N1, N, relu=True)
+
+            def chained():
+                ops.gemm_chain(A, B, sc, sh, M, N, K, W1, sc1, sh1, N1, residual=R, relu=True, second=second, out=y)
+
+            ts, tc = [], []
+            for _ in range(5):
+                ts.append(time_graph(separate))
+                tc.append(time_graph(chained))
+        us_s, us_c = sorted(ts)[2], sorted(tc)[2]
+        total += us_s - us_c
+        print("%-20s separate %7.1f us  chained %7.1f us  saving %6.1f us (%.1f%%)  SM clock %s"
+              % (name, us_s, us_c, us_s - us_c, 100.0 * (us_s - us_c) / us_s, smi("clocks.sm")), flush=True)
+        del A, B, W1, R, second, y
+    print("layer1 pairs of one forward: %.0f us saved" % total, flush=True)
+
+
 if __name__ == "__main__":
-    main(sys.argv[1:] or list(SHAPES))
+    if sys.argv[1:] == ["--chain"]:
+        main_chain()
+    else:
+        main(sys.argv[1:] or list(SHAPES))
