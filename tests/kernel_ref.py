@@ -57,12 +57,25 @@ def worst_ratio(got, ref, A, f16):
 
 
 def where_worst(got, ref, A, f16):
-    err = (got.double().cpu() - ref).abs()
+    return where_worst_of(got, ref, bound(ref, A, f16))
+
+
+def worst_ratio_of(got, ref, bnd):
+    """``worst_ratio`` against an explicit per-element bound (the pooled stem, the weight gradient and its dot product)."""
+    err = (got.double().cpu().reshape(ref.shape) - ref).abs()
     err = torch.where(torch.isfinite(err), err, torch.full_like(err, float("inf")))
-    r = err / bound(ref, A, f16)
+    return float((err / bnd).max())
+
+
+def where_worst_of(got, ref, bnd):
+    got = got.double().cpu().reshape(ref.shape)
+    err = (got - ref).abs()
+    err = torch.where(torch.isfinite(err), err, torch.full_like(err, float("inf")))
+    r = (err / bnd).reshape(ref.shape[0], -1)
     i = int(torch.argmax(r))
-    m, c = divmod(i, ref.shape[1])
-    return "row %d col %d: got %r ref %r A %r" % (m, c, float(got.reshape(ref.shape)[m, c]), float(ref[m, c]), float(A[m, c]))
+    m, c = divmod(i, r.shape[1])
+    return "row %d col %d: got %r ref %r bound %r" % (m, c, float(got.reshape(r.shape)[m, c]), float(ref.reshape(r.shape)[m, c]),
+                                                      float(bnd.reshape(r.shape)[m, c]))
 
 
 # ---------------------------------------------------------------------------------------------
@@ -197,3 +210,94 @@ def in_affine_acc(x, w, scale, shift, rows):
     if bool((other > 0).any()):
         mag = mag + (2.0 ** -10 / B_ACC) * (other @ w.double().cpu().abs().t())
     return acc, mag
+
+
+# ---------------------------------------------------------------------------------------------
+# stem convolution with the fused W max-pool, depthwise 3x3, weight gradient (tests/test_gpu_kernel_bounds.py,
+# tests/test_kernel_bounds_cpu.py): fp64 from exactly the operands each kernel reads.
+# ---------------------------------------------------------------------------------------------
+def stem_operands(x, weight):
+    """The stem's operands: x fp32/fp16 NCDHW [N, 3, T, H, W] -> fp16 NDHWC4 [N, T, H, W, 4] with channel 3 zero; the filter
+    weight [K, 3, kt, kh, kw] -> weight.half() (pack_weight_stem7_kernel rounds each weight with __float2half_rn; the BN affine
+    is applied afterwards, in the fp32 epilogue) as the [K, taps, 4] layout conv_ref reads, zero in channel 3."""
+    x = x.detach().cpu()
+    N, Cin, T, H, W = x.shape
+    x4 = torch.zeros(N, T, H, W, 4, dtype=torch.float16)
+    x4[..., :Cin] = x.half().permute(0, 2, 3, 4, 1)
+    w = weight.detach().cpu().half()
+    K, taps = w.shape[0], w.shape[2] * w.shape[3] * w.shape[4]
+    w4 = torch.zeros(K, taps, 4, dtype=torch.float16)
+    w4[..., :Cin] = w.permute(0, 2, 3, 4, 1).reshape(K, taps, Cin)
+    return x4, w4
+
+
+def pool_w(ref, A, Wo, f16=True):
+    """The stem's fused max-pool along W (k 3, stride 2, padding 1) of a ReLU'd fp64 result ref [rows * Wo, K] (rows = N To Ho)
+    with its bound.  Reference: the max over each window; bound: the largest per-element bound in the window -- the max is
+    1-Lipschitz in the inf-norm and fp16 rounding is monotone, so |max got - max ref| <= max |got - ref|.  Returns
+    (ref, bound), fp64 [rows * Wp, K] with Wp = (Wo - 1) // 2 + 1."""
+    K = ref.shape[1]
+
+    def pool(v):
+        v = v.reshape(-1, Wo, K).permute(0, 2, 1)
+        return F.max_pool1d(v, 3, 2, 1).permute(0, 2, 1).reshape(-1, K)
+    return pool(ref), pool(bound(ref, A, f16))
+
+
+def dw_ref(x, w9, scale, shift, stride, clamp_in, relu6):
+    """fp64 reference of b2_dwconv3x3_ndhwc (padding 1): x fp16 [B, H, W, C] (the C used channels), w9 fp32 [9][C] (tap
+    kh * 3 + kw), scale / shift fp32 [C].  The kernel reads min(x, 6) with clamp_in (exact in fp16).  A = |s| sum |x w| + |t|;
+    the ReLU6 clamp comes after the bound is formed (1-Lipschitz).  Returns (ref, A), fp64 [B * Ho * Wo, C]."""
+    x = x.double().cpu()
+    if clamp_in:
+        x = x.clamp(max=6.0)
+    C = x.shape[-1]
+    xt = x.permute(0, 3, 1, 2)
+    wt = w9.double().cpu().t().reshape(C, 1, 3, 3)
+    acc = F.conv2d(xt, wt, stride=stride, padding=1, groups=C).permute(0, 2, 3, 1).reshape(-1, C)
+    mag = F.conv2d(xt.abs(), wt.abs(), stride=stride, padding=1, groups=C).permute(0, 2, 3, 1).reshape(-1, C)
+    s, t = scale.double().cpu(), shift.double().cpu()
+    ref, A = acc * s + t, mag * s.abs() + t.abs()
+    if relu6:
+        ref = ref.clamp(0.0, 6.0)
+    return ref, A
+
+
+def wgrad_ref(x, g, k, stride, pad, scale=None, inv=None):
+    """fp64 weight gradient of b2_conv_wgrad_thw from its fp16 operands x [N, Cin, T, H, W] and g [N, Cout, To, Ho, Wo]:
+    G = conv3d_weight(x, g), M = conv3d_weight(|x|, |g|), dW = scale * inv * G, A = |scale| * inv * M.
+    Returns (G, M, dW, A), fp64 [Cout, Cin, kt, kh, kw]."""
+    x, g = x.double().cpu(), g.double().cpu()
+    shape = (g.shape[1], x.shape[1]) + tuple(k)
+    G = torch.nn.grad.conv3d_weight(x, shape, g, stride=stride, padding=pad)
+    M = torch.nn.grad.conv3d_weight(x.abs(), shape, g.abs(), stride=stride, padding=pad)
+    s = scale.double().cpu().view(-1, 1, 1, 1, 1) if scale is not None else torch.ones(1, dtype=torch.float64)
+    i = float(inv) if inv is not None else 1.0
+    return G, M, s * i * G, s.abs() * i * M
+
+
+def wgrad_b(nbox, splits):
+    """Accumulation coefficient of the fp32 weight gradient: one split sums 64 positions of each of its ceil(nbox / splits)
+    position blocks, then the reduce kernel adds the splits in order and applies inv and scale (2 roundings)."""
+    L = 64 * -(-nbox // splits)
+    return max(B_ACC, (L + splits + 2) * FLOOR)
+
+
+def wgrad_bound(A, nbox, splits):
+    """Per-element bound of dW (fp32 output: no output-rounding term)."""
+    return wgrad_b(nbox, splits) * A + FLOOR
+
+
+def wdot_ref(G, M, w, inv, nbox, splits):
+    """wdot[co] = inv * sum w G and its bound: the error of each inv * G element (b M) weighted by |w|, the reduce kernel's fp32
+    dot product chain (strided per-thread sum over ceil(n / 256) terms, a 5-level shuffle, 8 warp sums) on inv sum |w| |G|,
+    and the floor; n = Cin * taps.  Returns (ref, bound), fp64 [Cout]."""
+    Cout = G.shape[0]
+    i = float(inv) if inv is not None else 1.0
+    w = w.double().cpu().reshape(Cout, -1)
+    G, M = G.reshape(Cout, -1), M.reshape(Cout, -1)
+    n = G.shape[1]
+    ref = i * (w * G).sum(1)
+    bnd = (i * (w.abs() * (wgrad_b(nbox, splits) * M)).sum(1)
+           + (-(-n // 256) + 5 + 8) * FLOOR * i * (w.abs() * G.abs()).sum(1) + FLOOR)
+    return ref, bnd
