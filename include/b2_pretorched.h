@@ -168,6 +168,15 @@ int b2_gemm2_f16(const b2_gemm_args* a, const void* a2, int lda2, const void* b2
  * B2_ERR_UNSUPPORTED and the caller runs the two calls. */
 int b2_gemm_chain_f16(const b2_gemm_args* a, const void* a2, int lda2, const void* b2, int ldb2, int k2, const void* w1, int ldw1, int n1,
                       const float* scale1, const float* shift1, void* d1, int ldd1, void* stream);
+/* b2_gemm_f16 with a per-sample affine at ANY number of rows per sample (b2_gemm_f16 needs aff_rows % 128 == 0, so that a
+ * 128-row tile never straddles two samples):
+ *     D[m][n] = act(scale[m / aff_rows][n] * (A.B^T)[m][n] + shift[m / aff_rows][n] + residual[m][n])
+ * Each output row resolves its own sample.  The closing 1x1 convolution of an SE bottleneck (senet.py:111-131) with the
+ * squeeze-excite factor folded into the bn3 affine (b2_se_excite): at 224^2 its rows per sample are 3136 / 784 / 196 / 49.
+ * Contract: aff_ld > 0, aff_ld % 4 == 0, aff_ld >= N, scale / shift 16-byte aligned, aff_rows > 0, M % aff_rows == 0,
+ * N % 8 == 0; fp16 output (columns [N, ldd) written as zero; residual columns >= N never read); per_row, out_f32, accumulate,
+ * d2 and mask must be zero / NULL (B2_ERR_INVALID).  Always the persistent GEMM (b2_debug_last_gemm_path() == 2). */
+int b2_gemm_sample_affine_f16(const b2_gemm_args* a, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Non-local block core (nonlocalnet.py:143-211):
@@ -190,6 +199,11 @@ int b2_nonlocal_attention(const void* q, int ldq, const void* k, int ldk, const 
 /* nn.MaxPool3d (resnet3D.py:156): padding taps are skipped (== -inf padding). */
 int b2_maxpool3d_ndhwc(const void* x, void* y, int N, int T, int H, int W, int C, int kt, int kh, int kw,
                        int st, int sh, int sw, int pt, int ph, int pw, void* stream);
+/* The same pooling with the output extent (To, Ho, Wo) given by the caller, for windows that b2_maxpool3d_ndhwc's floor rule
+ * does not produce: nn.MaxPool2d(3, stride=2, ceil_mode=True) of the SENet stem (senet.py:279-282) maps 112 -> 56 with the last
+ * window clipped at the edge.  Taps outside the input are skipped; every window must overlap the input (B2_ERR_INVALID). */
+int b2_maxpool3d_ndhwc_out(const void* x, void* y, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh, int sw,
+                           int pt, int ph, int pw, int To, int Ho, int Wo, void* stream);
 /* nn.AdaptiveAvgPool3d(1) (resnet3D.py:161): x fp16 [N][S][C] -> y fp16 [N][C], fp32 accumulation. */
 int b2_avgpool_global_ndhwc(const void* x, void* y, int N, int S, int C, void* stream);
 /* fp32 NCDHW (the reference's input layout) -> fp16 NDHWC with channel pitch Cp (zero padded). */
@@ -348,6 +362,25 @@ int b2_rgb_head_gather_tanh(const void* partial, int ldp, const float* bias, voi
                             void* stream);
 /* y[n][c][s] = tanh(x[n*S + s][c]): fp16 channels-last (pitch ldx) -> NCHW planes, fp32 (out_f32) or fp16. */
 int b2_tanh_nhwc_to_nchw(const void* x, int ldx, void* y, int N, int C, long long S, int out_f32, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * SE-ResNet / SE-ResNeXt (senet.py:85-204)
+ * ------------------------------------------------------------------------------------------- */
+/* Squeeze-and-excitation of one SE bottleneck as per-sample affine rows for b2_gemm_sample_affine_f16.  SEModule
+ * (senet.py:85-104) scales x = bn3(conv3(h2)) by e = sigmoid(fc2(relu(fc1(avgpool(x))))); conv3 + bn3 is affine, so
+ * avgpool(x) = s3 * (W3 . m) + t3 with m the mean of h2 over the positions of a sample, and the caller passes fc1 composed with
+ * that map: w1 = W_fc1 . diag(s3) . W3 (fp32 [R][C2]), b1 = W_fc1 . t3 + b_fc1 (fp32 [R]).  Per sample n:
+ *     m[c]   = sum_p h[n*S + p][c] / S                 (fp32)
+ *     a[r]   = relu(sum_c w1[r][c] m[c] + b1[r])
+ *     e[k]   = sigmoid(sum_r w2[k][r] a[r] + b2[k])    (w2 fp32 [C][R] = fc2.weight, b2 = fc2.bias)
+ *     scale[n * ld_aff + k] = e[k] * s3[k],  shift[n * ld_aff + k] = e[k] * t3[k]      (k < C; columns >= C untouched)
+ * so that relu(scale * (W3 . h2) + shift + residual) is the block output (senet.py:127-131).  h: fp16 [N*S][ldh], C2 % 8 == 0,
+ * ldh % 8 == 0, 16-byte aligned.  ws: fp32 workspace of b2_se_excite_workspace_elems(N, C2, R) elements.  Three launches, fp32
+ * throughout, every sum in one fixed order (no atomics): bitwise repeatable, no host synchronisation. */
+size_t b2_se_excite_workspace_elems(int N, int C2, int R);
+int b2_se_excite(const void* h, int ldh, int N, int S, int C2, const float* w1, const float* b1, int R, const float* w2, const float* b2,
+                 int C, const float* s3, const float* t3, float* scale, float* shift, int ld_aff, float* ws, size_t ws_elems,
+                 void* stream);
 
 #ifdef __cplusplus
 }

@@ -103,6 +103,11 @@ SYMBOLS = {
     "b2_pack_grouped_conv_weight_elems": (ctypes.c_size_t, [c_int] * 6),
     "b2_pack_grouped_conv_weight": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
     "b2_conv_grouped_ndhwc_fprop": (c_int, [ctypes.POINTER(ConvArgs), c_int, c_void_p]),
+    "b2_gemm_sample_affine_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p]),
+    "b2_maxpool3d_ndhwc_out": (c_int, [c_void_p, c_void_p] + [c_int] * 17 + [c_void_p]),
+    "b2_se_excite_workspace_elems": (ctypes.c_size_t, [c_int] * 3),
+    "b2_se_excite": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                             c_void_p, c_void_p, c_void_p, c_int, c_void_p, ctypes.c_size_t, c_void_p]),
 }
 
 

@@ -596,6 +596,22 @@ int b2_maxpool3d_ndhwc(const void* x, void* y, int N, int T, int H, int W, int C
   return B2_OK;
 }
 
+int b2_maxpool3d_ndhwc_out(const void* x, void* y, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh, int sw,
+                           int pt, int ph, int pw, int To, int Ho, int Wo, void* stream) {
+  B2_CHECK_ARG(x && y && N > 0 && T > 0 && H > 0 && W > 0, "bad argument");
+  B2_CHECK_ARG(C % 8 == 0, "channel pitch %d is not a multiple of 8", C);
+  B2_CHECK_ARG(kt > 0 && kh > 0 && kw > 0 && st > 0 && sh > 0 && sw > 0 && pt >= 0 && ph >= 0 && pw >= 0, "bad window");
+  B2_CHECK_ARG(To > 0 && Ho > 0 && Wo > 0, "empty output");
+  // every window must overlap the input: its first tap lies before the input's end, its last one after the input's start
+  B2_CHECK_ARG((To - 1) * st - pt < T && (Ho - 1) * sh - ph < H && (Wo - 1) * sw - pw < W && kt > pt && kh > ph && kw > pw,
+               "output extent %dx%dx%d has a window outside the %dx%dx%d input", To, Ho, Wo, T, H, W);
+  const long long total = (long long)N * To * Ho * Wo * (C / 8);
+  maxpool3d_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      (const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw, total);
+  B2_CHECK_LAUNCH("maxpool3d");
+  return B2_OK;
+}
+
 int b2_avgpool_global_ndhwc(const void* x, void* y, int N, int S, int C, void* stream) {
   B2_CHECK_ARG(x && y && N > 0 && S > 0, "bad argument");
   B2_CHECK_ARG(C % 8 == 0, "channel pitch %d is not a multiple of 8", C);

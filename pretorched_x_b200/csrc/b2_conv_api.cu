@@ -843,6 +843,7 @@ static int launch_pgemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.in_scale = GAN ? ip.in_scale : nullptr; p.in_shift = ip.in_shift; p.in_ld = ip.in_ld; p.in_rows = ip.in_rows > 0 ? ip.in_rows : 128;
   p.dual = ip.y2 != nullptr; p.scale2 = ip.scale2; p.shift2 = ip.shift2; p.aff2_ld = ip.aff2_ld; p.aff2_rows = ip.aff2_rows > 0 ? ip.aff2_rows : 128;
   p.mask = ip.mask; p.ldm = ip.ldm;
+  p.fd_aff = make_fastdiv(ip.aff_rows > 0 ? ip.aff_rows : 1);
   const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
   B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, GAN, MASK>, dim3(grid), dim3(GAN ? kPgThreadsGan : kPgThreads), S::kTotal, stream, tmA, tmB, tmA2, tmB2, tmC, tmR, tmC2, p));
   B2_CHECK_LAUNCH("pgemm_kernel");
@@ -1195,9 +1196,25 @@ int b2_conv_grouped_ndhwc_fprop(const b2_conv_args* a, int groups, void* stream)
   return rc < 0 ? rc : B2_OK;
 }
 
-static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream);
+static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream,
+                       bool sample_rows = false);
 
 int b2_gemm_f16(const b2_gemm_args* g, void* stream) { return gemm_common(g, nullptr, 0, nullptr, 0, 0, stream); }
+
+int b2_gemm_sample_affine_f16(const b2_gemm_args* g, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(g != nullptr && g->scale && g->shift, "null args");
+  B2_CHECK_ARG(g->aff_ld > 0 && g->aff_ld % 4 == 0 && g->aff_ld >= g->N && g->aff_rows > 0 &&
+                   (reinterpret_cast<uintptr_t>(g->scale) & 15) == 0 && (reinterpret_cast<uintptr_t>(g->shift) & 15) == 0,
+               "per-sample affine needs 16-byte aligned fp32 [M / aff_rows][aff_ld] rows, aff_ld %% 4 == 0, aff_ld >= N, aff_rows > 0 "
+               "(got pitch %d, rows per sample %d)", g->aff_ld, g->aff_rows);
+  B2_CHECK_ARG(g->M > 0 && g->M % g->aff_rows == 0, "M %d is not a whole number of samples of %d rows", g->M, g->aff_rows);
+  B2_CHECK_ARG(g->N % 8 == 0, "N %d is not a multiple of 8", g->N);
+  B2_CHECK_ARG(!g->out_f32 && !g->per_row && !g->accumulate && !g->d2 && !g->mask,
+               "the per-sample-affine GEMM takes fp16 output without per-row affine, accumulation, second output or mask");
+  if (g_gemm_algo != 0) return set_error(B2_ERR_UNSUPPORTED, "the per-sample-affine GEMM needs the persistent kernel");
+  return gemm_common(g, nullptr, 0, nullptr, 0, 0, stream, true);
+}
 
 int b2_gemm2_f16(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream) {
   B2_CHECK_ARG(g != nullptr && a2 && b2 && k2 > 0, "null / empty second operand pair");
@@ -1232,7 +1249,8 @@ int b2_gemm_chain_f16(const b2_gemm_args* g, const void* a2, int lda2, const voi
                     : launch_pgemm_chain<128, 128>(g, a2, lda2, b2, ldb2, k2, w1, ldw1, n1, scale1, shift1, d1, ldd1, st);
 }
 
-static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream) {
+static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const void* b2, int ldb2, int k2, void* stream,
+                       bool sample_rows) {
   set_last_kernel(KID_NONE);
   B2_CHECK_ARG(g != nullptr, "null args");
   B2_CHECK_ARG(g->a && g->b && g->scale && g->shift && g->d, "null tensor pointer");
@@ -1260,8 +1278,8 @@ static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const vo
   p.y = g->d; p.ldy = g->ldd;
   p.relu = g->relu; p.per_row = g->per_row; p.accumulate = g->accumulate;
   p.epi = g->out_f32 ? EPI_DIRECT_F32 : EPI_TMA_F16;
-  B2_CHECK_ARG(g->aff_ld >= 0 && (g->aff_ld == 0 || (g->aff_ld >= g->N && g->aff_rows > 0 && g->aff_rows % 128 == 0 &&
-                                                     !g->out_f32 && !g->per_row)),
+  B2_CHECK_ARG(sample_rows || (g->aff_ld >= 0 && (g->aff_ld == 0 || (g->aff_ld >= g->N && g->aff_rows > 0 && g->aff_rows % 128 == 0 &&
+                                                                     !g->out_f32 && !g->per_row))),
                "bad per-sample affine (pitch %d, rows per sample %d)", g->aff_ld, g->aff_rows);
   p.aff_ld = g->aff_ld; p.aff_rows = g->aff_rows;
   p.mask = reinterpret_cast<const __half*>(g->mask); p.ldm = g->ldm;
@@ -1275,6 +1293,12 @@ static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const vo
   L.w = g->b; L.ldb = g->ldb; L.b_cols = g->Kd;
   L.a2 = a2; L.lda2 = lda2; L.w2 = b2; L.ldb2 = ldb2; L.k2 = k2;
   if (k2 > 0 && g_gemm_algo != 0) return set_error(B2_ERR_UNSUPPORTED, "two-operand GEMM needs the persistent kernel");
+  if (sample_rows) {
+    // the only kernel with the per-row sample decode; the dense-M and per-tile kernels never see this epilogue
+    g_last_gemm_path = 2;
+    const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return g->ldd <= 64 ? launch_pgemm<64, 0, 2>(L, st) : launch_pgemm<128, 0, 2>(L, st);
+  }
   return dispatch_igemm(L, reinterpret_cast<cudaStream_t>(stream));
 }
 

@@ -69,6 +69,9 @@ struct PgemmParams {
   int in_ld, in_rows;
   const __half* mask;       // pgemm_kernel<BN, 0, 1> only: fp16 [M][ldm] ReLU-derivative mask of the output (see IgemmParams)
   int ldm;
+  // pgemm_kernel<BN, 0, 2> only: per-sample affine at ANY rows per sample (aff_rows need not divide 128, so a tile may straddle
+  // samples).  Each fragment row resolves its own sample n = m / aff_rows with this divider and reads row n of scale / shift.
+  FastDiv fd_aff;
 };
 
 template <int BN, int GAN>
@@ -98,8 +101,9 @@ __device__ __forceinline__ uint32_t pg_sw_off(int row, int j, int c) {
          ((static_cast<uint32_t>(j & 7) ^ static_cast<uint32_t>(row & 7)) << 4) + static_cast<uint32_t>(c) * 2u;
 }
 
-template <int BN, int GAN, int MASK = 0>   // GAN = 1: instance with the generator extras (res_up gather, res_pre, dual output, A transform);
-                                           // 0: the classic epilogue.  MASK = 1 (with GAN = 0): ReLU-derivative mask operand (fine-tuning backward)
+template <int BN, int GAN, int EPI = 0>    // GAN = 1: instance with the generator extras (res_up gather, res_pre, dual output, A transform);
+                                           // 0: the classic epilogue.  With GAN = 0, EPI = 1: ReLU-derivative mask operand (fine-tuning
+                                           // backward); EPI = 2: per-sample affine resolved per fragment row (see PgemmParams::fd_aff)
 __global__ void __launch_bounds__(GAN ? kPgThreadsGan : kPgThreads, 1)
 pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -193,7 +197,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       const int m0 = (tile / p.tiles_n) * 128, n0 = (tile % p.tiles_n) * BN;
       // the tile's affine, fetched before the main loop and stored after it
       float aff[4] = {0.f, 0.f, 0.f, 0.f};
-      if (wt < BN && n0 + wt < p.Ncols) {
+      if (EPI != 2 && wt < BN && n0 + wt < p.Ncols) {
         // per-sample affine (class-conditional BN of the consumer): a 128-row tile never straddles two samples
         const size_t arow = p.aff_ld ? static_cast<size_t>(m0 / p.aff_rows) * p.aff_ld : 0;
         aff[0] = __ldg(&p.scale[arow + n0 + wt]);
@@ -237,6 +241,17 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       mbar_wait(&res_full[rb], (lt >> 1) & 1);
       uint8_t* stage = smem + S::kResOff + rb * S::kTile;
       int rsrc[2] = {fr, fr + 8};                          // row of the residual box each fragment row adds
+      const float* aff_rs[2] = {nullptr, nullptr};         // EPI = 2: scale / shift rows of the two fragment rows' samples
+      const float* aff_rh[2] = {nullptr, nullptr};
+      if constexpr (EPI == 2) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int m = min(m0 + fr + 8 * i, p.M - 1);    // rows past M (ragged last tile) are computed but never stored
+          const size_t off = static_cast<size_t>(fdiv(m, p.fd_aff)) * p.aff_ld;
+          aff_rs[i] = p.scale + off;
+          aff_rh[i] = p.shift + off;
+        }
+      }
       if (GAN && p.res_up) {
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
@@ -262,8 +277,18 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             a0 = a0 * sc.x + sh.x + rf.x;
             a1 = a1 * sc.y + sh.y + rf.y;
           }
+          if constexpr (EPI == 2) {
+            // this fragment row's sample: columns >= Ncols get a zero affine (and a TMA zero-filled residual), so the pitch stays zero
+            float2 rs = make_float2(0.f, 0.f), rh = make_float2(0.f, 0.f);
+            if (n0 + c < p.Ncols) {
+              rs = __ldg(reinterpret_cast<const float2*>(aff_rs[i] + n0 + c));
+              rh = __ldg(reinterpret_cast<const float2*>(aff_rh[i] + n0 + c));
+            }
+            a0 = acc[4 * j + 2 * i] * rs.x + rh.x + rf.x;
+            a1 = acc[4 * j + 2 * i + 1] * rs.y + rh.y + rf.y;
+          }
           if (p.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
-          if constexpr (MASK) {
+          if constexpr (EPI == 1) {
             const int mrow = m0 + fr + 8 * i, mcol = n0 + c;
             uint32_t mv = 0;
             if (mrow < p.M && mcol < p.ldm) mv = __ldg(reinterpret_cast<const unsigned int*>(p.mask + static_cast<size_t>(mrow) * p.ldm + mcol));

@@ -588,6 +588,104 @@ def run_mobilenet_features(features, x):
 
 
 # ---------------------------------------------------------------------------------------------
+# SE-ResNet / SE-ResNeXt (senet.py:85-366)
+# ---------------------------------------------------------------------------------------------
+def _strided_1x1(conv, bn, a, relu):
+    """A 1x1 Conv2d of stride s > 1 (SE-ResNet's conv1, senet.py:166-167, and every stage's projection): the strided pixel
+    subset is gathered once (1/s^2 of the input, b2_shortcut_a_ndhwc at T = 1) and the convolution runs as a stride-1 GEMM."""
+    s = _conv_geometry(conv)[0]
+    if s[1] == 1:
+        return conv_bn_act(conv, bn, a, relu=relu)
+    if not (_plain_1x1(conv) and s[1] == s[2] and a.T == 1):
+        raise NotImplementedError("strided 1x1 convolutions need equal in-plane strides on images")
+    sub = ops.shortcut_a(a, s[1], a.C)
+    pc = packed_conv(conv, bn, sub.ld, stride=(1, 1, 1))
+    return ops.conv(sub, pc, relu=relu)
+
+
+def _se_pack(block, C2):
+    """Closing-GEMM filter and squeeze-excite parameters of an SE bottleneck: conv3 as fp16 [K][C2], the bn3 affine (s3, t3),
+    fc1 composed with conv3 + bn3 -- w1 = W_fc1 diag(s3) W3, b1 = W_fc1 t3 + b_fc1, in fp64 then fp32 -- and fc2 in fp32."""
+    se = block.se_module
+    conv3, bn3 = block.conv3, block.bn3
+    dev = conv3.weight.device
+
+    def build():
+        K = conv3.weight.shape[0]
+        s3, t3 = ops.fold_affine(K, conv3.bias, bn3, dev)
+        w3d = _conv1x1_matrix(conv3).double()                                # [K][C]
+        C = w3d.shape[1]
+        w3 = torch.zeros((K, C2), dtype=torch.float16, device=dev)
+        w3[:, :C] = w3d.to(torch.float16)
+        f1 = _conv1x1_matrix(se.fc1).double()                                # [R][K]
+        b1 = se.fc1.bias.detach().double() if se.fc1.bias is not None else torch.zeros(f1.shape[0], dtype=torch.float64, device=dev)
+        w1 = torch.zeros((f1.shape[0], C2), dtype=torch.float64, device=dev)
+        w1[:, :C] = (f1 * s3.double()[None, :]) @ w3d
+        b1f = f1 @ t3.double() + b1
+        w2 = _conv1x1_matrix(se.fc2).float().contiguous()                   # [K][R]
+        b2 = se.fc2.bias.detach().float().contiguous() if se.fc2.bias is not None else torch.zeros(K, dtype=torch.float32, device=dev)
+        return w3, s3, t3, w1.float().contiguous(), b1f.float().contiguous(), w2, b2
+
+    sig = _sig(conv3.weight, conv3.bias, *_bn_tensors(bn3), se.fc1.weight, se.fc1.bias, se.fc2.weight, se.fc2.bias) + (C2,)
+    return _cached(block, "se", sig, build, reads=_bn_tensors(bn3))
+
+
+def run_se_bottleneck(block, a, out=None):
+    """SEResNetBottleneck / SEResNeXtBottleneck (senet.py:107-131) through its Function."""
+    return Fn.SEBottleneckFunction.run(block, a, out)
+
+
+def _se_bottleneck_body(block, a, out=None):
+    """conv1-bn1-relu, conv2-bn2-relu, then out = relu(e * bn3(conv3(h2)) + shortcut) with e the SE excitation.
+
+    The squeeze runs before conv3 (b2_se_excite: mean of h2, fc1 folded through conv3 + bn3, fc2, sigmoid) and hands the
+    closing GEMM per-sample affine rows e * s3, e * t3 (b2_gemm_sample_affine_f16).  A projection shortcut runs as its own
+    GEMM whose output is the closing GEMM's residual: SE scales the main path only, so the two-operand GEMM that fuses the
+    projection into the closing convolution elsewhere would scale the shortcut too, and a second accumulator set would double
+    the persistent kernel's accumulator registers for 4 of the 16 blocks."""
+    ds = block.downsample
+    if ds is None:
+        res = a
+    elif isinstance(ds, nn.Sequential) and len(ds) == 2 and _plain_1x1(ds[0]):
+        res = _strided_1x1(ds[0], ds[1], a, relu=False)
+    else:
+        raise NotImplementedError("SE bottlenecks with a projection other than a 1x1 convolution + BatchNorm (senet154) are outside "
+                                  "the engine's scope")
+    h1 = _strided_1x1(block.conv1, block.bn1, a, relu=True)
+    h2 = conv_bn_act(block.conv2, block.bn2, h1, relu=True)
+    w3, s3, t3, w1, b1, w2, b2 = _se_pack(block, h2.ld)
+    if (h2.N, h2.T, h2.H, h2.W) != (res.N, res.T, res.H, res.W):
+        raise RuntimeError("shortcut / main path shape mismatch")
+    scale, shift = ops.se_excite(h2, w1, b1, w2, b2, s3, t3)
+    K = w3.shape[0]
+    y = ops.gemm_sample_affine(h2.data, w3, scale, shift, h2.M, K, h2.ld, h2.positions, residual=res.data, relu=True, out=out)
+    return Act(y, h2.N, h2.T, h2.H, h2.W, K)
+
+
+def _se_stem_body(layer0, a, out=None):
+    """layer0 of the SENets (senet.py:272-283): 7x7 stride-2 conv -> bn1 -> ReLU on the stem kernel, then
+    MaxPool2d(3, stride=2, ceil_mode=True) on the pooling kernel with the ceil-mode output extent."""
+    mp = layer0.pool
+    k, s, p = mp.kernel_size, mp.stride, mp.padding
+    if not (isinstance(k, int) and isinstance(s, int) and isinstance(p, int)) or mp.dilation not in (1, (1, 1)):
+        raise NotImplementedError("the SENet stem pool must be a square, undilated MaxPool2d")
+    h = conv_bn_act(layer0.conv1, layer0.bn1, a, relu=True)
+    if mp.ceil_mode:
+        return ops.maxpool2d_ceil(h, k, s, p, out=out)
+    return ops.maxpool3d(h, (1, k, k), (1, s, s), (0, p, p), out=out)
+
+
+def run_senet_trunk(model, x):
+    """layer0 .. layer4 of an SENet: fp32 NCHW images (or an NDHWC4 Act) in, Act out."""
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x)
+    a = Fn.SEStemFunction.run(model.layer0, a)
+    for name in ("layer1", "layer2", "layer3", "layer4"):
+        for blk in getattr(model, name):
+            a = run_se_bottleneck(blk, a)
+    return a
+
+
+# ---------------------------------------------------------------------------------------------
 # stem / trunk / head
 # ---------------------------------------------------------------------------------------------
 def _pool_args(mp):

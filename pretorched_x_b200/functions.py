@@ -129,6 +129,24 @@ class InvertedResidualFunction(_FrozenFunction):
         return InvertedResidualFunction._finish(ctx, engine._inverted_residual_body(block, Act(x2d, *geom), out))
 
 
+class SEStemFunction(_FrozenFunction):
+    """layer0 of the SENets: conv1 -> bn1 -> relu1 -> ceil-mode pool (senet.py:272-283)."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, layer0, out=None):
+        from . import engine
+        return SEStemFunction._finish(ctx, engine._se_stem_body(layer0, Act(x2d, *geom), out))
+
+
+class SEBottleneckFunction(_FrozenFunction):
+    """SEResNetBottleneck / SEResNeXtBottleneck (senet.py:107-131): convolutions, squeeze-excite and the closing GEMM."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, block, out=None):
+        from . import engine
+        return SEBottleneckFunction._finish(ctx, engine._se_bottleneck_body(block, Act(x2d, *geom), out))
+
+
 class GBlockFunction(_FrozenFunction):
     """BigGAN-deep GBlock: ccbn-ReLU-1x1 -> ccbn-ReLU-[up]-3x3 -> ccbn-ReLU-3x3 -> ccbn-ReLU-1x1 (+ skip)."""
 

@@ -1,4 +1,4 @@
-from . import resnet3d, r2plus1d, nonlocalnet, resnet2d, resnext3d, trn, slowfast, mobilenet, utils, settings  # noqa: F401
+from . import resnet3d, r2plus1d, nonlocalnet, resnet2d, resnext3d, trn, slowfast, mobilenet, senet, utils, settings  # noqa: F401
 
 # the reference spells the module `resnet3D` (capital D); keep that import path working
 resnet3D = resnet3d

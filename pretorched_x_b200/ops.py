@@ -475,6 +475,51 @@ def gemm_chain(a2d, b2d, scale, shift, M, N, Kd, w1, scale1, shift1, n1, residua
     return out, h1
 
 
+@_on_device
+def gemm_sample_affine(a2d, b2d, scale, shift, M, N, Kd, aff_rows, residual=None, relu=False, out=None):
+    """D[M][N] = act(scale[m // aff_rows] * A[M][Kd] . B[N][Kd]^T + shift[m // aff_rows] + residual) with ``scale`` / ``shift``
+    fp32 [M // aff_rows][pitch] row views, at any rows per sample (b2_gemm_sample_affine_f16: the closing 1x1 GEMM of an SE
+    bottleneck, whose 49 .. 3136 positions per image do not fill whole 128-row tiles)."""
+    ldd = _round_up(N, 8)
+    out = torch.empty((M, ldd), dtype=torch.float16, device=a2d.device) if out is None else _out_rows(out, M, ldd)
+    if scale.shape != shift.shape or scale.stride(0) != shift.stride(0) or scale.shape[0] * aff_rows != M or scale.shape[1] < N:
+        raise ValueError("per-sample affine must be two fp32 [M / aff_rows][>= N] views with one pitch")
+    g = GemmArgs()
+    g.a, g.b, g.scale, g.shift = _ptr(a2d), _ptr(b2d), _ptr(scale), _ptr(shift)
+    g.residual = _ptr(residual)
+    g.d = _ptr(out)
+    g.M, g.N, g.Kd = M, N, Kd
+    g.lda, g.ldb, g.ldd = a2d.stride(0), b2d.stride(0), ldd
+    g.ldr = residual.stride(0) if residual is not None else 0
+    g.relu = int(relu)
+    g.aff_ld, g.aff_rows = scale.stride(0), int(aff_rows)
+    with _timed("gemm_se", "gemm M=%d N=%d K=%d sample-affine/%d" % (M, N, Kd, aff_rows), 2.0 * M * N * Kd,
+                2.0 * (M * Kd + N * Kd + M * ldd + (M * N if residual is not None else 0))):
+        _lib.check(_lib.load().b2_gemm_sample_affine_f16(ctypes.byref(g), _stream()), "b2_gemm_sample_affine_f16")
+    return out
+
+
+@_on_device
+def se_excite(h, w1, b1, w2, b2, s3, t3, out=None):
+    """Squeeze-excite of an SE bottleneck (b2_se_excite): h = the Act entering conv3, w1 / b1 = fc1 folded through conv3 + bn3
+    (fp32 [R][C2], [R]), w2 / b2 = fc2 (fp32 [C][R], [C]), s3 / t3 = the folded bn3 affine.  Returns fp32 (scale, shift)
+    [N][round_up(C, 4)] for ``gemm_sample_affine``."""
+    R, C2 = w1.shape
+    C = w2.shape[0]
+    if h.C != C2 or w2.shape[1] != R:
+        raise ValueError("squeeze-excite shapes: h %r, fc1 %s, fc2 %s" % (h, tuple(w1.shape), tuple(w2.shape)))
+    dev = h.data.device
+    lda = _round_up(C, 4)
+    aff = torch.empty((2, h.N, lda), dtype=torch.float32, device=dev) if out is None else out
+    lib = _lib.load()
+    ws = torch.empty(int(lib.b2_se_excite_workspace_elems(h.N, C2, R)), dtype=torch.float32, device=dev)
+    with _timed("se_excite", "se_excite N=%d S=%d C2=%d R=%d C=%d" % (h.N, h.positions, C2, R, C),
+                2.0 * h.N * (h.positions * C2 + R * C2 + C * R), 2.0 * h.M * C2 + 4.0 * (R * C2 + C * R + 2 * h.N * C)):
+        _lib.check(lib.b2_se_excite(_ptr(h.data), h.ld, h.N, h.positions, C2, _ptr(w1), _ptr(b1), R, _ptr(w2), _ptr(b2), C, _ptr(s3),
+                                    _ptr(t3), _ptr(aff[0]), _ptr(aff[1]), lda, _ptr(ws), ws.numel(), _stream()), "b2_se_excite")
+    return aff[0], aff[1]
+
+
 class PackedLinear:
     """nn.Linear weights as an fp16 [out][in_pitch] matrix + fp32 bias (resnet3D.py:162, trn.py:42-44)."""
     __slots__ = ("w", "scale", "shift", "out_features", "in_features", "in_pitch")
@@ -514,6 +559,27 @@ def maxpool3d(a, kernel, stride, padding, out=None):
         _lib.check(_lib.load().b2_maxpool3d_ndhwc(_ptr(a.data), _ptr(y), a.N, a.T, a.H, a.W, a.ld, kt, kh, kw, st, sh, sw,
                                                  pt, ph, pw, _stream()), "b2_maxpool3d_ndhwc")
     return Act(y, a.N, To, Ho, Wo, a.C)
+
+
+def ceil_pool_dim(i, k, s, p):
+    """Output size of a ceil-mode pooling window (torch's rule: the last window must start inside the input or left padding)."""
+    o = -(-(i + 2 * p - k) // s) + 1
+    if (o - 1) * s >= i + p:
+        o -= 1
+    return o
+
+
+@_on_device
+def maxpool2d_ceil(a, k, s, p=0, out=None):
+    """nn.MaxPool2d(k, stride=s, padding=p, ceil_mode=True) over every frame (the SENet stem pool, senet.py:260-263), on the
+    generic pooling kernel with an explicit output extent (b2_maxpool3d_ndhwc_out)."""
+    Ho, Wo = ceil_pool_dim(a.H, k, s, p), ceil_pool_dim(a.W, k, s, p)
+    My = a.N * a.T * Ho * Wo
+    y = _out_rows(out, My, a.ld) if out is not None else torch.empty((My, a.ld), dtype=torch.float16, device=a.data.device)
+    with _timed("maxpool", "maxpool ceil C%d M=%d->%d" % (a.C, a.M, My), 0.0, 2.0 * a.C * (a.M + My)):
+        _lib.check(_lib.load().b2_maxpool3d_ndhwc_out(_ptr(a.data), _ptr(y), a.N, a.T, a.H, a.W, a.ld, 1, k, k, 1, s, s, 0, p, p,
+                                                     a.T, Ho, Wo, _stream()), "b2_maxpool3d_ndhwc_out")
+    return Act(y, a.N, a.T, Ho, Wo, a.C)
 
 
 @_on_device

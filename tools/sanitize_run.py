@@ -46,6 +46,8 @@ case("preact_resnet3d50", lambda: P.preact_resnet3d50(num_classes=400), (2, 3, 8
 
 case("nonlocalresnet3d50", lambda: P.nonlocalresnet3d50(pretrained=None), (1, 3, 16, 96, 96))
 case("mobilenetv2", lambda: P.mobilenetv2(num_classes=1000, pretrained=None), (2, 3, 96, 64))
+case("se_resnet50", lambda: P.se_resnet50(pretrained=None), (2, 3, 224, 224))
+case("se_resnext50_32x4d", lambda: P.se_resnext50_32x4d(pretrained=None), (2, 3, 224, 224))
 case("slowfast18", lambda: P.slowfast.resnet18(mode="sf", num_classes=12), (1, 3, 32, 64, 64))
 
 if not only or "trn" in only:
