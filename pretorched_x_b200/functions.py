@@ -233,10 +233,30 @@ def _unit_affine(n, dev):
     return torch.ones(n, dtype=torch.float32, device=dev), torch.zeros(n, dtype=torch.float32, device=dev)
 
 
+def _pow2(k):
+    """int32 exponents in [-126, 126] -> fp32 2^k, exactly (built from the exponent bits)."""
+    return ((k + 127) << 23).view(torch.float32)
+
+
+def _row_exponents(g):
+    """Per-row power-of-two scale of an fp32 [rows][cols] gradient, on the device: k with max |g[r]| * 2^k in [2^7, 2^8) (the
+    target of ops.loss_scale_), 0 for an all-zero or non-finite row.  Returns (2^k, 2^-k), fp32 [rows][1]."""
+    amax = g.abs().amax(1)
+    _, e = torch.frexp(amax)                                         # amax = f * 2^e, f in [0.5, 1)
+    ok = (amax > 0) & torch.isfinite(amax)
+    k = torch.where(ok, 8 - e, torch.zeros_like(e)).clamp(-126, 126)
+    return _pow2(k)[:, None], _pow2(-k)[:, None]
+
+
 class LinearFunction(torch.autograd.Function):
     """y = x W^T + b on wgmma (fp16 operands, fp32 accumulate / output), with
     dL/dx = g W, dL/dW = g^T x, dL/db = sum_rows g computed by the same kernel (D = A . B^T with K-major operands:
-    the gradient products take the transposed fp16 copies as their operands)."""
+    the gradient products take the transposed fp16 copies as their operands).
+
+    The fp32 gradient g is rounded to fp16 for the products.  Cross-entropy gradients are (p - onehot) / B, mostly far below
+    fp16's normal range, so each row of the A operand (a sample row of g for dL/dx, a class row of g^T for dL/dW) is first
+    multiplied by its own power of two 2^k, which puts the row's peak in [2^7, 2^8); the fp32 product row is multiplied by
+    2^-k afterwards, which is exact."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, relu_input=False):
@@ -258,18 +278,22 @@ class LinearFunction(torch.autograd.Function):
         rows, out_f = gy.shape
         in_f = ctx.in_features
         gx = gw = gb = None
-        g16 = _f16_padded(gy)                                            # [rows][out_p]
+        gy = gy.float()
         if ctx.needs_input_grad[0]:
-            wt = _f16_padded(weight.detach().t())                        # [in][out_p]: B operand, K = out
+            up, down = _row_exponents(gy)
+            g16 = _f16_padded(gy * up)                                   # [rows][out_p]: A operand, K = out
+            wt = _f16_padded(weight.detach().t())                        # [in][out_p]: B operand
             one, zero = _unit_affine(in_f, dev)
-            gx = ops.gemm(g16, wt, one, zero, rows, in_f, out_f, out_f32=True)
+            gx = ops.gemm(g16, wt, one, zero, rows, in_f, out_f, out_f32=True) * down
             if ctx.relu_input:
                 gx = gx * (x16[:, :in_f] > 0)
         if ctx.needs_input_grad[1]:
-            gt = _f16_padded(gy.t())                                     # [out][rows_p]: A operand, K = rows
+            g_t = gy.t()
+            up, down = _row_exponents(g_t)
+            gt = _f16_padded(g_t * up)                                   # [out][rows_p]: A operand, K = rows
             xt = _f16_padded(x16[:, :in_f].t())                          # [in][rows_p]
             one, zero = _unit_affine(in_f, dev)
-            gw = ops.gemm(gt, xt, one, zero, out_f, in_f, rows, out_f32=True)
+            gw = ops.gemm(gt, xt, one, zero, out_f, in_f, rows, out_f32=True) * down
         if ctx.has_bias and ctx.needs_input_grad[2]:
             gb = gy.sum(0)
         return gx, gw, gb, None

@@ -267,11 +267,11 @@ def wgrad_ref(x, g, k, stride, pad, scale=None, inv=None):
     """fp64 weight gradient of b2_conv_wgrad_thw from its fp16 operands x [N, Cin, T, H, W] and g [N, Cout, To, Ho, Wo]:
     G = conv3d_weight(x, g), M = conv3d_weight(|x|, |g|), dW = scale * inv * G, A = |scale| * inv * M.
     Returns (G, M, dW, A), fp64 [Cout, Cin, kt, kh, kw]."""
-    x, g = x.double().cpu(), g.double().cpu()
+    x, g = x.double(), g.double().to(x.device)
     shape = (g.shape[1], x.shape[1]) + tuple(k)
     G = torch.nn.grad.conv3d_weight(x, shape, g, stride=stride, padding=pad)
     M = torch.nn.grad.conv3d_weight(x.abs(), shape, g.abs(), stride=stride, padding=pad)
-    s = scale.double().cpu().view(-1, 1, 1, 1, 1) if scale is not None else torch.ones(1, dtype=torch.float64)
+    s = scale.double().to(x.device).view(-1, 1, 1, 1, 1) if scale is not None else torch.ones(1, dtype=torch.float64, device=x.device)
     i = float(inv) if inv is not None else 1.0
     return G, M, s * i * G, s.abs() * i * M
 
@@ -283,21 +283,186 @@ def wgrad_b(nbox, splits):
     return max(B_ACC, (L + splits + 2) * FLOOR)
 
 
-def wgrad_bound(A, nbox, splits):
+def wgrad_bound(A, nbox, splits, floor=FLOOR):
     """Per-element bound of dW (fp32 output: no output-rounding term)."""
-    return wgrad_b(nbox, splits) * A + FLOOR
+    return wgrad_b(nbox, splits) * A + floor
 
 
-def wdot_ref(G, M, w, inv, nbox, splits):
+def wdot_ref(G, M, w, inv, nbox, splits, floor=FLOOR):
     """wdot[co] = inv * sum w G and its bound: the error of each inv * G element (b M) weighted by |w|, the reduce kernel's fp32
     dot product chain (strided per-thread sum over ceil(n / 256) terms, a 5-level shuffle, 8 warp sums) on inv sum |w| |G|,
     and the floor; n = Cin * taps.  Returns (ref, bound), fp64 [Cout]."""
     Cout = G.shape[0]
     i = float(inv) if inv is not None else 1.0
-    w = w.double().cpu().reshape(Cout, -1)
+    w = w.double().to(G.device).reshape(Cout, -1)
     G, M = G.reshape(Cout, -1), M.reshape(Cout, -1)
     n = G.shape[1]
     ref = i * (w * G).sum(1)
     bnd = (i * (w.abs() * (wgrad_b(nbox, splits) * M)).sum(1)
-           + (-(-n // 256) + 5 + 8) * FLOOR * i * (w.abs() * G.abs()).sum(1) + FLOOR)
+           + (-(-n // 256) + 5 + 8) * FLOOR * i * (w.abs() * G.abs()).sum(1) + floor)
     return ref, bnd
+
+
+# ---------------------------------------------------------------------------------------------
+# fine-tuning backward (tests/test_gpu_finetune_bounds.py on the GPU, tests/test_finetune_bounds_cpu.py on the CPU): the head's
+# gradient products, the pool hand-off and every stage of engine.block_backward, each in fp64 from the true operands.
+#
+# Bound of a gradient element, in the units it is stored in (the trunk's gradients carry the loss scale, the parameter
+# gradients do not):  a * 2^-11 |ref| + 2^-14 A + R + floor, with
+#   a, 2^-14 A   as above (a = 1 for fp16 output, 0 for fp32);
+#   R            the rounding of every operand the function under test rounds to fp16 itself, element by element:
+#                |fp16(v) - v| <= max(2^-11 |v|, 2^-25) for |v| < 65504 (2^-25 is half of fp16's subnormal quantum 2^-24), so
+#                R = sum_j max(2^-11 |u_j|, 2^-25 / s) |v_j| for a rounded operand u multiplied by 2^s before the cast (s = 1
+#                without a scale) and the other operand v.  Operands that arrive in fp16 (activations, incoming gradients)
+#                enter exactly and carry no R;
+#   floor        the fp16 quantum at the scale in use: 2^-24 / s (per row where the scale is per row), i.e. 2^-24 for a gradient
+#                stored with the loss scale.  Elements more than ~2^-31 below their row's peak may be flushed, none above.
+# ---------------------------------------------------------------------------------------------
+SUB_F16 = 2.0 ** -25
+
+
+def r16(v, scale=None):
+    """Bound on |fp16(v * scale) / scale - v|, element by element (fp64): max(2^-11 |v|, 2^-25 / scale); scale broadcasts
+    against v (a power of two per row, or None for an unscaled cast)."""
+    v = v.double()
+    q = SUB_F16 if scale is None else SUB_F16 / scale.double()
+    return torch.maximum(U_F16 * v.abs(), torch.as_tensor(q, dtype=torch.float64, device=v.device))
+
+
+def row_scale(g, dim):
+    """The power of two that puts the peak of each row (dim = 1) or column (dim = 0) of an fp32 gradient in [2^7, 2^8) (the
+    target of b2_loss_scale_f32), 1 for an all-zero row.  fp64, the reduced dimension kept."""
+    amax = g.double().abs().amax(dim, keepdim=True)
+    _, e = torch.frexp(amax)
+    k = torch.where(amax > 0, 8 - e, torch.zeros_like(e)).clamp(-126, 126)
+    return torch.pow(2.0, k.double())
+
+
+def head_ref(gy, w, x16, relu_mask=None):
+    """LinearFunction's two gradient products against the true gradients, from the fp32 logit gradient gy [B][C], the fp32 weight
+    w [C][F] and the fp16 input x16 [B][F] the forward saved:
+      dX = gy w (times relu_mask), A = |gy| |w|; gy is rounded with a power of two per sample row s_b (``row_scale``) and w is
+      rounded unscaled inside the backward: R = max(2^-11 |gy|, 2^-25 / s_b) |w| + |gy| max(2^-11 |w|, 2^-25); floor 2^-24 / s_b;
+      dW = gy^T x16, A = |gy^T| |x16|; gy^T is rounded with a power of two per class row s_c: R = max(2^-11 |gy^T|, 2^-25 / s_c)
+      |x16|; floor 2^-24 / s_c.
+    Both outputs are fp32 (no output-rounding term).  Returns (dx, dx bound, dw, dw bound), fp64."""
+    g, w, x = gy.double(), w.double(), x16.double()
+    sb, sc = row_scale(g, 1), row_scale(g.t(), 1)
+    dx = g @ w
+    bx = B_ACC * (g.abs() @ w.abs()) + r16(g, sb) @ w.abs() + g.abs() @ r16(w) + FLOOR / sb
+    if relu_mask is not None:
+        dx = dx * relu_mask.double()
+    gt = g.t()
+    dw = gt @ x
+    bw = B_ACC * (gt.abs() @ x.abs()) + r16(gt, sc) @ x.abs() + FLOOR / sc
+    return dx, bx, dw, bw
+
+
+def bias_grad_bound(gy):
+    """torch's fp32 column sum of gy [B][C]: any summation order of B terms errs by at most (B - 1) 2^-24 sum |g|."""
+    g = gy.double()
+    return g.sum(0), max(g.shape[0] - 1, 1) * FLOOR * g.abs().sum(0) + FLOOR * 2.0 ** -30
+
+
+def pool_backward_ref(gf, y_out, scale, S):
+    """FineTunePoolFunction.backward: fp16(gf[n] * (scale / S)) where the block output y_out [N * S][C] is positive.  The kernel
+    forms scale / S and the product in fp32 (two roundings, 2^-23 |ref|) and rounds once to fp16.  Returns (ref, bound)."""
+    ref = gf.double().repeat_interleave(S, dim=0) * (float(scale) / S)
+    ref = torch.where(y_out.double() > 0, ref, torch.zeros_like(ref))
+    return ref, (U_F16 + 2.0 ** -23) * ref.abs() + FLOOR
+
+
+def ncdhw(m, N, T, H, W):
+    """[N*T*H*W][C] rows (fp64) -> NCDHW."""
+    return m.double().reshape(N, T, H, W, -1).permute(0, 4, 1, 2, 3)
+
+
+def rows_of(t):
+    """NCDHW -> [N*T*H*W][C] rows."""
+    return t.permute(0, 2, 3, 4, 1).reshape(-1, t.shape[1])
+
+
+def zero_insert_ref(g, size, stride, channels=None):
+    """Adjoint of the type-A / strided subsampling (NCDHW, fp64): g at every ``stride``-th pixel of ``size``, its first ``channels``
+    channels, zeros elsewhere."""
+    N, C = g.shape[0], g.shape[1] if channels is None else channels
+    y = g.new_zeros((N, C) + tuple(size))
+    y[:, :, ::stride, ::stride, ::stride] = g[:, :C]
+    return y
+
+
+def folded(w, s):
+    """The BN-scaled filter s[co] * w[co] of a dgrad, formed in fp32 exactly as the engine forms it, as fp64."""
+    w = w.detach().float()
+    return (w * s.detach().float().to(w.device).view((-1,) + (1,) * (w.dim() - 1))).double()
+
+
+def folded_operand(w, s, pack):
+    """The dgrad's filter operand: with ``pack`` the fp16 rounding of the fp32 s W (what the engine packs, held to it bit for bit by
+    the derived-filter test), R = 0; without, the fp32 s W itself, whose rounding inside the backward R carries."""
+    f = folded(w, s)
+    return (f.half().double(), torch.zeros_like(f)) if pack else (f, r16(f))
+
+
+def dgrad_1x1(g, w, s, mask=None, residual=None, second=None, pack=True):
+    """Input gradient of a 1x1(x1) convolution followed by eval BN: g [M][Cout] (fp16, loss-scaled) . (s W) [Cout][Cin]
+    (+ residual [M][Cin]) (+ second = (g2, w2, s2), another such product), zeroed where mask [M][Cin] <= 0.  ``pack``: see
+    ``folded_operand``.  Returns (ref, A, R), fp64 [M][Cin]."""
+    terms = [(g, w, s)] + ([second] if second is not None else [])
+    ref = A = R = 0
+    for gg, ww, ss in terms:
+        gg = gg.double()
+        f, rf = (t.reshape(ww.shape[0], -1).to(gg.device) for t in folded_operand(ww, ss, pack))                   # [Cout][Cin]
+        ref, A, R = ref + gg @ f, A + gg.abs() @ f.abs(), R + gg.abs() @ rf
+    if residual is not None:
+        r = residual.double()
+        ref, A = ref + r, A + r.abs()
+    if mask is not None:
+        ref = torch.where(mask > 0, ref, torch.zeros_like(ref))
+    return ref, A, R
+
+
+def dgrad_3x3(z, w, s, mask=None, residual=None, pack=True):
+    """Input gradient of a 3x3x3 (or 2-D 3x3, as 1x3x3) convolution followed by eval BN, as the stride-1 convolution of the
+    zero-inserted gradient z (NCDHW fp16 values, loss-scaled) with the flipped, transposed, s-folded filter, padding k // 2.
+    (+ residual, NCDHW), zeroed where mask (NCDHW) <= 0.  ``pack``: see ``folded_operand``.  Returns (ref, A, R) as [rows][Cin],
+    fp64."""
+    f, rf = (t.to(z.device) for t in folded_operand(w, s, pack))
+    if f.dim() == 4:
+        f, rf = f.unsqueeze(2), rf.unsqueeze(2)
+    pad = tuple(k // 2 for k in f.shape[2:])
+    ft, rt = f.flip(2, 3, 4).transpose(0, 1), rf.flip(2, 3, 4).transpose(0, 1)
+    z = z.double()
+    ref = rows_of(F.conv3d(z, ft, padding=pad))
+    A = rows_of(F.conv3d(z.abs(), ft.abs(), padding=pad))
+    R = rows_of(F.conv3d(z.abs(), rt, padding=pad))
+    if residual is not None:
+        r = rows_of(residual.double())
+        ref, A = ref + r, A + r.abs()
+    if mask is not None:
+        ref = torch.where(rows_of(mask) > 0, ref, torch.zeros_like(ref))
+    return ref, A, R
+
+
+def grad_bound(ref, A, R):
+    """Bound of an fp16 loss-scaled gradient (floor: fp16's quantum in the scaled units)."""
+    return bound(ref, A, True) + R
+
+
+def colsum_bound(g, inv):
+    """dbeta = inv * column sums of the fp16 gradient g [rows][C] (b2_colsum_f16, the chain of its two fixed-order passes) and its
+    bound, floor 2^-24 * inv (fp16's quantum of g, unscaled).  Returns (ref, bound), fp64 [C]."""
+    g = g.double()
+    chain = g.shape[0] / (128 * 8) + 8 + 128 + 2
+    return inv * g.sum(0), chain * FLOOR * inv * g.abs().sum(0) + FLOOR * inv
+
+
+def dgamma_ref(wdot, wdot_bnd, dbeta, dbeta_bnd, mean, var, eps):
+    """dgamma = (wdot - mean * dbeta) * rsqrt(var + eps), two fp32 torch ops on top of the kernels' results.  The bound carries
+    the cancellation term r (bnd(wdot) + |mean| bnd(dbeta)) and the fp32 roundings of the product mean * dbeta, the difference,
+    var + eps, rsqrt (<= 2 ulp) and the last product, 7.5 units of 2^-24 at most: 2^-21 r (|wdot| + |mean dbeta|).
+    mean / var: the fp32 running statistics.  Returns (ref, bound), fp64 [C]."""
+    mean, var = mean.double().to(wdot.device), var.float().double().to(wdot.device)
+    r = 1.0 / torch.sqrt(var + float(torch.tensor(eps, dtype=torch.float32)))
+    ref = (wdot - mean * dbeta) * r
+    return ref, r * (wdot_bnd + mean.abs() * dbeta_bnd) + 2.0 ** -21 * r * (wdot.abs() + (mean * dbeta).abs()) + FLOOR * 2.0 ** -30
