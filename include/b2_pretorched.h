@@ -382,6 +382,40 @@ int b2_se_excite(const void* h, int ldh, int N, int S, int C2, const float* w1, 
                  int C, const float* s3, const float* t3, float* scale, float* shift, int ld_aff, float* ws, size_t ws_elems,
                  void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * BNInception (bninception.py:27-495): inception branches written in place into the concatenated block output
+ * ------------------------------------------------------------------------------------------- */
+/* Column-slice destinations.  A destination (y, ldy, cols) is columns [0, cols) of the rows of pitch ldy that start at y: y is
+ * the first column of the slice inside a wider row (16-byte aligned), cols % 8 == 0, ldy % 8 == 0, ldy >= cols.  The entries below
+ * write exactly those columns and leave every other column of the row untouched, so the branches of an inception block
+ * (torch.cat at bninception.py:288, 311, 328, 351, 374, 397, 420, 437, 460, 483) land in their slices of one [M][out] matrix. */
+
+/* Packed layout of a split GEMM: destination d owns the 64-column store boxes [box0[d], box0[d + 1]) of the packed B / affine,
+ * box0[0] = 0, box0[d + 1] = box0[d] + ceil(cols[d] / 64).  Returns the packed width 64 * box0[nd], or B2_ERR_INVALID (1 <= nd <= 4,
+ * cols[d] > 0 and cols[d] % 8 == 0).  Host only. */
+int b2_gemm_split_plan(int nd, const int* cols, int* box0);
+/* One GEMM, up to four column-slice destinations (the 1x1 heads of an inception block that read the same input, bninception.py:266-275):
+ *     D[m][n] = act(scale[n] * (A . B^T)[m][n] + shift[n]),  n < N = b2_gemm_split_plan(nd, cols)
+ * packed column 64 * box0[d] + j (j < cols[d]) is column j of destination d; B rows / affine entries of the padding columns (j >= cols[d]
+ * inside a destination's last box) are computed and dropped.  g: a, lda, b, ldb, Kd, M, N, scale, shift, relu as in b2_gemm_f16;
+ * d, ldd, residual, out_f32, per_row, accumulate, aff_ld, d2 and mask must be zero (B2_ERR_INVALID).  Always the persistent GEMM
+ * (b2_debug_last_kernel: KID 12, info = {N tile, nd, N}) with the N tile b2_gemm_f16 picks for an N-wide output (64 for N <= 64, else
+ * 128): with the same N tile each destination equals the stand-alone b2_gemm_f16 of its rows of B bit for bit. */
+int b2_gemm_split_f16(const b2_gemm_args* g, int nd, void* const* y, const int* ldy, const int* cols, void* stream);
+/* b2_conv_ndhwc_fprop with y a column slice (y, ldy, K) as above: columns [0, K) of each output row are written, K % 8 == 0, the rest
+ * of the row is untouched.  3x3 2-D convolutions (kt = 1, padding (0, 1, 1)) of stride 1 or 2 on the slab kernel only
+ * (b2_debug_last_kernel: KID 13).  Stem mode, mask, per-sample affine, upsampling, second output, pool_w, the generator fields and fp32
+ * output are refused (B2_ERR_INVALID); B2_ERR_UNSUPPORTED when no slab tiling of the image fits. */
+int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream);
+/* Pooling between column slices: x is [N*T*H*W] rows of pitch ldx (channels [0, C) read), y is a slice (y, ldy, C) of rows
+ * [N*To*Ho*Wo] with the output extent given by the caller (ceil mode).  avg = 0: max (nn.MaxPool2d, padding taps skipped);
+ * avg = 1: nn.AvgPool2d(count_include_pad=True) -- fp32 sum in a fixed tap order, divided by the window clipped to the padded input,
+ * one fp16 rounding.  The 3x3 stride-1 pools of the pool branches (bninception.py:61, :247) and the stride-2 ceil-mode pools whose
+ * output is a block's pass-through slice (:102, :206).  Every window must start inside the input or its left padding, padding <= half
+ * the window (B2_ERR_INVALID).  b2_debug_last_kernel: KID 14, info = {avg}. */
+int b2_pool_ndhwc_slice(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh,
+                        int sw, int pt, int ph, int pw, int To, int Ho, int Wo, int avg, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -108,6 +108,11 @@ SYMBOLS = {
     "b2_se_excite_workspace_elems": (ctypes.c_size_t, [c_int] * 3),
     "b2_se_excite": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p,
                              c_void_p, c_void_p, c_void_p, c_int, c_void_p, ctypes.c_size_t, c_void_p]),
+    "b2_gemm_split_plan": (c_int, [c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),
+    "b2_gemm_split_f16": (c_int, [ctypes.POINTER(GemmArgs), c_int, ctypes.POINTER(c_void_p), ctypes.POINTER(c_int),
+                                  ctypes.POINTER(c_int), c_void_p]),
+    "b2_conv_ndhwc_fprop_slice": (c_int, [ctypes.POINTER(ConvArgs), c_void_p]),
+    "b2_pool_ndhwc_slice": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 19 + [c_void_p]),
 }
 
 

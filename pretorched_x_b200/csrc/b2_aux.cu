@@ -122,9 +122,15 @@ __global__ void conv_simt_kernel(SimtConvParams p, long long total) {
 // ------------------------------------------------------------------------------------------
 // pooling
 // ------------------------------------------------------------------------------------------
+// MODE 0: max over a dense [..][C8 * 8] tensor (nn.MaxPool3d, the stem pools).  MODE 1 (max) / 2 (average): column slices --
+// the input rows have pitch ldx, the output rows pitch ldy, and only columns [0, C8 * 8) of an output row are written, so a pool
+// branch of an inception block lands in place in the block's concatenated output.  The average is nn.AvgPool2d with
+// count_include_pad=True: an fp32 sum over the taps in (dt, dh, dw) order (taps in the padding read zero), divided by the
+// window clipped to the padded input (the full window except where a ceil-mode window runs past the padding), one fp16 rounding.
+template <int MODE>
 __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restrict__ y, int N, int T, int H, int W,
                                  int C8, int To, int Ho, int Wo, int kt, int kh, int kw, int st, int sh, int sw, int pt,
-                                 int ph, int pw, long long total) {
+                                 int ph, int pw, long long total, int ldx = 0, int ldy = 0) {
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int c8 = (int)(i % C8);
@@ -133,29 +139,66 @@ __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restric
   const int ho = (int)(q % Ho); q /= Ho;
   const int to = (int)(q % To);
   const int n = (int)(q / To);
-  const __half2 ninf = __float2half2_rn(-65504.f);
-  __half2 m0 = ninf, m1 = ninf, m2 = ninf, m3 = ninf;
-  for (int dt = 0; dt < kt; ++dt) {
-    const int ti = to * st - pt + dt;
-    if ((unsigned)ti >= (unsigned)T) continue;
-    for (int dh = 0; dh < kh; ++dh) {
-      const int hi = ho * sh - ph + dh;
-      if ((unsigned)hi >= (unsigned)H) continue;
-      for (int dw = 0; dw < kw; ++dw) {
-        const int wi = wo * sw - pw + dw;
-        if ((unsigned)wi >= (unsigned)W) continue;
-        const uint4 v = __ldg(reinterpret_cast<const uint4*>(x + ((((size_t)n * T + ti) * H + hi) * W + wi) * (size_t)(C8 * 8)) + c8);
-        m0 = __hmax2(m0, *reinterpret_cast<const __half2*>(&v.x));
-        m1 = __hmax2(m1, *reinterpret_cast<const __half2*>(&v.y));
-        m2 = __hmax2(m2, *reinterpret_cast<const __half2*>(&v.z));
-        m3 = __hmax2(m3, *reinterpret_cast<const __half2*>(&v.w));
+  if constexpr (MODE == 2) {
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int dt = 0; dt < kt; ++dt) {
+      const int ti = to * st - pt + dt;
+      if ((unsigned)ti >= (unsigned)T) continue;
+      for (int dh = 0; dh < kh; ++dh) {
+        const int hi = ho * sh - ph + dh;
+        if ((unsigned)hi >= (unsigned)H) continue;
+        for (int dw = 0; dw < kw; ++dw) {
+          const int wi = wo * sw - pw + dw;
+          if ((unsigned)wi >= (unsigned)W) continue;
+          const uint4 v = __ldg(reinterpret_cast<const uint4*>(x + ((((size_t)n * T + ti) * H + hi) * W + wi) * (size_t)ldx + c8 * 8));
+          const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&u[e]));
+            acc[2 * e] += f.x;
+            acc[2 * e + 1] += f.y;
+          }
+        }
       }
     }
+    const int t0 = to * st - pt, h0 = ho * sh - ph, w0 = wo * sw - pw;
+    const int div = (min(t0 + kt, T + pt) - t0) * (min(h0 + kh, H + ph) - h0) * (min(w0 + kw, W + pw) - w0);
+    uint4 o;
+    uint32_t* op = reinterpret_cast<uint32_t*>(&o);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const __half2 h2 = __floats2half2_rn(acc[2 * e] / (float)div, acc[2 * e + 1] / (float)div);
+      op[e] = *reinterpret_cast<const uint32_t*>(&h2);
+    }
+    *reinterpret_cast<uint4*>(y + ((((size_t)n * To + to) * Ho + ho) * Wo + wo) * (size_t)ldy + c8 * 8) = o;
+  } else {
+    const __half2 ninf = __float2half2_rn(-65504.f);
+    __half2 m0 = ninf, m1 = ninf, m2 = ninf, m3 = ninf;
+    for (int dt = 0; dt < kt; ++dt) {
+      const int ti = to * st - pt + dt;
+      if ((unsigned)ti >= (unsigned)T) continue;
+      for (int dh = 0; dh < kh; ++dh) {
+        const int hi = ho * sh - ph + dh;
+        if ((unsigned)hi >= (unsigned)H) continue;
+        for (int dw = 0; dw < kw; ++dw) {
+          const int wi = wo * sw - pw + dw;
+          if ((unsigned)wi >= (unsigned)W) continue;
+          const uint4 v = MODE == 0
+              ? __ldg(reinterpret_cast<const uint4*>(x + ((((size_t)n * T + ti) * H + hi) * W + wi) * (size_t)(C8 * 8)) + c8)
+              : __ldg(reinterpret_cast<const uint4*>(x + ((((size_t)n * T + ti) * H + hi) * W + wi) * (size_t)ldx + c8 * 8));
+          m0 = __hmax2(m0, *reinterpret_cast<const __half2*>(&v.x));
+          m1 = __hmax2(m1, *reinterpret_cast<const __half2*>(&v.y));
+          m2 = __hmax2(m2, *reinterpret_cast<const __half2*>(&v.z));
+          m3 = __hmax2(m3, *reinterpret_cast<const __half2*>(&v.w));
+        }
+      }
+    }
+    uint4 o;
+    o.x = *reinterpret_cast<uint32_t*>(&m0); o.y = *reinterpret_cast<uint32_t*>(&m1);
+    o.z = *reinterpret_cast<uint32_t*>(&m2); o.w = *reinterpret_cast<uint32_t*>(&m3);
+    if constexpr (MODE == 0) reinterpret_cast<uint4*>(y)[i] = o;
+    else *reinterpret_cast<uint4*>(y + ((((size_t)n * To + to) * Ho + ho) * Wo + wo) * (size_t)ldy + c8 * 8) = o;
   }
-  uint4 o;
-  o.x = *reinterpret_cast<uint32_t*>(&m0); o.y = *reinterpret_cast<uint32_t*>(&m1);
-  o.z = *reinterpret_cast<uint32_t*>(&m2); o.w = *reinterpret_cast<uint32_t*>(&m3);
-  reinterpret_cast<uint4*>(y)[i] = o;
 }
 
 // The stem pool (3x3x3, stride 2, pad 1): branch-free so that the nine loads of a temporal tap are issued
@@ -589,7 +632,7 @@ int b2_maxpool3d_ndhwc(const void* x, void* y, int N, int T, int H, int W, int C
     maxpool3d_k331s221_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         (const __half*)x, (__half*)y, T, H, W, C / 8, To, Ho, total);
   } else {
-    maxpool3d_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+    maxpool3d_kernel<0><<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         (const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw, total);
   }
   B2_CHECK_LAUNCH("maxpool3d");
@@ -606,9 +649,36 @@ int b2_maxpool3d_ndhwc_out(const void* x, void* y, int N, int T, int H, int W, i
   B2_CHECK_ARG((To - 1) * st - pt < T && (Ho - 1) * sh - ph < H && (Wo - 1) * sw - pw < W && kt > pt && kh > ph && kw > pw,
                "output extent %dx%dx%d has a window outside the %dx%dx%d input", To, Ho, Wo, T, H, W);
   const long long total = (long long)N * To * Ho * Wo * (C / 8);
-  maxpool3d_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+  maxpool3d_kernel<0><<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       (const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh, sw, pt, ph, pw, total);
   B2_CHECK_LAUNCH("maxpool3d");
+  return B2_OK;
+}
+
+int b2_pool_ndhwc_slice(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh,
+                        int sw, int pt, int ph, int pw, int To, int Ho, int Wo, int avg, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(x && y && N > 0 && T > 0 && H > 0 && W > 0 && C > 0, "bad argument");
+  B2_CHECK_ARG(C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0 && ldx >= C && ldy >= C,
+               "channels %d, input pitch %d and output pitch %d must be multiples of 8 with both pitches >= the channels", C, ldx, ldy);
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "input / output slice not 16-byte aligned");
+  B2_CHECK_ARG(kt > 0 && kh > 0 && kw > 0 && st > 0 && sh > 0 && sw > 0 && pt >= 0 && ph >= 0 && pw >= 0, "bad window");
+  B2_CHECK_ARG(2 * pt <= kt && 2 * ph <= kh && 2 * pw <= kw, "padding exceeds half the window");
+  B2_CHECK_ARG(avg == 0 || avg == 1, "avg must be 0 (max) or 1 (average)");
+  B2_CHECK_ARG(To > 0 && Ho > 0 && Wo > 0, "empty output");
+  // every window must start inside the input or its left padding (torch's ceil-mode rule), so it overlaps the input
+  B2_CHECK_ARG((To - 1) * st - pt < T && (Ho - 1) * sh - ph < H && (Wo - 1) * sw - pw < W,
+               "output extent %dx%dx%d has a window outside the %dx%dx%d input", To, Ho, Wo, T, H, W);
+  const long long total = (long long)N * To * Ho * Wo * (C / 8);
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (avg)
+    maxpool3d_kernel<2><<<div_up(total, 256), 256, 0, s>>>((const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh,
+                                                             sw, pt, ph, pw, total, ldx, ldy);
+  else
+    maxpool3d_kernel<1><<<div_up(total, 256), 256, 0, s>>>((const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh,
+                                                             sw, pt, ph, pw, total, ldx, ldy);
+  B2_CHECK_LAUNCH("maxpool3d");
+  set_last_kernel(KID_POOL, avg);
   return B2_OK;
 }
 

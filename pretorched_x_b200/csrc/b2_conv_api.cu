@@ -1,6 +1,7 @@
 // b2_conv_api.cu -- C-ABI entry points for the wgmma implicit-GEMM convolution and the dense GEMM,
 // plus library-wide error/launch bookkeeping and the CUtensorMap builder.
 #include <atomic>
+#include <limits.h>
 #include <mutex>
 #include <stdlib.h>
 #include <string.h>
@@ -258,6 +259,15 @@ static bool slab_geometry(const b2_conv_args* a, SlabParams* p, int wc_hint) {
 
 template <int BNT, int TMT, int G = 0>
 static int run_slab(int grid, int smem_bytes, const CUtensorMap& tmX, const CUtensorMap& tmB, const SlabParams& p, cudaStream_t stream) {
+  if constexpr (G == 0) {
+    if (p.ldo) {                    // column-slice output (b2_conv_ndhwc_fprop_slice)
+      auto kernel = slabconv_kernel<BNT, TMT, kSlabSlice>;
+      B2_OPT_IN_SMEM(kernel, 227 * 1024);
+      B2_CHECK_CUDA(launch_pdl(kernel, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
+      B2_CHECK_LAUNCH("slabconv_kernel");
+      return B2_OK;
+    }
+  }
   auto kernel = slabconv_kernel<BNT, TMT, G>;
   B2_OPT_IN_SMEM(kernel, 227 * 1024);
   B2_CHECK_CUDA(launch_pdl(kernel, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
@@ -267,8 +277,9 @@ static int run_slab(int grid, int smem_bytes, const CUtensorMap& tmX, const CUte
 
 // BNT = 0: runtime N tile p.bn (set by the caller).  G != 0: grouped convolution (b2_groupconv.cuh) -- N tiles are the K / 64
 // channel slices, a.w is the packed grouped filter
+// ldo > 0: y is a column slice of rows of pitch ldo; a->ldy is then the slice width (the columns written)
 template <int BNT, int G = 0>
-static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cudaStream_t stream) {
+static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cudaStream_t stream, int ldo = 0) {
   if (BNT) { p.bn = BNT; p.wbytes = BNT * 128; p.accs = BNT; }
   if (G) { p.wbytes = G * 128; p.cchunks = 1; }
   const int BN = p.bn;
@@ -287,6 +298,7 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.ldr = a->ldr;
   p.y = reinterpret_cast<__half*>(a->y);
   p.ldy = a->ldy;
+  p.ldo = ldo;
   p.relu = a->relu;
   p.aff_ld = a->aff_ld;
   p.naff = slab_naff(a->ldy);
@@ -324,8 +336,9 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
 // Picks the N tile (fixed 64 / 128 or runtime), the M tiles per work item and the slab rows for a geometry; *best_mt == 0
 // when no configuration fits in shared memory.
 // G != 0 (grouped convolution): the N tiles are the K / 64 channel slices, each with a G-row weight stage per tap.
+// allow_flex = false: fixed 64 / 128 tiles only (the slice path's retry when the runtime-N tile finds no fit).
 static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out, bool* flex_out, int* best_mt_out, int* best_R_out,
-                              int G = 0) {
+                              int G = 0, bool allow_flex = true) {
   int BN = (G || a->ldy <= 64) ? 64 : 128;
   const int planes = a->N * p.To;
   int ntn = G ? a->K / 64 : (a->ldy + BN - 1) / BN;
@@ -333,7 +346,7 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   // tiles of <= 256 columns, each a multiple of 16 wide.
   bool flex = false;
   if (G) {
-  } else if (a->ldy > 128) {
+  } else if (a->ldy > 128 && allow_flex) {
     const int tn = (a->ldy + 255) / 256;
     const int bn = (((a->ldy + tn - 1) / tn) + 15) / 16 * 16;
     if (bn <= kSlabAccCols && ((long long)bn * tn * 21 <= (long long)ntn * 128 * 20 || (g_slab_wide == 1 && a->ldy % 256 == 0))) {
@@ -410,8 +423,9 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
 
 // returns 1 when the slab kernel took the convolution, 0 when it does not apply, <0 on error
 // G != 0: grouped convolution inside the contract of b2_conv_grouped_ndhwc_fprop (3x3 in plane, so never the temporal remap)
-static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0) {
-  if (g_conv_algo == 1 && !G) return 0;
+// ldo > 0: column-slice output, see launch_slab
+static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, int ldo = 0) {
+  if (g_conv_algo == 1 && !G && !ldo) return 0;
   SlabParams p;
   b2_conv_args remap = *a_in;
   const b2_conv_args* a = a_in;
@@ -443,7 +457,13 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0) {
     if (G) q.cchunks = 1;                                     // an item reads its own 64-channel slice only
     int bn_c = 0, mt_c = 0, r_c = 0;
     bool flex_c = false;
-    const double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G);
+    const SlabParams q0 = q;
+    double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G);
+    if (mt_c == 0 && ldo && flex_c) {
+      // a slice has no other kernel to fall back on: when the wide runtime-N tile does not fit, take 128-column tiles
+      q = q0;
+      cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G, false);
+    }
     if (mt_c == 0) continue;
     if (best_mt == 0 || cost < best_cost) { best_p = q; BN = bn_c; flex = flex_c; best_mt = mt_c; best_R = r_c; best_cost = cost; }
   }
@@ -451,9 +471,10 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0) {
   if (best_mt == 0) return 0;
   int rc = G == 16 ? launch_slab<64, 16>(a, p, best_mt, best_R, stream)
            : G == 32 ? launch_slab<64, 32>(a, p, best_mt, best_R, stream)
-           : flex ? launch_slab<0>(a, p, best_mt, best_R, stream)
-                  : (BN == 64) ? launch_slab<64>(a, p, best_mt, best_R, stream) : launch_slab<128>(a, p, best_mt, best_R, stream);
+           : flex ? launch_slab<0>(a, p, best_mt, best_R, stream, ldo)
+                  : (BN == 64) ? launch_slab<64>(a, p, best_mt, best_R, stream, ldo) : launch_slab<128>(a, p, best_mt, best_R, stream, ldo);
   if (rc == B2_OK && G) set_last_kernel(KID_GROUPCONV, G, best_mt, p.mp, p.wchunks);
+  else if (rc == B2_OK && ldo) set_last_kernel(KID_SLAB_SLICE, BN, best_mt, flex, p.wchunks);
   else if (rc == B2_OK) set_last_kernel(KID_SLAB, BN, best_mt, flex, p.wchunks, a != a_in);
   return rc == B2_OK ? 1 : rc;
 }
@@ -888,6 +909,38 @@ static int launch_pgemm_chain(const b2_gemm_args* g, const void* a2, int lda2, c
   return B2_OK;
 }
 
+// The split instance (b2_gemm_split_f16): pgemm_kernel<BN, 0, 3> with one tensor map per column-slice destination.
+template <int BN>
+static int launch_pgemm_split(const b2_gemm_args* g, int nd, void* const* y, const int* ldy, const int* cols, const int* box0,
+                              cudaStream_t stream) {
+  using S = PgemmSmem<BN, 0>;
+  B2_OPT_IN_SMEM((pgemm_kernel<BN, 0, 3>), S::kTotal);
+  CUtensorMap tmA, tmB, tmD[4];
+  int rc;
+  const int Npad = box0[nd] * 64;
+  if ((rc = make_tmap_2d_f16(&tmA, g->a, (uint64_t)g->Kd, (uint64_t)g->M, (uint64_t)g->lda, 64, 128, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmB, g->b, (uint64_t)g->Kd, (uint64_t)Npad, (uint64_t)g->ldb, 64, BN, true)) != B2_OK) return rc;
+  for (int d = 0; d < 4; ++d) {
+    const int s = d < nd ? d : 0;       // unused slots repeat destination 0 (never selected)
+    if ((rc = make_tmap_2d_f16(&tmD[d], y[s], (uint64_t)cols[s], (uint64_t)g->M, (uint64_t)ldy[s], 64, 64, true)) != B2_OK) return rc;
+  }
+  PgemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.M = g->M; p.Ncols = Npad; p.ldy = Npad; p.nkb = (g->Kd + 63) / 64; p.nkb2 = 0;
+  p.tiles_n = (Npad + BN - 1) / BN;
+  p.tiles_total = p.tiles_n * ((g->M + 127) / 128);
+  p.scale = g->scale; p.shift = g->shift;
+  p.relu = g->relu;
+  p.fd_Wh = make_fastdiv(2); p.fd_Hh = make_fastdiv(2); p.fd_aff = make_fastdiv(1);
+  for (int d = 0; d < 4; ++d) p.split_box[d] = d < nd ? box0[d] : INT_MAX;
+  const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
+  B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, 0, 3>, dim3(grid), dim3(kPgThreads), S::kTotal, stream, tmA, tmB, tmD[3], tmB, tmD[0], tmD[1],
+                           tmD[2], p));
+  B2_CHECK_LAUNCH("pgemm_kernel");
+  set_last_kernel(KID_PGEMM_SPLIT, BN, nd, Npad);
+  return B2_OK;
+}
+
 static int g_last_gemm_path = 0;   // kernel of the last GEMM-family launch: 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (tests pin it)
 
 static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
@@ -1300,6 +1353,66 @@ static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const vo
     return g->ldd <= 64 ? launch_pgemm<64, 0, 2>(L, st) : launch_pgemm<128, 0, 2>(L, st);
   }
   return dispatch_igemm(L, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_gemm_split_plan(int nd, const int* cols, int* box0) {
+  B2_CHECK_ARG(nd >= 1 && nd <= 4 && cols && box0, "a split GEMM has 1 to 4 destinations (got %d)", nd);
+  box0[0] = 0;
+  for (int d = 0; d < nd; ++d) {
+    B2_CHECK_ARG(cols[d] > 0 && cols[d] % 8 == 0, "destination %d: width %d is not a positive multiple of 8", d, cols[d]);
+    box0[d + 1] = box0[d] + (cols[d] + 63) / 64;
+  }
+  return box0[nd] * 64;
+}
+
+int b2_gemm_split_f16(const b2_gemm_args* g, int nd, void* const* y, const int* ldy, const int* cols, void* stream) {
+  set_last_kernel(KID_NONE);
+  int box0[5];
+  const int Npad = b2_gemm_split_plan(nd, cols, box0);
+  if (Npad < 0) return Npad;
+  B2_CHECK_ARG(g != nullptr && g->a && g->b && g->scale && g->shift && y && ldy, "null tensor pointer");
+  B2_CHECK_ARG(g->M > 0 && g->Kd > 0, "non-positive dimension");
+  B2_CHECK_ARG(g->N == Npad, "N %d is not the packed width %d of the destinations (whole 64-column boxes each)", g->N, Npad);
+  B2_CHECK_ARG(g->lda % 8 == 0 && g->ldb % 8 == 0 && g->lda >= g->Kd && g->ldb >= g->Kd, "bad operand pitch");
+  B2_CHECK_ARG(!g->d && !g->ldd && !g->residual && !g->out_f32 && !g->per_row && !g->accumulate && !g->aff_ld && !g->d2 && !g->mask,
+               "the split GEMM writes fp16 through its destinations with a per-column affine: d, ldd, residual, out_f32, per_row, "
+               "accumulate, aff_ld, d2 and mask must be zero");
+  for (int d = 0; d < nd; ++d) {
+    B2_CHECK_ARG(y[d] != nullptr && (reinterpret_cast<uintptr_t>(y[d]) & 15) == 0, "destination %d is null or not 16-byte aligned", d);
+    B2_CHECK_ARG(ldy[d] % 8 == 0 && ldy[d] >= cols[d], "destination %d: pitch %d is not a multiple of 8 >= its width %d", d, ldy[d], cols[d]);
+  }
+  if (g_gemm_algo != 0) return set_error(B2_ERR_UNSUPPORTED, "the split GEMM needs the persistent kernel");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  g_last_gemm_path = 2;
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // the N tile b2_gemm_f16 picks for an output of this width
+  return Npad <= 64 ? launch_pgemm_split<64>(g, nd, y, ldy, cols, box0, st) : launch_pgemm_split<128>(g, nd, y, ldy, cols, box0, st);
+}
+
+int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream) {
+  set_last_kernel(KID_NONE);
+  int rc = validate_conv(a);
+  if (rc != B2_OK) return rc;
+  B2_CHECK_ARG(a->mode == B2_CONV_AUTO && !a->mask && !a->ldm && !a->aff_ld && !a->upsample && !a->y2 && !a->scale2 && !a->shift2 &&
+                   !a->aff2_ld && !a->pool_w && !a->residual_up && !a->residual_pre && !a->in_scale && !a->in_shift && !a->in_aff_ld &&
+                   !a->out_f32 && !a->accumulate,
+               "the slice convolution takes a plain fp16 call: stem mode, mask, per-sample affine, upsampling, second output, pool_w, "
+               "generator fields and fp32 output must be zero");
+  B2_CHECK_ARG(a->kt == 1 && a->kh == 3 && a->kw == 3 && a->pt == 0 && a->ph == 1 && a->pw == 1 && a->st == 1 && a->sh == a->sw &&
+                   (a->sh == 1 || a->sh == 2),
+               "the slice convolution is a 3x3 2-D convolution with padding 1 and stride 1 or 2 (got %dx%dx%d, stride %d%d%d, padding %d%d%d)",
+               a->kt, a->kh, a->kw, a->st, a->sh, a->sw, a->pt, a->ph, a->pw);
+  B2_CHECK_ARG(a->K % 8 == 0, "slice width K %d is not a multiple of 8", a->K);
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(a->y) & 15) == 0, "slice start is not 16-byte aligned");
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  g_last_conv_path = 0;
+  g_last_gemm_path = 0;
+  b2_conv_args s = *a;
+  s.ldy = a->K;                         // the slab planner and epilogue see the slice width; ldo carries the row pitch
+  rc = try_slab(&s, reinterpret_cast<cudaStream_t>(stream), 0, a->ldy);
+  if (rc == 0) return set_error(B2_ERR_UNSUPPORTED, "no slab tiling of this image fits in shared memory (H=%d W=%d)", a->H, a->W);
+  return rc < 0 ? rc : B2_OK;
 }
 
 }  // extern "C"

@@ -76,7 +76,10 @@ int require_sm90();
 // (b2_debug_last_kernel: tests pin the variant a case exercised, so a dispatch change cannot silently move its coverage).
 enum LastKernel : int {
   KID_NONE = 0, KID_STEM = 1, KID_SLAB = 2, KID_SLABTS = 3 /* reserved: the temporal-group slab kernel, removed */, KID_TSTACK = 4, KID_DENSEM = 5, KID_PGEMM = 6, KID_IGEMM = 7,
-  KID_SIMT = 8, KID_ATTENTION = 9, KID_GROUPCONV = 10, KID_PGEMM_CHAIN = 11
+  KID_SIMT = 8, KID_ATTENTION = 9, KID_GROUPCONV = 10, KID_PGEMM_CHAIN = 11,
+  KID_PGEMM_SPLIT = 12 /* b2_gemm_split_f16: info = {BN, destinations, packed columns} */,
+  KID_SLAB_SLICE = 13 /* b2_conv_ndhwc_fprop_slice: info as KID_SLAB */,
+  KID_POOL = 14 /* b2_pool_ndhwc_slice: info = {average} */
 };
 void set_last_kernel(int id, int i0 = 0, int i1 = 0, int i2 = 0, int i3 = 0, int i4 = 0);
 

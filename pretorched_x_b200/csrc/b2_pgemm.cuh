@@ -72,6 +72,12 @@ struct PgemmParams {
   // pgemm_kernel<BN, 0, 2> only: per-sample affine at ANY rows per sample (aff_rows need not divide 128, so a tile may straddle
   // samples).  Each fragment row resolves its own sample n = m / aff_rows with this divider and reads row n of scale / shift.
   FastDiv fd_aff;
+  // pgemm_kernel<BN, 0, 3> only: column-slice destinations.  The Ncols = ldy packed columns are whole 64-column store boxes;
+  // destination d owns boxes [split_box[d], split_box[d + 1]) (split_box[d] = INT_MAX past the last one) and box b of it
+  // lands at its column 64 (b - split_box[d]) through tensor map d (tmC, tmR, tmC2, tmA2: the residual, second-output and
+  // second-operand maps this instance never reads).  Each map spans only its destination's columns, so TMA drops the
+  // padding columns of a ragged last box and nothing outside the slice is written.
+  int split_box[4];
 };
 
 template <int BN, int GAN>
@@ -313,7 +319,16 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       if (leader && m0 + wg * 64 < p.M) {
 #pragma unroll
         for (int b = 0; b < BN / 64; ++b)
-          if (n0 + b * 64 < p.ldy) tma_store_2d(&tmC, stage + b * (128 * 128) + wg * (64 * 128), n0 + b * 64, m0 + wg * 64);
+          if constexpr (EPI == 3) {
+            const int box = (n0 >> 6) + b;
+            int d = 0;
+#pragma unroll
+            for (int e = 1; e < 4; ++e) d = box >= p.split_box[e] ? e : d;
+            const CUtensorMap* tm = d == 0 ? &tmC : d == 1 ? &tmR : d == 2 ? &tmC2 : &tmA2;
+            if (n0 + b * 64 < p.ldy) tma_store_2d(tm, stage + b * (128 * 128) + wg * (64 * 128), (box - p.split_box[d]) * 64, m0 + wg * 64);
+          } else {
+            if (n0 + b * 64 < p.ldy) tma_store_2d(&tmC, stage + b * (128 * 128) + wg * (64 * 128), n0 + b * 64, m0 + wg * 64);
+          }
         tma_store_commit();
       }
       if (GAN && p.dual) {                                 // second output: next block's ccbn + ReLU on the fp32 value

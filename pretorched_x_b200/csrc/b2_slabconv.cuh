@@ -95,6 +95,7 @@ struct SlabParams {
   // 4-D TMA box brings the mp slabs ([plane][R][PW] in shared memory); tile j's A operand starts j * plane_stride bytes further.
   int mp, plane_stride, planes_total;
   FastDiv fd_tiles_n, fd_tiles_q, fd_wchunks, fd_To, fd_PW;   // dividers of the item decode (set by launch_slab)
+  int ldo;                 // slabconv_kernel<BN, TMT, kSlabSlice> only: row pitch of y (>= ldy, the columns written)
 };
 
 // scale/shift live in smem for all (padded) output channels: SlabParams::naff = round_up(ldy, 32) + 32 entries each; the
@@ -280,11 +281,15 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
 // G = 16 / 32 (BN = 64): grouped convolution with C == K (b2_groupconv.cuh).  N tile tn is the 64-channel slice tn of input AND
 // output, the item has one channel chunk (SlabParams::cchunks = 1) whose TMA channel coordinate is the slice's, and a weight stage
 // is the G-row tile of (slice, tap).
-template <int BN, int TMT = 0, int G = 0>
+// G = kSlabSlice: dense filter, y is a column slice of a wider row -- the epilogue writes columns [0, ldy) of rows of pitch
+// SlabParams::ldo and nothing else, so an inception branch lands in place in its block's concatenated output.
+constexpr int kSlabSlice = -1;
+template <int BN, int TMT = 0, int G_ = 0>
 __global__ void __launch_bounds__(kSlabThreads, 1)
 slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H, N*T), box (64, PW, R, 1)
                 const __grid_constant__ CUtensorMap tmB,   // weights [Ncols][taps*C], box (64, BN); G: [slices*taps*G][64], box (64, G)
                 const SlabParams p) {
+  constexpr int G = G_ > 0 ? G_ : 0;            // channels per group of the grouped form, 0 otherwise
   static_assert(G == 0 || (BN == 64 && TMT == 0), "the grouped form runs on the 64-wide tile with positions along M");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align<1024>(smem_raw);
@@ -463,7 +468,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
               // whole 32-column row segment would not fit the register budget
               const float* arow = at.p + static_cast<size_t>(erow) * at.ld + j * accs + jc * 32;
               if (ok[j]) {
-                __half* yrow = p.y + row[j] * p.ldy + c0;
+                __half* yrow = p.y + row[j] * (G_ == kSlabSlice ? p.ldo : p.ldy) + c0;
                 if (p.residual) {                              // uniform: residual added in fp32 before the single rounding
 #pragma unroll
                   for (int c8 = 0; c8 < 4; ++c8) {

@@ -686,6 +686,117 @@ def run_senet_trunk(model, x):
 
 
 # ---------------------------------------------------------------------------------------------
+# BNInception (bninception.py:27-495)
+# ---------------------------------------------------------------------------------------------
+def _split_pack(model, names, in_pitch):
+    """Packed B and affine of a split GEMM over the 1x1 convolutions ``names`` (each followed by ``name + '_bn'``) that read the
+    same input: destination d's fp16 filter rows and folded (conv bias + BN) affine from packed column 64 * box0[d] on, zero
+    rows in the padding of its last 64-column box (ops.split_plan).  Cached on the first convolution."""
+    convs = [getattr(model, n) for n in names]
+    bns = [getattr(model, n + '_bn') for n in names]
+    dev = convs[0].weight.device
+
+    def build():
+        npad, box0 = ops.split_plan([c.weight.shape[0] for c in convs])
+        w = torch.zeros((npad, in_pitch), dtype=torch.float16, device=dev)
+        scale = torch.zeros(npad, dtype=torch.float32, device=dev)
+        shift = torch.zeros(npad, dtype=torch.float32, device=dev)
+        for d, (c, bn) in enumerate(zip(convs, bns)):
+            K, r0 = c.weight.shape[0], 64 * box0[d]
+            w[r0:r0 + K, :c.weight.shape[1]] = _conv1x1_matrix(c).float().to(torch.float16)
+            scale[r0:r0 + K], shift[r0:r0 + K] = ops.fold_affine(K, c.bias, bn, dev)
+        return w, scale, shift
+
+    tensors = [t for c, bn in zip(convs, bns) for t in (c.weight, c.bias) + _bn_tensors(bn)]
+    reads = tuple(t for c, bn in zip(convs[1:], bns[1:]) for t in (c.weight, c.bias)) + tuple(t for bn in bns for t in _bn_tensors(bn))
+    return _cached(convs[0], "split", _sig(*tensors) + (in_pitch,), build, reads=reads)
+
+
+def _pool2d(pool):
+    """(kernel, stride, padding) of a square nn.MaxPool2d / nn.AvgPool2d with ceil_mode=True and no dilation."""
+    two = lambda v: (v, v) if isinstance(v, int) else tuple(v)
+    k, s, p = two(pool.kernel_size), two(pool.stride), two(pool.padding)
+    if (k[0] != k[1] or s[0] != s[1] or p[0] != p[1] or not pool.ceil_mode or getattr(pool, 'dilation', 1) not in (1, (1, 1))
+            or (isinstance(pool, nn.AvgPool2d) and not pool.count_include_pad)):
+        raise NotImplementedError("BNInception pools are square ceil-mode windows (average pools count the padding)")
+    return k[0], s[0], p[0]
+
+
+def run_inception(model, spec, a, out=None):
+    """One inception block of BNInception (``spec``: a row of models.bninception.BLOCKS) through its Function."""
+    return Fn.InceptionFunction.run(model, a, spec, out)
+
+
+def _inception_body(model, spec, a, out=None):
+    """The branches of an inception block (bninception.py:266-288 and the other blocks) each write their columns of the
+    concatenated output ``y`` [M][out] in place -- no copies, no padding columns:
+
+    * one split GEMM over the block input computes the 1x1 head straight into its slice and the two 3x3 reduces into their own
+      matrices (the three 1x1 convolutions that read the input, as one pass over it);
+    * the 3x3 branch and the second 3x3 of the double branch write their slices (slice convolutions, stride 2 in 3c / 4e);
+    * the pool branch pools the block input -- AvgPool2d(3, 1, 1) (MaxPool2d at 5b) into a dense matrix that its projection GEMM
+      reads and writes into its slice, or, in the stride-2 blocks, MaxPool2d(3, 2, ceil_mode) straight into the pass-through slice.
+
+    Six launches per stride-1 block (the block input is read by the split GEMM and the pool), five per stride-2 block."""
+    from .models.bninception import block_out_channels
+    n, cin, c1, (c3r, c3), (cdr, cd), (pk, proj) = spec
+    p = 'inception_%s_' % n
+    if a.C != cin or a.ld != cin:
+        raise ValueError("inception_%s takes a dense [M][%d] input, got %r" % (n, cin, a))
+    pool = getattr(model, p + 'pool')
+    k, s, pd = _pool2d(pool)
+    Ho, Wo = ops.ceil_pool_dim(a.H, k, s, pd), ops.ceil_pool_dim(a.W, k, s, pd)
+    if s > 1 and (Ho, Wo) != (ops._out_dim(a.H, 3, 2, 1), ops._out_dim(a.W, 3, 2, 1)):
+        raise ValueError("inception_%s: the stride-2 pool and convolutions disagree on a %dx%d map" % (n, a.H, a.W))
+    C = block_out_channels(spec)
+    M = a.N * a.T * Ho * Wo
+    dev = a.data.device
+    y = ops._out_rows(out, M, C) if out is not None else torch.empty((M, C), dtype=torch.float16, device=dev)
+    r3 = torch.empty((a.M, c3r), dtype=torch.float16, device=dev)
+    rd = torch.empty((a.M, cdr), dtype=torch.float16, device=dev)
+    heads = ([p + '1x1'] if c1 is not None else []) + [p + '3x3_reduce', p + 'double_3x3_reduce']
+    w, scale, shift = _split_pack(model, heads, a.ld)
+    col = c1 or 0
+    ops.gemm_split(a.data, w, scale, shift, a.M, a.ld, ([y[:, :col]] if c1 is not None else []) + [r3, rd], relu=True)
+    conv = getattr(model, p + '3x3')
+    ops.conv_slice(Act(r3, a.N, a.T, a.H, a.W, c3r), packed_conv(conv, getattr(model, p + '3x3_bn'), c3r), y[:, col:col + c3])
+    col += c3
+    d1 = conv_bn_act(getattr(model, p + 'double_3x3_1'), getattr(model, p + 'double_3x3_1_bn'), Act(rd, a.N, a.T, a.H, a.W, cdr),
+                     relu=True)
+    conv = getattr(model, p + 'double_3x3_2')
+    ops.conv_slice(d1, packed_conv(conv, getattr(model, p + 'double_3x3_2_bn'), d1.ld), y[:, col:col + cd])
+    col += cd
+    avg = isinstance(pool, nn.AvgPool2d)
+    if proj is None:
+        ops.pool_slice(a, k, s, pd, avg, y[:, col:])
+    else:
+        pooled = ops.pool_slice(a, k, s, pd, avg)
+        w, scale, shift = _split_pack(model, [p + 'pool_proj'], pooled.ld)
+        ops.gemm_split(pooled.data, w, scale, shift, pooled.M, pooled.ld, [y[:, col:col + proj]], relu=True)
+    return Act(y, a.N, a.T, Ho, Wo, C)
+
+
+def _bninception_stem_body(model, a, out=None):
+    """conv1_7x7_s2 -> BN -> ReLU on the stem kernel, pool1 (MaxPool2d(3, 2, ceil_mode)), conv2_3x3_reduce and conv2_3x3 (each
+    -> BN -> ReLU), pool2 (bninception.py:255-265)."""
+    h = conv_bn_act(model.conv1_7x7_s2, model.conv1_7x7_s2_bn, a, relu=True)
+    h = ops.maxpool2d_ceil(h, *_pool2d(model.pool1_3x3_s2))
+    h = conv_bn_act(model.conv2_3x3_reduce, model.conv2_3x3_reduce_bn, h, relu=True)
+    h = conv_bn_act(model.conv2_3x3, model.conv2_3x3_bn, h, relu=True)
+    return ops.maxpool2d_ceil(h, *_pool2d(model.pool2_3x3_s2), out=out)
+
+
+def run_bninception_trunk(model, x):
+    """The BNInception trunk: fp32 NCHW images (or an NDHWC4 Act) in, the 5b block output (an Act) out."""
+    from .models.bninception import BLOCKS
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x)
+    a = Fn.BNInceptionStemFunction.run(model, a)
+    for spec in BLOCKS:
+        a = run_inception(model, spec, a)
+    return a
+
+
+# ---------------------------------------------------------------------------------------------
 # stem / trunk / head
 # ---------------------------------------------------------------------------------------------
 def _pool_args(mp):

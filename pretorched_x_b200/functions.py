@@ -147,6 +147,25 @@ class SEBottleneckFunction(_FrozenFunction):
         return SEBottleneckFunction._finish(ctx, engine._se_bottleneck_body(block, Act(x2d, *geom), out))
 
 
+class BNInceptionStemFunction(_FrozenFunction):
+    """The BNInception stem: conv1_7x7_s2 .. pool2_3x3_s2 (bninception.py:255-265)."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, model, out=None):
+        from . import engine
+        return BNInceptionStemFunction._finish(ctx, engine._bninception_stem_body(model, Act(x2d, *geom), out))
+
+
+class InceptionFunction(_FrozenFunction):
+    """One BNInception block (``spec``: a row of models.bninception.BLOCKS): its branches written in place into the
+    concatenated output (bninception.py:266-483)."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, model, spec, out=None):
+        from . import engine
+        return InceptionFunction._finish(ctx, engine._inception_body(model, spec, Act(x2d, *geom), out))
+
+
 class GBlockFunction(_FrozenFunction):
     """BigGAN-deep GBlock: ccbn-ReLU-1x1 -> ccbn-ReLU-[up]-3x3 -> ccbn-ReLU-3x3 -> ccbn-ReLU-1x1 (+ skip)."""
 

@@ -6,8 +6,10 @@ from .resnet2d import pretrained_settings as resnet2d_settings
 from .resnext3d import pretrained_settings as resnext3d_settings      # settings.py:18,36 of the reference
 from .mobilenet import pretrained_settings as mobilenet_settings      # mobilenet.py:7-19 (not in the reference's registry)
 from .senet import pretrained_settings as senet_settings              # senet.py:15-82 (not in the reference's registry)
+from .bninception import pretrained_settings as bninception_settings  # bninception.py:10-25 (settings.py:3 of the reference)
 
-all_settings = [resnet2d_settings, resnet3d_settings, resnext3d_settings, nonlocal_settings, mobilenet_settings, senet_settings]
+all_settings = [resnet2d_settings, resnet3d_settings, resnext3d_settings, nonlocal_settings, mobilenet_settings, senet_settings,
+                bninception_settings]
 
 model_names = []
 pretrained_settings = {}

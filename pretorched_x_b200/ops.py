@@ -520,6 +520,97 @@ def se_excite(h, w1, b1, w2, b2, s3, t3, out=None):
     return aff[0], aff[1]
 
 
+# ---------------------------------------------------------------------------------------------
+# column-slice outputs (BNInception): inception branches written in place into the concatenated block output
+# ---------------------------------------------------------------------------------------------
+def _slice_view(y, what):
+    """(pointer, pitch, columns) of an fp16 2-D view whose columns are contiguous: ``out[:, c0:c0 + cols]`` of a wider matrix."""
+    if y.dtype != torch.float16 or y.dim() != 2 or y.stride(1) != 1 or y.data_ptr() % 16:
+        raise ValueError("%s must be a 16-byte aligned fp16 [rows][cols] view with contiguous columns" % what)
+    return _ptr(y), y.stride(0), y.shape[1]
+
+
+def split_plan(cols):
+    """(packed width, first 64-column box of each destination + the total) of a split GEMM (b2_gemm_split_plan)."""
+    n = len(cols)
+    c = (ctypes.c_int * max(n, 1))(*cols)
+    box0 = (ctypes.c_int * 5)()
+    npad = _lib.load().b2_gemm_split_plan(n, c, box0)
+    if npad < 0:
+        raise ValueError("split GEMM destinations %s: %s" % (list(cols), _lib.last_error()))
+    return npad, list(box0)[:n + 1]
+
+
+@_on_device
+def gemm_split(a2d, b2d, scale, shift, M, Kd, dests, relu=True):
+    """One GEMM A[M][Kd] . B[Npad][Kd]^T with a per-column affine (+ ReLU) whose columns go to up to four column slices
+    (b2_gemm_split_f16): ``dests`` are fp16 [M][cols_d] views (``out[:, c0:c0 + cols]`` of a block output, or a whole matrix);
+    B / scale / shift hold destination d's rows from packed column 64 * box0[d] on (``split_plan``)."""
+    nd = len(dests)
+    views = [_slice_view(y, "split GEMM destination %d" % d) for d, y in enumerate(dests)]
+    if any(y.shape[0] != M for y in dests):
+        raise ValueError("every split GEMM destination needs %d rows" % M)
+    cols = [v[2] for v in views]
+    npad, _ = split_plan(cols)
+    g = GemmArgs()
+    g.a, g.b, g.scale, g.shift = _ptr(a2d), _ptr(b2d), _ptr(scale), _ptr(shift)
+    g.M, g.N, g.Kd = M, npad, Kd
+    g.lda, g.ldb = a2d.stride(0), b2d.stride(0)
+    g.relu = int(relu)
+    ys = (ctypes.c_void_p * nd)(*[v[0] for v in views])
+    lds = (ctypes.c_int * nd)(*[v[1] for v in views])
+    cs = (ctypes.c_int * nd)(*cols)
+    with _timed("gemm_split", "gemm split M=%d N=%d(%s) K=%d" % (M, npad, "+".join(map(str, cols)), Kd), 2.0 * M * npad * Kd,
+                2.0 * (M * Kd + npad * Kd + M * sum(cols))):
+        _lib.check(_lib.load().b2_gemm_split_f16(ctypes.byref(g), nd, ys, lds, cs, _stream()), "b2_gemm_split_f16")
+
+
+@_on_device
+def conv_slice(a, pc, y, relu=True):
+    """``conv`` of a 3x3 filter (stride 1 or 2, padding 1) whose output is the column slice ``y`` (an fp16 [M][K] view of a
+    wider matrix): b2_conv_ndhwc_fprop_slice writes columns [0, K) of each row and nothing else."""
+    if a.ld != pc.C:
+        raise ValueError("activation pitch %d != packed filter pitch %d" % (a.ld, pc.C))
+    kt, kh, kw = pc.k
+    To, Ho, Wo = (_out_dim(a.T, kt, pc.s[0], pc.p[0]), _out_dim(a.H, kh, pc.s[1], pc.p[1]), _out_dim(a.W, kw, pc.s[2], pc.p[2]))
+    M = a.N * To * Ho * Wo
+    yp, ldy, cols = _slice_view(y, "slice convolution output")
+    if y.shape[0] != M or cols != pc.K:
+        raise ValueError("slice %s does not fit the %d x %d output" % (tuple(y.shape), M, pc.K))
+    args = ConvArgs()
+    args.x, args.w, args.scale, args.shift = _ptr(a.data), _ptr(pc.w), _ptr(pc.scale), _ptr(pc.shift)
+    args.y = yp
+    args.N, args.T, args.H, args.W, args.C = a.N, a.T, a.H, a.W, a.ld
+    args.K, args.ldy = pc.K, ldy
+    args.kt, args.kh, args.kw = kt, kh, kw
+    args.st, args.sh, args.sw = pc.s
+    args.pt, args.ph, args.pw = pc.p
+    args.relu, args.mode = int(relu), pc.mode
+    flops = 2.0 * M * pc.K * pc.Cin * kt * kh * kw
+    desc = "conv %dx%dx%d s%s C%d->%d M=%d slice" % (kt, kh, kw, "".join(map(str, pc.s)), pc.Cin, pc.K, M)
+    with _timed("conv_slice", desc, flops, 2.0 * (a.M * a.C + M * pc.K + pc.K * pc.Cin * kt * kh * kw)):
+        _lib.check(_lib.load().b2_conv_ndhwc_fprop_slice(ctypes.byref(args), _stream()), "b2_conv_ndhwc_fprop_slice")
+    return Act(y, a.N, To, Ho, Wo, pc.K)
+
+
+@_on_device
+def pool_slice(a, k, s, p, avg, y=None):
+    """nn.MaxPool2d / nn.AvgPool2d(count_include_pad=True) (k, stride s, padding p, ceil_mode=True) over every frame of ``a`` (its
+    ``data`` may itself be a column slice: rows of pitch ``data.stride(0)``) into the column slice ``y`` (fp16 [M_out][a.C] view; a fresh dense matrix when None) by b2_pool_ndhwc_slice."""
+    Ho, Wo = ceil_pool_dim(a.H, k, s, p), ceil_pool_dim(a.W, k, s, p)
+    My = a.N * a.T * Ho * Wo
+    if y is None:
+        y = torch.empty((My, _round_up(a.C, 8)), dtype=torch.float16, device=a.data.device)
+    yp, ldy, cols = _slice_view(y, "pool output")
+    if y.shape[0] != My or cols < a.C:
+        raise ValueError("pool output %s does not fit %d rows of %d channels" % (tuple(y.shape), My, a.C))
+    with _timed("pool", "%spool %dx%d s%d C%d M=%d->%d" % ("avg" if avg else "max", k, k, s, a.C, a.M, My), 0.0,
+                2.0 * a.C * (a.M + My)):
+        _lib.check(_lib.load().b2_pool_ndhwc_slice(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, k, k, 1, s, s, 0, p, p,
+                                                   a.T, Ho, Wo, int(bool(avg)), _stream()), "b2_pool_ndhwc_slice")
+    return Act(y, a.N, a.T, Ho, Wo, a.C)
+
+
 class PackedLinear:
     """nn.Linear weights as an fp16 [out][in_pitch] matrix + fp32 bias (resnet3D.py:162, trn.py:42-44)."""
     __slots__ = ("w", "scale", "shift", "out_features", "in_features", "in_pitch")
