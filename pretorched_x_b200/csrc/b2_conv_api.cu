@@ -11,6 +11,7 @@
 #include "b2_densem.cuh"
 #include "b2_pgemm.cuh"
 #include "b2_slabconv.cuh"
+#include "b2_slab_t128.cuh"
 #include "b2_tstack.cuh"
 #include "b2_stemconv.cuh"
 
@@ -421,12 +422,166 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   return best_cost;
 }
 
-// returns 1 when the slab kernel took the convolution, 0 when it does not apply, <0 on error
+// The slab kernel's plan of a convolution (a: after the temporal remap).  Returns false when the kernel does not apply or no tiling
+// fits in shared memory.
+struct SlabChoice {
+  SlabParams p;
+  int BN, MT, R;
+  bool flex;
+};
+static bool slab_choose(const b2_conv_args* a, int wc_hint, int G, int ldo, SlabChoice* c) {
+  // W chunking candidates: the default (whole rows, or <= 256-pixel chunks) and narrower chunks.  Narrow chunks make the
+  // slab of a work item shorter, which (a) lets 256-pixel rows fit the two slab stages at all and (b) admits more M tiles
+  // per item for wide images -- with few-tap 2-D filters the per-item costs (decode, epilogue set-up, slab latency) are
+  // what the cycle model trades against the extra halo columns.  The cheapest modelled configuration wins.
+  const int wc_try[3] = {wc_hint, 128, 64};
+  int best_mt = 0;
+  double best_cost = 0.0;
+  for (int attempt = 0; attempt < 3; ++attempt) {
+    if (attempt > 0 && (wc_hint > 0 || wc_try[attempt] >= a->W)) continue;
+    SlabParams q;
+    if (!slab_geometry(a, &q, wc_try[attempt])) { if (attempt == 0) return false; else continue; }
+    if (attempt > 0 && q.wchunks == 1) continue;              // same geometry as the default
+    if (g_conv_algo == 2 && q.ss != 1 && !G) return false;    // debug: strided convs through the gather kernel
+    if (G) q.cchunks = 1;                                     // an item reads its own 64-channel slice only
+    int bn_c = 0, mt_c = 0, r_c = 0;
+    bool flex_c = false;
+    const SlabParams q0 = q;
+    double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G);
+    if (mt_c == 0 && ldo && flex_c) {
+      // a slice has no other kernel to fall back on: when the wide runtime-N tile does not fit, take 128-column tiles
+      q = q0;
+      cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G, false);
+    }
+    if (mt_c == 0) continue;
+    if (best_mt == 0 || cost < best_cost) { c->p = q; c->BN = bn_c; c->flex = flex_c; c->MT = best_mt = mt_c; c->R = r_c; best_cost = cost; }
+  }
+  return best_mt != 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// 128-wide slab tiles as the transposed product (b2_slab_t128.cuh)
+// ------------------------------------------------------------------------------------------
+static int g_slab_t128 = -1;       // -1 the rule (slab_t128_wanted), 0 never, 1 wherever the form applies (tests, A/B sweeps)
+static const int kT128Widths[3] = {216, 224, 256};   // compiled item widths NP
+
+struct T128Plan {
+  SlabParams p;                    // geometry (slab_geometry) + qitem
+  int np, rows, R, items, smem;
+};
+
+static int t128_smem(int slab_bytes, int np, int ldy) {
+  return kSlabSStages * slab_bytes + kSlabWStages * kT128WBytes + np * kT128RowBytes + 256 + 2 * slab_naff(ldy) * 4 + 1024;
+}
+
+// Whether the form takes the convolution at all, and its plan: the fewest row groups per plane whose padded positions fit 256, the
+// narrowest compiled width that holds one, and the slab rows every item's positions and taps reach.
+static bool slab_t128_geometry(const b2_conv_args* a, T128Plan* t) {
+  if (a->upsample || a->aff_ld || a->residual || a->y2 || a->residual_up || a->residual_pre || a->in_scale || a->mask) return false;
+  if (a->kh != 3 || a->kw != 3 || (a->kt != 1 && a->kt != 3)) return false;
+  if (a->C % 64 != 0 || a->K % 128 != 0) return false;
+  SlabParams& p = t->p;
+  if (!slab_geometry(a, &p, 0) || p.wchunks != 1 || p.up) return false;
+  const int max_rows = 256 / p.PW;
+  if (max_rows < 1) return false;
+  const int groups = (p.Ho + max_rows - 1) / max_rows;
+  t->rows = (p.Ho + groups - 1) / groups;
+  p.qitem = t->rows * p.PW;
+  t->np = 0;
+  for (int np : kT128Widths)
+    if (np >= p.qitem) { t->np = np; break; }
+  if (t->np == 0) return false;
+  int R = 0;
+  for (int q0 = 0; q0 < p.P; q0 += p.qitem) {
+    int lo = q0 - p.reach;
+    lo = (lo >= 0) ? lo / p.PW : -((-lo + p.PW - 1) / p.PW);
+    const int hi = (q0 + t->np - 1 + p.reach) / p.PW;
+    R = (hi - lo + 1) > R ? (hi - lo + 1) : R;
+  }
+  if (p.ss * (R - 1) + 1 > 256) return false;
+  t->R = R;
+  p.R = R;
+  p.slab_bytes = (R * p.PW * 128 + 1023) / 1024 * 1024;
+  p.MT = 1;
+  p.tiles_n = (a->ldy + 127) / 128;
+  p.tiles_q = groups;
+  const long long items = (long long)p.tiles_n * groups * a->N * p.To;
+  if (items >= (1ll << 31)) return false;
+  t->items = (int)items;
+  t->smem = t128_smem(p.slab_bytes, t->np, a->ldy);
+  return t->smem <= 227 * 1024;
+}
+
+// Items the slab kernel's plan c runs for the convolution
+static long long slab_items(const b2_conv_args* a, const SlabChoice& c) {
+  const SlabParams& p = c.p;
+  const long long planes = p.mp > 1 ? ((long long)a->N * p.To + p.mp - 1) / p.mp : (long long)a->N * p.To;
+  const long long tq = p.mp > 1 ? 1 : (p.P + c.MT * 128 - 1) / (c.MT * 128);
+  return (long long)((a->ldy + c.BN - 1) / c.BN) * tq * p.wchunks * planes * (p.up ? 4 : 1);
+}
+
+// The rule: an item of the form runs NP / 128 times the MMA columns of a one-tile slab item and there are fewer of them, so it
+// is taken where rounds of items x MMA columns per item -- the critical path of the persistent grid -- is not longer than the slab
+// kernel's plan: ceil(items / SMs) * NP / 128 <= ceil(slab items / SMs) * MT.  At small sizes halving the items idles SMs and the
+// rule declines.  A forced slab plan (set_slab_mt, set_slab_wide) and multi-plane slab items stay on the slab kernel.
+static bool slab_t128_wanted(const b2_conv_args* a, const SlabChoice& c, T128Plan* t) {
+  if (g_slab_t128 == 0 || !slab_t128_geometry(a, t)) return false;
+  if (g_slab_t128 == 1) return true;
+  if (g_slab_force_mt != 0 || g_slab_wide == 1 || c.p.mp > 1) return false;
+  const long long sms = sm_count();
+  const long long cur = slab_items(a, c);
+  return ((t->items + sms - 1) / sms) * t->np <= ((cur + sms - 1) / sms) * c.MT * 128;
+}
+
+template <int NP>
+static int run_slab_t128(int grid, int smem_bytes, const CUtensorMap& tmX, const CUtensorMap& tmB, const SlabParams& p,
+                         cudaStream_t stream) {
+  B2_OPT_IN_SMEM(slab_t128_kernel<NP>, 227 * 1024);
+  B2_CHECK_CUDA(launch_pdl(slab_t128_kernel<NP>, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
+  B2_CHECK_LAUNCH("slab_t128_kernel");
+  return B2_OK;
+}
+
+static int launch_slab_t128(const b2_conv_args* a, T128Plan& t, cudaStream_t stream) {
+  SlabParams& p = t.p;
+  p.bn = 128; p.wbytes = kT128WBytes; p.accs = 128;
+  p.mp = 0;
+  p.planes_total = a->N * p.To;
+  p.plane_stride = p.R * p.PW * 128;
+  p.Ncols = a->K;
+  p.scale = a->scale; p.shift = a->shift;
+  p.residual = nullptr; p.ldr = 0;
+  p.y = reinterpret_cast<__half*>(a->y);
+  p.ldy = a->ldy;
+  p.ldo = 0;
+  p.relu = a->relu;
+  p.aff_ld = 0;
+  p.naff = slab_naff(a->ldy);
+  p.items_total = t.items;
+  p.fd_tiles_n = make_fastdiv(p.tiles_n); p.fd_tiles_q = make_fastdiv(p.tiles_q); p.fd_wchunks = make_fastdiv(p.wchunks);
+  p.fd_To = make_fastdiv(p.To); p.fd_PW = make_fastdiv(p.PW);
+  CUtensorMap tmX, tmB;
+  int rc;
+  const int taps = a->kt * a->kh * a->kw;
+  if ((rc = make_tmap_ndhwc_slab(&tmX, a->x, (uint64_t)a->C, (uint64_t)a->W, (uint64_t)a->H, (uint64_t)a->N * a->T, (uint32_t)p.PW,
+                                 (uint32_t)t.R, (uint32_t)p.ss)) != B2_OK)
+    return rc;
+  if ((rc = make_tmap_2d_f16(&tmB, a->w, (uint64_t)taps * a->C, (uint64_t)a->K, (uint64_t)taps * a->C, 64, 128, true)) != B2_OK)
+    return rc;
+  const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
+  switch (t.np) {
+    case 216: return run_slab_t128<216>(grid, t.smem, tmX, tmB, p, stream);
+    case 224: return run_slab_t128<224>(grid, t.smem, tmX, tmB, p, stream);
+    case 256: return run_slab_t128<256>(grid, t.smem, tmX, tmB, p, stream);
+    default: return set_error(B2_ERR_INVALID, "slab item width %d is not one of the compiled widths", t.np);
+  }
+}
+
+// returns 1 when the slab kernel (or its 128-wide transposed form) took the convolution, 0 when it does not apply, <0 on error
 // G != 0: grouped convolution inside the contract of b2_conv_grouped_ndhwc_fprop (3x3 in plane, so never the temporal remap)
 // ldo > 0: column-slice output, see launch_slab
 static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, int ldo = 0) {
   if (g_conv_algo == 1 && !G && !ldo) return 0;
-  SlabParams p;
   b2_conv_args remap = *a_in;
   const b2_conv_args* a = a_in;
   int wc_hint = 0;
@@ -439,36 +594,19 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, in
     a = &remap;
     wc_hint = 64;
   }
-  // W chunking candidates: the default (whole rows, or <= 256-pixel chunks) and narrower chunks.  Narrow chunks make the
-  // slab of a work item shorter, which (a) lets 256-pixel rows fit the two slab stages at all and (b) admits more M tiles
-  // per item for wide images -- with few-tap 2-D filters the per-item costs (decode, epilogue set-up, slab latency) are
-  // what the cycle model trades against the extra halo columns.  The cheapest modelled configuration wins.
-  const int wc_try[3] = {wc_hint, 128, 64};
-  int BN = 0, best_mt = 0, best_R = 0;
-  bool flex = false;
-  double best_cost = 0.0;
-  SlabParams best_p;
-  for (int attempt = 0; attempt < 3; ++attempt) {
-    if (attempt > 0 && (wc_hint > 0 || wc_try[attempt] >= a->W)) continue;
-    SlabParams q;
-    if (!slab_geometry(a, &q, wc_try[attempt])) { if (attempt == 0) return 0; else continue; }
-    if (attempt > 0 && q.wchunks == 1) continue;              // same geometry as the default
-    if (g_conv_algo == 2 && q.ss != 1 && !G) return 0;        // debug: strided convs through the gather kernel
-    if (G) q.cchunks = 1;                                     // an item reads its own 64-channel slice only
-    int bn_c = 0, mt_c = 0, r_c = 0;
-    bool flex_c = false;
-    const SlabParams q0 = q;
-    double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G);
-    if (mt_c == 0 && ldo && flex_c) {
-      // a slice has no other kernel to fall back on: when the wide runtime-N tile does not fit, take 128-column tiles
-      q = q0;
-      cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G, false);
+  SlabChoice c;
+  if (!slab_choose(a, wc_hint, G, ldo, &c)) return 0;
+  if (!G && !ldo) {
+    T128Plan t;
+    if (slab_t128_wanted(a, c, &t)) {
+      const int rc = launch_slab_t128(a, t, stream);
+      if (rc == B2_OK) set_last_kernel(KID_SLAB_T128, t.np, t.rows, 128, t.p.ss, t.R);
+      return rc == B2_OK ? 1 : rc;
     }
-    if (mt_c == 0) continue;
-    if (best_mt == 0 || cost < best_cost) { best_p = q; BN = bn_c; flex = flex_c; best_mt = mt_c; best_R = r_c; best_cost = cost; }
   }
-  if (best_mt != 0) p = best_p;
-  if (best_mt == 0) return 0;
+  SlabParams& p = c.p;
+  const int BN = c.BN, best_mt = c.MT, best_R = c.R;
+  const bool flex = c.flex;
   int rc = G == 16 ? launch_slab<64, 16>(a, p, best_mt, best_R, stream)
            : G == 32 ? launch_slab<64, 32>(a, p, best_mt, best_R, stream)
            : flex ? launch_slab<0>(a, p, best_mt, best_R, stream, ldo)
@@ -1055,6 +1193,26 @@ int b2_debug_stem_row_plan(int G, int kh, int* out) {
 }
 int b2_debug_last_gemm_path(void) { return g_last_gemm_path; }   /* 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (last GEMM-family launch) */   /* 1: the temporal stack kernel took the last convolution */
 int b2_debug_set_tstack(int mode) { g_tstack = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }   /* temporal stack kernel: -1 rule, 0 never, 1 whenever eligible */
+/* 128-wide slab tiles as the transposed product (b2_slab_t128.cuh): mode -1 = the rule, 0 = never, 1 = wherever the form applies.
+   Host-only view of its decision for a convolution (no launch, no GPU needed) under the current knobs: out = {taken, applies, NP,
+   rows per item, slab rows R, items, dynamic shared memory bytes, slab kernel items, slab kernel MT, SM count the rule used}.
+   b2_debug_last_kernel's info
+   of a launch of the form (KID_SLAB_T128): {NP, rows per item, N tile 128, spatial stride, R}. */
+int b2_debug_set_slab_t128(int mode) { g_slab_t128 = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }
+int b2_debug_slab_t128_plan(const b2_conv_args* a, int* out) {
+  memset(out, 0, 10 * sizeof(int));
+  out[9] = sm_count();
+  T128Plan t;
+  memset(&t, 0, sizeof(t));
+  SlabChoice c;
+  const bool remapped = a->kt > 1 && a->kh == 1 && a->kw == 1;      // the remapped temporal form is never this one's
+  if (remapped || !slab_choose(a, 0, 0, 0, &c)) return B2_OK;
+  out[0] = slab_t128_wanted(a, c, &t);
+  out[1] = slab_t128_geometry(a, &t);
+  out[2] = t.np; out[3] = t.rows; out[4] = t.R; out[5] = t.items; out[6] = t.smem;
+  out[7] = (int)slab_items(a, c); out[8] = c.MT;
+  return B2_OK;
+}
 int b2_debug_set_slab_mt(int mt) { g_slab_force_mt = mt < 0 ? 0 : mt; return B2_OK; }
 int b2_debug_set_densem(int maxm, int force_s) { g_densem_maxm = maxm < 0 ? -2 : maxm; g_densem_force_s = force_s; return B2_OK; }
 /* The temporal-group slab kernel this selected is gone (the slab kernel's 64-wide tile does what it was for); the entry point

@@ -96,6 +96,7 @@ struct SlabParams {
   int mp, plane_stride, planes_total;
   FastDiv fd_tiles_n, fd_tiles_q, fd_wchunks, fd_To, fd_PW;   // dividers of the item decode (set by launch_slab)
   int ldo;                 // slabconv_kernel<BN, TMT, kSlabSlice> only: row pitch of y (>= ldy, the columns written)
+  int qitem;               // slab_t128_kernel only: padded positions of the whole output rows of one work item
 };
 
 // scale/shift live in smem for all (padded) output channels: SlabParams::naff = round_up(ldy, 32) + 32 entries each; the
@@ -277,6 +278,67 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
   }
 }
 
+// TMA producer of the slab kernels (one warp); item_at(item) decodes a work item (slab_item, or slab_t128_item of b2_slab_t128.cuh).
+// Walks (item, slab) pairs; the slab after the current one -- possibly the first slab of the NEXT item -- is
+// requested after weight tap min(kSlabWStages, ntaps - 1) of the current slab: from tap kSlabWStages on, the weight ring
+// guarantees the consumers have retired the slab that occupied the target slot, so that wait never stalls weight issue;
+// a slab with fewer taps issues all of its weights first (the previous slab is released only once this one's first tap runs).
+template <int G, class ItemAt>
+__device__ __forceinline__ void slab_producer(const SlabParams& p, const CUtensorMap* tmX, const CUtensorMap* tmB, uint8_t* slab_base,
+                                              uint8_t* w_base, int kWBytes, int bn, uint64_t* slab_full, uint64_t* slab_empty,
+                                              uint64_t* w_full, uint64_t* w_empty, ItemAt item_at) {
+  int wit = 0, sg = 0;                     // global weight-tile / slab counters (ring phases persist across items)
+  int item = blockIdx.x;
+  if (item < p.items_total) {
+    SlabItem cur = item_at(item);
+    int nxt_item = item, nxt_si = 0;       // (item, slab) of the next slab to load
+    SlabItem nxt = cur;
+    // slab index si of an item enumerates (cc, dt, sub) with sub fastest
+    auto load_next = [&]() {
+      const int sub = nxt_si % p.n_sub;
+      const int r2 = nxt_si / p.n_sub;
+      const int cc = r2 / nxt.n_dt, dt = nxt.dt_lo + (r2 - cc * nxt.n_dt);
+      const int s = sg % kSlabSStages;
+      mbar_wait(&slab_empty[s], ((sg / kSlabSStages) & 1) ^ 1);
+      if (elect_one()) {
+        mbar_expect_tx(&slab_full[s], static_cast<uint32_t>(p.R * p.PW * 128 * (p.mp > 1 ? p.mp : 1)));
+        tma_load_4d(slab_base + s * p.slab_bytes, tmX, &slab_full[s], G ? nxt.n0 : cc * 64,
+                    p.sub_w0[sub] + p.ss * nxt.wc * p.WC, p.ss * nxt.r_lo + p.sub_h0[sub], nxt.plane_i0 + dt);
+      }
+      __syncwarp();
+      ++sg;
+      if (++nxt_si == nxt.n_slabs) {       // advance to the first slab of the following item
+        nxt_si = 0;
+        nxt_item += gridDim.x;
+        if (nxt_item < p.items_total) nxt = item_at(nxt_item);
+      }
+    };
+    load_next();
+    for (; item < p.items_total; item += gridDim.x) {
+      cur = item_at(item);
+      for (int si = 0; si < cur.n_slabs; ++si) {
+        const int sub = p.up ? cur.phase : si % p.n_sub;          // tap-table row (== slab index unless p.up)
+        const int r2 = si / p.n_sub;
+        const int cc = r2 / cur.n_dt, dt = cur.dt_lo + (r2 - cc * cur.n_dt);
+        const int ntaps = p.sub_ntaps[sub];
+        const int pf = min(kSlabWStages, ntaps - 1);
+        for (int ti = 0; ti < ntaps; ++ti, ++wit) {
+          const int ws = wit % kSlabWStages;
+          mbar_wait(&w_empty[ws], ((wit / kSlabWStages) & 1) ^ 1);
+          const int tap = dt * p.khw + p.sub_tap[sub][ti];
+          if (elect_one()) {
+            mbar_expect_tx(&w_full[ws], static_cast<uint32_t>(G ? G * 128 : bn * 128));
+            if constexpr (G != 0) tma_load_2d(w_base + ws * kWBytes, tmB, &w_full[ws], 0, ((cur.n0 >> 6) * p.kt * p.khw + tap) * G);
+            else tma_load_2d(w_base + ws * kWBytes, tmB, &w_full[ws], tap * p.C + cc * 64, cur.n0);
+          }
+          __syncwarp();
+          if (ti == pf && nxt_item < p.items_total) load_next();
+        }
+      }
+    }
+  }
+}
+
 // BN = 0: N tile taken from SlabParams::bn at run time.  TMT: the 64-wide tile's MMA form (slab_consumer; 0 for the other tiles).
 // G = 16 / 32 (BN = 64): grouped convolution with C == K (b2_groupconv.cuh).  N tile tn is the 64-channel slice tn of input AND
 // output, the item has one channel chunk (SlabParams::cchunks = 1) whose TMA channel coordinate is the slice's, and a weight stage
@@ -330,60 +392,8 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
 
   if (warp == kSlabTmaWarp) {
     // ================================ TMA producer ======================================
-    // Walks (item, slab) pairs; the slab after the current one -- possibly the first slab of the NEXT item -- is
-    // requested after weight tap min(kSlabWStages, ntaps - 1) of the current slab: from tap kSlabWStages on, the weight ring
-    // guarantees the consumers have retired the slab that occupied the target slot, so that wait never stalls weight issue;
-    // a slab with fewer taps issues all of its weights first (the previous slab is released only once this one's first tap runs).
-    int wit = 0, sg = 0;                     // global weight-tile / slab counters (ring phases persist across items)
-    int item = blockIdx.x;
-    if (item < p.items_total) {
-      SlabItem cur = slab_item(p, item, bn);
-      int nxt_item = item, nxt_si = 0;       // (item, slab) of the next slab to load
-      SlabItem nxt = cur;
-      // slab index si of an item enumerates (cc, dt, sub) with sub fastest
-      auto load_next = [&]() {
-        const int sub = nxt_si % p.n_sub;
-        const int r2 = nxt_si / p.n_sub;
-        const int cc = r2 / nxt.n_dt, dt = nxt.dt_lo + (r2 - cc * nxt.n_dt);
-        const int s = sg % kSlabSStages;
-        mbar_wait(&slab_empty[s], ((sg / kSlabSStages) & 1) ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(&slab_full[s], static_cast<uint32_t>(p.R * p.PW * 128 * (p.mp > 1 ? p.mp : 1)));
-          tma_load_4d(slab_base + s * p.slab_bytes, &tmX, &slab_full[s], G ? nxt.n0 : cc * 64,
-                      p.sub_w0[sub] + p.ss * nxt.wc * p.WC, p.ss * nxt.r_lo + p.sub_h0[sub], nxt.plane_i0 + dt);
-        }
-        __syncwarp();
-        ++sg;
-        if (++nxt_si == nxt.n_slabs) {       // advance to the first slab of the following item
-          nxt_si = 0;
-          nxt_item += gridDim.x;
-          if (nxt_item < p.items_total) nxt = slab_item(p, nxt_item, bn);
-        }
-      };
-      load_next();
-      for (; item < p.items_total; item += gridDim.x) {
-        cur = slab_item(p, item, bn);
-        for (int si = 0; si < cur.n_slabs; ++si) {
-          const int sub = p.up ? cur.phase : si % p.n_sub;          // tap-table row (== slab index unless p.up)
-          const int r2 = si / p.n_sub;
-          const int cc = r2 / cur.n_dt, dt = cur.dt_lo + (r2 - cc * cur.n_dt);
-          const int ntaps = p.sub_ntaps[sub];
-          const int pf = min(kSlabWStages, ntaps - 1);
-          for (int ti = 0; ti < ntaps; ++ti, ++wit) {
-            const int ws = wit % kSlabWStages;
-            mbar_wait(&w_empty[ws], ((wit / kSlabWStages) & 1) ^ 1);
-            const int tap = dt * p.khw + p.sub_tap[sub][ti];
-            if (elect_one()) {
-              mbar_expect_tx(&w_full[ws], static_cast<uint32_t>(G ? G * 128 : bn * 128));
-              if constexpr (G != 0) tma_load_2d(w_base + ws * kWBytes, &tmB, &w_full[ws], 0, ((cur.n0 >> 6) * p.kt * p.khw + tap) * G);
-              else tma_load_2d(w_base + ws * kWBytes, &tmB, &w_full[ws], tap * p.C + cc * 64, cur.n0);
-            }
-            __syncwarp();
-            if (ti == pf && nxt_item < p.items_total) load_next();
-          }
-        }
-      }
-    }
+    slab_producer<G>(p, &tmX, &tmB, slab_base, w_base, kWBytes, bn, slab_full, slab_empty, w_full, w_empty,
+                     [&](int it) { return slab_item(p, it, bn); });
   } else if (warp < kSlabEpiWarp0) {
     // ================================ consumer warpgroups ===============================
     const uint32_t slab0 = smem_u32(slab_base), w0s = smem_u32(w_base);

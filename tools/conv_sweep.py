@@ -19,6 +19,8 @@ lib.b2_debug_set_slab_wide.restype = ctypes.c_int
 lib.b2_debug_set_slab_wide.argtypes = [ctypes.c_int]          # 4th field of a setting: 256-column N tiles 1 = always, 0 = never, -1 / absent = the library's rule
 lib.b2_debug_set_tstack.restype = ctypes.c_int
 lib.b2_debug_set_tstack.argtypes = [ctypes.c_int]             # 5th field: temporal stack kernel 1 = whenever eligible, 0 = never, -1 / absent = the library's rule
+lib.b2_debug_set_slab_t128.restype = ctypes.c_int
+lib.b2_debug_set_slab_t128.argtypes = [ctypes.c_int]          # 6th field: 128-wide transposed slab form 1 = wherever it applies, 0 = never, -1 / absent = the rule
 dev = torch.device("cuda:0")
 REP = 20
 for sp in specs:
@@ -47,6 +49,7 @@ for sp in specs:
             lib.b2_debug_set_slab_mt(mt)
             lib.b2_debug_set_slab_wide(st[3] if len(st) > 3 else -1)
             lib.b2_debug_set_tstack(st[4] if len(st) > 4 else -1)
+            lib.b2_debug_set_slab_t128(st[5] if len(st) > 5 else -1)
             for _ in range(2):
                 y = engine.conv_bn_act(conv, bn, x, residual=res, relu=True)
             torch.cuda.synchronize()
@@ -62,6 +65,9 @@ for sp in specs:
                 g.replay()
             e1.record(); torch.cuda.synchronize()
             us = e0.elapsed_time(e1) / (3 * REP) * 1e3
-            out.append("[%s] %7.1f us %6.0f TF/s %s" % (":".join(map(str, st)), us, fl / us / 1e6, "" if err < 2e-3 else "ERR %.1e" % err))
+            info = (ctypes.c_int * 5)()
+            kid = lib.b2_debug_last_kernel(info)
+            out.append("[%s] %7.1f us %6.0f TF/s k%d%s %s" % (":".join(map(str, st)), us, fl / us / 1e6, kid, tuple(info),
+                                                          "" if err < 2e-3 else "ERR %.1e" % err))
             del g
         print("  ".join(out), flush=True)

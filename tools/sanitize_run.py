@@ -44,6 +44,14 @@ case("resnext3d50", lambda: P.resnext3d50(num_classes=400), (1, 3, 8, 64, 64))
 case("preact_resnet3d50", lambda: P.preact_resnet3d50(num_classes=400), (2, 3, 8, 64, 64))
 
 
+if not only or "resnet3d50_t128" in only:
+    # the slab kernel's 128-wide transposed form, forced (the rule takes it only at large batches), at stride 1 and 2
+    lib = _lib.load()
+    lib.b2_debug_set_densem(0, 0)
+    lib.b2_debug_set_slab_t128(1)
+    case("resnet3d50_t128", lambda: P.resnet3d50(num_classes=400, pretrained=None), (2, 3, 8, 64, 64))
+    lib.b2_debug_set_slab_t128(-1)
+    lib.b2_debug_set_densem(-1, 0)
 case("nonlocalresnet3d50", lambda: P.nonlocalresnet3d50(pretrained=None), (1, 3, 16, 96, 96))
 case("mobilenetv2", lambda: P.mobilenetv2(num_classes=1000, pretrained=None), (2, 3, 96, 64))
 case("se_resnet50", lambda: P.se_resnet50(pretrained=None), (2, 3, 224, 224))
