@@ -71,7 +71,8 @@ typedef struct b2_conv_args {
   int32_t aff_ld;       /* 0: scale/shift are [K].  > 0: per-SAMPLE affine, scale/shift are fp32 [N][aff_ld], 16-byte aligned,
                            aff_ld % 4 == 0
                            (class-conditional BatchNorm of the layer that FOLLOWS this convolution, BigGAN GBlock);
-                           multi-tap "same" convolutions and 1x1x1 convolutions with To*Ho*Wo % 128 == 0 only      */
+                           multi-tap convolutions with in-plane padding between 0 and "same" (temporal "same") and
+                           1x1x1 convolutions with To*Ho*Wo % 128 == 0 only                                        */
   int32_t upsample;     /* 1: y = conv3x3(nearest_upsample_2x(x)) without materialising the upsampled image (GBlock conv2):
                            x is the LOW-resolution input [N,1,H,W,C], y has (2H) x (2W) pixels per image, and w is the
                            phase-folded filter bank [K][16][C] written by b2_pack_upconv3x3_weight.  kt=1, kh=kw=3,
@@ -403,7 +404,8 @@ int b2_gemm_split_plan(int nd, const int* cols, int* box0);
  * 128): with the same N tile each destination equals the stand-alone b2_gemm_f16 of its rows of B bit for bit. */
 int b2_gemm_split_f16(const b2_gemm_args* g, int nd, void* const* y, const int* ldy, const int* cols, void* stream);
 /* b2_conv_ndhwc_fprop with y a column slice (y, ldy, K) as above: columns [0, K) of each output row are written, K % 8 == 0, the rest
- * of the row is untouched.  3x3 2-D convolutions (kt = 1, padding (0, 1, 1)) of stride 1 or 2 on the slab kernel only
+ * of the row is untouched.  2-D convolutions (kt = 1) with an odd kh x kw filter other than 1x1 (3x3, 1x3, 3x1, 1x7, 7x1, 5x5 ...),
+ * in-plane padding from 0 ("valid") to (k - 1) / 2 ("same") per axis, stride 1 or 2, on the slab kernel only
  * (b2_debug_last_kernel: KID 13).  Stem mode, mask, per-sample affine, upsampling, second output, pool_w, the generator fields and fp32
  * output are refused (B2_ERR_INVALID); B2_ERR_UNSUPPORTED when no slab tiling of the image fits. */
 int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream);
@@ -415,6 +417,12 @@ int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream);
  * the window (B2_ERR_INVALID).  b2_debug_last_kernel: KID 14, info = {avg}. */
 int b2_pool_ndhwc_slice(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh,
                         int sw, int pt, int ph, int pw, int To, int Ho, int Wo, int avg, void* stream);
+/* b2_pool_ndhwc_slice's average with count_include_pad=False (nn.AvgPool2d(3, 1, 1, count_include_pad=False), the pool branches of
+ * inceptionv4.py:124, :180, :238 and inceptionresnetv2.py:73): fp32 sum over the in-input taps in (dt, dh, dw) order, divided by
+ * their number, one fp16 rounding.  Same argument contract as b2_pool_ndhwc_slice (every window overlaps the input).
+ * b2_debug_last_kernel: KID 14, info = {2}. */
+int b2_avgpool_ndhwc_slice_exclude_pad(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw,
+                                       int st, int sh, int sw, int pt, int ph, int pw, int To, int Ho, int Wo, void* stream);
 
 #ifdef __cplusplus
 }

@@ -113,6 +113,7 @@ SYMBOLS = {
                                   ctypes.POINTER(c_int), c_void_p]),
     "b2_conv_ndhwc_fprop_slice": (c_int, [ctypes.POINTER(ConvArgs), c_void_p]),
     "b2_pool_ndhwc_slice": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 19 + [c_void_p]),
+    "b2_avgpool_ndhwc_slice_exclude_pad": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 18 + [c_void_p]),
 }
 
 

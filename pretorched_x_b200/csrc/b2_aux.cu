@@ -127,6 +127,8 @@ __global__ void conv_simt_kernel(SimtConvParams p, long long total) {
 // branch of an inception block lands in place in the block's concatenated output.  The average is nn.AvgPool2d with
 // count_include_pad=True: an fp32 sum over the taps in (dt, dh, dw) order (taps in the padding read zero), divided by the
 // window clipped to the padded input (the full window except where a ceil-mode window runs past the padding), one fp16 rounding.
+// MODE 3: the same sum divided by the taps inside the input (count_include_pad=False, the pool branches of Inception-v4 /
+// Inception-ResNet-v2).
 template <int MODE>
 __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restrict__ y, int N, int T, int H, int W,
                                  int C8, int To, int Ho, int Wo, int kt, int kh, int kw, int st, int sh, int sw, int pt,
@@ -139,7 +141,7 @@ __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restric
   const int ho = (int)(q % Ho); q /= Ho;
   const int to = (int)(q % To);
   const int n = (int)(q / To);
-  if constexpr (MODE == 2) {
+  if constexpr (MODE >= 2) {
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     for (int dt = 0; dt < kt; ++dt) {
       const int ti = to * st - pt + dt;
@@ -162,7 +164,8 @@ __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restric
       }
     }
     const int t0 = to * st - pt, h0 = ho * sh - ph, w0 = wo * sw - pw;
-    const int div = (min(t0 + kt, T + pt) - t0) * (min(h0 + kh, H + ph) - h0) * (min(w0 + kw, W + pw) - w0);
+    const int div = MODE == 2 ? (min(t0 + kt, T + pt) - t0) * (min(h0 + kh, H + ph) - h0) * (min(w0 + kw, W + pw) - w0)
+                              : (min(t0 + kt, T) - max(t0, 0)) * (min(h0 + kh, H) - max(h0, 0)) * (min(w0 + kw, W) - max(w0, 0));
     uint4 o;
     uint32_t* op = reinterpret_cast<uint32_t*>(&o);
 #pragma unroll
@@ -655,31 +658,54 @@ int b2_maxpool3d_ndhwc_out(const void* x, void* y, int N, int T, int H, int W, i
   return B2_OK;
 }
 
-int b2_pool_ndhwc_slice(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh,
-                        int sw, int pt, int ph, int pw, int To, int Ho, int Wo, int avg, void* stream) {
-  set_last_kernel(KID_NONE);
+}  // extern "C"
+
+// The argument contract shared by the slice pools (b2_pool_ndhwc_slice, b2_avgpool_ndhwc_slice_exclude_pad): mode 1 max, 2 average
+// counting the padding, 3 average over the in-input taps.  Every window overlaps the input, so mode 3 never divides by zero.
+static int pool_slice(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh,
+                      int sw, int pt, int ph, int pw, int To, int Ho, int Wo, int mode, void* stream) {
   B2_CHECK_ARG(x && y && N > 0 && T > 0 && H > 0 && W > 0 && C > 0, "bad argument");
   B2_CHECK_ARG(C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0 && ldx >= C && ldy >= C,
                "channels %d, input pitch %d and output pitch %d must be multiples of 8 with both pitches >= the channels", C, ldx, ldy);
   B2_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "input / output slice not 16-byte aligned");
   B2_CHECK_ARG(kt > 0 && kh > 0 && kw > 0 && st > 0 && sh > 0 && sw > 0 && pt >= 0 && ph >= 0 && pw >= 0, "bad window");
   B2_CHECK_ARG(2 * pt <= kt && 2 * ph <= kh && 2 * pw <= kw, "padding exceeds half the window");
-  B2_CHECK_ARG(avg == 0 || avg == 1, "avg must be 0 (max) or 1 (average)");
   B2_CHECK_ARG(To > 0 && Ho > 0 && Wo > 0, "empty output");
   // every window must start inside the input or its left padding (torch's ceil-mode rule), so it overlaps the input
   B2_CHECK_ARG((To - 1) * st - pt < T && (Ho - 1) * sh - ph < H && (Wo - 1) * sw - pw < W,
                "output extent %dx%dx%d has a window outside the %dx%dx%d input", To, Ho, Wo, T, H, W);
   const long long total = (long long)N * To * Ho * Wo * (C / 8);
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (avg)
+  if (mode == 3)
+    maxpool3d_kernel<3><<<div_up(total, 256), 256, 0, s>>>((const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh,
+                                                             sw, pt, ph, pw, total, ldx, ldy);
+  else if (mode == 2)
     maxpool3d_kernel<2><<<div_up(total, 256), 256, 0, s>>>((const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh,
                                                              sw, pt, ph, pw, total, ldx, ldy);
   else
     maxpool3d_kernel<1><<<div_up(total, 256), 256, 0, s>>>((const __half*)x, (__half*)y, N, T, H, W, C / 8, To, Ho, Wo, kt, kh, kw, st, sh,
                                                              sw, pt, ph, pw, total, ldx, ldy);
   B2_CHECK_LAUNCH("maxpool3d");
-  set_last_kernel(KID_POOL, avg);
   return B2_OK;
+}
+
+extern "C" {
+
+int b2_pool_ndhwc_slice(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw, int st, int sh,
+                        int sw, int pt, int ph, int pw, int To, int Ho, int Wo, int avg, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(avg == 0 || avg == 1, "avg must be 0 (max) or 1 (average)");
+  const int rc = pool_slice(x, ldx, y, ldy, N, T, H, W, C, kt, kh, kw, st, sh, sw, pt, ph, pw, To, Ho, Wo, avg ? 2 : 1, stream);
+  if (rc == B2_OK) set_last_kernel(KID_POOL, avg);
+  return rc;
+}
+
+int b2_avgpool_ndhwc_slice_exclude_pad(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw,
+                                       int st, int sh, int sw, int pt, int ph, int pw, int To, int Ho, int Wo, void* stream) {
+  set_last_kernel(KID_NONE);
+  const int rc = pool_slice(x, ldx, y, ldy, N, T, H, W, C, kt, kh, kw, st, sh, sw, pt, ph, pw, To, Ho, Wo, 3, stream);
+  if (rc == B2_OK) set_last_kernel(KID_POOL, 2);
+  return rc;
 }
 
 int b2_avgpool_global_ndhwc(const void* x, void* y, int N, int S, int C, void* stream) {

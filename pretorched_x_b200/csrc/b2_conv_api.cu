@@ -156,7 +156,7 @@ int make_tmap_ndhwc_5d(CUtensorMap* out, const void* base, uint64_t C, uint64_t 
 }
 
 // ------------------------------------------------------------------------------------------
-// slab convolution launcher (stride 1, "same" padding)
+// slab convolution launcher (stride 1 or 2, in-plane padding from 0 to "same")
 // ------------------------------------------------------------------------------------------
 static int g_conv_algo = 0;   // 0 auto, 1 force gather (debug / A-B comparisons)
 static int g_slab_wide = -1;       // 1: request 256-column N tiles for channel counts that are multiples of 256 (tuning; they only run
@@ -182,7 +182,8 @@ static int slab_rows(int MT, int PW, int reach, int P) {
 static bool slab_geometry(const b2_conv_args* a, SlabParams* p, int wc_hint) {
   if (a->mode != B2_CONV_AUTO || a->out_f32) return false;
   if ((a->kt & 1) == 0 || (a->kh & 1) == 0 || (a->kw & 1) == 0) return false;
-  if (a->pt != (a->kt - 1) / 2 || a->ph != (a->kh - 1) / 2 || a->pw != (a->kw - 1) / 2) return false;
+  // temporal padding "same"; in-plane padding anywhere from "valid" (0) to "same" ((k - 1) / 2)
+  if (a->pt != (a->kt - 1) / 2 || a->ph < 0 || a->ph > (a->kh - 1) / 2 || a->pw < 0 || a->pw > (a->kw - 1) / 2) return false;
   if (a->sh != a->sw || (a->sh != 1 && a->sh != 2) || (a->st != 1 && a->st != 2)) return false;
   if (a->kh * a->kw > kSlabMaxTaps) return false;
   const int ss = a->sh;
@@ -196,8 +197,16 @@ static bool slab_geometry(const b2_conv_args* a, SlabParams* p, int wc_hint) {
   p->cchunks = (a->C + 63) / 64;
   // tap (dh, dw) reads input (ss*ho + dh - ph, ss*wo + dw - pw) = phase (rh, rw), sub-image pixel (ho + oi, wo + oj)
   int oi[8], rh[8], oj[8], rw[8];
-  int min_oj = 0, max_oj = 0;
-  for (int d = 0; d < a->kh; ++d) { int v = d - a->ph; rh[d] = ((v % ss) + ss) % ss; oi[d] = (v - rh[d]) / ss; }
+  int min_oj = 0, max_oj = 0, min_oi = 0, max_oi = 0;
+  for (int d = 0; d < a->kh; ++d) {
+    int v = d - a->ph; rh[d] = ((v % ss) + ss) % ss; oi[d] = (v - rh[d]) / ss;
+    if (oi[d] < min_oi) min_oi = oi[d];
+    if (oi[d] > max_oi) max_oi = oi[d];
+  }
+  // Row offsets are taken relative to the middle row of the taps, so that the slab rows an item loads (reach above and below its
+  // positions) are not doubled by a one-sided window: below-"same" padding (valid 3x3: rows +0..+2) becomes -1..+1 with the
+  // slab starting one sub-image row lower.  Every "same" window is already centred (|min + max| <= 1 truncates to 0).
+  const int row_c = (min_oi + max_oi) / 2;
   for (int d = 0; d < a->kw; ++d) {
     int v = d - a->pw; rw[d] = ((v % ss) + ss) % ss; oj[d] = (v - rw[d]) / ss;
     if (oj[d] < min_oj) min_oj = oj[d];
@@ -226,7 +235,7 @@ static bool slab_geometry(const b2_conv_args* a, SlabParams* p, int wc_hint) {
       for (int dh = 0; dh < a->kh; ++dh)
         for (int dw = 0; dw < a->kw; ++dw)
           if (rh[dh] == ph_ && rw[dw] == pw_) {
-            const int off = oi[dh] * p->PW + oj[dw];
+            const int off = (oi[dh] - row_c) * p->PW + oj[dw];
             p->sub_off[sidx][n] = (short)off;
             p->sub_tap[sidx][n] = (unsigned char)(dh * a->kw + dw);
             if (off > p->reach) p->reach = off;
@@ -235,7 +244,7 @@ static bool slab_geometry(const b2_conv_args* a, SlabParams* p, int wc_hint) {
           }
       if (n == 0) continue;
       p->sub_ntaps[sidx] = n;
-      p->sub_h0[sidx] = ph_;                               // + ss * r_lo at run time
+      p->sub_h0[sidx] = ph_ + ss * row_c;                  // + ss * r_lo at run time
       p->sub_w0[sidx] = pw_ - ss * p->halo_l;              // slab column 0 = sub-image column -halo_l
       ++p->n_sub;
     }
@@ -1128,8 +1137,9 @@ int b2_version(void) { return 103; }   // 103: split-K / fused (2+1)D / pooled-s
 int b2_debug_set_conv_algo(int algo) { g_conv_algo = algo; return B2_OK; }
 int b2_debug_set_gemm_algo(int algo) { g_gemm_algo = algo; return B2_OK; }
 /* host-only view of the slab kernel's tiling decision for a convolution (no launch, no GPU needed): out = {applies, BN, MT, R, PW,
-   WC, wchunks, items, flex, remapped}.  Used by tests/test_host_logic.py and by tuning scripts. */
-int b2_debug_slab_plan(const b2_conv_args* a_in, int* out) {
+   WC, wchunks, items, flex, remapped}.  Used by tests/test_host_logic.py and by tuning scripts.  slice != 0: the plan of
+   b2_conv_ndhwc_fprop_slice (a->ldy the slice width), which takes 128-column tiles where the runtime-N tile finds no fit. */
+static int slab_plan_view(const b2_conv_args* a_in, int* out, bool slice) {
   b2_conv_args remap = *a_in;
   const b2_conv_args* a = a_in;
   int wc_hint = 0, remapped = 0;
@@ -1137,25 +1147,18 @@ int b2_debug_slab_plan(const b2_conv_args* a_in, int* out) {
     remap.T = 1; remap.H = a_in->T; remap.W = a_in->H * a_in->W; remap.kt = 1; remap.kh = a_in->kt; remap.kw = 1;
     remap.pt = 0; remap.ph = a_in->pt; remap.pw = 0; a = &remap; wc_hint = 64; remapped = 1;
   }
-  const int wc_try[3] = {wc_hint, 128, 64};
-  int BN = 0, best_mt = 0, best_R = 0; bool flex = false; double best_cost = 0.0; SlabParams best_p;
-  memset(&best_p, 0, sizeof(best_p));
-  for (int attempt = 0; attempt < 3; ++attempt) {
-    if (attempt > 0 && (wc_hint > 0 || wc_try[attempt] >= a->W)) continue;
-    SlabParams q;
-    if (!slab_geometry(a, &q, wc_try[attempt])) { if (attempt == 0) break; else continue; }
-    if (attempt > 0 && q.wchunks == 1) continue;
-    int bn_c = 0, mt_c = 0, r_c = 0; bool flex_c = false;
-    const double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c);
-    if (mt_c == 0) continue;
-    if (best_mt == 0 || cost < best_cost) { best_p = q; BN = bn_c; flex = flex_c; best_mt = mt_c; best_R = r_c; best_cost = cost; }
-  }
-  out[0] = best_mt != 0; out[1] = BN; out[2] = best_mt; out[3] = best_R; out[4] = best_p.PW; out[5] = best_p.WC; out[6] = best_p.wchunks;
-  const long long tq = best_mt ? (best_p.P + best_mt * 128 - 1) / (best_mt * 128) : 0;
-  out[7] = (int)(((a->ldy + BN - 1) / (BN ? BN : 1)) * tq * best_p.wchunks * a->N * best_p.To);
-  out[8] = flex; out[9] = remapped;
+  SlabChoice c;
+  memset(&c, 0, sizeof(c));
+  const bool ok = slab_choose(a, wc_hint, 0, slice ? 1 : 0, &c);   // the launchers' own planner (ldo only selects the slice rules)
+  const int BN = ok ? c.BN : 0, best_mt = ok ? c.MT : 0;
+  out[0] = ok; out[1] = BN; out[2] = best_mt; out[3] = ok ? c.R : 0; out[4] = c.p.PW; out[5] = c.p.WC; out[6] = c.p.wchunks;
+  const long long tq = best_mt ? (c.p.P + best_mt * 128 - 1) / (best_mt * 128) : 0;
+  out[7] = (int)(((a->ldy + BN - 1) / (BN ? BN : 1)) * tq * c.p.wchunks * a->N * c.p.To);
+  out[8] = ok && c.flex; out[9] = remapped;
   return B2_OK;
 }
+int b2_debug_slab_plan(const b2_conv_args* a_in, int* out) { return slab_plan_view(a_in, out, false); }
+int b2_debug_slab_slice_plan(const b2_conv_args* a_in, int* out) { return slab_plan_view(a_in, out, true); }
 /* debug knobs of the small-M path: layers with M <= maxm take the dense-M kernel (0 = never); force_s > 0 caps the cluster size */
 int b2_debug_set_slab_wide(int on) { g_slab_wide = on; return B2_OK; }   /* 1: request 256-column tiles; -1 / 0: the rule */
 /* host-only view of the temporal stack kernel's decision for a convolution (no launch, no GPU needed): out = {applies, items, frame
@@ -1557,10 +1560,11 @@ int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream) {
                    !a->out_f32 && !a->accumulate,
                "the slice convolution takes a plain fp16 call: stem mode, mask, per-sample affine, upsampling, second output, pool_w, "
                "generator fields and fp32 output must be zero");
-  B2_CHECK_ARG(a->kt == 1 && a->kh == 3 && a->kw == 3 && a->pt == 0 && a->ph == 1 && a->pw == 1 && a->st == 1 && a->sh == a->sw &&
-                   (a->sh == 1 || a->sh == 2),
-               "the slice convolution is a 3x3 2-D convolution with padding 1 and stride 1 or 2 (got %dx%dx%d, stride %d%d%d, padding %d%d%d)",
-               a->kt, a->kh, a->kw, a->st, a->sh, a->sw, a->pt, a->ph, a->pw);
+  B2_CHECK_ARG(a->kt == 1 && a->pt == 0 && a->st == 1 && (a->kh & 1) && (a->kw & 1) && a->kh * a->kw > 1 && a->kh * a->kw <= kSlabMaxTaps &&
+                   a->ph >= 0 && 2 * a->ph <= a->kh - 1 && a->pw >= 0 && 2 * a->pw <= a->kw - 1 && a->sh == a->sw && (a->sh == 1 || a->sh == 2),
+               "the slice convolution is a 2-D convolution with an odd kh x kw filter other than 1x1 (at most %d taps), padding from 0 to "
+               "(k - 1) / 2 per axis and stride 1 or 2 (got %dx%dx%d, stride %d%d%d, padding %d%d%d)",
+               kSlabMaxTaps, a->kt, a->kh, a->kw, a->st, a->sh, a->sw, a->pt, a->ph, a->pw);
   B2_CHECK_ARG(a->K % 8 == 0, "slice width K %d is not a multiple of 8", a->K);
   B2_CHECK_ARG((reinterpret_cast<uintptr_t>(a->y) & 15) == 0, "slice start is not 16-byte aligned");
   if ((rc = require_sm90()) != B2_OK) return rc;

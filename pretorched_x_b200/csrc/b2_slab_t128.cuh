@@ -18,8 +18,10 @@
 // staging tile; the three epilogue warps copy its valid rows to y.  Every output element keeps the slab kernel's accumulation order
 // (temporal tap, channel chunk, phase, in-plane tap, K step), so the outputs are bitwise those of the slab kernel.
 //
-// Scope (slab_t128_geometry in b2_conv_api.cu): "same" 3x3 or 3x3x3 filters, spatial stride 1 or 2 (the phase sub-images of the
-// slab producer, unchanged), C % 64 == 0, K % 128 == 0, rows that fit one TMA box; no residual, per-sample affine or upsampling.
+// Scope (slab_t128_geometry in b2_conv_api.cu): 3x3 or 3x3x3 filters with in-plane padding 0 ("valid") or 1 ("same") and temporal
+// padding "same" -- slab_geometry's tap table, whose row offsets are centred on the window -- spatial stride 1 or 2 (the phase
+// sub-images of the slab producer, unchanged), C % 64 == 0, K % 128 == 0, rows that fit one TMA box; no residual, per-sample affine
+// or upsampling.
 #pragma once
 
 #include "b2_slabconv.cuh"

@@ -1,5 +1,5 @@
-// b2_slabconv.cuh -- "same"-padded convolution (3x3x3, 1x3x3, 3x1x1, 7x1x1 ...; spatial stride 1 or 2) as an
-// implicit GEMM whose A operand is never re-fetched per filter tap.
+// b2_slabconv.cuh -- convolution (3x3x3, 1x3x3, 3x1x1, 7x1x1, 1x7, 5x5 ...; spatial stride 1 or 2; temporal padding "same", in-plane
+// padding from 0 to "same") as an implicit GEMM whose A operand is never re-fetched per filter tap.
 //
 // The generic gather kernel (b2_igemm.cuh) moves 16 KB of activations from L2 for every (tap, 64-channel)
 // K block: 27 x for a 3x3x3 filter, which makes those layers L2-bandwidth bound at ~20% of tensor peak.

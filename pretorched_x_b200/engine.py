@@ -692,8 +692,11 @@ def _split_pack(model, names, in_pitch):
     """Packed B and affine of a split GEMM over the 1x1 convolutions ``names`` (each followed by ``name + '_bn'``) that read the
     same input: destination d's fp16 filter rows and folded (conv bias + BN) affine from packed column 64 * box0[d] on, zero
     rows in the padding of its last 64-column box (ops.split_plan).  Cached on the first convolution."""
-    convs = [getattr(model, n) for n in names]
-    bns = [getattr(model, n + '_bn') for n in names]
+    return _split_pack_convs([getattr(model, n) for n in names], [getattr(model, n + '_bn') for n in names], in_pitch)
+
+
+def _split_pack_convs(convs, bns, in_pitch):
+    """``_split_pack`` over 1x1 convolutions ``convs``, each followed by BatchNorm ``bns[i]``."""
     dev = convs[0].weight.device
 
     def build():
@@ -793,6 +796,162 @@ def run_bninception_trunk(model, x):
     a = Fn.BNInceptionStemFunction.run(model, a)
     for spec in BLOCKS:
         a = run_inception(model, spec, a)
+    return a
+
+
+# ---------------------------------------------------------------------------------------------
+# Inception-v4 / Inception-ResNet-v2 (inceptionv4.py:34-309, inceptionresnetv2.py:34-331)
+# ---------------------------------------------------------------------------------------------
+def _is_head(u):
+    """A BasicConv2d whose convolution is 1x1, stride 1, padding 0: it runs inside a split GEMM."""
+    c = u.conv
+    return tuple(c.kernel_size) == (1, 1) and tuple(c.stride) == (1, 1) and tuple(c.padding) == (0, 0)
+
+
+def _max3s2(a, y=None):
+    """nn.MaxPool2d(3, stride=2) (floor mode) on the slice pool; on the odd maps of these networks it is the ceil-mode window."""
+    if (a.H - 3) % 2 or (a.W - 3) % 2:
+        raise ValueError("MaxPool2d(3, stride=2) runs on odd maps here (299x299 inputs), got %dx%d" % (a.H, a.W))
+    return ops.pool_slice(a, 3, 2, 0, False, y)
+
+
+def _basic_unit(u, a, y=None):
+    """BasicConv2d ``u`` (conv -> BN -> ReLU) of ``a``: a 1x1 on the GEMM, any filter with taps on the slab kernel's slice entry,
+    written into ``y`` (an fp16 [M][K] column slice) or a fresh dense matrix."""
+    if _is_head(u):
+        if y is None:
+            return conv_bn_act(u.conv, u.bn, a, relu=True)
+        w, scale, shift = _split_pack_convs([u.conv], [u.bn], a.ld)
+        ops.gemm_split(a.data, w, scale, shift, a.M, a.ld, [y], relu=True)
+        return Act(y, a.N, a.T, a.H, a.W, y.shape[1])
+    pc = packed_conv(u.conv, u.bn, a.ld)
+    if y is None:
+        (_, sh, sw), (_, ph, pw) = _conv_geometry(u.conv)
+        M = a.N * a.T * ops._out_dim(a.H, pc.k[1], sh, ph) * ops._out_dim(a.W, pc.k[2], sw, pw)
+        y = torch.empty((M, ops._round_up(pc.K, 8)), dtype=torch.float16, device=a.data.device)[:, :pc.K]
+    return ops.conv_slice(a, pc, y)
+
+
+def _inception_stem_body(units, a, out=None):
+    """The units before the first block (BasicConv2d / MaxPool2d(3, 2)) in sequence, and Inception-ResNet-v2's closing conv2d_7b.
+    The 3-channel input has pitch 8: the 3x3 stride-2 valid convolution runs on the slab kernel like MobileNetV2's stem."""
+    for i, u in enumerate(units):
+        last = i == len(units) - 1
+        if isinstance(u, nn.MaxPool2d):
+            a = _max3s2(a, None if not last or out is None else out)
+        else:
+            a = _basic_unit(u, a, out if last and out is not None else None)
+    return a
+
+
+def _branch_width(block, a, br):
+    if br[0] == 'max':
+        return a.C
+    if br[0] == 'fork':
+        return sum(block.get_submodule(p).conv.out_channels for p in br[2])
+    return block.get_submodule(br[1][-1]).conv.out_channels
+
+
+def _branch_hw(block, a, br):
+    """Output map of a branch: MaxPool2d(3, 2), or its chain's convolutions in sequence (every branch of a block agrees)."""
+    if br[0] == 'max':
+        return ops._out_dim(a.H, 3, 2, 0), ops._out_dim(a.W, 3, 2, 0)
+    H, W = a.H, a.W
+    for p in (br[1] if br[0] != 'fork' else br[1] + [br[2][0]]):
+        (_, sh, sw), (_, ph, pw) = _conv_geometry(block.get_submodule(p).conv)
+        kh, kw = block.get_submodule(p).conv.kernel_size
+        H, W = ops._out_dim(H, kh, sh, ph), ops._out_dim(W, kw, sw, pw)
+    return H, W
+
+
+def _inception_block_body(block, a, out=None):
+    """One block of Inception-v4 / Inception-ResNet-v2 from its row of models.inception.BRANCHES.  The branches write their
+    columns of the concatenated output ``y`` in place:
+
+    * the 1x1 units that read the block input (a lone 1x1 branch straight into its slice, the first unit of a longer chain into its
+      own matrix) run as one split GEMM -- one pass over the block input;
+    * every later unit of a chain runs on the slab kernel's slice entry, the last one into the branch's slice; a fork's two units
+      read the same matrix and write adjacent slices;
+    * a max branch pools the block input into its slice; an average branch pools it (count_include_pad=False) into a matrix that
+      its 1x1 projection reads, writing its slice;
+    * a residual block (Block35 / 17 / 8) closes with one GEMM over ``y``: per-column scale ``block.scale``, shift
+      ``scale * bias``, the block input as residual, ReLU unless ``noReLU`` (inceptionresnetv2.py:113-117)."""
+    from .models.inception import BRANCHES, RESIDUAL
+    kind = type(block).kind
+    branches = BRANCHES[kind]
+    get = block.get_submodule
+    if a.ld != a.C:
+        raise ValueError("%s takes a dense [M][C] input, got %r" % (kind, a))
+    Ho, Wo = _branch_hw(block, a, branches[0])
+    widths = [_branch_width(block, a, br) for br in branches]
+    cols = [sum(widths[:i]) for i in range(len(widths))]
+    C = sum(widths)
+    M = a.N * a.T * Ho * Wo
+    dev = a.data.device
+    residual = kind in RESIDUAL
+    if out is not None and not residual:
+        y = ops._out_rows(out, M, C)
+    else:
+        y = torch.empty((M, C), dtype=torch.float16, device=dev)
+    heads, dests, temps = [], [], {}
+    for br, c0, wd in zip(branches, cols, widths):
+        if br[0] in ('chain', 'fork') and _is_head(get(br[1][0])):
+            u = get(br[1][0])
+            K = u.conv.out_channels
+            if br[0] == 'chain' and len(br[1]) == 1:
+                dests.append(y[:, c0:c0 + K])
+            else:
+                temps[br[1][0]] = torch.empty((a.M, K), dtype=torch.float16, device=dev)
+                dests.append(temps[br[1][0]])
+            heads.append(u)
+    if heads:
+        w, scale, shift = _split_pack_convs([u.conv for u in heads], [u.bn for u in heads], a.ld)
+        ops.gemm_split(a.data, w, scale, shift, a.M, a.ld, dests, relu=True)
+    for br, c0, wd in zip(branches, cols, widths):
+        if br[0] == 'max':
+            _max3s2(a, y[:, c0:c0 + wd])
+        elif br[0] == 'avg':
+            pooled = ops.pool_slice(a, 3, 1, 1, True, count_include_pad=False)
+            _basic_unit(get(br[1][-1]), pooled, y[:, c0:c0 + wd])
+        else:
+            paths = br[1]
+            h = Act(temps[paths[0]], a.N, a.T, a.H, a.W, temps[paths[0]].shape[1]) if paths[0] in temps else a
+            rest = [get(p) for p in paths[(1 if paths[0] in temps or _is_head(get(paths[0])) else 0):]]
+            ends = [get(p) for p in br[2]] if br[0] == 'fork' else rest[-1:]
+            for u in (rest if br[0] == 'fork' else rest[:-1]):
+                h = _basic_unit(u, h)
+            c = c0
+            for u in ends:
+                K = u.conv.out_channels
+                _basic_unit(u, h, y[:, c:c + K])
+                c += K
+    if not residual:
+        return Act(y, a.N, a.T, Ho, Wo, C)
+    conv = block.conv2d
+    K = conv.out_channels
+
+    def build():
+        s = torch.full((K,), float(block.scale), dtype=torch.float64, device=dev)
+        return (_conv1x1_matrix(conv).float().to(torch.float16).contiguous(), s.float().contiguous(),
+                (s * conv.bias.detach().double()).float().contiguous())
+
+    w, scale, shift = _cached(conv, "res", _sig(conv.weight, conv.bias) + (float(block.scale),), build)
+    z = ops.gemm(y, w, scale, shift, M, K, C, residual=a.data, relu=not getattr(block, 'noReLU', False), out=out)
+    return Act(z, a.N, a.T, Ho, Wo, K)
+
+
+def run_inception_trunk(n_stem, units, x):
+    """The trunk of Inception-v4 (``units`` = ``features``) or Inception-ResNet-v2: fp32 NCHW images (or an Act with channel
+    pitch 8) in, the final 1536-channel map (an Act) out.  ``units[:n_stem]`` run as one stem Function, every block as one
+    ``InceptionBlockFunction``, a trailing BasicConv2d (conv2d_7b) as a stem Function of its own."""
+    from .models.inception import BasicConv2d
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
+    if (a.H, a.W) != (299, 299):
+        # the final pool is the reference's fixed AvgPool2d(8): only an 8x8 final map gives one vector per image
+        raise ValueError("the final pool is AvgPool2d(8): it needs an 8x8 final map (299x299 inputs), got a %dx%d input" % (a.H, a.W))
+    a = Fn.InceptionStemFunction.run(tuple(units[:n_stem]), a)
+    for u in units[n_stem:]:
+        a = Fn.InceptionStemFunction.run((u,), a) if isinstance(u, BasicConv2d) else Fn.InceptionBlockFunction.run(u, a)
     return a
 
 

@@ -166,6 +166,26 @@ class InceptionFunction(_FrozenFunction):
         return InceptionFunction._finish(ctx, engine._inception_body(model, spec, Act(x2d, *geom), out))
 
 
+class InceptionStemFunction(_FrozenFunction):
+    """Units of Inception-v4 / Inception-ResNet-v2 outside the blocks, in sequence (``units``: a tuple of BasicConv2d /
+    MaxPool2d): the stems (inceptionv4.py:274-276, inceptionresnetv2.py:305-311) and conv2d_7b (:319)."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, units, out=None):
+        from . import engine
+        return InceptionStemFunction._finish(ctx, engine._inception_stem_body(units, Act(x2d, *geom), out))
+
+
+class InceptionBlockFunction(_FrozenFunction):
+    """One block of Inception-v4 / Inception-ResNet-v2 (models.inception.BRANCHES): its branches written in place into the
+    concatenated output, and the residual close of Block35 / 17 / 8."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, block, out=None):
+        from . import engine
+        return InceptionBlockFunction._finish(ctx, engine._inception_block_body(block, Act(x2d, *geom), out))
+
+
 class GBlockFunction(_FrozenFunction):
     """BigGAN-deep GBlock: ccbn-ReLU-1x1 -> ccbn-ReLU-[up]-3x3 -> ccbn-ReLU-3x3 -> ccbn-ReLU-1x1 (+ skip)."""
 

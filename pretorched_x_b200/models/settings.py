@@ -7,9 +7,10 @@ from .resnext3d import pretrained_settings as resnext3d_settings      # settings
 from .mobilenet import pretrained_settings as mobilenet_settings      # mobilenet.py:7-19 (not in the reference's registry)
 from .senet import pretrained_settings as senet_settings              # senet.py:15-82 (not in the reference's registry)
 from .bninception import pretrained_settings as bninception_settings  # bninception.py:10-25 (settings.py:3 of the reference)
+from .inception import pretrained_settings as inception_settings      # inceptionv4.py:10-31, inceptionresnetv2.py:10-31
 
 all_settings = [resnet2d_settings, resnet3d_settings, resnext3d_settings, nonlocal_settings, mobilenet_settings, senet_settings,
-                bninception_settings]
+                bninception_settings, inception_settings]
 
 model_names = []
 pretrained_settings = {}

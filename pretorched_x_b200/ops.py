@@ -567,8 +567,9 @@ def gemm_split(a2d, b2d, scale, shift, M, Kd, dests, relu=True):
 
 @_on_device
 def conv_slice(a, pc, y, relu=True):
-    """``conv`` of a 3x3 filter (stride 1 or 2, padding 1) whose output is the column slice ``y`` (an fp16 [M][K] view of a
-    wider matrix): b2_conv_ndhwc_fprop_slice writes columns [0, K) of each row and nothing else."""
+    """``conv`` of a 2-D filter with taps (3x3, 1x7, 7x1, 5x5 ...; stride 1 or 2; padding from 0 to "same") whose output is the
+    column slice ``y`` (an fp16 [M][K] view of a wider matrix, or a whole [M][K] matrix): b2_conv_ndhwc_fprop_slice writes columns
+    [0, K) of each row and nothing else, always on the slab kernel."""
     if a.ld != pc.C:
         raise ValueError("activation pitch %d != packed filter pitch %d" % (a.ld, pc.C))
     kt, kh, kw = pc.k
@@ -594,9 +595,11 @@ def conv_slice(a, pc, y, relu=True):
 
 
 @_on_device
-def pool_slice(a, k, s, p, avg, y=None):
-    """nn.MaxPool2d / nn.AvgPool2d(count_include_pad=True) (k, stride s, padding p, ceil_mode=True) over every frame of ``a`` (its
-    ``data`` may itself be a column slice: rows of pitch ``data.stride(0)``) into the column slice ``y`` (fp16 [M_out][a.C] view; a fresh dense matrix when None) by b2_pool_ndhwc_slice."""
+def pool_slice(a, k, s, p, avg, y=None, count_include_pad=True):
+    """nn.MaxPool2d / nn.AvgPool2d (k, stride s, padding p, ceil_mode=True) over every frame of ``a`` (its ``data`` may itself be a
+    column slice: rows of pitch ``data.stride(0)``) into the column slice ``y`` (fp16 [M_out][a.C] view; a fresh dense matrix when
+    None) by b2_pool_ndhwc_slice, or, for an average with ``count_include_pad=False``, b2_avgpool_ndhwc_slice_exclude_pad.  (The
+    floor-mode windows of Inception-v4 / Inception-ResNet-v2 are ceil-mode windows on their odd maps.)"""
     Ho, Wo = ceil_pool_dim(a.H, k, s, p), ceil_pool_dim(a.W, k, s, p)
     My = a.N * a.T * Ho * Wo
     if y is None:
@@ -606,8 +609,13 @@ def pool_slice(a, k, s, p, avg, y=None):
         raise ValueError("pool output %s does not fit %d rows of %d channels" % (tuple(y.shape), My, a.C))
     with _timed("pool", "%spool %dx%d s%d C%d M=%d->%d" % ("avg" if avg else "max", k, k, s, a.C, a.M, My), 0.0,
                 2.0 * a.C * (a.M + My)):
-        _lib.check(_lib.load().b2_pool_ndhwc_slice(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, k, k, 1, s, s, 0, p, p,
-                                                   a.T, Ho, Wo, int(bool(avg)), _stream()), "b2_pool_ndhwc_slice")
+        if avg and not count_include_pad:
+            _lib.check(_lib.load().b2_avgpool_ndhwc_slice_exclude_pad(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, k,
+                                                                      k, 1, s, s, 0, p, p, a.T, Ho, Wo, _stream()),
+                       "b2_avgpool_ndhwc_slice_exclude_pad")
+        else:
+            _lib.check(_lib.load().b2_pool_ndhwc_slice(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, k, k, 1, s, s, 0,
+                                                       p, p, a.T, Ho, Wo, int(bool(avg)), _stream()), "b2_pool_ndhwc_slice")
     return Act(y, a.N, a.T, Ho, Wo, a.C)
 
 
