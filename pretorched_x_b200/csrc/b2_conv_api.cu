@@ -469,42 +469,54 @@ static bool slab_choose(const b2_conv_args* a, int wc_hint, int G, int ldo, Slab
 }
 
 // ------------------------------------------------------------------------------------------
-// 128-wide slab tiles as the transposed product (b2_slab_t128.cuh)
+// 128- and 64-wide slab tiles as the transposed product (b2_slab_t128.cuh)
 // ------------------------------------------------------------------------------------------
 static int g_slab_t128 = -1;       // -1 the rule (slab_t128_wanted), 0 never, 1 wherever the form applies (tests, A/B sweeps)
-static const int kT128Widths[3] = {216, 224, 256};   // compiled item widths NP
+static int g_slab_t64 = -1;        // the same for the 64-wide form (slab_t64_wanted)
+static const int kT128Widths[3] = {216, 224, 256};   // compiled item widths NP of the 128-wide form
+static const int kT64Width = 168;  // positions per warpgroup of the 64-wide form: 20 half-items cover a 56 x 58 padded plane
 
-struct T128Plan {
+struct TPlan {
   SlabParams p;                    // geometry (slab_geometry) + qitem
-  int np, rows, R, items, smem;
+  int np, rows, R, items, smem;    // rows: whole output rows per item (128-wide form), 0 for the 64-wide form
 };
 
-static int t128_smem(int slab_bytes, int np, int ldy) {
-  return kSlabSStages * slab_bytes + kSlabWStages * kT128WBytes + np * kT128RowBytes + 256 + 2 * slab_naff(ldy) * 4 + 1024;
+static int slab_t_smem(int BN, int slab_bytes, int np, int ldy) {
+  return kSlabSStages * slab_bytes + kSlabWStages * BN * 128 + np * 256 + 256 + 2 * slab_naff(ldy) * 4 + 1024;
 }
 
-// Whether the form takes the convolution at all, and its plan: the fewest row groups per plane whose padded positions fit 256, the
-// narrowest compiled width that holds one, and the slab rows every item's positions and taps reach.
-static bool slab_t128_geometry(const b2_conv_args* a, T128Plan* t) {
+// Whether the BN-wide form takes the convolution at all, and its plan.  BN = 128: the fewest row groups per plane whose padded
+// positions fit 256, and the narrowest compiled width that holds one.  BN = 64: items of 2 NP consecutive positions.  Then the slab
+// rows that every item's MMA columns and taps reach.
+static bool slab_t_geometry(const b2_conv_args* a, int BN, TPlan* t) {
   if (a->upsample || a->aff_ld || a->residual || a->y2 || a->residual_up || a->residual_pre || a->in_scale || a->mask) return false;
   if (a->kh != 3 || a->kw != 3 || (a->kt != 1 && a->kt != 3)) return false;
-  if (a->C % 64 != 0 || a->K % 128 != 0) return false;
+  if (a->C % 64 != 0 || (BN == 128 ? a->K % 128 != 0 : a->ldy > 64)) return false;
   SlabParams& p = t->p;
   if (!slab_geometry(a, &p, 0) || p.wchunks != 1 || p.up) return false;
-  const int max_rows = 256 / p.PW;
-  if (max_rows < 1) return false;
-  const int groups = (p.Ho + max_rows - 1) / max_rows;
-  t->rows = (p.Ho + groups - 1) / groups;
-  p.qitem = t->rows * p.PW;
-  t->np = 0;
-  for (int np : kT128Widths)
-    if (np >= p.qitem) { t->np = np; break; }
-  if (t->np == 0) return false;
+  int groups, span;                // position groups per plane, MMA columns from each item start
+  if (BN == 128) {
+    const int max_rows = 256 / p.PW;
+    if (max_rows < 1) return false;
+    groups = (p.Ho + max_rows - 1) / max_rows;
+    t->rows = (p.Ho + groups - 1) / groups;
+    p.qitem = t->rows * p.PW;
+    t->np = 0;
+    for (int np : kT128Widths)
+      if (np >= p.qitem) { t->np = np; break; }
+    if (t->np == 0) return false;
+    span = t->np;
+  } else {
+    t->np = kT64Width;
+    t->rows = 0;
+    p.qitem = span = 2 * t->np;
+    groups = (p.P + p.qitem - 1) / p.qitem;
+  }
   int R = 0;
   for (int q0 = 0; q0 < p.P; q0 += p.qitem) {
     int lo = q0 - p.reach;
     lo = (lo >= 0) ? lo / p.PW : -((-lo + p.PW - 1) / p.PW);
-    const int hi = (q0 + t->np - 1 + p.reach) / p.PW;
+    const int hi = (q0 + span - 1 + p.reach) / p.PW;
     R = (hi - lo + 1) > R ? (hi - lo + 1) : R;
   }
   if (p.ss * (R - 1) + 1 > 256) return false;
@@ -512,12 +524,12 @@ static bool slab_t128_geometry(const b2_conv_args* a, T128Plan* t) {
   p.R = R;
   p.slab_bytes = (R * p.PW * 128 + 1023) / 1024 * 1024;
   p.MT = 1;
-  p.tiles_n = (a->ldy + 127) / 128;
+  p.tiles_n = (a->ldy + BN - 1) / BN;
   p.tiles_q = groups;
   const long long items = (long long)p.tiles_n * groups * a->N * p.To;
   if (items >= (1ll << 31)) return false;
   t->items = (int)items;
-  t->smem = t128_smem(p.slab_bytes, t->np, a->ldy);
+  t->smem = slab_t_smem(BN, p.slab_bytes, t->np, a->ldy);
   return t->smem <= 227 * 1024;
 }
 
@@ -533,8 +545,8 @@ static long long slab_items(const b2_conv_args* a, const SlabChoice& c) {
 // is taken where rounds of items x MMA columns per item -- the critical path of the persistent grid -- is not longer than the slab
 // kernel's plan: ceil(items / SMs) * NP / 128 <= ceil(slab items / SMs) * MT.  At small sizes halving the items idles SMs and the
 // rule declines.  A forced slab plan (set_slab_mt, set_slab_wide) and multi-plane slab items stay on the slab kernel.
-static bool slab_t128_wanted(const b2_conv_args* a, const SlabChoice& c, T128Plan* t) {
-  if (g_slab_t128 == 0 || !slab_t128_geometry(a, t)) return false;
+static bool slab_t128_wanted(const b2_conv_args* a, const SlabChoice& c, TPlan* t) {
+  if (g_slab_t128 == 0 || !slab_t_geometry(a, 128, t)) return false;
   if (g_slab_t128 == 1) return true;
   if (g_slab_force_mt != 0 || g_slab_wide == 1 || c.p.mp > 1) return false;
   const long long sms = sm_count();
@@ -542,18 +554,39 @@ static bool slab_t128_wanted(const b2_conv_args* a, const SlabChoice& c, T128Pla
   return ((t->items + sms - 1) / sms) * t->np <= ((cur + sms - 1) / sms) * c.MT * 128;
 }
 
-template <int NP>
-static int run_slab_t128(int grid, int smem_bytes, const CUtensorMap& tmX, const CUtensorMap& tmB, const SlabParams& p,
-                         cudaStream_t stream) {
-  B2_OPT_IN_SMEM(slab_t128_kernel<NP>, 227 * 1024);
-  B2_CHECK_CUDA(launch_pdl(slab_t128_kernel<NP>, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
-  B2_CHECK_LAUNCH("slab_t128_kernel");
+// The 64-wide form's rule.  Its items hold 2 NP = 336 positions against the slab kernel's MT * 128, and one of its MMA columns
+// costs less: a weight stage serves 1.3x the positions, and the consumers store fp16 through stmatrix instead of fp32 scalars into an
+// accumulator tile.  Measured per column (kernel time / (rounds of items x columns per item), H100 SXM at 700 W, 1980 MHz) on 64 ->
+// 64 3x3 convolutions over 56 x 56 planes, the form's column cost 0.64 - 0.75 of the slab kernel's at 2 - 32 clips of 8 frames and
+// 32 - 256 images, so it is taken where rounds x columns x kT64ColCost % is not longer than the slab plan's rounds x columns.  Below
+// kT64MinItemsPerSm items per SM (fewer than ~26 planes of 56 x 56) the slab kernel keeps the convolution: there a launch is a
+// round or two of items, and the form's larger items gain at most a few microseconds.  A forced slab plan and multi-plane slab
+// items stay on the slab kernel.
+static const int kT64ColCost = 75;
+static const int kT64MinItemsPerSm = 2;
+static bool slab_t64_wanted(const b2_conv_args* a, const SlabChoice& c, TPlan* t) {
+  if (g_slab_t64 == 0 || !slab_t_geometry(a, 64, t)) return false;
+  if (g_slab_t64 == 1) return true;
+  if (g_slab_force_mt != 0 || g_slab_wide == 1 || c.p.mp > 1) return false;
+  const long long sms = sm_count();
+  const long long cur = slab_items(a, c);
+  return t->items >= kT64MinItemsPerSm * sms &&
+         ((t->items + sms - 1) / sms) * 2 * t->np * kT64ColCost <= ((cur + sms - 1) / sms) * c.MT * 128 * 100;
+}
+
+template <int BN, int NP>
+static int run_slab_t(int grid, int smem_bytes, const CUtensorMap& tmX, const CUtensorMap& tmB, const SlabParams& p,
+                      cudaStream_t stream) {
+  B2_OPT_IN_SMEM((slab_t_kernel<BN, NP>), 227 * 1024);
+  B2_CHECK_CUDA(launch_pdl(slab_t_kernel<BN, NP>, dim3(grid), dim3(kSlabThreads), smem_bytes, stream, tmX, tmB, p));
+  B2_CHECK_LAUNCH("slab_t_kernel");
   return B2_OK;
 }
 
-static int launch_slab_t128(const b2_conv_args* a, T128Plan& t, cudaStream_t stream) {
+template <int BN>
+static int launch_slab_t(const b2_conv_args* a, TPlan& t, cudaStream_t stream) {
   SlabParams& p = t.p;
-  p.bn = 128; p.wbytes = kT128WBytes; p.accs = 128;
+  p.bn = BN; p.wbytes = BN * 128; p.accs = BN;
   p.mp = 0;
   p.planes_total = a->N * p.To;
   p.plane_stride = p.R * p.PW * 128;
@@ -575,18 +608,19 @@ static int launch_slab_t128(const b2_conv_args* a, T128Plan& t, cudaStream_t str
   if ((rc = make_tmap_ndhwc_slab(&tmX, a->x, (uint64_t)a->C, (uint64_t)a->W, (uint64_t)a->H, (uint64_t)a->N * a->T, (uint32_t)p.PW,
                                  (uint32_t)t.R, (uint32_t)p.ss)) != B2_OK)
     return rc;
-  if ((rc = make_tmap_2d_f16(&tmB, a->w, (uint64_t)taps * a->C, (uint64_t)a->K, (uint64_t)taps * a->C, 64, 128, true)) != B2_OK)
+  if ((rc = make_tmap_2d_f16(&tmB, a->w, (uint64_t)taps * a->C, (uint64_t)a->K, (uint64_t)taps * a->C, 64, BN, true)) != B2_OK)
     return rc;
   const int grid = p.items_total < sm_count() ? p.items_total : sm_count();
-  switch (t.np) {
-    case 216: return run_slab_t128<216>(grid, t.smem, tmX, tmB, p, stream);
-    case 224: return run_slab_t128<224>(grid, t.smem, tmX, tmB, p, stream);
-    case 256: return run_slab_t128<256>(grid, t.smem, tmX, tmB, p, stream);
-    default: return set_error(B2_ERR_INVALID, "slab item width %d is not one of the compiled widths", t.np);
+  switch (BN * 1000 + t.np) {
+    case 128216: return run_slab_t<128, 216>(grid, t.smem, tmX, tmB, p, stream);
+    case 128224: return run_slab_t<128, 224>(grid, t.smem, tmX, tmB, p, stream);
+    case 128256: return run_slab_t<128, 256>(grid, t.smem, tmX, tmB, p, stream);
+    case 64168: return run_slab_t<64, 168>(grid, t.smem, tmX, tmB, p, stream);
+    default: return set_error(B2_ERR_INVALID, "slab item width %d is not one of the compiled widths of the %d-wide form", t.np, BN);
   }
 }
 
-// returns 1 when the slab kernel (or its 128-wide transposed form) took the convolution, 0 when it does not apply, <0 on error
+// returns 1 when the slab kernel (or one of its transposed forms) took the convolution, 0 when it does not apply, <0 on error
 // G != 0: grouped convolution inside the contract of b2_conv_grouped_ndhwc_fprop (3x3 in plane, so never the temporal remap)
 // ldo > 0: column-slice output, see launch_slab
 static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, int ldo = 0) {
@@ -606,10 +640,15 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, in
   SlabChoice c;
   if (!slab_choose(a, wc_hint, G, ldo, &c)) return 0;
   if (!G && !ldo) {
-    T128Plan t;
+    TPlan t;
     if (slab_t128_wanted(a, c, &t)) {
-      const int rc = launch_slab_t128(a, t, stream);
+      const int rc = launch_slab_t<128>(a, t, stream);
       if (rc == B2_OK) set_last_kernel(KID_SLAB_T128, t.np, t.rows, 128, t.p.ss, t.R);
+      return rc == B2_OK ? 1 : rc;
+    }
+    if (slab_t64_wanted(a, c, &t)) {
+      const int rc = launch_slab_t<64>(a, t, stream);
+      if (rc == B2_OK) set_last_kernel(KID_SLAB_T64, t.np, t.items, t.R);
       return rc == B2_OK ? 1 : rc;
     }
   }
@@ -1205,15 +1244,34 @@ int b2_debug_set_slab_t128(int mode) { g_slab_t128 = mode < -1 ? -1 : (mode > 1 
 int b2_debug_slab_t128_plan(const b2_conv_args* a, int* out) {
   memset(out, 0, 10 * sizeof(int));
   out[9] = sm_count();
-  T128Plan t;
+  TPlan t;
   memset(&t, 0, sizeof(t));
   SlabChoice c;
   const bool remapped = a->kt > 1 && a->kh == 1 && a->kw == 1;      // the remapped temporal form is never this one's
   if (remapped || !slab_choose(a, 0, 0, 0, &c)) return B2_OK;
   out[0] = slab_t128_wanted(a, c, &t);
-  out[1] = slab_t128_geometry(a, &t);
+  out[1] = slab_t_geometry(a, 128, &t);
   out[2] = t.np; out[3] = t.rows; out[4] = t.R; out[5] = t.items; out[6] = t.smem;
   out[7] = (int)slab_items(a, c); out[8] = c.MT;
+  return B2_OK;
+}
+/* 64-wide slab tiles as the transposed product (b2_slab_t128.cuh): mode -1 = the rule, 0 = never, 1 = wherever the form applies.
+   Host-only view of its decision for a convolution (no launch, no GPU needed) under the current knobs: out = {taken, applies, NP,
+   slab rows R, items, dynamic shared memory bytes, slab kernel items, slab kernel MT, SM count the rule used}.
+   b2_debug_last_kernel's info of a launch of the form (KID_SLAB_T64): {NP, items, R}. */
+int b2_debug_set_slab_t64(int mode) { g_slab_t64 = mode < -1 ? -1 : (mode > 1 ? 1 : mode); return B2_OK; }
+int b2_debug_slab_t64_plan(const b2_conv_args* a, int* out) {
+  memset(out, 0, 9 * sizeof(int));
+  out[8] = sm_count();
+  TPlan t;
+  memset(&t, 0, sizeof(t));
+  SlabChoice c;
+  const bool remapped = a->kt > 1 && a->kh == 1 && a->kw == 1;      // the remapped temporal form is never this one's
+  if (remapped || !slab_choose(a, 0, 0, 0, &c)) return B2_OK;
+  out[0] = slab_t64_wanted(a, c, &t);
+  out[1] = slab_t_geometry(a, 64, &t);
+  out[2] = t.np; out[3] = t.R; out[4] = t.items; out[5] = t.smem;
+  out[6] = (int)slab_items(a, c); out[7] = c.MT;
   return B2_OK;
 }
 int b2_debug_set_slab_mt(int mt) { g_slab_force_mt = mt < 0 ? 0 : mt; return B2_OK; }

@@ -96,7 +96,7 @@ struct SlabParams {
   int mp, plane_stride, planes_total;
   FastDiv fd_tiles_n, fd_tiles_q, fd_wchunks, fd_To, fd_PW;   // dividers of the item decode (set by launch_slab)
   int ldo;                 // slabconv_kernel<BN, TMT, kSlabSlice> only: row pitch of y (>= ldy, the columns written)
-  int qitem;               // slab_t128_kernel only: padded positions of the whole output rows of one work item
+  int qitem;               // slab_t_kernel only: padded positions of one work item (whole output rows for BN = 128, 2 NP for 64)
 };
 
 // scale/shift live in smem for all (padded) output channels: SlabParams::naff = round_up(ldy, 32) + 32 entries each; the
@@ -278,7 +278,7 @@ __device__ __forceinline__ void slab_consumer(const SlabParams& p, const AccTile
   }
 }
 
-// TMA producer of the slab kernels (one warp); item_at(item) decodes a work item (slab_item, or slab_t128_item of b2_slab_t128.cuh).
+// TMA producer of the slab kernels (one warp); item_at(item) decodes a work item (slab_item, or slab_t_item of b2_slab_t128.cuh).
 // Walks (item, slab) pairs; the slab after the current one -- possibly the first slab of the NEXT item -- is
 // requested after weight tap min(kSlabWStages, ntaps - 1) of the current slab: from tap kSlabWStages on, the weight ring
 // guarantees the consumers have retired the slab that occupied the target slot, so that wait never stalls weight issue;

@@ -21,6 +21,8 @@ lib.b2_debug_set_tstack.restype = ctypes.c_int
 lib.b2_debug_set_tstack.argtypes = [ctypes.c_int]             # 5th field: temporal stack kernel 1 = whenever eligible, 0 = never, -1 / absent = the library's rule
 lib.b2_debug_set_slab_t128.restype = ctypes.c_int
 lib.b2_debug_set_slab_t128.argtypes = [ctypes.c_int]          # 6th field: 128-wide transposed slab form 1 = wherever it applies, 0 = never, -1 / absent = the rule
+lib.b2_debug_set_slab_t64.restype = ctypes.c_int
+lib.b2_debug_set_slab_t64.argtypes = [ctypes.c_int]           # 7th field: 64-wide transposed slab form 1 = wherever it applies, 0 = never, -1 / absent = the rule
 dev = torch.device("cuda:0")
 REP = 20
 for sp in specs:
@@ -50,6 +52,7 @@ for sp in specs:
             lib.b2_debug_set_slab_wide(st[3] if len(st) > 3 else -1)
             lib.b2_debug_set_tstack(st[4] if len(st) > 4 else -1)
             lib.b2_debug_set_slab_t128(st[5] if len(st) > 5 else -1)
+            lib.b2_debug_set_slab_t64(st[6] if len(st) > 6 else -1)
             for _ in range(2):
                 y = engine.conv_bn_act(conv, bn, x, residual=res, relu=True)
             torch.cuda.synchronize()
