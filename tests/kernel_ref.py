@@ -9,6 +9,9 @@ Bound, per output element:  |got - ref| <= a * 2^-11 * |ref| + b * A + 2^-24, wi
       of roundoff on the sum of magnitudes -- far below what one dropped tap, channel chunk or output row costs.
 The generator epilogues (per-sample affine, fused upsample, upsampled / pre-affine residual, second output, input affine) use
 the same bound with the magnitude of each epilogue's own terms; see ``epilogue`` below.
+
+The builders take ``device=`` (default the CPU): whole-model audits (tests/model_audit.py) build the same fp64 references on
+the GPU, where a CPU reference of a full-batch forward would take hours.
 """
 import torch
 import torch.nn.functional as F
@@ -18,12 +21,12 @@ B_ACC = 2.0 ** -14
 FLOOR = 2.0 ** -24
 
 
-def conv_ref(x, w, scale, shift, k, s, p, residual=None, relu=False, base=None):
+def conv_ref(x, w, scale, shift, k, s, p, residual=None, relu=False, base=None, device="cpu"):
     """fp64 reference of b2_conv_ndhwc_fprop from exactly the kernel's operands.
 
     x: [N, T, H, W, C] (C the channel pitch), w: [K, taps, C] (the packed filter), scale / shift: [K]; residual: [M, >= K];
     base: [M, K], the prior contents of an fp32 output with ``accumulate``.  Returns (ref, A), both fp64 [M, K]."""
-    x, w = x.double().cpu(), w.double().cpu()
+    x, w = x.double().to(device), w.double().to(device)
     K, C = w.shape[0], x.shape[-1]
     wt = w.reshape(K, k[0], k[1], k[2], C).permute(0, 4, 1, 2, 3)
     xt = x.permute(0, 4, 1, 2, 3)
@@ -31,16 +34,16 @@ def conv_ref(x, w, scale, shift, k, s, p, residual=None, relu=False, base=None):
     mag = F.conv3d(xt.abs(), wt.abs(), stride=s, padding=p)
     acc = acc.permute(0, 2, 3, 4, 1).reshape(-1, K)
     mag = mag.permute(0, 2, 3, 4, 1).reshape(-1, K)
-    sc, sh = scale.double().cpu(), shift.double().cpu()
+    sc, sh = scale.double().to(device), shift.double().to(device)
     ref = acc * sc + sh
     A = mag * sc.abs() + sh.abs()
     if residual is not None:
-        r = residual[:, :K].double().cpu()
+        r = residual[:, :K].double().to(device)
         ref, A = ref + r, A + r.abs()
     if relu:
         ref = ref.clamp_min(0.0)
     if base is not None:
-        b = base.double().cpu()
+        b = base.double().to(device)
         ref, A = ref + b, A + b.abs()
     return ref, A
 
@@ -83,9 +86,9 @@ def where_worst_of(got, ref, bnd):
 # come from one of the *_acc functions, the epilogue from ``epilogue`` -- all in fp64 from exactly the operands the kernel reads,
 # every element held to the same bound as above.
 # ---------------------------------------------------------------------------------------------
-def conv_acc(x, w, k, s, p):
+def conv_acc(x, w, k, s, p, device="cpu"):
     """sum_{tap,c} x * w and sum |x * w| of a convolution (x [N, T, H, W, C], w [K, taps, C]): fp64 [M, K] each."""
-    x, w = x.double().cpu(), w.double().cpu()
+    x, w = x.double().to(device), w.double().to(device)
     K, C = w.shape[0], x.shape[-1]
     wt = w.reshape(K, k[0], k[1], k[2], C).permute(0, 4, 1, 2, 3)
     xt = x.permute(0, 4, 1, 2, 3)
@@ -94,24 +97,24 @@ def conv_acc(x, w, k, s, p):
     return acc, mag
 
 
-def gemm_acc(a, b):
+def gemm_acc(a, b, device="cpu"):
     """A[M][Kd] . B[N][Kd]^T and its magnitude, fp64."""
-    a, b = a.double().cpu(), b.double().cpu()
+    a, b = a.double().to(device), b.double().to(device)
     return a @ b.t(), a.abs() @ b.abs().t()
 
 
-def upconv_acc(x, wph):
+def upconv_acc(x, wph, device="cpu"):
     """conv3x3(nearest_up2(x)) as the kernel computes it: four 2x2 phase convolutions of the LOW-res image x [N, H, W, C]
     (or [N, 1, H, W, C]) with the packed phase filter wph [K, 16, C] read back from the pack.  Output pixel (2h + py, 2w + px)
     reads low-res pixel (h - 1 + py + a, w - 1 + px + b) with tap (2 py + px) * 4 + 2 a + b.  fp64 [N * 2H * 2W, K] each."""
-    x = x.double().cpu()
+    x = x.double().to(device)
     if x.dim() == 5:
         x = x[:, 0]
     N, H, W, C = x.shape
-    wph = wph.double().cpu()
+    wph = wph.double().to(device)
     K = wph.shape[0]
     xp = F.pad(x.permute(0, 3, 1, 2), (1, 1, 1, 1))
-    acc = torch.zeros(N, K, 2 * H, 2 * W, dtype=torch.float64)
+    acc = torch.zeros(N, K, 2 * H, 2 * W, dtype=torch.float64, device=device)
     mag = torch.zeros_like(acc)
     for py in (0, 1):
         for px in (0, 1):
@@ -146,41 +149,41 @@ def upconv_fold(w):
     return fold, mag
 
 
-def nearest_up2(skip, N, H, W, K):
+def nearest_up2(skip, N, H, W, K, device="cpu"):
     """The first K channels of a low-res skip tensor [N * (H/2) * (W/2)][>= K], nearest-2x upsampled to [N * H * W][K] (fp64)."""
-    s = skip[:, :K].double().cpu().reshape(N, H // 2, W // 2, K)
+    s = skip[:, :K].double().to(device).reshape(N, H // 2, W // 2, K)
     return s.repeat_interleave(2, dim=1).repeat_interleave(2, dim=2).reshape(-1, K)
 
 
-def per_row(v, rows, M, K):
+def per_row(v, rows, M, K, device="cpu"):
     """Per-sample rows [N][>= K] -> the [M][K] rows the elements use (row m takes sample m // rows); [K] stays [K]."""
-    v = v.double().cpu()
+    v = v.double().to(device)
     if v.dim() == 1:
         return v[:K]
     return v[:, :K].repeat_interleave(rows, dim=0)[:M]
 
 
-def epilogue(acc, mag, scale, shift, residual=None, pre=False, relu=False):
+def epilogue(acc, mag, scale, shift, residual=None, pre=False, relu=False, device="cpu"):
     """Value of an output element before its fp16 rounding, and its magnitude A.  scale / shift: [K] or per-row [M][K] (see
     ``per_row``); residual: fp64 [M][K].  pre: the residual joins before the affine, v = s * (acc + r) + t with
     A = |s| * (sum |xw| + |r|) + |t|; otherwise v = s * acc + t + r with A = |s| * sum |xw| + |t| + |r|."""
-    s, t = scale.double().cpu(), shift.double().cpu()
+    s, t = scale.double().to(device), shift.double().to(device)
     if residual is not None and pre:
-        r = residual.double().cpu()
+        r = residual.double().to(device)
         v, A = s * (acc + r) + t, s.abs() * (mag + r.abs()) + t.abs()
     else:
         v, A = s * acc + t, s.abs() * mag + t.abs()
         if residual is not None:
-            r = residual.double().cpu()
+            r = residual.double().to(device)
             v, A = v + r, A + r.abs()
     if relu:
         v = v.clamp_min(0.0)
     return v, A
 
 
-def second_output(v, A, scale2, shift2):
+def second_output(v, A, scale2, shift2, device="cpu"):
     """y2 = relu(s2 * v + t2) from the first output's value v BEFORE its fp16 rounding: (ref2, A2 = |s2| A + |t2|)."""
-    s2, t2 = scale2.double().cpu(), shift2.double().cpu()
+    s2, t2 = scale2.double().to(device), shift2.double().to(device)
     return (s2 * v + t2).clamp_min(0.0), s2.abs() * A + t2.abs()
 
 
@@ -188,28 +191,59 @@ def second_output(v, A, scale2, shift2):
 MIDPOINT_REL = 2.0 ** -23
 
 
-def in_affine_operand(x, scale, shift, rows):
+def in_affine_operand(x, scale, shift, rows, device="cpu"):
     """The A operand of a convolution with an input affine: x' = fp16(relu(x * s_n + t_n)), x fp16 [M][C], scale / shift fp32
     [N][>= C].  Returns (x', other): x' the fp16 rounding of the fp64 value, ``other`` the magnitude of the neighbouring fp16
     value where the fp64 value lies within MIDPOINT_REL of a rounding midpoint (the kernel's fp32 FMA may land on either side;
     0 elsewhere)."""
-    x = x.double().cpu()
+    x = x.double().to(device)
     M, C = x.shape
-    v = (x * per_row(scale, rows, M, C) + per_row(shift, rows, M, C)).clamp_min(0.0)
+    v = (x * per_row(scale, rows, M, C, device) + per_row(shift, rows, M, C, device)).clamp_min(0.0)
     lo = (v * (1 - MIDPOINT_REL)).half().double()
     hi = (v * (1 + MIDPOINT_REL)).half().double()
     amb = lo != hi
     return v.half().double(), torch.where(amb, torch.maximum(lo.abs(), hi.abs()), torch.zeros_like(v))
 
 
-def in_affine_acc(x, w, scale, shift, rows):
+def in_affine_acc(x, w, scale, shift, rows, device="cpu"):
     """acc / magnitude of relu(x * s_n + t_n) . w^T (w [K][C]).  An operand that may round either way moves by at most one
     fp16 unit, 2^-10 |x'|: its products enter A with the weight 2^-10 / B_ACC, so the bound B_ACC * A covers the flip."""
-    xq, other = in_affine_operand(x, scale, shift, rows)
-    acc, mag = gemm_acc(xq, w)
+    xq, other = in_affine_operand(x, scale, shift, rows, device)
+    acc, mag = gemm_acc(xq, w, device)
     if bool((other > 0).any()):
-        mag = mag + (2.0 ** -10 / B_ACC) * (other @ w.double().cpu().abs().t())
+        mag = mag + (2.0 ** -10 / B_ACC) * (other @ w.double().to(device).abs().t())
     return acc, mag
+
+
+# ---------------------------------------------------------------------------------------------
+# non-local attention (tests/test_gpu_kernel_matrix.py, tests/model_audit.py)
+# ---------------------------------------------------------------------------------------------
+ATT_C = 4.0
+
+
+def att_ref(q, k, v, B, Nq, Nk, mode):
+    """fp64 softmax(Q K^T) V (mode 0), (Q K^T / Nk) V (mode 1) or (relu(Q K^T) / Nk) V (mode 2) of q [B * Nq][d], k [B * Nk][d],
+    v [B * Nk][dv], on their device.  Returns (ref [B * Nq][dv], |P| |V| [B][Nq][dv])."""
+    q, k, v = (t.double().view(B, -1, t.shape[1]) for t in (q, k, v))
+    s = q @ k.transpose(1, 2)
+    if mode == 0:
+        p = torch.softmax(s, dim=-1)
+    else:
+        p = (s if mode == 1 else s.clamp_min(0.0)) / Nk
+    return (p @ v).reshape(B * Nq, -1), p.abs() @ v.abs()
+
+
+def att_bound(ref, pv, v, B, Nq, Nk, mode):
+    """Per-element bound of the attention output.  Mode 0: a convex combination of the values, with fp16 P and output roundings,
+    relative to max_j |v_j| of its sample: ATT_C 2^-11 max_j |v_j|.  Modes 1 / 2: 2^-11 |ref| + ATT_C 2^-11 |P| |V|.  Plus the
+    floor 2^-24."""
+    dv = ref.shape[1]
+    if mode == 0:
+        vmax = v.double().abs().view(B, Nk, dv).amax(dim=1)
+        bnd = ATT_C * U_F16 * vmax.repeat_interleave(Nq, dim=0)
+    else:
+        bnd = U_F16 * ref.abs() + ATT_C * U_F16 * pv.reshape(B * Nq, dv)
+    return bnd + FLOOR
 
 
 # ---------------------------------------------------------------------------------------------
@@ -244,19 +278,19 @@ def pool_w(ref, A, Wo, f16=True):
     return pool(ref), pool(bound(ref, A, f16))
 
 
-def dw_ref(x, w9, scale, shift, stride, clamp_in, relu6):
+def dw_ref(x, w9, scale, shift, stride, clamp_in, relu6, device="cpu"):
     """fp64 reference of b2_dwconv3x3_ndhwc (padding 1): x fp16 [B, H, W, C] (the C used channels), w9 fp32 [9][C] (tap
     kh * 3 + kw), scale / shift fp32 [C].  The kernel reads min(x, 6) with clamp_in (exact in fp16).  A = |s| sum |x w| + |t|;
     the ReLU6 clamp comes after the bound is formed (1-Lipschitz).  Returns (ref, A), fp64 [B * Ho * Wo, C]."""
-    x = x.double().cpu()
+    x = x.double().to(device)
     if clamp_in:
         x = x.clamp(max=6.0)
     C = x.shape[-1]
     xt = x.permute(0, 3, 1, 2)
-    wt = w9.double().cpu().t().reshape(C, 1, 3, 3)
+    wt = w9.double().to(device).t().reshape(C, 1, 3, 3)
     acc = F.conv2d(xt, wt, stride=stride, padding=1, groups=C).permute(0, 2, 3, 1).reshape(-1, C)
     mag = F.conv2d(xt.abs(), wt.abs(), stride=stride, padding=1, groups=C).permute(0, 2, 3, 1).reshape(-1, C)
-    s, t = scale.double().cpu(), shift.double().cpu()
+    s, t = scale.double().to(device), shift.double().to(device)
     ref, A = acc * s + t, mag * s.abs() + t.abs()
     if relu6:
         ref = ref.clamp(0.0, 6.0)

@@ -17,7 +17,7 @@ import torch.nn.functional as F
 
 from oracle import functional as OF
 from tests.conftest import has_h100
-from tests.kernel_ref import conv_ref, where_worst, worst_ratio
+from tests.kernel_ref import att_bound, att_ref, conv_ref, where_worst, worst_ratio
 
 KNOB_ENV = ("B2_CONV_ALGO", "B2_GEMM_ALGO", "B2_DENSEM_MAXM", "B2_DENSEM_S", "B2_TSTACK", "B2_SLABTS")
 
@@ -476,7 +476,6 @@ ATT_CASES = [
     (1, 0, 1, 128, 128, 64, 64), (1, 0, 3, 260, 65, 128, 192), (1, 0, 1, 100, 17, 512, 256),
     (2, 0, 3, 129, 129, 64, 128), (2, 0, 1, 256, 64, 256, 64), (2, 0, 3, 99, 17, 192, 192),
 ]
-ATT_C = 4.0
 
 
 def att_operands(dev, B, Nq, Nk, d, dv, seed):
@@ -486,16 +485,6 @@ def att_operands(dev, B, Nq, Nk, d, dv, seed):
     kv = torch.randn(B * Nk, d + dv + 24, generator=g).half()
     kv[:, :d] = (kv[:, :d].float() * 0.3).half()
     return qm, kv
-
-
-def att_ref(q, k, v, B, Nq, Nk, mode):
-    q, k, v = (t.double().view(B, -1, t.shape[1]) for t in (q, k, v))
-    s = q @ k.transpose(1, 2)
-    if mode == 0:
-        p = torch.softmax(s, dim=-1)
-    else:
-        p = (s if mode == 1 else s.clamp_min(0.0)) / Nk
-    return (p @ v).reshape(B * Nq, -1), p.abs() @ v.abs()
 
 
 @pytest.mark.parametrize("case", ATT_CASES, ids=["m%d%s_B%d_q%d_k%d_d%d_dv%d" % (c[0], "tp" if c[1] else "", *c[2:]) for c in ATT_CASES])
@@ -512,12 +501,7 @@ def test_attention_against_fp64(dev, lib, case):
     assert (kid, info[:2]) == (ATTENTION, (online, 128 if online and dv % 128 == 0 else 64))
     ref, pv = att_ref(qm[:, :d], kv[:, :d], kv[:, d:d + dv], B, Nq, Nk, mode)
     err = (o[:, :dv].cpu().double() - ref).abs()
-    if mode == 0:           # a convex combination of the values: fp16 P and output roundings, relative to max_j |v_j|
-        vmax = kv[:, d:d + dv].double().abs().view(B, Nk, dv).amax(dim=1)
-        bnd = ATT_C * 2.0 ** -11 * vmax.repeat_interleave(Nq, dim=0)
-    else:
-        bnd = 2.0 ** -11 * ref.abs() + ATT_C * 2.0 ** -11 * pv.reshape(B * Nq, dv)
-    ratio = float((err / (bnd + 2.0 ** -24)).max())
+    ratio = float((err / att_bound(ref, pv, kv[:, d:d + dv], B, Nq, Nk, mode)).max())
     report("attention %s" % (case,), ratio)
     assert ratio <= 1.0
     o2 = ops.attention(qd, kvd, kvd[:, d:], d, dv, B, Nq, Nk, mode=mode)
