@@ -409,6 +409,11 @@ int b2_gemm_split_f16(const b2_gemm_args* g, int nd, void* const* y, const int* 
  * (b2_debug_last_kernel: KID 13).  Stem mode, mask, per-sample affine, upsampling, second output, pool_w, the generator fields and fp32
  * output are refused (B2_ERR_INVALID); B2_ERR_UNSUPPORTED when no slab tiling of the image fits. */
 int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream);
+/* b2_conv_ndhwc_fprop_slice with one N tile exactly K = 32 or 48 columns wide (one m64n32k16 / m64n48k16 per K step, positions along
+ * M) instead of the 64-wide tile that pads those widths: the growth-rate 3x3 convolutions of DenseNet's dense layers.  Same contract
+ * as b2_conv_ndhwc_fprop_slice, plus K in {32, 48} (B2_ERR_INVALID).  Each output element is accumulated in the same order as on the
+ * 64-wide tile and goes through the same epilogue.  b2_debug_last_kernel: KID 13, info = {K, MT, 1, wchunks}. */
+int b2_conv_ndhwc_fprop_slice_narrow(const b2_conv_args* a, void* stream);
 /* Pooling between column slices: x is [N*T*H*W] rows of pitch ldx (channels [0, C) read), y is a slice (y, ldy, C) of rows
  * [N*To*Ho*Wo] with the output extent given by the caller (ceil mode).  avg = 0: max (nn.MaxPool2d, padding taps skipped);
  * avg = 1: nn.AvgPool2d(count_include_pad=True) -- fp32 sum in a fixed tap order, divided by the window clipped to the padded input,
@@ -423,6 +428,30 @@ int b2_pool_ndhwc_slice(const void* x, int ldx, void* y, int ldy, int N, int T, 
  * b2_debug_last_kernel: KID 14, info = {2}. */
 int b2_avgpool_ndhwc_slice_exclude_pad(const void* x, int ldx, void* y, int ldy, int N, int T, int H, int W, int C, int kt, int kh, int kw,
                                        int st, int sh, int sw, int pt, int ph, int pw, int To, int Ho, int Wo, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * DenseNet (torchvision densenet.py, wrapped by torchvision_models.py:254-380)
+ * ------------------------------------------------------------------------------------------- */
+/* The 1x1 convolution of a dense layer with its pre-activation applied to the A operand on chip:
+ *     D[m][n] = act(scale[n] * sum_k relu(in_scale[k] * A[m][k] + in_shift[k]) * B[n][k] + shift[n])
+ * A is the first Kd columns of the dense block's matrix (pitch lda, any Kd % 8 == 0): columns >= Kd are never read -- the A and
+ * B tensor maps span Kd columns and TMA zero-fills the rest of the last 64-column K block -- so in_scale / in_shift must be
+ * 16-byte aligned fp32 arrays of round_up(Kd, 64) entries that are ZERO past Kd (relu(0 * 0 + 0) = 0), and B zero there.  The
+ * transformed operand is rounded to fp16 once before the MMA.  g: as b2_gemm_f16 with fp16 output (columns [N, ldd) written
+ * as zero); residual, per_row, out_f32, accumulate, aff_ld, d2 and mask must be zero (B2_ERR_INVALID).  Always the persistent
+ * GEMM's generator instance (b2_debug_last_kernel: KID 6, info = {N tile, 0, 1}). */
+int b2_gemm_preact_f16(const b2_gemm_args* g, const float* in_scale, const float* in_shift, void* stream);
+/* A dense transition's BatchNorm + ReLU + AvgPool2d(2, 2) (densenet.py _Transition, pooled before its 1x1 convolution):
+ *     y[n][ho][wo][c] = fp16(sum_{dh, dw < 2} relu(scale[c] * x[n][2 ho + dh][2 wo + dw][c] + shift[c]) / 4)
+ * fp32 sum in (dh, dw) order, one rounding; Ho = H / 2, Wo = W / 2 (floor: an odd last row / column is dropped, as nn.AvgPool2d).
+ * x: rows of pitch ldx (channels [0, C) read), y: a slice (y, ldy, C).  C, ldx, ldy multiples of 8, x / y 16-byte aligned, scale /
+ * shift fp32 [C].  b2_debug_last_kernel: KID 14, info = {3}. */
+int b2_bn_relu_avgpool2_ndhwc(const void* x, int ldx, void* y, int ldy, int N, int H, int W, int C, const float* scale, const float* shift,
+                              void* stream);
+/* b2_avgpool_global_ndhwc with relu(scale[c] * x + shift[c]) applied to every element before the sum (DenseNet's norm5 + ReLU +
+ * 7x7 mean, torchvision_models.py:262-264): fp32 accumulation, one fp16 rounding.  scale / shift fp32 [C].
+ * b2_debug_last_kernel: KID 14, info = {4}. */
+int b2_avgpool_global_affine_ndhwc(const void* x, void* y, int N, int S, int C, const float* scale, const float* shift, void* stream);
 
 #ifdef __cplusplus
 }

@@ -128,11 +128,13 @@ __global__ void conv_simt_kernel(SimtConvParams p, long long total) {
 // count_include_pad=True: an fp32 sum over the taps in (dt, dh, dw) order (taps in the padding read zero), divided by the
 // window clipped to the padded input (the full window except where a ceil-mode window runs past the padding), one fp16 rounding.
 // MODE 3: the same sum divided by the taps inside the input (count_include_pad=False, the pool branches of Inception-v4 /
-// Inception-ResNet-v2).
+// Inception-ResNet-v2).  MODE 4: MODE 2 with relu(scale[c] * x + shift[c]) applied to every tap before the sum (a DenseNet
+// transition's BatchNorm + ReLU ahead of its 2x2 average; its windows have no padding, so the divisor is the window).
 template <int MODE>
 __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restrict__ y, int N, int T, int H, int W,
                                  int C8, int To, int Ho, int Wo, int kt, int kh, int kw, int st, int sh, int sw, int pt,
-                                 int ph, int pw, long long total, int ldx = 0, int ldy = 0) {
+                                 int ph, int pw, long long total, int ldx = 0, int ldy = 0, const float* __restrict__ scale = nullptr,
+                                 const float* __restrict__ shift = nullptr) {
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int c8 = (int)(i % C8);
@@ -143,6 +145,11 @@ __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restric
   const int n = (int)(q / To);
   if constexpr (MODE >= 2) {
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    float sc[8], sf[8];
+    if constexpr (MODE == 4) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { sc[e] = __ldg(scale + c8 * 8 + e); sf[e] = __ldg(shift + c8 * 8 + e); }
+    }
     for (int dt = 0; dt < kt; ++dt) {
       const int ti = to * st - pt + dt;
       if ((unsigned)ti >= (unsigned)T) continue;
@@ -157,14 +164,19 @@ __global__ void maxpool3d_kernel(const __half* __restrict__ x, __half* __restric
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&u[e]));
-            acc[2 * e] += f.x;
-            acc[2 * e + 1] += f.y;
+            if constexpr (MODE == 4) {
+              acc[2 * e] += fmaxf(fmaf(f.x, sc[2 * e], sf[2 * e]), 0.f);
+              acc[2 * e + 1] += fmaxf(fmaf(f.y, sc[2 * e + 1], sf[2 * e + 1]), 0.f);
+            } else {
+              acc[2 * e] += f.x;
+              acc[2 * e + 1] += f.y;
+            }
           }
         }
       }
     }
     const int t0 = to * st - pt, h0 = ho * sh - ph, w0 = wo * sw - pw;
-    const int div = MODE == 2 ? (min(t0 + kt, T + pt) - t0) * (min(h0 + kh, H + ph) - h0) * (min(w0 + kw, W + pw) - w0)
+    const int div = MODE != 3 ? (min(t0 + kt, T + pt) - t0) * (min(h0 + kh, H + ph) - h0) * (min(w0 + kw, W + pw) - w0)
                               : (min(t0 + kt, T) - max(t0, 0)) * (min(h0 + kh, H) - max(h0, 0)) * (min(w0 + kw, W) - max(w0, 0));
     uint4 o;
     uint32_t* op = reinterpret_cast<uint32_t*>(&o);
@@ -289,13 +301,21 @@ maxpool3d_k331s221_kernel(const __half* __restrict__ x, __half* __restrict__ y, 
 
 // global average: grid (C8 chunks / 32, N), 1024 threads.  Lane = one 8-channel chunk (a warp reads 512 contiguous
 // bytes of a pixel), warp w walks positions w, w+32, ... ; the 32 partial sums meet in shared memory in a fixed order.
-__global__ void __launch_bounds__(1024) avgpool_kernel(const __half* __restrict__ x, __half* __restrict__ y, int S, int C8) {
+// AFF = 1: relu(scale[c] * x + shift[c]) per element before the sum (b2_avgpool_global_affine_ndhwc: DenseNet's norm5 + ReLU).
+template <int AFF>
+__global__ void __launch_bounds__(1024) avgpool_kernel(const __half* __restrict__ x, __half* __restrict__ y, int S, int C8,
+                                                       const float* __restrict__ scale = nullptr, const float* __restrict__ shift = nullptr) {
   __shared__ float part[32][32][9];                 // [slice][lane][8 + pad]
   const int lane = threadIdx.x & 31, slice = threadIdx.x >> 5;
   const int c8 = blockIdx.x * 32 + lane;
   const int n = blockIdx.y;
   float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   if (c8 < C8) {
+    float sc[8], sf[8];
+    if constexpr (AFF) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { sc[e] = __ldg(scale + c8 * 8 + e); sf[e] = __ldg(shift + c8 * 8 + e); }
+    }
     const uint4* base = reinterpret_cast<const uint4*>(x + (size_t)n * S * (C8 * 8)) + c8;
 #pragma unroll 4
     for (int s = slice; s < S; s += 32) {
@@ -303,7 +323,11 @@ __global__ void __launch_bounds__(1024) avgpool_kernel(const __half* __restrict_
       const uint32_t u[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&u[e]));
+        float2 f = __half22float2(*reinterpret_cast<const __half2*>(&u[e]));
+        if constexpr (AFF) {
+          f.x = fmaxf(fmaf(f.x, sc[2 * e], sf[2 * e]), 0.f);
+          f.y = fmaxf(fmaf(f.y, sc[2 * e + 1], sf[2 * e + 1]), 0.f);
+        }
         acc[2 * e] += f.x; acc[2 * e + 1] += f.y;
       }
     }
@@ -712,8 +736,35 @@ int b2_avgpool_global_ndhwc(const void* x, void* y, int N, int S, int C, void* s
   B2_CHECK_ARG(x && y && N > 0 && S > 0, "bad argument");
   B2_CHECK_ARG(C % 8 == 0, "channel pitch %d is not a multiple of 8", C);
   dim3 grid(div_up(C / 8, 32), N);
-  avgpool_kernel<<<grid, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>((const __half*)x, (__half*)y, S, C / 8);
+  avgpool_kernel<0><<<grid, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>((const __half*)x, (__half*)y, S, C / 8);
   B2_CHECK_LAUNCH("avgpool");
+  return B2_OK;
+}
+
+int b2_avgpool_global_affine_ndhwc(const void* x, void* y, int N, int S, int C, const float* scale, const float* shift, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(x && y && scale && shift && N > 0 && S > 0 && C > 0, "bad argument");
+  B2_CHECK_ARG(C % 8 == 0, "channel pitch %d is not a multiple of 8", C);
+  dim3 grid(div_up(C / 8, 32), N);
+  avgpool_kernel<1><<<grid, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>((const __half*)x, (__half*)y, S, C / 8, scale, shift);
+  B2_CHECK_LAUNCH("avgpool");
+  set_last_kernel(KID_POOL, 4);
+  return B2_OK;
+}
+
+int b2_bn_relu_avgpool2_ndhwc(const void* x, int ldx, void* y, int ldy, int N, int H, int W, int C, const float* scale, const float* shift,
+                              void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(x && y && scale && shift && N > 0 && H >= 2 && W >= 2 && C > 0, "bad argument (the 2x2 window needs H, W >= 2)");
+  B2_CHECK_ARG(C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0 && ldx >= C && ldy >= C,
+               "channels %d, input pitch %d and output pitch %d must be multiples of 8 with both pitches >= the channels", C, ldx, ldy);
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "input / output slice not 16-byte aligned");
+  const int Ho = H / 2, Wo = W / 2;
+  const long long total = (long long)N * Ho * Wo * (C / 8);
+  maxpool3d_kernel<4><<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      (const __half*)x, (__half*)y, N, 1, H, W, C / 8, 1, Ho, Wo, 1, 2, 2, 1, 2, 2, 0, 0, 0, total, ldx, ldy, scale, shift);
+  B2_CHECK_LAUNCH("maxpool3d");
+  set_last_kernel(KID_POOL, 3);
   return B2_OK;
 }
 

@@ -300,7 +300,7 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.MT = MT;
   if (MT * BN > kSlabAccCols)
     return set_error(B2_ERR_INVALID, "slab plan MT=%d x N=%d exceeds the %d register accumulator columns", MT, BN, kSlabAccCols);
-  if (!BNT && BN != 16 && (BN < 144 || BN > kSlabAccCols || BN % 16 != 0))
+  if (!BNT && BN != 16 && BN != 32 && BN != 48 && (BN < 144 || BN > kSlabAccCols || BN % 16 != 0))
     return set_error(B2_ERR_INVALID, "slab runtime N tile %d is not one of the compiled widths", BN);
   p.Ncols = a->K;
   p.scale = a->scale; p.shift = a->shift;
@@ -347,8 +347,9 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
 // when no configuration fits in shared memory.
 // G != 0 (grouped convolution): the N tiles are the K / 64 channel slices, each with a G-row weight stage per tap.
 // allow_flex = false: fixed 64 / 128 tiles only (the slice path's retry when the runtime-N tile finds no fit).
+// narrow = 32 / 48 (b2_conv_ndhwc_fprop_slice_narrow, a->ldy == narrow): one runtime N tile of exactly the output width.
 static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out, bool* flex_out, int* best_mt_out, int* best_R_out,
-                              int G = 0, bool allow_flex = true) {
+                              int G = 0, bool allow_flex = true, int narrow = 0) {
   int BN = (G || a->ldy <= 64) ? 64 : 128;
   const int planes = a->N * p.To;
   int ntn = G ? a->K / 64 : (a->ldy + BN - 1) / BN;
@@ -356,6 +357,9 @@ static double slab_pick_tiles(const b2_conv_args* a, SlabParams& p, int* BN_out,
   // tiles of <= 256 columns, each a multiple of 16 wide.
   bool flex = false;
   if (G) {
+  } else if (narrow) {
+    flex = true; BN = narrow; ntn = 1;
+    p.bn = narrow; p.wbytes = (narrow * 128 + 1023) / 1024 * 1024; p.accs = (narrow + 31) / 32 * 32;
   } else if (a->ldy > 128 && allow_flex) {
     const int tn = (a->ldy + 255) / 256;
     const int bn = (((a->ldy + tn - 1) / tn) + 15) / 16 * 16;
@@ -438,7 +442,7 @@ struct SlabChoice {
   int BN, MT, R;
   bool flex;
 };
-static bool slab_choose(const b2_conv_args* a, int wc_hint, int G, int ldo, SlabChoice* c) {
+static bool slab_choose(const b2_conv_args* a, int wc_hint, int G, int ldo, SlabChoice* c, int narrow = 0) {
   // W chunking candidates: the default (whole rows, or <= 256-pixel chunks) and narrower chunks.  Narrow chunks make the
   // slab of a work item shorter, which (a) lets 256-pixel rows fit the two slab stages at all and (b) admits more M tiles
   // per item for wide images -- with few-tap 2-D filters the per-item costs (decode, epilogue set-up, slab latency) are
@@ -456,8 +460,8 @@ static bool slab_choose(const b2_conv_args* a, int wc_hint, int G, int ldo, Slab
     int bn_c = 0, mt_c = 0, r_c = 0;
     bool flex_c = false;
     const SlabParams q0 = q;
-    double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G);
-    if (mt_c == 0 && ldo && flex_c) {
+    double cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G, true, narrow);
+    if (mt_c == 0 && ldo && flex_c && !narrow) {
       // a slice has no other kernel to fall back on: when the wide runtime-N tile does not fit, take 128-column tiles
       q = q0;
       cost = slab_pick_tiles(a, q, &bn_c, &flex_c, &mt_c, &r_c, G, false);
@@ -623,7 +627,8 @@ static int launch_slab_t(const b2_conv_args* a, TPlan& t, cudaStream_t stream) {
 // returns 1 when the slab kernel (or one of its transposed forms) took the convolution, 0 when it does not apply, <0 on error
 // G != 0: grouped convolution inside the contract of b2_conv_grouped_ndhwc_fprop (3x3 in plane, so never the temporal remap)
 // ldo > 0: column-slice output, see launch_slab
-static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, int ldo = 0) {
+// narrow: see slab_pick_tiles
+static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, int ldo = 0, int narrow = 0) {
   if (g_conv_algo == 1 && !G && !ldo) return 0;
   b2_conv_args remap = *a_in;
   const b2_conv_args* a = a_in;
@@ -638,7 +643,7 @@ static int try_slab(const b2_conv_args* a_in, cudaStream_t stream, int G = 0, in
     wc_hint = 64;
   }
   SlabChoice c;
-  if (!slab_choose(a, wc_hint, G, ldo, &c)) return 0;
+  if (!slab_choose(a, wc_hint, G, ldo, &c, narrow)) return 0;
   if (!G && !ldo) {
     TPlan t;
     if (slab_t128_wanted(a, c, &t)) {
@@ -1178,7 +1183,7 @@ int b2_debug_set_gemm_algo(int algo) { g_gemm_algo = algo; return B2_OK; }
 /* host-only view of the slab kernel's tiling decision for a convolution (no launch, no GPU needed): out = {applies, BN, MT, R, PW,
    WC, wchunks, items, flex, remapped}.  Used by tests/test_host_logic.py and by tuning scripts.  slice != 0: the plan of
    b2_conv_ndhwc_fprop_slice (a->ldy the slice width), which takes 128-column tiles where the runtime-N tile finds no fit. */
-static int slab_plan_view(const b2_conv_args* a_in, int* out, bool slice) {
+static int slab_plan_view(const b2_conv_args* a_in, int* out, bool slice, int narrow = 0) {
   b2_conv_args remap = *a_in;
   const b2_conv_args* a = a_in;
   int wc_hint = 0, remapped = 0;
@@ -1188,7 +1193,7 @@ static int slab_plan_view(const b2_conv_args* a_in, int* out, bool slice) {
   }
   SlabChoice c;
   memset(&c, 0, sizeof(c));
-  const bool ok = slab_choose(a, wc_hint, 0, slice ? 1 : 0, &c);   // the launchers' own planner (ldo only selects the slice rules)
+  const bool ok = slab_choose(a, wc_hint, 0, slice ? 1 : 0, &c, narrow);   // the launchers' own planner (ldo only selects the slice rules)
   const int BN = ok ? c.BN : 0, best_mt = ok ? c.MT : 0;
   out[0] = ok; out[1] = BN; out[2] = best_mt; out[3] = ok ? c.R : 0; out[4] = c.p.PW; out[5] = c.p.WC; out[6] = c.p.wchunks;
   const long long tq = best_mt ? (c.p.P + best_mt * 128 - 1) / (best_mt * 128) : 0;
@@ -1198,6 +1203,8 @@ static int slab_plan_view(const b2_conv_args* a_in, int* out, bool slice) {
 }
 int b2_debug_slab_plan(const b2_conv_args* a_in, int* out) { return slab_plan_view(a_in, out, false); }
 int b2_debug_slab_slice_plan(const b2_conv_args* a_in, int* out) { return slab_plan_view(a_in, out, true); }
+/* the plan of b2_conv_ndhwc_fprop_slice_narrow (a->ldy = a->K = 32 or 48) */
+int b2_debug_slab_slice_narrow_plan(const b2_conv_args* a_in, int* out) { return slab_plan_view(a_in, out, true, a_in->K); }
 /* debug knobs of the small-M path: layers with M <= maxm take the dense-M kernel (0 = never); force_s > 0 caps the cluster size */
 int b2_debug_set_slab_wide(int on) { g_slab_wide = on; return B2_OK; }   /* 1: request 256-column tiles; -1 / 0: the rule */
 /* host-only view of the temporal stack kernel's decision for a convolution (no launch, no GPU needed): out = {applies, items, frame
@@ -1574,6 +1581,41 @@ static int gemm_common(const b2_gemm_args* g, const void* a2, int lda2, const vo
   return dispatch_igemm(L, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int b2_gemm_preact_f16(const b2_gemm_args* g, const float* in_scale, const float* in_shift, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(g != nullptr && g->a && g->b && g->scale && g->shift && g->d && in_scale && in_shift, "null tensor pointer");
+  B2_CHECK_ARG(g->M > 0 && g->N > 0 && g->Kd > 0 && g->Kd % 8 == 0, "non-positive dimension or Kd %d not a multiple of 8", g->Kd);
+  B2_CHECK_ARG(g->lda % 8 == 0 && g->ldb % 8 == 0 && g->lda >= g->Kd && g->ldb >= g->Kd, "bad operand pitch");
+  B2_CHECK_ARG(g->ldd % 8 == 0 && g->ldd >= g->N, "bad output pitch %d", g->ldd);
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(in_scale) & 15) == 0 && (reinterpret_cast<uintptr_t>(in_shift) & 15) == 0,
+               "in_scale / in_shift must be 16-byte aligned fp32 arrays of round_up(Kd, 64) entries");
+  B2_CHECK_ARG(!g->residual && !g->ldr && !g->per_row && !g->out_f32 && !g->accumulate && !g->aff_ld && !g->aff_rows && !g->d2 && !g->mask,
+               "the pre-activated GEMM takes fp16 output with a per-column affine: residual, per_row, out_f32, accumulate, aff_ld, d2 "
+               "and mask must be zero");
+  if (g_gemm_algo != 0) return set_error(B2_ERR_UNSUPPORTED, "the pre-activated GEMM needs the persistent kernel");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  IgemmLaunch L;
+  memset(&L, 0, sizeof(L));
+  IgemmParams& p = L.p;
+  p.amode = AMODE_TMA;
+  p.M_total = g->M;
+  p.Ncols = g->N;
+  p.nkb = (g->Kd + kBK - 1) / kBK;
+  p.scale = g->scale; p.shift = g->shift;
+  p.y = g->d; p.ldy = g->ldd;
+  p.relu = g->relu;
+  p.epi = EPI_TMA_F16;
+  // one per-channel row for every tile: in_ld = 0 makes the transform warps' row offset (m0 / in_rows) * in_ld zero
+  p.in_scale = in_scale; p.in_shift = in_shift; p.in_ld = 0; p.in_rows = 128;
+  p.x = reinterpret_cast<const __half*>(g->a);
+  L.a_mat = g->a; L.lda = g->lda; L.a_cols = g->Kd;
+  L.w = g->b; L.ldb = g->ldb; L.b_cols = g->Kd;
+  g_last_gemm_path = 2;
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return g->ldd <= 64 ? launch_pgemm<64, 1>(L, st) : launch_pgemm<128, 1>(L, st);
+}
+
 int b2_gemm_split_plan(int nd, const int* cols, int* box0) {
   B2_CHECK_ARG(nd >= 1 && nd <= 4 && cols && box0, "a split GEMM has 1 to 4 destinations (got %d)", nd);
   box0[0] = 0;
@@ -1609,7 +1651,7 @@ int b2_gemm_split_f16(const b2_gemm_args* g, int nd, void* const* y, const int* 
   return Npad <= 64 ? launch_pgemm_split<64>(g, nd, y, ldy, cols, box0, st) : launch_pgemm_split<128>(g, nd, y, ldy, cols, box0, st);
 }
 
-int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream) {
+static int conv_slice(const b2_conv_args* a, void* stream, int narrow) {
   set_last_kernel(KID_NONE);
   int rc = validate_conv(a);
   if (rc != B2_OK) return rc;
@@ -1624,15 +1666,26 @@ int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream) {
                "(k - 1) / 2 per axis and stride 1 or 2 (got %dx%dx%d, stride %d%d%d, padding %d%d%d)",
                kSlabMaxTaps, a->kt, a->kh, a->kw, a->st, a->sh, a->sw, a->pt, a->ph, a->pw);
   B2_CHECK_ARG(a->K % 8 == 0, "slice width K %d is not a multiple of 8", a->K);
+  B2_CHECK_ARG(!narrow || a->K == narrow, "the narrow slice convolution takes K = 32 or 48 output channels (got %d)", a->K);
   B2_CHECK_ARG((reinterpret_cast<uintptr_t>(a->y) & 15) == 0, "slice start is not 16-byte aligned");
   if ((rc = require_sm90()) != B2_OK) return rc;
   g_last_conv_path = 0;
   g_last_gemm_path = 0;
   b2_conv_args s = *a;
   s.ldy = a->K;                         // the slab planner and epilogue see the slice width; ldo carries the row pitch
-  rc = try_slab(&s, reinterpret_cast<cudaStream_t>(stream), 0, a->ldy);
+  rc = try_slab(&s, reinterpret_cast<cudaStream_t>(stream), 0, a->ldy, narrow);
   if (rc == 0) return set_error(B2_ERR_UNSUPPORTED, "no slab tiling of this image fits in shared memory (H=%d W=%d)", a->H, a->W);
   return rc < 0 ? rc : B2_OK;
+}
+
+int b2_conv_ndhwc_fprop_slice(const b2_conv_args* a, void* stream) { return conv_slice(a, stream, 0); }
+
+int b2_conv_ndhwc_fprop_slice_narrow(const b2_conv_args* a, void* stream) {
+  if (a != nullptr && a->K != 32 && a->K != 48) {
+    set_last_kernel(KID_NONE);
+    return set_error(B2_ERR_INVALID, "the narrow slice convolution takes K = 32 or 48 output channels (got %d)", a->K);
+  }
+  return conv_slice(a, stream, a ? a->K : 0);
 }
 
 }  // extern "C"

@@ -79,7 +79,7 @@ enum LastKernel : int {
   KID_SIMT = 8, KID_ATTENTION = 9, KID_GROUPCONV = 10, KID_PGEMM_CHAIN = 11,
   KID_PGEMM_SPLIT = 12 /* b2_gemm_split_f16: info = {BN, destinations, packed columns} */,
   KID_SLAB_SLICE = 13 /* b2_conv_ndhwc_fprop_slice: info as KID_SLAB */,
-  KID_POOL = 14 /* b2_pool_ndhwc_slice: info = {average} */,
+  KID_POOL = 14 /* b2_pool_ndhwc_slice: info = {average}; 2 exclude-pad, 3 DenseNet transition, 4 global mean with affine */,
   KID_SLAB_T128 = 15 /* the slab kernel's 128-wide transposed form (b2_slab_t128.cuh): info = {NP, rows per item, 128, stride, R} */,
   KID_SLAB_T64 = 16 /* the slab kernel's 64-wide transposed form (b2_slab_t128.cuh): info = {NP, items, R} */
 };

@@ -269,6 +269,19 @@ __device__ __forceinline__ void wgmma_ss(float* d, uint64_t a, uint64_t b);
 template <>
 __device__ __forceinline__ void wgmma_ss<16>(float* d, uint64_t a, uint64_t b) { wgmma_n16<0>(*reinterpret_cast<float(*)[8]>(d), a, b); }
 template <>
+__device__ __forceinline__ void wgmma_ss<32>(float* d, uint64_t a, uint64_t b) { wgmma_n32<0>(*reinterpret_cast<float(*)[16]>(d), a, b); }
+// N = 32 / 48: the growth-rate outputs of a dense layer (slab kernel, DenseNet)
+template <>
+__device__ __forceinline__ void wgmma_ss<48>(float* d, uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, 1, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(a), "l"(b));
+}
+template <>
 __device__ __forceinline__ void wgmma_ss<64>(float* d, uint64_t a, uint64_t b) { wgmma_n64<0>(*reinterpret_cast<float(*)[32]>(d), a, b); }
 // N = 112: one whole 112-column output row of the transposed stem (positions along N)
 template <>

@@ -68,7 +68,8 @@ struct SlabParams {
   int slab_bytes;          // R * PW * 128, rounded up to 1024
   int MT;                  // M tiles per work item (MT * N tile <= kSlabAccCols)
   // runtime N tile (slabconv_kernel<0> only; the <64>/<128> instances use their template value): Cout = 144, 288,
-  // 576 ... of the (2+1)D factorisation would waste up to 44% of the MMA columns on 128-wide tiles
+  // 576 ... of the (2+1)D factorisation would waste up to 44% of the MMA columns on 128-wide tiles; N = 32 / 48 for the
+  // growth-rate outputs of a dense layer (b2_conv_ndhwc_fprop_slice_narrow), which a 64-wide tile half / a quarter pads
   int bn;                  // N per MMA / per tile, multiple of 16, <= 256
   int wbytes;              // weight stage stride in smem: bn * 128 rounded up to 1024
   int accs;                // accumulator column stride between the MT accumulators: bn rounded up to 32
@@ -403,7 +404,7 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
       // runtime N: one compiled main loop per width the tile planner can pick (launch_slab rejects any other)
       switch (bn) {
 #define B2_SLAB_N(n) case n: slab_consumer<n, 0>(p, at, accs, slab0, w0s, kWBytes, slab_full, slab_empty, w_full, w_empty, acc_full, acc_empty); break;
-        B2_SLAB_N(16) B2_SLAB_N(144) B2_SLAB_N(160) B2_SLAB_N(176) B2_SLAB_N(192)
+        B2_SLAB_N(16) B2_SLAB_N(32) B2_SLAB_N(48) B2_SLAB_N(144) B2_SLAB_N(160) B2_SLAB_N(176) B2_SLAB_N(192)
 #undef B2_SLAB_N
         default: __trap();
       }

@@ -956,6 +956,144 @@ def run_inception_trunk(n_stem, units, x):
 
 
 # ---------------------------------------------------------------------------------------------
+# DenseNet (torchvision densenet.py behind torchvision_models.py:254-380)
+# ---------------------------------------------------------------------------------------------
+# Each dense block owns one fp16 [M][C_final] matrix.  Its first C0 columns are written by the stem's pool (first block) or the
+# previous transition's GEMM; layer L reads columns [0, C_L) and writes [C_L, C_L + k): every column is written before it is
+# read, so the concatenations of torchvision's forward are never materialised and no memset is needed.
+def _bn_affine(bn, width=None):
+    """Folded eval-mode affine of ``bn`` as fp32 [width] arrays, zero past bn.num_features (cached on ``bn``)."""
+    C = bn.num_features
+    width = C if width is None else width
+
+    def build():
+        s, t = ops.fold_affine(C, None, bn, bn.running_mean.device)
+        sp = torch.zeros(width, dtype=torch.float32, device=s.device)
+        tp = torch.zeros(width, dtype=torch.float32, device=s.device)
+        sp[:C], tp[:C] = s, t
+        return sp, tp
+    return _cached(bn, "dense_aff%d" % width, _sig(*_bn_tensors(bn)) + (width,), build)
+
+
+def _dense_layer_pack(layer):
+    """conv1 of a dense layer as fp16 [4k][C_L], its norm1 affine padded with zeros to whole 64-column K blocks (the A transform
+    of b2_gemm_preact_f16) and its norm2 affine (the epilogue)."""
+    conv = layer.conv1
+    C_L = conv.in_channels
+
+    def build():
+        s1, t1 = ops.fold_affine(C_L, None, layer.norm1, conv.weight.device)
+        kpad = ops._round_up(C_L, 64)
+        s1p = torch.zeros(kpad, dtype=torch.float32, device=s1.device)
+        t1p = torch.zeros(kpad, dtype=torch.float32, device=s1.device)
+        s1p[:C_L], t1p[:C_L] = s1, t1
+        s2, t2 = ops.fold_affine(conv.out_channels, None, layer.norm2, conv.weight.device)
+        return _conv1x1_matrix(conv).to(torch.float16).contiguous(), s1p, t1p, s2, t2
+    reads = _bn_tensors(layer.norm1) + _bn_tensors(layer.norm2)
+    return _cached(conv, "preact", _sig(conv.weight, *reads), build, reads=reads)
+
+
+# Growth-rate 3x3 convolutions (4k -> k) that run on an N tile exactly k wide (b2_conv_ndhwc_fprop_slice_narrow) instead of the
+# 64-wide one: the (k, map size) pairs where the narrow tile measured faster at both 32 and 256 images (the 7x7 maps of the last
+# block; at 14 - 56 the 64-wide tile is as fast or faster at 256 images, DESIGN section 5).  Both give bitwise the same output.
+_NARROW_GROWTH = frozenset({(32, 7), (48, 7)})
+
+
+def _dense_layer(layer, blk):
+    """One _DenseLayer (densenet.py: norm1 -> relu1 -> conv1 -> norm2 -> relu2 -> conv2) on the block matrix ``blk`` (an Act
+    whose C is the block's final width): conv1 reads columns [0, C_L) through the pre-activated GEMM, with norm2 + ReLU in its
+    epilogue; conv2 (3x3, no affine) writes its k columns [C_L, C_L + k) in place."""
+    C_L, k = layer.conv1.in_channels, layer.conv2.out_channels
+    if tuple(layer.conv1.kernel_size) != (1, 1) or tuple(layer.conv2.kernel_size) != (3, 3) or tuple(layer.conv2.padding) != (1, 1):
+        raise NotImplementedError("dense layers are 1x1 -> 3x3 'same' convolutions")
+    if C_L % 8 or k % 8:
+        raise NotImplementedError("dense layers need input widths and a growth rate that are multiples of 8 (got %d, %d)" % (C_L, k))
+    w1, s1, t1, s2, t2 = _dense_layer_pack(layer)
+    K1 = w1.shape[0]
+    h = ops.gemm_preact(blk.data, w1, s2, t2, s1, t1, blk.M, K1, C_L, relu=True)
+    pc = packed_conv(layer.conv2, None, h.shape[1])
+    ops.conv_slice(Act(h, blk.N, 1, blk.H, blk.W, K1), pc, blk.data[:, C_L:C_L + k], relu=False, narrow=(k, blk.H) in _NARROW_GROWTH)
+
+
+def _dense_transition(tr, blk, y):
+    """_Transition (densenet.py: norm -> relu -> conv 1x1 -> AvgPool2d(2, 2)) as norm + ReLU + pool in one pass, then the 1x1
+    convolution on a quarter of the positions, written into the slice ``y`` (the next block's first C / 2 columns).  The pool and
+    the bias-free 1x1 convolution are both linear, so pooling first is exact in real arithmetic."""
+    s, t = _bn_affine(tr.norm)
+    pooled = ops.bn_relu_avgpool2(blk, s, t)
+    w, scale, shift = _split_pack_convs([tr.conv], [None], pooled.ld)
+    ops.gemm_split(pooled.data, w, scale, shift, pooled.M, pooled.ld, [y], relu=False)
+
+
+def _dense_stem(features, a, y):
+    """conv0 -> norm0 -> relu0 on the stem kernel, pool0 (MaxPool2d(3, 2, 1)) into the slice ``y`` (the first block's first
+    columns).  On the stem kernel's pooled-W path the convolution takes the pool's W direction in its epilogue."""
+    conv = features.conv0
+    if (a.ld == 4 and _is_stem_shape(conv) and ops._out_dim(a.W, 7, 2, 3) <= 120 and a.W % 2 == 0
+            and os.environ.get("B2_STEM_POOLW", "1") != "0"):
+        h = conv_bn_act(conv, features.norm0, a, relu=True, pool_w=True)
+        return ops.pool_slice(h, (3, 1), (2, 1), (1, 0), False, y, ceil_mode=False)
+    h = conv_bn_act(conv, features.norm0, a, relu=True)
+    return ops.pool_slice(h, 3, 2, 1, False, y, ceil_mode=False)
+
+
+def _densenet_trunk_body(features, a):
+    """The DenseNet trunk up to the last block's output (norm5 not applied): fp16 NDHWC4 images in, an Act out."""
+    mods = features._modules
+    blocks = [m for n, m in mods.items() if n.startswith('denseblock')]
+    trans = [m for n, m in mods.items() if n.startswith('transition')]
+    pool = features.pool0
+    if not (isinstance(pool, nn.MaxPool2d) and _pool_args(pool) == ((1, 3, 3), (1, 2, 2), (0, 1, 1)) and not pool.ceil_mode):
+        raise NotImplementedError("DenseNet's pool0 is MaxPool2d(3, stride=2, padding=1)")
+    dev = a.data.device
+    C = features.conv0.out_channels
+    H, W = ops._out_dim(a.H, 7, 2, 3), ops._out_dim(a.W, 7, 2, 3)
+    H, W = ops._out_dim(H, 3, 2, 1), ops._out_dim(W, 3, 2, 1)
+    y = None
+    for i, block in enumerate(blocks):
+        layers = list(block.children())
+        Cf = C + sum(l.conv2.out_channels for l in layers)
+        blk = Act(torch.empty((a.N * H * W, Cf), dtype=torch.float16, device=dev), a.N, 1, H, W, Cf)
+        if i == 0:
+            _dense_stem(features, a, blk.data[:, :C])
+        else:
+            _dense_transition(trans[i - 1], y, blk.data[:, :C])
+        for layer in layers:
+            _dense_layer(layer, blk)
+        y = blk
+        if i < len(trans):
+            C, H, W = trans[i].conv.out_channels, H // 2, W // 2
+    return y
+
+
+def run_densenet_trunk(features, x):
+    """DenseNet ``features`` up to norm5 through its Function: fp32 NCHW images (or an NDHWC4 Act) in, the last dense block's
+    output (an Act, norm5 not applied) out."""
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x)
+    return Fn.DenseNetTrunkFunction.run(features, a)
+
+
+def densenet_norm5(features, a):
+    """norm5 of the last block's output as an Act (``features()``'s tensor; off the hot path: the head applies it in its pool)."""
+    s, t = _bn_affine(features.norm5, a.ld)
+    return ops.ccbn_act(a, s.view(1, -1), t.view(1, -1), relu=False)
+
+
+def run_densenet_head(model, a, bn=None):
+    """relu(bn(x)) -> 7x7 mean -> view -> last_linear (torchvision_models.py:262-266) on the last block's output ``a``: the
+    affine (norm5, or none when ``a`` already holds features()'s tensor) and the ReLU are applied inside the pool."""
+    if (a.T, a.H, a.W) != (1, 7, 7):
+        raise NotImplementedError("DenseNet's logits take F.avg_pool2d(kernel_size=7, stride=1) of a 7x7 final map (224x224 inputs), "
+                                  "got %dx%d" % (a.H, a.W))
+    if bn is None:
+        s = torch.ones(a.ld, dtype=torch.float32, device=a.data.device)
+        t = torch.zeros(a.ld, dtype=torch.float32, device=a.data.device)
+    else:
+        s, t = _bn_affine(bn, a.ld)
+    return _head_on_pooled(model.last_linear, ops.avgpool_global_affine(a, s, t), a.C)
+
+
+# ---------------------------------------------------------------------------------------------
 # stem / trunk / head
 # ---------------------------------------------------------------------------------------------
 def _pool_args(mp):
@@ -1298,7 +1436,11 @@ def run_head(model, a, head):
         # fine-tuning: fp32 pooled features, so that the head's input gradient reaches the pool backward unrounded
         pooled = Fn.FineTunePoolFunction.apply(a.data, (a.N, a.T, a.H, a.W, a.C), a.loss_scale)
         return Fn.linear(pooled, head.weight, head.bias) if isinstance(head, nn.Linear) else head(pooled)
-    pooled = ops.avgpool_global(a)                     # fp16 [N][ld]
+    return _head_on_pooled(head, ops.avgpool_global(a), a.C)
+
+
+def _head_on_pooled(head, pooled, C):
+    """``head`` on the fp16 pooled features [N][ld] (``C`` of them used) -> fp32 [N][classes]."""
     if isinstance(head, nn.Linear) and torch.is_grad_enabled() and any(p.requires_grad for p in head.parameters()):
         # trainable head on frozen engine features: differentiable GEMM (functions.LinearFunction), same kernel
         return Fn.linear(pooled[:, :head.in_features], head.weight, head.bias)
@@ -1306,4 +1448,4 @@ def run_head(model, a, head):
         pl = _cached(head, "pl", _sig(head.weight, head.bias), lambda: ops.PackedLinear(head.weight, head.bias))
         return ops.linear(pooled, pl, out_f32=True)
     # user-swapped head (Identity, Dropout, custom module): hand it the pooled features like the reference does
-    return head(pooled[:, :a.C].float())
+    return head(pooled[:, :C].float())

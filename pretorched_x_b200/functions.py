@@ -186,6 +186,16 @@ class InceptionBlockFunction(_FrozenFunction):
         return InceptionBlockFunction._finish(ctx, engine._inception_block_body(block, Act(x2d, *geom), out))
 
 
+class DenseNetTrunkFunction(_FrozenFunction):
+    """The DenseNet trunk up to norm5 (torchvision densenet.py ``features`` without its last BatchNorm): every dense block as one
+    matrix that its layers and the preceding transition (or the stem's pool) write in place."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, features):
+        from . import engine
+        return DenseNetTrunkFunction._finish(ctx, engine._densenet_trunk_body(features, Act(x2d, *geom)))
+
+
 class GBlockFunction(_FrozenFunction):
     """BigGAN-deep GBlock: ccbn-ReLU-1x1 -> ccbn-ReLU-[up]-3x3 -> ccbn-ReLU-3x3 -> ccbn-ReLU-1x1 (+ skip)."""
 

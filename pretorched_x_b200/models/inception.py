@@ -14,6 +14,7 @@ import torch.nn as nn
 from .. import engine, ops
 from ..ops import Act
 from .resnet3d import _attach_settings
+from .utils import Trunk
 
 __all__ = ['InceptionV4', 'inceptionv4', 'InceptionResNetV2', 'inceptionresnetv2']
 
@@ -219,27 +220,13 @@ for _k in BRANCHES:
     globals()[_k].kind = _k
 
 
-class _Trunk(nn.Sequential):
-    """``InceptionV4.features`` (inceptionv4.py:273-296): the reference's Sequential, so its keys are ``features.<i>.*``.  Calling
-    it runs the whole trunk on the engine and returns fp32 NCHW [B, 1536, 8, 8] for 299x299 inputs.  A slice (``features[a:b]``) is
-    a ``_Trunk`` too and refuses to run: the engine runs the trunk whole, never a part of it."""
+class _Trunk(Trunk):
+    """``InceptionV4.features`` (inceptionv4.py:273-296): the reference's Sequential.  Returns fp32 NCHW [B, 1536, 8, 8] for
+    299x299 inputs."""
 
-    _partial = False
+    _model = 'InceptionV4'
 
-    def __getitem__(self, idx):
-        out = super().__getitem__(idx)
-        if isinstance(idx, slice):
-            out._partial = True
-        return out
-
-    def forward(self, input):
-        return ops.to_ncdhw(self.run_act(input)).squeeze(2)
-
-    def run_act(self, x):
-        if self._partial:
-            raise NotImplementedError("InceptionV4.features[a:b] does not run on the engine: only the whole trunk does")
-        if self.training:
-            raise RuntimeError("the forward engine is inference-only: call model.eval() first")
+    def _run(self, x):
         return engine.run_inception_trunk(V4_STEM, list(self), x)
 
 

@@ -566,10 +566,11 @@ def gemm_split(a2d, b2d, scale, shift, M, Kd, dests, relu=True):
 
 
 @_on_device
-def conv_slice(a, pc, y, relu=True):
+def conv_slice(a, pc, y, relu=True, narrow=False):
     """``conv`` of a 2-D filter with taps (3x3, 1x7, 7x1, 5x5 ...; stride 1 or 2; padding from 0 to "same") whose output is the
     column slice ``y`` (an fp16 [M][K] view of a wider matrix, or a whole [M][K] matrix): b2_conv_ndhwc_fprop_slice writes columns
-    [0, K) of each row and nothing else, always on the slab kernel."""
+    [0, K) of each row and nothing else, always on the slab kernel.  ``narrow`` (K = 32 or 48): one N tile exactly K wide
+    (b2_conv_ndhwc_fprop_slice_narrow) instead of the 64-wide tile, with bitwise the same result."""
     if a.ld != pc.C:
         raise ValueError("activation pitch %d != packed filter pitch %d" % (a.ld, pc.C))
     kt, kh, kw = pc.k
@@ -588,35 +589,96 @@ def conv_slice(a, pc, y, relu=True):
     args.pt, args.ph, args.pw = pc.p
     args.relu, args.mode = int(relu), pc.mode
     flops = 2.0 * M * pc.K * pc.Cin * kt * kh * kw
-    desc = "conv %dx%dx%d s%s C%d->%d M=%d slice" % (kt, kh, kw, "".join(map(str, pc.s)), pc.Cin, pc.K, M)
+    desc = "conv %dx%dx%d s%s C%d->%d M=%d slice%s" % (kt, kh, kw, "".join(map(str, pc.s)), pc.Cin, pc.K, M, " n%d" % pc.K if narrow else "")
+    entry = "b2_conv_ndhwc_fprop_slice_narrow" if narrow else "b2_conv_ndhwc_fprop_slice"
     with _timed("conv_slice", desc, flops, 2.0 * (a.M * a.C + M * pc.K + pc.K * pc.Cin * kt * kh * kw)):
-        _lib.check(_lib.load().b2_conv_ndhwc_fprop_slice(ctypes.byref(args), _stream()), "b2_conv_ndhwc_fprop_slice")
+        _lib.check(getattr(_lib.load(), entry)(ctypes.byref(args), _stream()), entry)
     return Act(y, a.N, To, Ho, Wo, pc.K)
 
 
+def _pair(v):
+    return (v, v) if isinstance(v, int) else tuple(v)
+
+
 @_on_device
-def pool_slice(a, k, s, p, avg, y=None, count_include_pad=True):
-    """nn.MaxPool2d / nn.AvgPool2d (k, stride s, padding p, ceil_mode=True) over every frame of ``a`` (its ``data`` may itself be a
-    column slice: rows of pitch ``data.stride(0)``) into the column slice ``y`` (fp16 [M_out][a.C] view; a fresh dense matrix when
-    None) by b2_pool_ndhwc_slice, or, for an average with ``count_include_pad=False``, b2_avgpool_ndhwc_slice_exclude_pad.  (The
-    floor-mode windows of Inception-v4 / Inception-ResNet-v2 are ceil-mode windows on their odd maps.)"""
-    Ho, Wo = ceil_pool_dim(a.H, k, s, p), ceil_pool_dim(a.W, k, s, p)
+def pool_slice(a, k, s, p, avg, y=None, count_include_pad=True, ceil_mode=True):
+    """nn.MaxPool2d / nn.AvgPool2d (k, stride s, padding p: ints or (h, w) pairs; ceil_mode=True unless ``ceil_mode=False``) over
+    every frame of ``a`` (its ``data`` may itself be a column slice: rows of pitch ``data.stride(0)``) into the column slice ``y``
+    (fp16 [M_out][a.C] view; a fresh dense matrix when None) by b2_pool_ndhwc_slice, or, for an average with
+    ``count_include_pad=False``, b2_avgpool_ndhwc_slice_exclude_pad.  (The floor-mode windows of Inception-v4 /
+    Inception-ResNet-v2 are ceil-mode windows on their odd maps; DenseNet's pool0 is a floor-mode window.)"""
+    (kh, kw), (sh, sw), (ph, pw) = _pair(k), _pair(s), _pair(p)
+    dim = ceil_pool_dim if ceil_mode else _out_dim
+    Ho, Wo = dim(a.H, kh, sh, ph), dim(a.W, kw, sw, pw)
     My = a.N * a.T * Ho * Wo
     if y is None:
         y = torch.empty((My, _round_up(a.C, 8)), dtype=torch.float16, device=a.data.device)
     yp, ldy, cols = _slice_view(y, "pool output")
     if y.shape[0] != My or cols < a.C:
         raise ValueError("pool output %s does not fit %d rows of %d channels" % (tuple(y.shape), My, a.C))
-    with _timed("pool", "%spool %dx%d s%d C%d M=%d->%d" % ("avg" if avg else "max", k, k, s, a.C, a.M, My), 0.0,
+    with _timed("pool", "%spool %dx%d s%d C%d M=%d->%d" % ("avg" if avg else "max", kh, kw, sh, a.C, a.M, My), 0.0,
                 2.0 * a.C * (a.M + My)):
         if avg and not count_include_pad:
-            _lib.check(_lib.load().b2_avgpool_ndhwc_slice_exclude_pad(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, k,
-                                                                      k, 1, s, s, 0, p, p, a.T, Ho, Wo, _stream()),
+            _lib.check(_lib.load().b2_avgpool_ndhwc_slice_exclude_pad(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, kh,
+                                                                      kw, 1, sh, sw, 0, ph, pw, a.T, Ho, Wo, _stream()),
                        "b2_avgpool_ndhwc_slice_exclude_pad")
         else:
-            _lib.check(_lib.load().b2_pool_ndhwc_slice(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, k, k, 1, s, s, 0,
-                                                       p, p, a.T, Ho, Wo, int(bool(avg)), _stream()), "b2_pool_ndhwc_slice")
+            _lib.check(_lib.load().b2_pool_ndhwc_slice(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.T, a.H, a.W, a.C, 1, kh, kw, 1, sh, sw, 0,
+                                                       ph, pw, a.T, Ho, Wo, int(bool(avg)), _stream()), "b2_pool_ndhwc_slice")
     return Act(y, a.N, a.T, Ho, Wo, a.C)
+
+
+# ---------------------------------------------------------------------------------------------
+# DenseNet: dense layers read and write column slices of one block matrix
+# ---------------------------------------------------------------------------------------------
+@_on_device
+def gemm_preact(a2d, b2d, scale, shift, in_scale, in_shift, M, N, Kd, relu=True):
+    """D[M][N] = act(scale * relu(in_scale * A[M][:Kd] + in_shift) . B[N][Kd]^T + shift) (b2_gemm_preact_f16): a dense layer's
+    norm1 + ReLU applied to the first ``Kd`` columns of the block matrix ``a2d`` on their way to the tensor core.  ``in_scale`` /
+    ``in_shift``: fp32 [round_up(Kd, 64)], zero past Kd."""
+    if in_scale.numel() < _round_up(Kd, 64) or in_shift.numel() < _round_up(Kd, 64):
+        raise ValueError("the input affine needs round_up(Kd, 64) = %d entries" % _round_up(Kd, 64))
+    out = torch.empty((M, _round_up(N, 8)), dtype=torch.float16, device=a2d.device)
+    g = GemmArgs()
+    g.a, g.b, g.scale, g.shift = _ptr(a2d), _ptr(b2d), _ptr(scale), _ptr(shift)
+    g.d = _ptr(out)
+    g.M, g.N, g.Kd = M, N, Kd
+    g.lda, g.ldb, g.ldd = a2d.stride(0), b2d.stride(0), out.stride(0)
+    g.relu = int(relu)
+    with _timed("gemm_preact", "gemm M=%d N=%d K=%d preact" % (M, N, Kd), 2.0 * M * N * Kd,
+                2.0 * (M * Kd + N * Kd + M * out.shape[1])):
+        _lib.check(_lib.load().b2_gemm_preact_f16(ctypes.byref(g), _ptr(in_scale), _ptr(in_shift), _stream()), "b2_gemm_preact_f16")
+    return out
+
+
+@_on_device
+def bn_relu_avgpool2(a, scale, shift, y=None):
+    """relu(scale * x + shift) -> AvgPool2d(2, 2) over every image of ``a`` (a dense transition's norm + ReLU + pool,
+    b2_bn_relu_avgpool2_ndhwc) into the slice ``y`` (fp16 [M / 4][C] view; a fresh dense matrix when None)."""
+    if a.T != 1:
+        raise ValueError("the transition pool works on images (T == 1)")
+    Ho, Wo = a.H // 2, a.W // 2
+    My = a.N * Ho * Wo
+    if y is None:
+        y = torch.empty((My, _round_up(a.C, 8)), dtype=torch.float16, device=a.data.device)
+    yp, ldy, cols = _slice_view(y, "transition pool output")
+    if y.shape[0] != My or cols < a.C:
+        raise ValueError("transition pool output %s does not fit %d rows of %d channels" % (tuple(y.shape), My, a.C))
+    with _timed("pool", "bn+relu+avgpool 2x2 C%d M=%d->%d" % (a.C, a.M, My), 0.0, 2.0 * a.C * (a.M + My)):
+        _lib.check(_lib.load().b2_bn_relu_avgpool2_ndhwc(_ptr(a.data), a.data.stride(0), yp, ldy, a.N, a.H, a.W, a.C, _ptr(scale),
+                                                         _ptr(shift), _stream()), "b2_bn_relu_avgpool2_ndhwc")
+    return Act(y, a.N, 1, Ho, Wo, a.C)
+
+
+@_on_device
+def avgpool_global_affine(a, scale, shift):
+    """relu(scale * x + shift) averaged over every clip's positions (b2_avgpool_global_affine_ndhwc: DenseNet's norm5 + ReLU +
+    7x7 mean) -> fp16 [N][ld].  ``scale`` / ``shift``: fp32 [ld]."""
+    y = torch.empty((a.N, a.ld), dtype=torch.float16, device=a.data.device)
+    with _timed("avgpool", "bn+relu+avgpool C%d M=%d" % (a.C, a.M), 0.0, 2.0 * a.C * (a.M + a.N)):
+        _lib.check(_lib.load().b2_avgpool_global_affine_ndhwc(_ptr(a.data), _ptr(y), a.N, a.positions, a.ld, _ptr(scale), _ptr(shift),
+                                                              _stream()), "b2_avgpool_global_affine_ndhwc")
+    return y
 
 
 class PackedLinear:

@@ -23,6 +23,9 @@ lib.b2_debug_set_slab_t128.restype = ctypes.c_int
 lib.b2_debug_set_slab_t128.argtypes = [ctypes.c_int]          # 6th field: 128-wide transposed slab form 1 = wherever it applies, 0 = never, -1 / absent = the rule
 lib.b2_debug_set_slab_t64.restype = ctypes.c_int
 lib.b2_debug_set_slab_t64.argtypes = [ctypes.c_int]           # 7th field: 64-wide transposed slab form 1 = wherever it applies, 0 = never, -1 / absent = the rule
+# 8th field: -1 / absent = the plain entry; 0 = the slice entry (b2_conv_ndhwc_fprop_slice, its own N tile); 1 = the slice entry with the
+# N tile exactly K wide (b2_conv_ndhwc_fprop_slice_narrow, K = 32 or 48).  Slice settings run without BatchNorm or ReLU (DenseNet's
+# growth-rate convolutions) and report the largest difference from the first slice setting's output (bits: 0 = bitwise equal).
 dev = torch.device("cuda:0")
 REP = 20
 for sp in specs:
@@ -44,8 +47,33 @@ for sp in specs:
         M = want.data.shape[0]
         fl = 2.0 * M * K * Cin * kt * kh * kw
         out = ["%-44s M=%-7d" % (" ".join(sp[:12]) + (" +res" if with_res else ""), M)]
+        ref_slice = None
         for st in settings:
             maxm, fs = st[0], st[1]
+            if len(st) > 7 and st[7] >= 0:
+                pc = engine.packed_conv(conv, None, x.ld)
+                ys = torch.empty((M, K), dtype=torch.float16, device=dev)
+                run = lambda: ops.conv_slice(x, pc, ys, relu=False, narrow=st[7] == 1)
+                run(); torch.cuda.synchronize()
+                if ref_slice is None:
+                    ref_slice = ys.clone()
+                diff = int((ys.view(torch.int16) != ref_slice.view(torch.int16)).sum())
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    for _ in range(REP):
+                        run()
+                g.replay(); torch.cuda.synchronize()
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(3):
+                    g.replay()
+                e1.record(); torch.cuda.synchronize()
+                us = e0.elapsed_time(e1) / (3 * REP) * 1e3
+                info = (ctypes.c_int * 5)()
+                kid = lib.b2_debug_last_kernel(info)
+                out.append("[%s] %7.1f us %6.0f TF/s k%d%s bits!=%d" % (":".join(map(str, st)), us, fl / us / 1e6, kid, tuple(info), diff))
+                del g
+                continue
             mt = st[2] if len(st) > 2 else 0
             lib.b2_debug_set_densem(maxm, fs)
             lib.b2_debug_set_slab_mt(mt)

@@ -57,6 +57,8 @@ case("mobilenetv2", lambda: P.mobilenetv2(num_classes=1000, pretrained=None), (2
 case("se_resnet50", lambda: P.se_resnet50(pretrained=None), (2, 3, 224, 224))
 case("se_resnext50_32x4d", lambda: P.se_resnext50_32x4d(pretrained=None), (2, 3, 224, 224))
 case("slowfast18", lambda: P.slowfast.resnet18(mode="sf", num_classes=12), (1, 3, 32, 64, 64))
+case("densenet121", lambda: P.densenet121(pretrained=None), (2, 3, 224, 224))
+case("densenet161", lambda: P.densenet161(pretrained=None), (1, 3, 224, 224))
 
 if not only or "trn" in only:
     torch.manual_seed(0)
