@@ -247,6 +247,46 @@ def att_bound(ref, pv, v, B, Nq, Nk, mode):
 
 
 # ---------------------------------------------------------------------------------------------
+# squeeze-and-excitation (tests/test_gpu_senet.py, tests/model_audit.py)
+# ---------------------------------------------------------------------------------------------
+def excite_mean(h, N, S, C2, device="cpu"):
+    """Per-sample channel means of h (fp16 [N * S][>= C2]) and of |h|: fp64 [N][C2] each."""
+    hd = h[:, :C2].double().to(device).reshape(N, S, C2)
+    return hd.mean(1), hd.abs().mean(1)
+
+
+def excite_ref(m, habs, w1, b1, w2, b2, s3, t3):
+    """fp64 excitation from the operands b2_se_excite reads: the means ``m`` (and mean |h|, ``habs``) of ``excite_mean``, fc1
+    folded through conv3 + bn3 (w1 [R][C2], b1 [R]), fc2 (w2 [C][R], b2 [C]) and the bn3 affine (s3, t3 [C]).  Returns the dict
+    ``excite_bound`` reads: m, habs, a = relu(fc1), e = sigmoid(fc2), scale = e s3, shift = e t3."""
+    dev = m.device
+    w1, b1, w2, b2, s3, t3 = (t.double().to(dev) for t in (w1, b1, w2, b2, s3, t3))
+    a = (m @ w1.t() + b1).clamp_min(0)
+    e = torch.sigmoid(a @ w2.t() + b2)
+    return dict(m=m, habs=habs, a=a, e=e, scale=e * s3, shift=e * t3)
+
+
+def excite_bound(r, w1, b1, w2, b2, s3, t3, S, fold_rounding=False):
+    """Per-element bound of (scale, shift), from fp32 roundoff (u = 2^-24) stage by stage, r the dict of ``excite_ref``:
+      mean   |dm| <= (S + 34) u mean|h|          (stripe sums of <= ceil(S/32) terms, 32-term stripe sum, one division)
+      fc1    |da| <= (C2 + 1) u (sum |w1| |m| + |b1|) + sum |w1| |dm|    (one fmaf chain and the bias)
+      fc2    |dv| <= (R + 1) u (sum |w2| |a| + |b2|) + sum |w2| |da|
+      sigmoid |de| <= |dv| / 4 + 2^-19        (Lipschitz 1/4; the fast-math exp and reciprocal)
+      output |d(e s)| <= |s| |de| + u |e s|
+    ``fold_rounding``: r was computed from the unfolded fp64 weights, so fc1 also carries the fp32 rounding of the fold
+    w1 = W_fc1 diag(s3) W3, b1 = W_fc1 t3 + b_fc1: (C2 + 2) u."""
+    dev = r["m"].device
+    w1a, b1a, w2a, b2a = (t.double().to(dev).abs() for t in (w1, b1, w2, b2))
+    s3d, t3d = s3.double().to(dev), t3.double().to(dev)
+    C2, R = w1a.shape[1], w1a.shape[0]
+    dm = (S + 34) * FLOOR * r["habs"]
+    da = (C2 + 1 + int(fold_rounding)) * FLOOR * (r["m"].abs() @ w1a.t() + b1a) + dm @ w1a.t()
+    dv = (R + 1) * FLOOR * (r["a"].abs() @ w2a.t() + b2a) + da @ w2a.t()
+    de = dv / 4 + 2.0 ** -19
+    return de * s3d.abs() + FLOOR * r["scale"].abs(), de * t3d.abs() + FLOOR * r["shift"].abs()
+
+
+# ---------------------------------------------------------------------------------------------
 # stem convolution with the fused W max-pool, depthwise 3x3, weight gradient (tests/test_gpu_kernel_bounds.py,
 # tests/test_kernel_bounds_cpu.py): fp64 from exactly the operands each kernel reads.
 # ---------------------------------------------------------------------------------------------

@@ -10,6 +10,9 @@ GPU from exactly the operands the kernel read.  Nothing is skipped silently:
   * the launch-count delta of the whole forward must equal the sum of the deltas of the wrapped entries;
   * an entry without a check (``UNAUDITED`` lists the layout helpers and why), or an argument combination the checks below do not
     understand, raises ``AuditError``;
+  * an entry that writes column slices of a wider matrix leaves every other column of those rows bit for bit as it was
+    (``SliceGuard``), and the pre-activated GEMM's output depends on nothing of A, B or its input affine past Kd
+    (``preact_contract``);
   * the composite entries (``PASS_THROUGH``) launch nothing themselves: the inner entry they call is audited, once.
 
 Filters: ordinary packs are read back from ``pc.w`` as [K][taps][C] (as tests/test_gpu_kernel_matrix.py's ``Problem`` does); the
@@ -52,8 +55,6 @@ UNAUDITED = {
 }
 # composite entries: they launch only through the named entry, which is audited
 PASS_THROUGH = {"linear": "gemm", "nonlocal_attention": "attention", "concat_channels": "concat_rows"}
-# launching entries no benchmarked forward reaches and the audit has no check for yet: reaching one fails the audit
-NO_CHECK = ("se_excite", "gemm_split", "conv_slice", "pool_slice")
 
 
 # the parameters each audited entry's check models: a parameter an entry gains later fails the audit until its check learns it
@@ -77,7 +78,17 @@ KNOWN = {
     "embed_concat": ("z", "labels", "table", "split"),
     "rgb_head": ("partial", "bias", "N", "H", "W", "K", "out_dtype", "out"),
     "tanh_to_nchw": ("a", "out_dtype", "out"),
+    "conv_slice": ("a", "pc", "y", "relu", "narrow"),
+    "gemm_split": ("a2d", "b2d", "scale", "shift", "M", "Kd", "dests", "relu"),
+    "pool_slice": ("a", "k", "s", "p", "avg", "y", "count_include_pad", "ceil_mode"),
+    "gemm_preact": ("a2d", "b2d", "scale", "shift", "in_scale", "in_shift", "M", "N", "Kd", "relu"),
+    "bn_relu_avgpool2": ("a", "scale", "shift", "y"),
+    "avgpool_global_affine": ("a", "scale", "shift"),
+    "se_excite": ("h", "w1", "b1", "w2", "b2", "s3", "t3", "out"),
 }
+# entries whose launch records the kernel and plan it ran (b2_debug_last_kernel)
+RECORDS_KERNEL = ("conv", "gemm", "gemm_chain", "gemm_sample_affine", "attention", "conv_slice", "gemm_split", "gemm_preact",
+                  "pool_slice", "bn_relu_avgpool2", "avgpool_global_affine")
 
 
 class AuditError(AssertionError):
@@ -123,6 +134,11 @@ class _Worst:
             self.ratio = float("inf")
             self.where = "%s row %d col %d: got %r want %r (bit-exact)" % (what, row0 + m, c, float(got.reshape(-1)[i]),
                                                                            float(want.reshape(-1)[i]))
+
+    def merge(self, what, ratio, where):
+        """Fold in the (ratio, where) of a sub-check; NaN counts as infinite."""
+        if not ratio <= self.ratio or self.where == "no elements":
+            self.ratio, self.where = ratio if ratio == ratio else float("inf"), "%s: %s" % (what, where)
 
     def result(self):
         return self.ratio, self.where
@@ -409,6 +425,196 @@ def check_dwconv(x2d, N, H, W, C, w9, scale, shift, stride, clamp_in, relu6, y):
 
 
 # ---------------------------------------------------------------------------------------------
+# column-slice outputs (BNInception, Inception-v4, DenseNet), pre-activated GEMM, DenseNet pools, squeeze-excite
+# ---------------------------------------------------------------------------------------------
+class SliceGuard:
+    """The slice contract of an entry that writes column slices of wider matrices: after the call, every column of the parent
+    rows outside the slices is bit for bit what it was before (compared as int16, so NaN patterns in uninitialised columns
+    compare equal).  ``views``: (fp16 [rows][cols] view, columns the entry writes from the view's first column on).  The parent
+    is the view's base, which must be a 2-D matrix of the view's row pitch: its rows, not an assumed row grid of the storage,
+    locate the slice (a view into a flat workspace raises).  A view of whole rows has nothing outside it; slices of the same
+    rows are checked together."""
+
+    def __init__(self, views):
+        groups = {}
+        for y, width in views:
+            pitch, rows = y.stride(0), y.shape[0]
+            if y.shape[1] == pitch:
+                continue
+            base = y._base
+            if base is None or base.dim() != 2 or base.stride() != (pitch, 1):
+                raise AuditError("the parent of a %s column slice of pitch %d is not a 2-D matrix of that pitch (%s): its rows "
+                                 "cannot be located" % (tuple(y.shape), pitch, None if base is None else tuple(base.shape)))
+            r0, c0 = divmod(y.storage_offset() - base.storage_offset(), pitch)
+            if r0 < 0 or r0 + rows > base.shape[0] or c0 + width > pitch:
+                raise AuditError("a %s column slice at row %d col %d does not lie inside its %s parent" % (tuple(y.shape), r0, c0,
+                                                                                                      tuple(base.shape)))
+            groups.setdefault((base.data_ptr(), r0, rows), (base, []))[1].append((c0, c0 + width))
+        self.spans = []
+        for (_, r0, rows), (base, cols) in groups.items():
+            keep = torch.ones(base.shape[1], dtype=torch.bool, device=base.device)
+            for c0, c1 in cols:
+                keep[c0:c1] = False
+            if bool(keep.any()):
+                span = base[r0:r0 + rows].view(torch.int16)
+                self.spans.append((span, keep, span.clone()))
+
+    def check(self):
+        """(0, ...) when every column outside the slices is unchanged, else (inf, the first changed element; its row counts from
+        the slices' first row, as the output rows of the entry do)."""
+        wst = _Worst()
+        for span, keep, before in self.spans:
+            diff = (span != before) & keep
+            if bool(diff.any()):
+                m, c = (int(v) for v in torch.nonzero(diff)[0])
+                wst.ratio = float("inf")
+                wst.where = "outside the slice row %d col %d: bits %#06x, were %#06x" % (m, c, int(span[m, c]) & 0xFFFF,
+                                                                                         int(before[m, c]) & 0xFFFF)
+                break
+        return wst.result()
+
+
+def check_gemm_split(a, b, scale, shift, M, Kd, dests, relu=True):
+    """Destination d (fp16 [M][cols_d]) = act(scale * A[:, :Kd] . B[rows]^T + shift) over the packed rows
+    [64 box0[d], 64 box0[d] + cols_d) of B / scale / shift (``ops.split_plan``): each held to the GEMM bound of ``check_gemm``."""
+    from pretorched_x_b200 import ops
+    _, box0 = ops.split_plan([y.shape[1] for y in dests])
+    wst = _Worst()
+    for d, y in enumerate(dests):
+        r0, n = 64 * box0[d], y.shape[1]
+        wst.merge("dest %d" % d, *check_gemm(a, b[r0:r0 + n], scale[r0:r0 + n], shift[r0:r0 + n], M, n, Kd, y, relu=relu))
+    return wst.result()
+
+
+def check_pool_slice(x2d, N, T, H, W, C, k, s, p, avg, y, count_include_pad=True, ceil_mode=True):
+    """nn.MaxPool2d / nn.AvgPool2d over every frame of x2d (fp16 rows [N T H W][>= C], any row pitch) into y (fp16 rows
+    [N T Ho Wo][>= C]); k, s, p are (h, w) pairs.  Max: bit-exact against F.max_pool2d of the same fp16 values.  Average: an fp32
+    sum of at most kh kw taps (each addition errs by 2^-24 of the partial sum, at most the sum of the taps' magnitudes), one
+    division by the divisor (2^-24) and the fp16 rounding, so |got - ref| <= 2^-11 |ref| + max(16, kh kw) 2^-24 mean|x| + 2^-24
+    with mean|x| the same average of |x| (the padding counted or not): 2^-20 mean|x| for windows of at most 16 taps."""
+    S = T * H * W
+    wst = _Worst()
+    rows_out = None
+    for n0, n1 in _chunks(N, 8 * 6 * S * C):
+        xs = x2d[n0 * S:n1 * S, :C].double().reshape((n1 - n0) * T, H, W, C).permute(0, 3, 1, 2)
+        if avg:
+            ref = F.avg_pool2d(xs, k, s, p, ceil_mode=ceil_mode, count_include_pad=count_include_pad)
+            mag = F.avg_pool2d(xs.abs(), k, s, p, ceil_mode=ceil_mode, count_include_pad=count_include_pad)
+        else:
+            ref = F.max_pool2d(xs, k, s, p, ceil_mode=ceil_mode)
+        Ho, Wo = ref.shape[2:]
+        So = T * Ho * Wo
+        if rows_out is None:
+            rows_out = N * So
+            if y.shape[0] != rows_out:
+                raise AuditError("pool output has %d rows, torch gives %d" % (y.shape[0], rows_out))
+        ref = ref.permute(0, 2, 3, 1).reshape(-1, C)
+        yc = y[n0 * So:n1 * So, :C]
+        if avg:
+            mag = mag.permute(0, 2, 3, 1).reshape(-1, C)
+            wst.add("y", yc, ref, KR.U_F16 * ref.abs() + max(16, k[0] * k[1]) * KR.FLOOR * mag + KR.FLOOR, n0 * So)
+        else:
+            wst.exact("y", yc, ref, n0 * So)
+    return wst.result()
+
+
+def check_gemm_preact(a, b, scale, shift, in_scale, in_shift, M, N, Kd, d, relu=True):
+    """D[M][N] = act(scale * relu(in_scale * A[:, :Kd] + in_shift) . B[:N, :Kd]^T + shift), the in-affine operand rounded to fp16
+    once (``KR.in_affine_acc``), held to the GEMM bound; the pad columns [N, ldd) of D are zero."""
+    dev = d.device
+    wst = _Worst()
+    for m0, m1 in _chunks(M, 8 * 8 * (Kd + N)):
+        acc, mag = KR.in_affine_acc(a[m0:m1, :Kd], b[:N, :Kd], in_scale[:Kd], in_shift[:Kd], m1 - m0, device=dev)
+        v, A = KR.epilogue(acc, mag, scale[:N], shift[:N], relu=relu, device=dev)
+        del acc, mag
+        wst.add("d", d[m0:m1, :N], v, KR.bound(v, A, True), m0)
+        _pad_zero(wst, "d", d[m0:m1], N, m0)
+    return wst.result()
+
+
+# What ``preact_contract`` puts past Kd: A's columns [Kd, lda) hold PREACT_A, the input affine's entries [Kd, round_up(Kd, 64))
+# PREACT_IN (scale, shift) and B is handed over at a wider pitch whose extra columns hold PREACT_B.  Every value is finite and
+# relu(PREACT_A s + t) > 0, so a kernel that reads any of them moves its output by about PREACT_B relu(PREACT_A s + t) per column
+# read, far past the bound.
+PREACT_A, PREACT_IN, PREACT_B = 2.0, (1.0, 0.5), 0.125
+
+
+def preact_contract(ba):
+    """The pre-activated GEMM's contract: its output depends only on A[:, :Kd], B[:N, :Kd] and in_scale / in_shift[:Kd] (its A
+    and B tensor maps span Kd columns, and the hardware zero-fills the rest of the last 64-column K block).
+
+    A poison has to survive the kernel's A transform to be seen: that computes fmaxf(fmaf(x, s, t), 0), and fmaxf returns its
+    non-NaN operand, so a NaN (or fmaf(Inf, 0, 0)) past Kd would turn into 0 and vanish.  The call therefore gets finite
+    values past Kd everywhere the kernel could look: A's columns [Kd, lda) are set to PREACT_A in place (their exact bits come
+    back afterwards), and the call receives copies of the input affine that are PREACT_IN past Kd and a copy of B at a pitch 64
+    columns wider, PREACT_B there.  Returns (the call's keyword arguments, the restoring function)."""
+    a, b, M, Kd = ba["a2d"], ba["b2d"], ba["M"], ba["Kd"]
+    lda = a.stride(0)
+    call = dict(ba)
+    restore = lambda: None                                   # noqa: E731
+    if lda > Kd:
+        if (a.storage_offset() + M * lda) * a.element_size() > a.untyped_storage().nbytes():
+            raise AuditError("the %d rows of pitch %d of the pre-activated GEMM's A run past its storage" % (M, lda))
+        tail = a.as_strided((M, lda - Kd), (lda, 1), a.storage_offset() + Kd).view(torch.int16)
+        saved = tail.clone()
+        tail.view(torch.float16).fill_(PREACT_A)
+        restore = lambda: tail.copy_(saved)                  # noqa: E731
+    for key, v in (("in_scale", PREACT_IN[0]), ("in_shift", PREACT_IN[1])):
+        t = ba[key].clone()
+        t[Kd:] = v
+        call[key] = t
+    wide = torch.full((b.shape[0], b.stride(0) + 64), PREACT_B, dtype=b.dtype, device=b.device)
+    wide[:, :Kd] = b[:, :Kd]
+    call["b2d"] = wide
+    return call, restore
+
+
+def _affine_relu(xs, scale, shift, C):
+    """relu(scale * x + shift) of fp64 rows [..][C] and the magnitude |scale x| + |shift| of its terms."""
+    sc, sh = scale[:C].double().to(xs.device), shift[:C].double().to(xs.device)
+    return (xs * sc + sh).clamp_min(0.0), (xs * sc).abs() + sh.abs()
+
+
+def check_transition_pool(x2d, N, H, W, C, scale, shift, y):
+    """y = the 2x2 mean of relu(scale * x + shift) (floor extents): per tap one fp32 FMA (2^-24 of |s x| + |t|), three additions
+    and a division, then the fp16 rounding: |got - ref| <= 2^-11 |ref| + 2^-20 mean(|s x| + |t|) + 2^-24."""
+    S, Ho, Wo = H * W, H // 2, W // 2
+    So = Ho * Wo
+    wst = _Worst()
+    for n0, n1 in _chunks(N, 8 * 6 * S * C):
+        v, A = _affine_relu(x2d[n0 * S:n1 * S, :C].double(), scale, shift, C)
+        ref, mag = (F.avg_pool2d(t.reshape(n1 - n0, H, W, C).permute(0, 3, 1, 2), 2, 2).permute(0, 2, 3, 1).reshape(-1, C)
+                    for t in (v, A))
+        wst.add("y", y[n0 * So:n1 * So, :C], ref, KR.U_F16 * ref.abs() + 2.0 ** -20 * mag + KR.FLOOR, n0 * So)
+    return wst.result()
+
+
+def check_head_pool(x2d, N, S, C, scale, shift, y):
+    """y[n] = the mean over the S positions of relu(scale * x + shift): one FMA per term, S - 1 fp32 additions in any order, the
+    multiplication by a rounded 1 / S (two roundings), the fp16 rounding: |got - ref| <= 2^-11 |ref| + max(64, S + 2) 2^-24
+    mean(|s x| + |t|) + 2^-24 (2^-18 mean(|s x| + |t|) up to S = 62)."""
+    wst = _Worst()
+    for n0, n1 in _chunks(N, 8 * 6 * S * C):
+        v, A = _affine_relu(x2d[n0 * S:n1 * S, :C].double(), scale, shift, C)
+        ref, mag = (t.reshape(n1 - n0, S, C).mean(1) for t in (v, A))
+        wst.add("y", y[n0:n1, :C], ref, KR.U_F16 * ref.abs() + max(64, S + 2) * KR.FLOOR * mag + KR.FLOOR, n0)
+    return wst.result()
+
+
+def check_se_excite(h2d, N, S, C2, w1, b1, w2, b2, s3, t3, scale, shift):
+    """(scale, shift) fp32 [N][>= C] against ``KR.excite_ref`` of the kernel's own operands (the folded fp32 w1 / b1, then w2, b2,
+    s3, t3) under ``KR.excite_bound``."""
+    m, habs = KR.excite_mean(h2d, N, S, C2, device=scale.device)
+    r = KR.excite_ref(m, habs, w1, b1, w2, b2, s3, t3)
+    bs, bh = KR.excite_bound(r, w1, b1, w2, b2, s3, t3, S)
+    C = w2.shape[0]
+    wst = _Worst()
+    wst.add("scale", scale[:, :C], r["scale"], bs)
+    wst.add("shift", shift[:, :C], r["shift"], bh)
+    return wst.result()
+
+
+# ---------------------------------------------------------------------------------------------
 # BigGAN helpers
 # ---------------------------------------------------------------------------------------------
 # One fp32 FMA or product (2^-24 of its magnitude), at most one fp32 sum on top, then the fp16 rounding: an element of a
@@ -577,23 +783,28 @@ class _Auditor:
             bound.apply_defaults()
             ba = dict(bound.arguments)
             snap = self.snapshot(name, ba)
+            guard = SliceGuard(self.slices(name, ba))
+            call, restore = preact_contract(ba) if name == "gemm_preact" else (None, lambda: None)
             self.depth += 1
             try:
                 torch.cuda.synchronize()
                 c0 = self.lib.b2_launch_count()
-                out = orig(*args, **kwargs)
+                out = orig(*args, **kwargs) if call is None else orig(**call)
                 torch.cuda.synchronize()
                 n = self.lib.b2_launch_count() - c0
             finally:
                 self.depth -= 1
+                restore()
             if name in UNAUDITED:
                 self.record(name, "", n)
                 return out
-            kernel, info = _last_kernel(self.lib) if name in ("conv", "gemm", "gemm_chain", "gemm_sample_affine", "attention") \
-                else ("-", "-")
+            kernel, info = _last_kernel(self.lib) if name in RECORDS_KERNEL else ("-", "-")
             if n < 1:
                 raise AuditError("%s returned without a launch" % name)
             geometry, (ratio, where) = getattr(self, "audit_" + name)(snap, out)
+            r_out, w_out = guard.check()
+            if not r_out <= ratio:
+                ratio, where = r_out, w_out
             self.record(name, geometry, n, ratio, where, kernel, str(info))
             return out
         return wrapped
@@ -617,6 +828,17 @@ class _Auditor:
                 if isinstance(t, torch.Tensor) and _storage_of(t) in ptrs:
                     ba[key] = self.ops.Act(t.clone(), v.N, v.T, v.H, v.W, v.C) if isinstance(v, self.ops.Act) else t.clone()
         return ba
+
+    @staticmethod
+    def slices(name, ba):
+        """(view, columns written) of every column slice of a wider matrix the entry writes (``SliceGuard``)."""
+        if name == "conv_slice":
+            return [(ba["y"], ba["pc"].K)]
+        if name == "gemm_split":
+            return [(y, y.shape[1]) for y in ba["dests"]]
+        if name in ("pool_slice", "bn_relu_avgpool2") and ba["y"] is not None:
+            return [(ba["y"], ba["a"].C)]
+        return []
 
     # -- packs --
     def wrap_init(self, cls, kind):
@@ -780,9 +1002,58 @@ class _Auditor:
         a = b["a"]
         return "tanh N%d %dx%d C%d" % (a.N, a.H, a.W, a.C), check_tanh(a.data, a.N, a.C, a.T * a.H * a.W, y)
 
+    def audit_conv_slice(self, b, out):
+        a, pc, y = b["a"], b["pc"], b["y"]
+        w = self.filter_of(pc, a.ld)
+        x = a.data.view(a.N, a.T, a.H, a.W, a.ld)
+        geom = "conv_slice N%d %dx%dx%d C%d->%d k%s s%s p%s%s%s" % (a.N, a.T, a.H, a.W, a.ld, pc.K, "".join(map(str, pc.k)),
+                                                                "".join(map(str, pc.s)), "".join(map(str, pc.p)),
+                                                                " relu" if b["relu"] else "", " narrow" if b["narrow"] else "")
+        self.report.ref_flops += 2 * 2.0 * y.shape[0] * pc.K * a.ld * pc.k[0] * pc.k[1] * pc.k[2]
+        return geom, check_conv(x, w, pc.scale, pc.shift, pc.k, pc.s, pc.p, y, pc.K, relu=b["relu"])
+
+    def audit_gemm_split(self, b, out):
+        cols = [y.shape[1] for y in b["dests"]]
+        self.report.ref_flops += 2 * 2.0 * b["M"] * sum(cols) * b["Kd"]
+        geom = "gemm_split M%d K%d -> %s%s" % (b["M"], b["Kd"], "+".join(map(str, cols)), " relu" if b["relu"] else "")
+        return geom, check_gemm_split(b["a2d"], b["b2d"], b["scale"], b["shift"], b["M"], b["Kd"], b["dests"], relu=b["relu"])
+
+    def audit_pool_slice(self, b, y):
+        a = b["a"]
+        k, s, p = (self.ops._pair(b[f]) for f in ("k", "s", "p"))
+        kind = ("avg" if b["count_include_pad"] else "avg_excl") if b["avg"] else "max"
+        geom = "pool_slice %s N%d %dx%dx%d C%d k%dx%d s%dx%d p%dx%d %s" % (kind, a.N, a.T, a.H, a.W, a.C, k[0], k[1], s[0], s[1],
+                                                                       p[0], p[1], "ceil" if b["ceil_mode"] else "floor")
+        return geom, check_pool_slice(a.data, a.N, a.T, a.H, a.W, a.C, k, s, p, b["avg"], y.data,
+                                      count_include_pad=b["count_include_pad"], ceil_mode=b["ceil_mode"])
+
+    def audit_gemm_preact(self, b, d):
+        self.report.ref_flops += 2 * 2.0 * b["M"] * b["N"] * b["Kd"]
+        geom = "gemm_preact M%d N%d K%d lda%d" % (b["M"], b["N"], b["Kd"], b["a2d"].stride(0))
+        return geom, check_gemm_preact(b["a2d"], b["b2d"], b["scale"], b["shift"], b["in_scale"], b["in_shift"], b["M"], b["N"],
+                                       b["Kd"], d, relu=b["relu"])
+
+    def audit_bn_relu_avgpool2(self, b, y):
+        a = b["a"]
+        geom = "bn_relu_avgpool2 N%d %dx%d C%d" % (a.N, a.H, a.W, a.C)
+        return geom, check_transition_pool(a.data, a.N, a.H, a.W, a.C, b["scale"], b["shift"], y.data)
+
+    def audit_avgpool_global_affine(self, b, y):
+        a = b["a"]
+        # the kernel averages every one of the ld columns with the affine of that column
+        return ("avgpool_affine N%d S%d C%d" % (a.N, a.positions, a.ld),
+                check_head_pool(a.data, a.N, a.positions, a.ld, b["scale"], b["shift"], y))
+
+    def audit_se_excite(self, b, out):
+        h = b["h"]
+        R, C2 = b["w1"].shape
+        return ("se_excite N%d S%d C2 %d R%d C%d" % (h.N, h.positions, C2, R, b["w2"].shape[0]),
+                check_se_excite(h.data, h.N, h.positions, C2, b["w1"], b["b1"], b["w2"], b["b2"], b["s3"], b["t3"], *out))
+
 
 ENTRIES = ("conv", "gemm", "gemm_chain", "gemm_sample_affine", "attention", "maxpool3d", "maxpool2d_ceil", "avgpool_global",
-           "shortcut_a", "concat_rows", "relu6_", "dwconv3x3", "ccbn_act", "embed_concat", "rgb_head", "tanh_to_nchw")
+           "shortcut_a", "concat_rows", "relu6_", "dwconv3x3", "ccbn_act", "embed_concat", "rgb_head", "tanh_to_nchw", "conv_slice",
+           "gemm_split", "pool_slice", "gemm_preact", "bn_relu_avgpool2", "avgpool_global_affine", "se_excite")
 
 
 @contextlib.contextmanager
@@ -792,7 +1063,7 @@ def patched(chain_bitwise=True):
     lib = _lib.load()
     lib.b2_launch_count.restype = ctypes.c_uint64
     aud = _Auditor(lib, ops, chain_bitwise)
-    names = ENTRIES + tuple(UNAUDITED) + tuple(PASS_THROUGH) + NO_CHECK
+    names = ENTRIES + tuple(UNAUDITED) + tuple(PASS_THROUGH)
     saved = {n: getattr(ops, n) for n in names}
     aud._orig = saved
     inits = {}

@@ -4,7 +4,7 @@
    (2^-11 |ref| + 2^-14 A + 2^-24, A = |scale| sum |a w| + |shift| + |r|), at every rows-per-sample of the 224^2 networks and
    at ones that do not divide a 128-row tile, with the persistent kernel pinned and the pitch contract asserted.
 2. b2_se_excite against an fp64 restatement of SEModule (unfolded: conv3 + bn3, avgpool, fc1, fc2) under the bound derived in
-   ``excite_bound``.
+   ``tests/kernel_ref.excite_bound``.
 3. The ceil-mode stem pool bit-exact against F.max_pool2d(..., ceil_mode=True).
 4. Every SE block kind against the fp64 oracle block (oracle/senet.py) on the engine's own fp16 input: 5e-3 of max |ref|.
 5. se_resnet50 / se_resnext50_32x4d / TRN-MSTRN against the reference's fixtures (per-stage samples 1e-2, logits 5e-3 of
@@ -34,7 +34,6 @@ pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not has_h100(), reason="needs 
 
 dev = torch.device("cuda:0")
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
-U32 = 2.0 ** -24
 PGEMM = 6          # KID_PGEMM of csrc/b2_host.h
 
 
@@ -137,34 +136,12 @@ EXCITE_CASES = [
 
 
 def excite_ref(h, w3, s3, t3, f1, b1, f2, b2, N, S, C2):
-    """fp64 SEModule on bn3(conv3(h)) pooled first (unfolded), plus the magnitudes the bound needs."""
-    hd = h.double().cpu()[:, :C2].reshape(N, S, C2)
-    m = hd.mean(1)
+    """fp64 SEModule on bn3(conv3(h)) pooled first (unfolded), plus the magnitudes ``KR.excite_bound`` needs: the fc1 of
+    ``KR.excite_ref`` applied to the unfolded affine map bn3(W3 m)."""
+    m, habs = KR.excite_mean(h, N, S, C2)
     w3d, s3d, t3d = w3.double().cpu(), s3.double().cpu(), t3.double().cpu()
-    z = (m @ w3d.t()) * s3d + t3d
-    a = (z @ f1.double().cpu().t() + b1.double().cpu()).clamp_min(0)
-    v = a @ f2.double().cpu().t() + b2.double().cpu()
-    e = torch.sigmoid(v)
-    return dict(m=m, habs=hd.abs().mean(1), a=a, e=e, scale=e * s3d, shift=e * t3d)
-
-
-def excite_bound(r, w1f, b1f, f2, b2, s3, t3, S):
-    """Per-element bound of (scale, shift), from fp32 roundoff (u = 2^-24) stage by stage:
-      mean   |dm| <= (S + 34) u mean|h|          (stripe sums of <= ceil(S/32) terms, 32-term stripe sum, one division)
-      fc1    |da| <= (C2 + 2) u (sum |w1| |m| + |b1|) + sum |w1| |dm|    (one fmaf chain, the bias, the fp32 rounding of the
-                                                                           fp64 fold w1 = W_fc1 diag(s3) W3, b1 = W_fc1 t3 + b_fc1)
-      fc2    |dv| <= (R + 1) u (sum |w2| |a| + |b2|) + sum |w2| |da|
-      sigmoid |de| <= |dv| / 4 + 2^-19        (Lipschitz 1/4; the fast-math exp and reciprocal)
-      output |d(e s)| <= |s| |de| + u |e s|"""
-    w1a, b1a = w1f.double().cpu().abs(), b1f.double().cpu().abs()
-    f2a, b2a = f2.double().cpu().abs(), b2.double().cpu().abs()
-    C2, R = w1a.shape[1], w1a.shape[0]
-    dm = (S + 34) * U32 * r["habs"]
-    da = (C2 + 2) * U32 * (r["m"].abs() @ w1a.t() + b1a) + dm @ w1a.t()
-    dv = (R + 1) * U32 * (r["a"].abs() @ f2a.t() + b2a) + da @ f2a.t()
-    de = dv / 4 + 2.0 ** -19
-    s3d, t3d = s3.double().cpu(), t3.double().cpu()
-    return de * s3d.abs() + U32 * r["scale"].abs(), de * t3d.abs() + U32 * r["shift"].abs()
+    f1d = f1.double().cpu()
+    return KR.excite_ref(m, habs, (f1d * s3d[None, :]) @ w3d, f1d @ t3d + b1.double().cpu(), f2, b2, s3, t3)
 
 
 @pytest.mark.parametrize("N,S,C2,ldh,C", EXCITE_CASES)
@@ -187,7 +164,7 @@ def test_se_excite_matches_fp64(N, S, C2, ldh, C):
     torch.cuda.synchronize()
     assert torch.equal(scale, scale2) and torch.equal(shift, shift2), "not bitwise repeatable"
     r = excite_ref(h, w3, s3, t3, f1, b1, f2, b2, N, S, C2)
-    bs, bh = excite_bound(r, w1f, b1f, f2, b2, s3, t3, S)
+    bs, bh = KR.excite_bound(r, w1f, b1f, f2, b2, s3, t3, S, fold_rounding=True)
     for got, want, bnd, what in ((scale, r["scale"], bs, "scale"), (shift, r["shift"], bh, "shift")):
         worst = KR.worst_ratio_of(got[:, :C], want, bnd)
         assert worst <= 1.0, "%s: %s" % (what, KR.where_worst_of(got[:, :C], want, bnd))
