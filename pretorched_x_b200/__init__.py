@@ -28,6 +28,7 @@ from .models.senet import (se_resnet50, se_resnet101, se_resnet152, se_resnext50
 from .models.bninception import bninception  # noqa: F401  (pretorched/models/bninception.py:497)
 from .models.inception import inceptionv4, inceptionresnetv2  # noqa: F401  (pretorched/__init__.py:16-17)
 from .models.densenet import densenet121, densenet161, densenet169, densenet201  # noqa: F401  (pretorched/__init__.py:21-24)
+from .models.inceptionv3 import inceptionv3  # noqa: F401  (pretorched/__init__.py:30)
 from .models.trn import Relation, MultiScaleRelation, HierarchicalRelation, TRN, trn  # noqa: F401
 from .models.utils import Identity  # noqa: F401
 # BigGAN-deep generator (BASELINE.json configs[4]; not in the reference tree -- see models/biggan_deep.py)

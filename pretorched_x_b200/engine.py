@@ -800,7 +800,8 @@ def run_bninception_trunk(model, x):
 
 
 # ---------------------------------------------------------------------------------------------
-# Inception-v4 / Inception-ResNet-v2 (inceptionv4.py:34-309, inceptionresnetv2.py:34-331)
+# Inception-v4 / Inception-ResNet-v2 (inceptionv4.py:34-309, inceptionresnetv2.py:34-331) and Inception-v3 (torchvision's
+# Inception3 behind torchvision_models.py:380-437): torchvision's BasicConv2d has the same conv / bn (eps 0.001) fields
 # ---------------------------------------------------------------------------------------------
 def _is_head(u):
     """A BasicConv2d whose convolution is 1x1, stride 1, padding 0: it runs inside a split GEMM."""
@@ -865,15 +866,15 @@ def _branch_hw(block, a, br):
 
 
 def _inception_block_body(block, a, out=None):
-    """One block of Inception-v4 / Inception-ResNet-v2 from its row of models.inception.BRANCHES.  The branches write their
-    columns of the concatenated output ``y`` in place:
+    """One block of Inception-v4 / Inception-ResNet-v2 / Inception-v3 from its row of models.inception.BRANCHES.  The branches
+    write their columns of the concatenated output ``y`` in place:
 
     * the 1x1 units that read the block input (a lone 1x1 branch straight into its slice, the first unit of a longer chain into its
       own matrix) run as one split GEMM -- one pass over the block input;
     * every later unit of a chain runs on the slab kernel's slice entry, the last one into the branch's slice; a fork's two units
       read the same matrix and write adjacent slices;
-    * a max branch pools the block input into its slice; an average branch pools it (count_include_pad=False) into a matrix that
-      its 1x1 projection reads, writing its slice;
+    * a max branch pools the block input into its slice; an average branch pools it (count_include_pad as its row says: False in
+      Inception-v4 / Inception-ResNet-v2, True in Inception-v3) into a matrix that its 1x1 projection reads, writing its slice;
     * a residual block (Block35 / 17 / 8) closes with one GEMM over ``y``: per-column scale ``block.scale``, shift
       ``scale * bias``, the block input as residual, ReLU unless ``noReLU`` (inceptionresnetv2.py:113-117)."""
     from .models.inception import BRANCHES, RESIDUAL
@@ -911,7 +912,7 @@ def _inception_block_body(block, a, out=None):
         if br[0] == 'max':
             _max3s2(a, y[:, c0:c0 + wd])
         elif br[0] == 'avg':
-            pooled = ops.pool_slice(a, 3, 1, 1, True, count_include_pad=False)
+            pooled = ops.pool_slice(a, 3, 1, 1, True, count_include_pad=br[2])
             _basic_unit(get(br[1][-1]), pooled, y[:, c0:c0 + wd])
         else:
             paths = br[1]
@@ -941,9 +942,10 @@ def _inception_block_body(block, a, out=None):
 
 
 def run_inception_trunk(n_stem, units, x):
-    """The trunk of Inception-v4 (``units`` = ``features``) or Inception-ResNet-v2: fp32 NCHW images (or an Act with channel
-    pitch 8) in, the final 1536-channel map (an Act) out.  ``units[:n_stem]`` run as one stem Function, every block as one
-    ``InceptionBlockFunction``, a trailing BasicConv2d (conv2d_7b) as a stem Function of its own."""
+    """The trunk of Inception-v4 (``units`` = ``features``), Inception-ResNet-v2 or Inception-v3: fp32 NCHW images (or an Act
+    with channel pitch 8) in, the final 8x8 map (an Act; 1536 channels, 2048 for Inception-v3) out.  ``units[:n_stem]`` run as
+    one stem Function, every block as one ``InceptionBlockFunction``, a trailing BasicConv2d (conv2d_7b) as a stem Function of its
+    own."""
     from .models.inception import BasicConv2d
     a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
     if (a.H, a.W) != (299, 299):

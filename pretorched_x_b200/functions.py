@@ -167,8 +167,9 @@ class InceptionFunction(_FrozenFunction):
 
 
 class InceptionStemFunction(_FrozenFunction):
-    """Units of Inception-v4 / Inception-ResNet-v2 outside the blocks, in sequence (``units``: a tuple of BasicConv2d /
-    MaxPool2d): the stems (inceptionv4.py:274-276, inceptionresnetv2.py:305-311) and conv2d_7b (:319)."""
+    """Units of Inception-v4 / Inception-ResNet-v2 / Inception-v3 outside the blocks, in sequence (``units``: a tuple of
+    BasicConv2d / MaxPool2d): the stems (inceptionv4.py:274-276, inceptionresnetv2.py:305-311, torchvision_models.py:397-403)
+    and conv2d_7b (inceptionresnetv2.py:319)."""
 
     @staticmethod
     def forward(ctx, x2d, geom, units, out=None):
@@ -177,8 +178,8 @@ class InceptionStemFunction(_FrozenFunction):
 
 
 class InceptionBlockFunction(_FrozenFunction):
-    """One block of Inception-v4 / Inception-ResNet-v2 (models.inception.BRANCHES): its branches written in place into the
-    concatenated output, and the residual close of Block35 / 17 / 8."""
+    """One block of Inception-v4 / Inception-ResNet-v2 / Inception-v3 (models.inception.BRANCHES): its branches written in place
+    into the concatenated output, and the residual close of Block35 / 17 / 8."""
 
     @staticmethod
     def forward(ctx, x2d, geom, block, out=None):

@@ -54,32 +54,47 @@ def _pool_branch(cin, proj):
 # Blocks as data (engine._inception_block_body): BRANCHES[kind] lists the branches in the order of the reference's torch.cat.
 #   ('chain', paths)        BasicConv2d units in sequence from the block input, the last one writes the branch's slice
 #   ('fork', paths, (a, b)) a chain whose output feeds two units that write adjacent slices (Inception-C, inceptionv4.py:245-255)
-#   ('max', path)           MaxPool2d(3, stride=2) of the block input, its slice the block input's channels
-#   ('avg', paths)          AvgPool2d(3, 1, 1, count_include_pad=False) of the block input, then the unit(s) in ``paths``
+#   ('max', path)           MaxPool2d(3, stride=2) of the block input, its slice the block input's channels (``path`` None: a
+#                           functional F.max_pool2d(3, 2), as in torchvision's blocks)
+#   ('avg', paths, incl)    AvgPool2d(3, 1, 1) of the block input, the padding counted in the divisor when ``incl``
+#                           (count_include_pad), then the unit(s) in ``paths``
 # RESIDUAL kinds close with ``conv2d`` (1x1 with bias): out = relu(conv2d(cat) * scale + x) (inceptionresnetv2.py:109-117).
+# The Inception* rows are torchvision's Inception3 blocks (models/inceptionv3.py), whose pools are functional calls.
 BRANCHES = {
     'Mixed_3a': [('max', 'maxpool'), ('chain', ['conv'])],
     'Mixed_4a': [('chain', ['branch0.0', 'branch0.1']), ('chain', ['branch1.0', 'branch1.1', 'branch1.2', 'branch1.3'])],
     'Mixed_5a': [('chain', ['conv']), ('max', 'maxpool')],
     'Inception_A': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1']), ('chain', ['branch2.0', 'branch2.1', 'branch2.2']),
-                    ('avg', ['branch3.1'])],
+                    ('avg', ['branch3.1'], False)],
     'Reduction_A': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1', 'branch1.2']), ('max', 'branch2')],
     'Inception_B': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1', 'branch1.2']),
-                    ('chain', ['branch2.0', 'branch2.1', 'branch2.2', 'branch2.3', 'branch2.4']), ('avg', ['branch3.1'])],
+                    ('chain', ['branch2.0', 'branch2.1', 'branch2.2', 'branch2.3', 'branch2.4']), ('avg', ['branch3.1'], False)],
     'Reduction_B': [('chain', ['branch0.0', 'branch0.1']), ('chain', ['branch1.0', 'branch1.1', 'branch1.2', 'branch1.3']),
                     ('max', 'branch2')],
     'Inception_C': [('chain', ['branch0']), ('fork', ['branch1_0'], ('branch1_1a', 'branch1_1b')),
-                    ('fork', ['branch2_0', 'branch2_1', 'branch2_2'], ('branch2_3a', 'branch2_3b')), ('avg', ['branch3.1'])],
+                    ('fork', ['branch2_0', 'branch2_1', 'branch2_2'], ('branch2_3a', 'branch2_3b')), ('avg', ['branch3.1'], False)],
     'Mixed_5b': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1']), ('chain', ['branch2.0', 'branch2.1', 'branch2.2']),
-                 ('avg', ['branch3.1'])],
+                 ('avg', ['branch3.1'], False)],
     'Block35': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1']), ('chain', ['branch2.0', 'branch2.1', 'branch2.2'])],
     'Mixed_6a': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1', 'branch1.2']), ('max', 'branch2')],
     'Block17': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1', 'branch1.2'])],
     'Mixed_7a': [('chain', ['branch0.0', 'branch0.1']), ('chain', ['branch1.0', 'branch1.1']),
                  ('chain', ['branch2.0', 'branch2.1', 'branch2.2']), ('max', 'branch3')],
     'Block8': [('chain', ['branch0']), ('chain', ['branch1.0', 'branch1.1', 'branch1.2'])],
+    'InceptionA': [('chain', ['branch1x1']), ('chain', ['branch5x5_1', 'branch5x5_2']),
+                   ('chain', ['branch3x3dbl_1', 'branch3x3dbl_2', 'branch3x3dbl_3']), ('avg', ['branch_pool'], True)],
+    'InceptionB': [('chain', ['branch3x3']), ('chain', ['branch3x3dbl_1', 'branch3x3dbl_2', 'branch3x3dbl_3']), ('max', None)],
+    'InceptionC': [('chain', ['branch1x1']), ('chain', ['branch7x7_1', 'branch7x7_2', 'branch7x7_3']),
+                   ('chain', ['branch7x7dbl_1', 'branch7x7dbl_2', 'branch7x7dbl_3', 'branch7x7dbl_4', 'branch7x7dbl_5']),
+                   ('avg', ['branch_pool'], True)],
+    'InceptionD': [('chain', ['branch3x3_1', 'branch3x3_2']), ('chain', ['branch7x7x3_1', 'branch7x7x3_2', 'branch7x7x3_3',
+                                                                         'branch7x7x3_4']), ('max', None)],
+    'InceptionE': [('chain', ['branch1x1']), ('fork', ['branch3x3_1'], ('branch3x3_2a', 'branch3x3_2b')),
+                   ('fork', ['branch3x3dbl_1', 'branch3x3dbl_2'], ('branch3x3dbl_3a', 'branch3x3dbl_3b')),
+                   ('avg', ['branch_pool'], True)],
 }
 RESIDUAL = ('Block35', 'Block17', 'Block8')
+V3_KINDS = ('InceptionA', 'InceptionB', 'InceptionC', 'InceptionD', 'InceptionE')   # their classes are in models/inceptionv3.py
 
 
 class _Block(engine.CacheOwner, nn.Module):
@@ -217,7 +232,8 @@ class Block8(_Block):
 
 
 for _k in BRANCHES:
-    globals()[_k].kind = _k
+    if _k not in V3_KINDS:
+        globals()[_k].kind = _k
 
 
 class _Trunk(Trunk):

@@ -13,6 +13,7 @@ import torch  # noqa: E402
 import pretorched_x_b200 as P  # noqa: E402
 from pretorched_x_b200 import _lib, engine  # noqa: E402
 from oracle import functional as OF  # noqa: E402  (seeded BN statistics only)
+from oracle import inceptionv3 as OV3  # noqa: E402  (Inception-v3's weights rescaled to stay in fp16 range)
 
 dev = torch.device("cuda:0")
 only = set(sys.argv[1:])
@@ -59,6 +60,7 @@ case("se_resnext50_32x4d", lambda: P.se_resnext50_32x4d(pretrained=None), (2, 3,
 case("slowfast18", lambda: P.slowfast.resnet18(mode="sf", num_classes=12), (1, 3, 32, 64, 64))
 case("densenet121", lambda: P.densenet121(pretrained=None), (2, 3, 224, 224))
 case("densenet161", lambda: P.densenet161(pretrained=None), (1, 3, 224, 224))
+case("inceptionv3", lambda: OV3.fan_in_scale_(P.inceptionv3(pretrained=None)), (1, 3, 299, 299))
 
 if not only or "trn" in only:
     torch.manual_seed(0)
