@@ -178,6 +178,19 @@ int b2_gemm_chain_f16(const b2_gemm_args* a, const void* a2, int lda2, const voi
  * N % 8 == 0; fp16 output (columns [N, ldd) written as zero; residual columns >= N never read); per_row, out_f32, accumulate,
  * d2 and mask must be zero / NULL (B2_ERR_INVALID).  Always the persistent GEMM (b2_debug_last_gemm_path() == 2). */
 int b2_gemm_sample_affine_f16(const b2_gemm_args* a, void* stream);
+/* Two fp16 outputs from one fp32 accumulator acc = A.B^T:
+ *     d  = act(scale[n] * acc + shift[n] + residual[m][n])          (as b2_gemm_f16; a: its args, act = ReLU when a->relu)
+ *     d2 = relu(scale2[n] * acc + shift2[n])                         fp16 [M][ldd2], scale2 / shift2 fp32 [N]
+ * The closing 1x1 convolution of one application of a PolyNet poly-3 module (polynet.py:229-326): with (sb, tb) the folded
+ * BatchNorm of that application's conv2d and s the module's scale, scale = s * sb, shift = s * tb, residual = the running sum,
+ * so d is the new running sum and d2 = relu(sb * acc + tb) the next application's input.  d2 is not relu(d * scale2 + shift2)
+ * (the generator's second output, b2_gemm_args.d2): it is taken from the accumulator, before the residual joins.
+ * Contract: fp16 d with a per-column affine (columns [N, ldd) written as zero, residual columns >= N never read); d2 has d's
+ * pitch (ldd2 == ldd; its columns [N, ldd) are written as zero too), is 16-byte aligned and shares no byte with d, A, B or the
+ * residual (B2_ERR_INVALID).  out_f32, per_row, accumulate, aff_ld / aff_rows (per-sample affines), mask, and the args' own d2 / scale2 /
+ * shift2 / aff2 fields must be zero (B2_ERR_UNSUPPORTED).  Always the persistent GEMM (b2_debug_last_gemm_path() == 2;
+ * b2_debug_last_kernel: KID 6, info = {N tile, 4, 0}).  d is bitwise what b2_gemm_f16 writes for the same arguments. */
+int b2_gemm_dual_f16(const b2_gemm_args* a, const float* scale2, const float* shift2, void* d2, int ldd2, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Non-local block core (nonlocalnet.py:143-211):

@@ -29,6 +29,7 @@ from .models.bninception import bninception  # noqa: F401  (pretorched/models/bn
 from .models.inception import inceptionv4, inceptionresnetv2  # noqa: F401  (pretorched/__init__.py:16-17)
 from .models.densenet import densenet121, densenet161, densenet169, densenet201  # noqa: F401  (pretorched/__init__.py:21-24)
 from .models.inceptionv3 import inceptionv3  # noqa: F401  (pretorched/__init__.py:30)
+from .models.polynet import polynet  # noqa: F401  (pretorched/__init__.py:55)
 from .models.trn import Relation, MultiScaleRelation, HierarchicalRelation, TRN, trn  # noqa: F401
 from .models.utils import Identity  # noqa: F401
 # BigGAN-deep generator (BASELINE.json configs[4]; not in the reference tree -- see models/biggan_deep.py)

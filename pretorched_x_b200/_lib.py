@@ -116,6 +116,7 @@ SYMBOLS = {
     "b2_pool_ndhwc_slice": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 19 + [c_void_p]),
     "b2_avgpool_ndhwc_slice_exclude_pad": (c_int, [c_void_p, c_int, c_void_p] + [c_int] * 18 + [c_void_p]),
     "b2_gemm_preact_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p, c_void_p, c_void_p]),
+    "b2_gemm_dual_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "b2_bn_relu_avgpool2_ndhwc": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_int] * 4 + [c_void_p, c_void_p, c_void_p]),
     "b2_avgpool_global_affine_ndhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
 }

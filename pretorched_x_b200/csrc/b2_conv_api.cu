@@ -1132,6 +1132,37 @@ static int launch_pgemm_split(const b2_gemm_args* g, int nd, void* const* y, con
   return B2_OK;
 }
 
+// The dual instance (b2_gemm_dual_f16): pgemm_kernel<BN, 0, 4>, d through tmC as b2_gemm_f16 writes it, d2 through tmC2.
+template <int BN>
+static int launch_pgemm_dual(const b2_gemm_args* g, const float* scale2, const float* shift2, void* d2, int ldd2, cudaStream_t stream) {
+  using S = PgemmSmem<BN, 0, 1>;
+  B2_OPT_IN_SMEM((pgemm_kernel<BN, 0, 4>), S::kTotal);
+  CUtensorMap tmA, tmB, tmC, tmR, tmC2;
+  int rc;
+  if ((rc = make_tmap_2d_f16(&tmA, g->a, (uint64_t)g->Kd, (uint64_t)g->M, (uint64_t)g->lda, 64, 128, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmB, g->b, (uint64_t)g->Kd, (uint64_t)g->N, (uint64_t)g->ldb, 64, BN, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmC, g->d, (uint64_t)g->ldd, (uint64_t)g->M, (uint64_t)g->ldd, 64, 64, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmC2, d2, (uint64_t)ldd2, (uint64_t)g->M, (uint64_t)ldd2, 64, 64, true)) != B2_OK) return rc;
+  tmR = tmC;
+  if (g->residual && (rc = make_tmap_2d_f16(&tmR, g->residual, (uint64_t)g->N, (uint64_t)g->M, (uint64_t)g->ldr, 64, 128, true)) != B2_OK)
+    return rc;
+  PgemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.M = g->M; p.Ncols = g->N; p.ldy = g->ldd; p.nkb = (g->Kd + 63) / 64; p.nkb2 = 0;
+  p.tiles_n = (g->ldd + BN - 1) / BN;
+  p.tiles_total = p.tiles_n * ((g->M + 127) / 128);
+  p.scale = g->scale; p.shift = g->shift;
+  p.has_residual = g->residual != nullptr;
+  p.relu = g->relu;
+  p.dual = 1; p.scale2 = scale2; p.shift2 = shift2; p.aff2_ld = 0; p.aff2_rows = 128;   // one per-column row for every tile
+  p.fd_Wh = make_fastdiv(2); p.fd_Hh = make_fastdiv(2); p.fd_aff = make_fastdiv(1);
+  const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
+  B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, 0, 4>, dim3(grid), dim3(kPgThreads), S::kTotal, stream, tmA, tmB, tmA, tmB, tmC, tmR, tmC2, p));
+  B2_CHECK_LAUNCH("pgemm_kernel");
+  set_last_kernel(KID_PGEMM, BN, 4, 0);
+  return B2_OK;
+}
+
 static int g_last_gemm_path = 0;   // kernel of the last GEMM-family launch: 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (tests pin it)
 
 static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
@@ -1614,6 +1645,40 @@ int b2_gemm_preact_f16(const b2_gemm_args* g, const float* in_scale, const float
   g_last_gemm_path = 2;
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return g->ldd <= 64 ? launch_pgemm<64, 1>(L, st) : launch_pgemm<128, 1>(L, st);
+}
+
+static bool spans_overlap(const void* p, size_t pn, const void* q, size_t qn) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+  return p && q && a < b + qn && b < a + pn;
+}
+
+int b2_gemm_dual_f16(const b2_gemm_args* g, const float* scale2, const float* shift2, void* d2, int ldd2, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(g != nullptr && g->a && g->b && g->scale && g->shift && g->d && scale2 && shift2 && d2, "null tensor pointer");
+  B2_CHECK_ARG(g->M > 0 && g->N > 0 && g->Kd > 0, "non-positive dimension");
+  B2_CHECK_ARG(g->lda % 8 == 0 && g->ldb % 8 == 0 && g->lda >= g->Kd && g->ldb >= g->Kd, "bad operand pitch");
+  B2_CHECK_ARG(g->ldd % 8 == 0 && g->ldd >= g->N && ldd2 == g->ldd, "bad output pitch (ldd %d, ldd2 %d, N %d): d2 has d's pitch",
+               g->ldd, ldd2, g->N);
+  B2_CHECK_ARG(g->residual == nullptr || (g->ldr % 8 == 0 && g->ldr >= g->N), "bad residual pitch");
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(d2) & 15) == 0, "d2 must be 16-byte aligned");
+  if (g->out_f32 || g->per_row || g->accumulate || g->aff_ld || g->aff_rows || g->d2 || g->scale2 || g->shift2 || g->aff2_ld ||
+      g->aff2_rows || g->mask || g->ldm)
+    return set_error(B2_ERR_UNSUPPORTED, "the dual GEMM takes fp16 output with per-column affines: out_f32, per_row, accumulate, "
+                     "aff_ld / aff_rows, the args' own d2 / scale2 / shift2 / aff2 fields and mask must be zero");
+  // d2 is written while A, the residual and d are live: it may share no byte with them
+  const size_t d2n = static_cast<size_t>(g->M) * ldd2 * 2;
+  B2_CHECK_ARG(!spans_overlap(d2, d2n, g->d, static_cast<size_t>(g->M) * g->ldd * 2) &&
+                   !spans_overlap(d2, d2n, g->a, (static_cast<size_t>(g->M - 1) * g->lda + g->Kd) * 2) &&
+                   !spans_overlap(d2, d2n, g->b, (static_cast<size_t>(g->N - 1) * g->ldb + g->Kd) * 2) &&
+                   !spans_overlap(d2, d2n, g->residual, (static_cast<size_t>(g->M - 1) * g->ldr + g->N) * 2),
+               "d2 overlaps d, A, B or the residual");
+  if (g_gemm_algo != 0) return set_error(B2_ERR_UNSUPPORTED, "the dual GEMM needs the persistent kernel");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  g_last_gemm_path = 2;
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // the N tile b2_gemm_f16 picks for an output of this pitch
+  return g->ldd <= 64 ? launch_pgemm_dual<64>(g, scale2, shift2, d2, ldd2, st) : launch_pgemm_dual<128>(g, scale2, shift2, d2, ldd2, st);
 }
 
 int b2_gemm_split_plan(int nd, const int* cols, int* box0) {

@@ -19,6 +19,11 @@
 //   warps 0-7   two consumer warpgroups: wgmma main loop, epilogue, TMA store of their 64 rows
 //   warp 8      producer: the K blocks of tile i (A and B boxes, 128B-swizzled), then its residual tile
 //   warps 9-12  generator instance only: A-operand transform (see PgemmParams::in_scale)
+//
+// Dual instance (pgemm_kernel<BN, 0, 4>, b2_gemm_dual_f16): a second fp16 output taken from the same fp32 accumulator,
+//     d2 = relu(scale2[n] * acc + shift2[n]),
+// next to d = act(scale[n] * acc + shift[n] + residual).  One application of a PolyNet poly-3 module closes with it: d is the
+// running sum, d2 the next application's input, from one pass over the concatenated branches.
 #pragma once
 
 #include "b2_ptx.cuh"
@@ -55,7 +60,7 @@ struct PgemmParams {
   int res_pre;              // 1: y = act(scale * (acc + residual) + shift) instead of act(scale * acc + shift + residual)
   // Second output (pgemm_kernel<BN, 1>): y2 = relu(y * scale2[m / aff2_rows][n] + shift2[...]) -- the class-conditional
   // BatchNorm + ReLU of the NEXT block applied to this block's fp32 result, staged in a tile of its own and written through tmC2.
-  int dual;
+  int dual;                 // pgemm_kernel<BN, 0, 4> too: d2 = relu(scale2[n] * acc + shift2[n]) of the accumulator (aff2_ld = 0)
   const float* scale2;
   const float* shift2;
   int aff2_ld, aff2_rows;
@@ -80,19 +85,19 @@ struct PgemmParams {
   int split_box[4];
 };
 
-template <int BN, int GAN>
+template <int BN, int GAN, int C2 = GAN>   // C2: a second-output staging tile (generator and dual instances)
 struct PgemmSmem {
   static constexpr int kABytes = 128 * 128;
   static constexpr int kBBytes = BN * 128;
   static constexpr int kStage = kABytes + kBBytes;
   static constexpr int kTile = 128 * BN * 2;                 // fp16 128 x BN tile: BN / 64 boxes of [128 rows][128 B], 128B-swizzled
   static constexpr int kAffBytes = 2 * 4 * BN * 4;           // per consumer warpgroup: scale, shift, scale2, shift2 of the tile
-  static constexpr int kFixed = 2 * kTile + (GAN ? kTile : 0) + 256 + kAffBytes + 1024;
+  static constexpr int kFixed = 2 * kTile + (C2 ? kTile : 0) + 256 + kAffBytes + 1024;
   // operand ring: as deep as the budget allows, up to kPgMaxStages (BN = 128: 4 stages, 3 with the generator's second-output tile)
   static constexpr int kStages = (227 * 1024 - kFixed) / kStage < kPgMaxStages ? (227 * 1024 - kFixed) / kStage : kPgMaxStages;
   static constexpr int kResOff = kStages * kStage;           // 2 residual / output staging tiles
   static constexpr int kC2Off = kResOff + 2 * kTile;         // second-output staging tile (generator instance)
-  static constexpr int kBarOff = kC2Off + (GAN ? kTile : 0);
+  static constexpr int kBarOff = kC2Off + (C2 ? kTile : 0);
   static constexpr int kAffOff = kBarOff + 256;
   static constexpr int kTotal = kAffOff + kAffBytes + 1024;
   static_assert(kStages >= 3 && kTotal <= 227 * 1024, "shared memory budget");
@@ -109,13 +114,14 @@ __device__ __forceinline__ uint32_t pg_sw_off(int row, int j, int c) {
 
 template <int BN, int GAN, int EPI = 0>    // GAN = 1: instance with the generator extras (res_up gather, res_pre, dual output, A transform);
                                            // 0: the classic epilogue.  With GAN = 0, EPI = 1: ReLU-derivative mask operand (fine-tuning
-                                           // backward); EPI = 2: per-sample affine resolved per fragment row (see PgemmParams::fd_aff)
+                                           // backward); EPI = 2: per-sample affine resolved per fragment row (see PgemmParams::fd_aff);
+                                           // EPI = 3: column-slice destinations; EPI = 4: second output from the accumulator (dual)
 __global__ void __launch_bounds__(GAN ? kPgThreadsGan : kPgThreads, 1)
 pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
              const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
              const __grid_constant__ CUtensorMap tmC2, const PgemmParams p) {
-  using S = PgemmSmem<BN, GAN>;
+  using S = PgemmSmem<BN, GAN, GAN || EPI == 4>;
   constexpr int kSt = S::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align<1024>(smem_raw);
@@ -208,7 +214,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         const size_t arow = p.aff_ld ? static_cast<size_t>(m0 / p.aff_rows) * p.aff_ld : 0;
         aff[0] = __ldg(&p.scale[arow + n0 + wt]);
         aff[1] = __ldg(&p.shift[arow + n0 + wt]);
-        if (GAN && p.dual) {
+        if ((GAN || EPI == 4) && p.dual) {
           const size_t arow2 = static_cast<size_t>(m0 / p.aff2_rows) * p.aff2_ld;
           aff[2] = __ldg(&p.scale2[arow2 + n0 + wt]);
           aff[3] = __ldg(&p.shift2[arow2 + n0 + wt]);
@@ -246,6 +252,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       const int rb = lt & 1;
       mbar_wait(&res_full[rb], (lt >> 1) & 1);
       uint8_t* stage = smem + S::kResOff + rb * S::kTile;
+      uint8_t* stage2 = smem + S::kC2Off;                  // second output (generator / dual instances): free since the bar above
       int rsrc[2] = {fr, fr + 8};                          // row of the residual box each fragment row adds
       const float* aff_rs[2] = {nullptr, nullptr};         // EPI = 2: scale / shift rows of the two fragment rows' samples
       const float* aff_rh[2] = {nullptr, nullptr};
@@ -276,6 +283,13 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           float2 rf = make_float2(0.f, 0.f);
           if (p.has_residual) rf = unpack_half2(*reinterpret_cast<const uint32_t*>(stage + pg_sw_off(rsrc[i], j, fc)));
           float a0 = acc[4 * j + 2 * i], a1 = acc[4 * j + 2 * i + 1];
+          if constexpr (EPI == 4) {
+            // d2 from the accumulator before the first epilogue overwrites it (columns >= Ncols: zero affine, relu(0) = 0)
+            const float2 sc2 = *reinterpret_cast<const float2*>(s_aff + 2 * BN + c);
+            const float2 sh2 = *reinterpret_cast<const float2*>(s_aff + 3 * BN + c);
+            *reinterpret_cast<uint32_t*>(stage2 + pg_sw_off(fr + 8 * i, j, fc)) =
+                pack_half2(fmaxf(a0 * sc2.x + sh2.x, 0.f), fmaxf(a1 * sc2.y + sh2.y, 0.f));
+          }
           if (GAN && p.res_pre) {
             a0 = (a0 + rf.x) * sc.x + sh.x;
             a1 = (a1 + rf.y) * sc.y + sh.y;
@@ -329,10 +343,15 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           } else {
             if (n0 + b * 64 < p.ldy) tma_store_2d(&tmC, stage + b * (128 * 128) + wg * (64 * 128), n0 + b * 64, m0 + wg * 64);
           }
+        if constexpr (EPI == 4) {
+          // d2 has d's pitch: its columns [Ncols, ldy) are written as zero too (zero affine, zero-filled B rows)
+#pragma unroll
+          for (int b = 0; b < BN / 64; ++b)
+            if (n0 + b * 64 < p.ldy) tma_store_2d(&tmC2, stage2 + b * (128 * 128) + wg * (64 * 128), n0 + b * 64, m0 + wg * 64);
+        }
         tma_store_commit();
       }
       if (GAN && p.dual) {                                 // second output: next block's ccbn + ReLU on the fp32 value
-        uint8_t* stage2 = smem + S::kC2Off;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int c = 8 * j + fc;

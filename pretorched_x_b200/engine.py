@@ -23,12 +23,14 @@ Function's ``forward`` is the ctypes call sequence, its outputs are marked non-d
 semantics), except for the stages a ``fine_tune(k)`` call (``ResNet3D``, ``ResNet2D``, ``TRN``) made trainable (``block_backward``), and the dense heads (``last_linear``, the TRN
 relation MLPs) have a real backward on the same wgmma GEMM so that a head can be trained on engine features.
 """
+import copy
 import os
 
 import torch
 import torch.nn as nn
 
 from . import ops
+from . import ops_dual
 from . import functions as Fn
 from .ops import Act
 
@@ -865,49 +867,27 @@ def _branch_hw(block, a, br):
     return H, W
 
 
-def _inception_block_body(block, a, out=None):
-    """One block of Inception-v4 / Inception-ResNet-v2 / Inception-v3 from its row of models.inception.BRANCHES.  The branches
-    write their columns of the concatenated output ``y`` in place:
-
-    * the 1x1 units that read the block input (a lone 1x1 branch straight into its slice, the first unit of a longer chain into its
-      own matrix) run as one split GEMM -- one pass over the block input;
-    * every later unit of a chain runs on the slab kernel's slice entry, the last one into the branch's slice; a fork's two units
-      read the same matrix and write adjacent slices;
-    * a max branch pools the block input into its slice; an average branch pools it (count_include_pad as its row says: False in
-      Inception-v4 / Inception-ResNet-v2, True in Inception-v3) into a matrix that its 1x1 projection reads, writing its slice;
-    * a residual block (Block35 / 17 / 8) closes with one GEMM over ``y``: per-column scale ``block.scale``, shift
-      ``scale * bias``, the block input as residual, ReLU unless ``noReLU`` (inceptionresnetv2.py:113-117)."""
-    from .models.inception import BRANCHES, RESIDUAL
-    kind = type(block).kind
-    branches = BRANCHES[kind]
-    get = block.get_submodule
-    if a.ld != a.C:
-        raise ValueError("%s takes a dense [M][C] input, got %r" % (kind, a))
-    Ho, Wo = _branch_hw(block, a, branches[0])
-    widths = [_branch_width(block, a, br) for br in branches]
-    cols = [sum(widths[:i]) for i in range(len(widths))]
-    C = sum(widths)
-    M = a.N * a.T * Ho * Wo
-    dev = a.data.device
-    residual = kind in RESIDUAL
-    if out is not None and not residual:
-        y = ops._out_rows(out, M, C)
-    else:
-        y = torch.empty((M, C), dtype=torch.float16, device=dev)
-    heads, dests, temps = [], [], {}
-    for br, c0, wd in zip(branches, cols, widths):
+def _branch_heads(get, branches, a, y, cols, temps):
+    """The 1x1 units of a row that read the block input ``a`` (``get``: the block's get_submodule) and their split-GEMM
+    destinations: a lone 1x1 branch writes its slice of ``y``, the first unit of a longer chain a fresh matrix (kept in ``temps``
+    under its path)."""
+    heads, dests = [], []
+    for br, c0 in zip(branches, cols):
         if br[0] in ('chain', 'fork') and _is_head(get(br[1][0])):
             u = get(br[1][0])
             K = u.conv.out_channels
             if br[0] == 'chain' and len(br[1]) == 1:
                 dests.append(y[:, c0:c0 + K])
             else:
-                temps[br[1][0]] = torch.empty((a.M, K), dtype=torch.float16, device=dev)
+                temps[br[1][0]] = torch.empty((a.M, K), dtype=torch.float16, device=a.data.device)
                 dests.append(temps[br[1][0]])
             heads.append(u)
-    if heads:
-        w, scale, shift = _split_pack_convs([u.conv for u in heads], [u.bn for u in heads], a.ld)
-        ops.gemm_split(a.data, w, scale, shift, a.M, a.ld, dests, relu=True)
+    return heads, dests
+
+
+def _branch_bodies(get, branches, a, y, cols, widths, temps):
+    """Everything of a row after its split GEMM: pools, and the units of each chain / fork after its head, each branch ending in
+    its slice of ``y``."""
     for br, c0, wd in zip(branches, cols, widths):
         if br[0] == 'max':
             _max3s2(a, y[:, c0:c0 + wd])
@@ -926,6 +906,44 @@ def _inception_block_body(block, a, out=None):
                 K = u.conv.out_channels
                 _basic_unit(u, h, y[:, c:c + K])
                 c += K
+
+
+def _inception_block_body(block, a, out=None, row=None):
+    """One block of Inception-v4 / Inception-ResNet-v2 / Inception-v3 from its row of models.inception.BRANCHES (or ``row``: a
+    row of another table in that format, as PolyNet's).  The branches write their columns of the concatenated output ``y`` in
+    place:
+
+    * the 1x1 units that read the block input (a lone 1x1 branch straight into its slice, the first unit of a longer chain into its
+      own matrix) run as one split GEMM -- one pass over the block input;
+    * every later unit of a chain runs on the slab kernel's slice entry, the last one into the branch's slice; a fork's two units
+      read the same matrix and write adjacent slices;
+    * a max branch pools the block input into its slice; an average branch pools it (count_include_pad as its row says: False in
+      Inception-v4 / Inception-ResNet-v2, True in Inception-v3) into a matrix that its 1x1 projection reads, writing its slice;
+    * a residual block (Block35 / 17 / 8) closes with one GEMM over ``y``: per-column scale ``block.scale``, shift
+      ``scale * bias``, the block input as residual, ReLU unless ``noReLU`` (inceptionresnetv2.py:113-117)."""
+    from .models.inception import BRANCHES, RESIDUAL
+    kind = getattr(type(block), 'kind', None) or type(block).__name__
+    branches = BRANCHES[kind] if row is None else row
+    get = block.get_submodule
+    if a.ld != a.C:
+        raise ValueError("%s takes a dense [M][C] input, got %r" % (kind, a))
+    Ho, Wo = _branch_hw(block, a, branches[0])
+    widths = [_branch_width(block, a, br) for br in branches]
+    cols = [sum(widths[:i]) for i in range(len(widths))]
+    C = sum(widths)
+    M = a.N * a.T * Ho * Wo
+    dev = a.data.device
+    residual = row is None and kind in RESIDUAL
+    if out is not None and not residual:
+        y = ops._out_rows(out, M, C)
+    else:
+        y = torch.empty((M, C), dtype=torch.float16, device=dev)
+    temps = {}
+    heads, dests = _branch_heads(get, branches, a, y, cols, temps)
+    if heads:
+        w, scale, shift = _split_pack_convs([u.conv for u in heads], [u.bn for u in heads], a.ld)
+        ops.gemm_split(a.data, w, scale, shift, a.M, a.ld, dests, relu=True)
+    _branch_bodies(get, branches, a, y, cols, widths, temps)
     if not residual:
         return Act(y, a.N, a.T, Ho, Wo, C)
     conv = block.conv2d
@@ -954,6 +972,179 @@ def run_inception_trunk(n_stem, units, x):
     a = Fn.InceptionStemFunction.run(tuple(units[:n_stem]), a)
     for u in units[n_stem:]:
         a = Fn.InceptionStemFunction.run((u,), a) if isinstance(u, BasicConv2d) else Fn.InceptionBlockFunction.run(u, a)
+    return a
+
+
+# ---------------------------------------------------------------------------------------------
+# PolyNet (polynet.py): the Inception block path above, 2-way modules closed by one two-operand GEMM, poly-3 modules by the dual GEMM
+# ---------------------------------------------------------------------------------------------
+def _polynet_stem_body(stem, a):
+    """conv1 (three BasicConv2d units), then the stem's three concatenations as rows Stem1-3 of models.polynet.BRANCHES
+    (polynet.py:91-105)."""
+    from .models.polynet import BRANCHES
+    a = _inception_stem_body(tuple(stem.conv1), a)
+    for k in ('Stem1', 'Stem2', 'Stem3'):
+        a = _inception_block_body(stem, a, row=BRANCHES[k])
+    return a
+
+
+def _polynet_2way_body(module, a):
+    """out = relu(x + s * A(x) + s * B(x)) (MultiWay, polynet.py:329-344).  Both blocks write their branches into their own
+    concatenation matrix; their 1x1 heads, which all read x, run as one split GEMM (two when there are more heads than its four
+    destinations: Inception-ResNet-A's three per block).  The close is ONE two-operand GEMM over both matrices, with
+    s * (closing BatchNorm scale) folded into each fp16 filter and the shifts summed, x as residual and ReLU: x + s * A(x) is never
+    written out."""
+    from .models.polynet import BRANCHES
+    blocks = list(module.blocks)
+    if len(blocks) != 2:
+        raise NotImplementedError("the engine runs 2-way modules, got %d blocks" % len(blocks))
+    branches = BRANCHES[type(blocks[0]).__name__]
+    if a.ld != a.C:
+        raise ValueError("%s takes a dense [M][C] input, got %r" % (type(module).__name__, a))
+    widths = [_branch_width(blocks[0], a, br) for br in branches]
+    cols = [sum(widths[:i]) for i in range(len(widths))]
+    C = sum(widths)
+    dev = a.data.device
+    ys, temps, heads, dests = [], [], [], []
+    for b in blocks:
+        y = torch.empty((a.M, C), dtype=torch.float16, device=dev)
+        t = {}
+        h, d = _branch_heads(b.get_submodule, branches, a, y, cols, t)
+        ys.append(y)
+        temps.append(t)
+        heads.append(h)
+        dests.append(d)
+    groups = [(heads[0] + heads[1], dests[0] + dests[1])] if len(heads[0]) + len(heads[1]) <= 4 else list(zip(heads, dests))
+    for hs, ds in groups:
+        w, scale, shift = _split_pack_convs([u.conv for u in hs], [u.bn for u in hs], a.ld)
+        ops.gemm_split(a.data, w, scale, shift, a.M, a.ld, ds, relu=True)
+    for b, y, t in zip(blocks, ys, temps):
+        _branch_bodies(b.get_submodule, branches, a, y, cols, widths, t)
+    units = [b.conv2d for b in blocks]
+    K = units[0].conv.out_channels
+
+    def build():
+        s = float(module.scale)
+        ws, shift = [], torch.zeros(K, dtype=torch.float64, device=dev)
+        for u in units:
+            sb, tb = ops.fold_affine(K, None, u.bn, dev)
+            ws.append((_conv1x1_matrix(u.conv).double() * (s * sb.double())[:, None]).to(torch.float16).contiguous())
+            shift = shift + s * tb.double()
+        return ws[0], ws[1], torch.ones(K, dtype=torch.float32, device=dev), shift.float().contiguous()
+
+    sig = _sig(*[t for u in units for t in (u.conv.weight,) + _bn_tensors(u.bn)]) + (float(module.scale),)
+    w0, w1, ones, shift = _cached(module, "close2", sig, build)
+    z = ops.gemm(ys[0], w0, ones, shift, a.M, K, C, residual=a.data, relu=True, second=(ys[1], w1, C))
+    return Act(z, a.N, a.T, a.H, a.W, K)
+
+
+def _poly_split_pack(module, heads, i, in_pitch):
+    """The split GEMM of one poly application's 1x1 heads (PolyConv2d units reading x_i): the fp16 filter rows packed once per
+    module, the folded affine of BatchNorms ``bn_blocks[i]`` per application (its cache key holds those BatchNorms)."""
+    dev = heads[0].conv.weight.device
+
+    def build(bns):
+        npad, box0 = ops.split_plan([u.conv.out_channels for u in heads])
+        w = torch.zeros((npad, in_pitch), dtype=torch.float16, device=dev)
+        scale = torch.zeros(npad, dtype=torch.float32, device=dev)
+        shift = torch.zeros(npad, dtype=torch.float32, device=dev)
+        for d, (u, bn) in enumerate(zip(heads, bns)):
+            K, r0 = u.conv.out_channels, 64 * box0[d]
+            w[r0:r0 + K, :u.conv.in_channels] = _conv1x1_matrix(u.conv).float().to(torch.float16)
+            scale[r0:r0 + K], shift[r0:r0 + K] = ops.fold_affine(K, None, bn, dev)
+        return w, scale, shift
+
+    bns = [u.bn_blocks[i] for u in heads]
+    w = _cached(module, "poly_split_w", _sig(*[u.conv.weight for u in heads]) + (in_pitch,), lambda: build([None] * len(heads))[0])
+    sig = _sig(*[t for bn in bns for t in _bn_tensors(bn)]) + (id(bns[0]), in_pitch)
+    scale, shift = _cached(module, "poly_split_aff%d" % i, sig, lambda: build(bns)[1:], reads=tuple(t for bn in bns for t in _bn_tensors(bn)))
+    return w, scale, shift
+
+
+def _poly_conv(unit, i, in_pitch):
+    """PackedConv of PolyConv2d ``unit`` with BatchNorm ``bn_blocks[i]``: the fp16 filter is packed once (cached on the unit) and
+    shared by every application; each application's pack carries only its own folded affine (cached on its BatchNorm)."""
+    conv, bn = unit.conv, unit.bn_blocks[i]
+    stride, padding = _conv_geometry(conv)
+    base = _cached(unit, "poly_w", _sig(conv.weight) + (in_pitch,),
+                   lambda: ops.PackedConv(conv.weight.detach(), None, None, stride, padding, in_pitch=in_pitch))
+
+    def build():
+        pc = copy.copy(base)
+        pc.scale, pc.shift = ops.fold_affine(conv.out_channels, None, bn, conv.weight.device)
+        return pc
+
+    return _cached(bn, "poly_pc", _sig(conv.weight, *_bn_tensors(bn)) + (in_pitch,), build, reads=(conv.weight,))
+
+
+def _polynet_poly_body(module, a):
+    """out = x; for i: f = F_i(x_i); out += s * f; x_{i+1} = relu(f); relu(out) (InceptionResNetB/CPoly, polynet.py:229-326).
+    Application i: its 1x1 heads over x_i as one split GEMM (the 1x1 into a matrix, ``path1`` into its slice), the 1xn and nx1
+    convolutions on the slab kernel (the second into its slice), and the close over the concatenation: with (sb, tb) the folded
+    BatchNorm of ``conv2d_blocks[i]``, scale s * sb, shift s * tb and the running sum as residual.  Every application but the last
+    closes with the dual GEMM, which also writes x_{i+1} = relu(sb * acc + tb) from the same accumulator; the last one is the
+    residual GEMM with ReLU."""
+    from .models.polynet import BRANCHES
+    (_, chain), (_, (lone,)) = BRANCHES[module.kind]
+    h1x1, ha, hb = (getattr(module, n) for n in chain)
+    p1 = getattr(module, lone)
+    if a.ld != a.C:
+        raise ValueError("%s takes a dense [M][C] input, got %r" % (type(module).__name__, a))
+    K0, Ka, Kb = h1x1.conv.out_channels, ha.conv.out_channels, hb.conv.out_channels
+    C = Kb + p1.conv.out_channels
+    K = module.conv2d_blocks[0].conv.out_channels
+    dev = a.data.device
+    M = a.M
+    geo = (a.N, a.T, a.H, a.W)
+    x, total = a, a.data
+    s = float(module.scale)
+    n = module.num_blocks
+    for i in range(n):
+        y = torch.empty((M, C), dtype=torch.float16, device=dev)
+        t0 = torch.empty((M, K0), dtype=torch.float16, device=dev)
+        w, scale, shift = _poly_split_pack(module, [h1x1, p1], i, x.ld)
+        ops.gemm_split(x.data, w, scale, shift, M, x.ld, [t0, y[:, Kb:]], relu=True)
+        ta = torch.empty((M, Ka), dtype=torch.float16, device=dev)
+        ops.conv_slice(Act(t0, *geo, K0), _poly_conv(ha, i, K0), ta)
+        ops.conv_slice(Act(ta, *geo, Ka), _poly_conv(hb, i, Ka), y[:, :Kb])
+        unit = module.conv2d_blocks[i]
+
+        def build(unit=unit):
+            sb, tb = ops.fold_affine(K, None, unit.bn, dev)
+            return (_conv1x1_matrix(unit.conv).float().to(torch.float16).contiguous(), (s * sb.double()).float().contiguous(),
+                    (s * tb.double()).float().contiguous(), sb, tb)
+
+        wc, sc, sh, sb, tb = _cached(unit, "poly_close", _sig(unit.conv.weight, *_bn_tensors(unit.bn)) + (s,), build)
+        if i < n - 1:
+            total, xn = ops_dual.gemm_dual(y, wc, sc, sh, sb, tb, M, K, C, residual=total)
+            x = Act(xn, *geo, K)
+        else:
+            total = ops.gemm(y, wc, sc, sh, M, K, C, residual=total, relu=True)
+    return Act(total, *geo, K)
+
+
+def _polynet_block_body(module, a):
+    """One module of the PolyNet trunk (PolyNet.modules_in_order)."""
+    from .models import polynet as PN
+    if isinstance(module, PN.Stem):
+        return _polynet_stem_body(module, a)
+    if isinstance(module, PN.MultiWay):
+        return _polynet_2way_body(module, a)
+    if isinstance(module, (PN.InceptionResNetBPoly, PN.InceptionResNetCPoly)):
+        return _polynet_poly_body(module, a)
+    return _inception_block_body(module, a, row=PN.BRANCHES[module.kind])
+
+
+def run_polynet_trunk(model, x):
+    """The PolyNet trunk: fp32 NCHW images (or an Act with channel pitch 8) in, the 9x9x2048 stage_c output (an Act) out; every
+    module is one ``PolyNetBlockFunction``."""
+    H, W = (x.H, x.W) if isinstance(x, Act) else tuple(x.shape[-2:])
+    if (H, W) != (331, 331):
+        # the final pool is the reference's fixed AvgPool2d(9): only a 9x9 final map gives one vector per image
+        raise ValueError("the final pool is AvgPool2d(9): it needs a 9x9 final map (331x331 inputs), got a %dx%d input" % (H, W))
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
+    for m in model.modules_in_order():
+        a = Fn.PolyNetBlockFunction.run(m, a)
     return a
 
 

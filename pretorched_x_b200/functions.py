@@ -187,6 +187,16 @@ class InceptionBlockFunction(_FrozenFunction):
         return InceptionBlockFunction._finish(ctx, engine._inception_block_body(block, Act(x2d, *geom), out))
 
 
+class PolyNetBlockFunction(_FrozenFunction):
+    """One module of the PolyNet trunk (polynet.py:71-371): the stem, a reduction, a 2-way module or a poly-3 module, every
+    branch written in place into its concatenation matrix."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, module):
+        from . import engine
+        return PolyNetBlockFunction._finish(ctx, engine._polynet_block_body(module, Act(x2d, *geom)))
+
+
 class DenseNetTrunkFunction(_FrozenFunction):
     """The DenseNet trunk up to norm5 (torchvision densenet.py ``features`` without its last BatchNorm): every dense block as one
     matrix that its layers and the preceding transition (or the stem's pool) write in place."""

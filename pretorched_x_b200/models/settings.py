@@ -10,9 +10,10 @@ from .bninception import pretrained_settings as bninception_settings  # bnincept
 from .inception import pretrained_settings as inception_settings      # inceptionv4.py:10-31, inceptionresnetv2.py:10-31
 from .densenet import pretrained_settings as densenet_settings        # torchvision_models.py:80-130
 from .inceptionv3 import pretrained_settings as inceptionv3_settings  # torchvision_models.py:39, 74-92
+from .polynet import pretrained_settings as polynet_settings          # polynet.py:8-21 (settings.py:15 of the reference)
 
 all_settings = [resnet2d_settings, resnet3d_settings, resnext3d_settings, nonlocal_settings, mobilenet_settings, senet_settings,
-                bninception_settings, inception_settings, densenet_settings, inceptionv3_settings]
+                bninception_settings, inception_settings, densenet_settings, inceptionv3_settings, polynet_settings]
 
 model_names = []
 pretrained_settings = {}
