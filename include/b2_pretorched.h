@@ -466,6 +466,32 @@ int b2_bn_relu_avgpool2_ndhwc(const void* x, int ldx, void* y, int ldy, int N, i
  * b2_debug_last_kernel: KID 14, info = {4}. */
 int b2_avgpool_global_affine_ndhwc(const void* x, void* y, int N, int S, int C, const float* scale, const float* shift, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * VGG / AlexNet (torchvision vgg.py / alexnet.py behind torchvision_models.py:195-248, 597-725)
+ * ------------------------------------------------------------------------------------------- */
+/* AlexNet's first convolution (nn.Conv2d(3, 64, 11, stride=4, padding=2)) as a valid 3x3 stride-1 convolution over a 4x4
+ * space-to-depth image: x fp32 NCHW [N][3][H][W] -> y fp16 [N*Hs*Ws][48] with Ho = (H + 4 - 11) / 4 + 1, Hs = Ho + 2 (same for W),
+ *     y[(n, hs, ws)][(dh * 4 + dw) * 3 + c] = x[n][c][4 hs + dh - 2][4 ws + dw - 2]      (0 outside the image)
+ * so that conv11x11/4(x)[ho][wo] = sum_{a, b < 3} y[ho + a][wo + b] . W3[a][b] with W3[k][(dh * 4 + dw) * 3 + c][a][b] =
+ * W[k][c][4 a + dh][4 b + dw] (zero where 4 a + dh or 4 b + dw reaches 11).  One rounding to fp16 per element.  H, W >= 7, y 16-byte
+ * aligned.  Replaces the layout pass of the generic input path for this network. */
+int b2_space_to_depth4_nchw(const float* x, void* y, int N, int H, int W, void* stream);
+/* Split-K GEMM for the fully connected classifiers (torchvision_models.py:211-224, 613-626), whose M is the batch:
+ *     D[M][N] = act(scale[n] * sum_{s < S} P_s[m][n] + shift[n]),   P_s = A[:, K_s] . B[:, K_s]^T over K blocks
+ *                                                                 K_s = [s * nkb / S, (s + 1) * nkb / S) of 64 (nkb = ceil(Kd / 64))
+ * One persistent-GEMM launch writes every P_s in fp32 into its own slice of the caller's workspace ws ([S][M][round_up(N, 8)] floats,
+ * b2_gemm_splitk_workspace_elems), then one pass sums the slices in the order 0..S-1, applies the per-column affine, the ReLU
+ * (g->relu) and writes fp16 (columns [N, ldd) zero) or fp32 (g->out_f32, ldd >= N, only columns [0, N) written).  No atomics: the
+ * result is bitwise repeatable, and the same under CUDA-graph replay.  g: a, lda, b, ldb, M, N, Kd, scale, shift, d, ldd, relu,
+ * out_f32 as in b2_gemm_f16; a residual, a mask, per_row, a per-sample affine (aff_ld / aff_rows), a second output (d2 / scale2 /
+ * shift2 / aff2_*) and accumulate are refused (B2_ERR_INVALID), as is 1 > S or S > min(64, nkb).  Two launches;
+ * b2_debug_last_kernel: KID 17, info = {N tile, S}, with the N tile b2_gemm_f16 picks for an output of pitch round_up(N, 8). */
+size_t b2_gemm_splitk_workspace_elems(int M, int N, int splits);
+int b2_gemm_splitk_f16(const b2_gemm_args* g, int splits, float* ws, size_t ws_elems, void* stream);
+/* The number of splits S for an M x N x Kd product on `sm_count` SMs: 1 when the output tiles (128 rows x the N tile) fill the SMs,
+ * else SMs / tiles, capped so that every split keeps at least 8 K blocks of 64 and at 16 splits; at least 1.  Host only. */
+int b2_gemm_splitk_plan(int M, int N, int Kd, int sm_count);
+
 #ifdef __cplusplus
 }
 #endif

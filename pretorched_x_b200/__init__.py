@@ -30,6 +30,8 @@ from .models.inception import inceptionv4, inceptionresnetv2  # noqa: F401  (pre
 from .models.densenet import densenet121, densenet161, densenet169, densenet201  # noqa: F401  (pretorched/__init__.py:21-24)
 from .models.inceptionv3 import inceptionv3  # noqa: F401  (pretorched/__init__.py:30)
 from .models.polynet import polynet  # noqa: F401  (pretorched/__init__.py:55)
+from .models.vgg import (alexnet, vgg11, vgg11_bn, vgg13, vgg13_bn, vgg16, vgg16_bn, vgg19,  # noqa: F401
+                         vgg19_bn)                          # pretorched/__init__.py (torchvision_models.py:23-31)
 from .models.trn import Relation, MultiScaleRelation, HierarchicalRelation, TRN, trn  # noqa: F401
 from .models.utils import Identity  # noqa: F401
 # BigGAN-deep generator (BASELINE.json configs[4]; not in the reference tree -- see models/biggan_deep.py)

@@ -119,6 +119,10 @@ SYMBOLS = {
     "b2_gemm_dual_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "b2_bn_relu_avgpool2_ndhwc": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_int] * 4 + [c_void_p, c_void_p, c_void_p]),
     "b2_avgpool_global_affine_ndhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "b2_space_to_depth4_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "b2_gemm_splitk_workspace_elems": (ctypes.c_size_t, [c_int, c_int, c_int]),
+    "b2_gemm_splitk_f16": (c_int, [ctypes.POINTER(GemmArgs), c_int, c_void_p, ctypes.c_size_t, c_void_p]),
+    "b2_gemm_splitk_plan": (c_int, [c_int, c_int, c_int, c_int]),
 }
 
 

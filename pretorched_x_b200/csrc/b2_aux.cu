@@ -780,6 +780,39 @@ int b2_ncdhw_f32_to_ndhwc_f16(const float* x, void* y, int N, int C, int T, int 
   return B2_OK;
 }
 
+// AlexNet's stem input as a 4x4 space-to-depth image: one thread per 8-channel chunk of an output row (6 chunks per row), one 16-byte
+// store.  Channel ch = (dh * 4 + dw) * 3 + c of row (n, hs, ws) is x[n][c][4 hs + dh - 2][4 ws + dw - 2], zero outside the image.
+__global__ void space_to_depth4_kernel(const float* __restrict__ x, __half* __restrict__ y, int H, int W, int Hs, int Ws, long long total) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int q = static_cast<int>(idx % 6);
+  const long long row = idx / 6;
+  const int ws = static_cast<int>(row % Ws);
+  const long long t = row / Ws;
+  const int hs = static_cast<int>(t % Hs);
+  const long long n = t / Hs;
+  const float* xn = x + n * 3 * H * W;
+  __align__(16) __half v[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const int ch = q * 8 + e, c = ch % 3, tap = ch / 3;
+    const int h = 4 * hs + tap / 4 - 2, w = 4 * ws + tap % 4 - 2;
+    v[e] = __float2half_rn((h >= 0 && h < H && w >= 0 && w < W) ? __ldg(xn + (static_cast<long long>(c) * H + h) * W + w) : 0.f);
+  }
+  *reinterpret_cast<uint4*>(y + row * 48 + q * 8) = *reinterpret_cast<const uint4*>(v);
+}
+
+int b2_space_to_depth4_nchw(const float* x, void* y, int N, int H, int W, void* stream) {
+  B2_CHECK_ARG(x && y, "null tensor pointer");
+  B2_CHECK_ARG(N > 0 && H >= 7 && W >= 7, "bad image size %d x %d x %d (the 11x11 stride-4 filter needs at least 7 x 7)", N, H, W);
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(y) & 15) == 0, "output must be 16-byte aligned");
+  const int Hs = (H + 4 - 11) / 4 + 3, Ws = (W + 4 - 11) / 4 + 3;
+  const long long total = (long long)N * Hs * Ws * 6;
+  space_to_depth4_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, (__half*)y, H, W, Hs, Ws, total);
+  B2_CHECK_LAUNCH("space_to_depth4");
+  return B2_OK;
+}
+
 int b2_ncdhw_f16_to_ndhwc_f16(const void* x, void* y, int N, int C, int T, int H, int W, int Cp, void* stream) {
   B2_CHECK_ARG(x && y && Cp >= C && (Cp == 4 || Cp % 8 == 0), "bad argument (Cp must be 4 or a multiple of 8, >= C)");
   const long long S = (long long)T * H * W, total = (long long)N * S;

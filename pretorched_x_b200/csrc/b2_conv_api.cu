@@ -1163,6 +1163,40 @@ static int launch_pgemm_dual(const b2_gemm_args* g, const float* scale2, const f
   return B2_OK;
 }
 
+// The split-K instance (b2_gemm_splitk_f16): pgemm_kernel<BN, 0, 5> writes the fp32 partial accumulators of every (split, tile)
+// into the workspace, splitk_reduce_kernel sums them in split order and applies the epilogue.
+template <int BN>
+static int launch_pgemm_splitk(const b2_gemm_args* g, int splits, float* ws, int ldw, cudaStream_t stream) {
+  using S = PgemmSmem<BN, 0, 0>;
+  B2_OPT_IN_SMEM((pgemm_kernel<BN, 0, 5>), S::kTotal);
+  CUtensorMap tmA, tmB;
+  int rc;
+  if ((rc = make_tmap_2d_f16(&tmA, g->a, (uint64_t)g->Kd, (uint64_t)g->M, (uint64_t)g->lda, 64, 128, true)) != B2_OK) return rc;
+  if ((rc = make_tmap_2d_f16(&tmB, g->b, (uint64_t)g->Kd, (uint64_t)g->N, (uint64_t)g->ldb, 64, BN, true)) != B2_OK) return rc;
+  PgemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.M = g->M; p.Ncols = g->N; p.ldy = ldw; p.nkb = (g->Kd + 63) / 64; p.nkb2 = 0;
+  p.tiles_n = (ldw + BN - 1) / BN;
+  p.tiles_mn = p.tiles_n * ((g->M + 127) / 128);
+  p.splits = splits;
+  p.tiles_total = p.tiles_mn * splits;
+  p.ldw = ldw; p.ws = ws;
+  p.aff2_rows = 128;
+  p.fd_Wh = make_fastdiv(2); p.fd_Hh = make_fastdiv(2); p.fd_aff = make_fastdiv(1);
+  const int grid = p.tiles_total < sm_count() ? p.tiles_total : sm_count();
+  // the maps this instance never reads are given tmA (every map argument must be a valid descriptor)
+  B2_CHECK_CUDA(launch_pdl(pgemm_kernel<BN, 0, 5>, dim3(grid), dim3(kPgThreads), S::kTotal, stream, tmA, tmB, tmA, tmB, tmA, tmA, tmA, p));
+  B2_CHECK_LAUNCH("pgemm_kernel");
+  const int width = g->out_f32 ? g->N : g->ldd;
+  const int quads = (width + 3) / 4;
+  const long long threads = (long long)g->M * quads;
+  splitk_reduce_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(ws, splits, g->M, g->N, ldw, g->scale, g->shift, g->relu, g->d,
+                                                                             g->ldd, g->out_f32, quads);
+  B2_CHECK_LAUNCH("splitk_reduce_kernel");
+  set_last_kernel(KID_PGEMM_SPLITK, BN, splits);
+  return B2_OK;
+}
+
 static int g_last_gemm_path = 0;   // kernel of the last GEMM-family launch: 1 dense-M, 2 persistent GEMM, 3 implicit GEMM (tests pin it)
 
 static int dispatch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
@@ -1679,6 +1713,54 @@ int b2_gemm_dual_f16(const b2_gemm_args* g, const float* scale2, const float* sh
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // the N tile b2_gemm_f16 picks for an output of this pitch
   return g->ldd <= 64 ? launch_pgemm_dual<64>(g, scale2, shift2, d2, ldd2, st) : launch_pgemm_dual<128>(g, scale2, shift2, d2, ldd2, st);
+}
+
+// The split-K planner: N tile as b2_gemm_f16 picks it for an output of pitch round_up(N, 8), at least kSplitkMinKb K blocks of 64 per
+// split, at most kSplitkMaxSplits splits.
+static constexpr int kSplitkMinKb = 8;
+static constexpr int kSplitkMaxSplits = 16;
+
+static int splitk_bn(int N) { return (N + 7) / 8 * 8 <= 64 ? 64 : 128; }
+
+int b2_gemm_splitk_plan(int M, int N, int Kd, int sms) {
+  B2_CHECK_ARG(M > 0 && N > 0 && Kd > 0 && sms > 0, "non-positive dimension or SM count");
+  const int BN = splitk_bn(N);
+  const long long tiles = (long long)((M + 127) / 128) * (((N + 7) / 8 * 8 + BN - 1) / BN);
+  if (tiles >= sms) return 1;                    // the output tiles alone fill the SMs
+  long long s = sms / tiles;
+  const int nkb = (Kd + 63) / 64;
+  if (s > nkb / kSplitkMinKb) s = nkb / kSplitkMinKb;
+  if (s > kSplitkMaxSplits) s = kSplitkMaxSplits;
+  return s < 1 ? 1 : (int)s;
+}
+
+size_t b2_gemm_splitk_workspace_elems(int M, int N, int splits) {
+  if (M <= 0 || N <= 0 || splits <= 0) return 0;
+  return (size_t)splits * M * ((N + 7) / 8 * 8);
+}
+
+int b2_gemm_splitk_f16(const b2_gemm_args* g, int splits, float* ws, size_t ws_elems, void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(g != nullptr && g->a && g->b && g->scale && g->shift && g->d && ws, "null tensor pointer");
+  B2_CHECK_ARG(g->M > 0 && g->N > 0 && g->Kd > 0, "non-positive dimension");
+  B2_CHECK_ARG(g->lda % 8 == 0 && g->ldb % 8 == 0 && g->lda >= g->Kd && g->ldb >= g->Kd, "bad operand pitch");
+  B2_CHECK_ARG(g->out_f32 ? g->ldd >= g->N : (g->ldd % 8 == 0 && g->ldd >= g->N), "bad output pitch (ldd %d, N %d)", g->ldd, g->N);
+  const int nkb = (g->Kd + 63) / 64;
+  B2_CHECK_ARG(splits >= 1 && splits <= nkb && splits <= 64, "splits %d outside [1, min(64, K blocks %d)]", splits, nkb);
+  B2_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "workspace must be 16-byte aligned");
+  B2_CHECK_ARG(ws_elems >= b2_gemm_splitk_workspace_elems(g->M, g->N, splits), "workspace of %zu floats, %zu needed", ws_elems,
+               b2_gemm_splitk_workspace_elems(g->M, g->N, splits));
+  B2_CHECK_ARG(g->residual == nullptr && g->ldr == 0, "the split-K GEMM takes no residual");
+  B2_CHECK_ARG(g->mask == nullptr && g->ldm == 0, "the split-K GEMM takes no mask");
+  B2_CHECK_ARG(!g->per_row && !g->aff_ld && !g->aff_rows, "the split-K GEMM takes a per-column affine only (no per-row or per-sample affine)");
+  B2_CHECK_ARG(!g->d2 && !g->scale2 && !g->shift2 && !g->aff2_ld && !g->aff2_rows, "the split-K GEMM has no second output");
+  B2_CHECK_ARG(!g->accumulate, "the split-K GEMM does not accumulate into its output");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  g_last_gemm_path = 2;
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int ldw = (g->N + 7) / 8 * 8;
+  return splitk_bn(g->N) == 64 ? launch_pgemm_splitk<64>(g, splits, ws, ldw, st) : launch_pgemm_splitk<128>(g, splits, ws, ldw, st);
 }
 
 int b2_gemm_split_plan(int nd, const int* cols, int* box0) {

@@ -81,7 +81,8 @@ enum LastKernel : int {
   KID_SLAB_SLICE = 13 /* b2_conv_ndhwc_fprop_slice: info as KID_SLAB */,
   KID_POOL = 14 /* b2_pool_ndhwc_slice: info = {average}; 2 exclude-pad, 3 DenseNet transition, 4 global mean with affine */,
   KID_SLAB_T128 = 15 /* the slab kernel's 128-wide transposed form (b2_slab_t128.cuh): info = {NP, rows per item, 128, stride, R} */,
-  KID_SLAB_T64 = 16 /* the slab kernel's 64-wide transposed form (b2_slab_t128.cuh): info = {NP, items, R} */
+  KID_SLAB_T64 = 16 /* the slab kernel's 64-wide transposed form (b2_slab_t128.cuh): info = {NP, items, R} */,
+  KID_PGEMM_SPLITK = 17 /* b2_gemm_splitk_f16: info = {N tile, splits} */
 };
 void set_last_kernel(int id, int i0 = 0, int i1 = 0, int i2 = 0, int i3 = 0, int i4 = 0);
 

@@ -24,6 +24,13 @@
 //     d2 = relu(scale2[n] * acc + shift2[n]),
 // next to d = act(scale[n] * acc + shift[n] + residual).  One application of a PolyNet poly-3 module closes with it: d is the
 // running sum, d2 the next application's input, from one pass over the concatenated branches.
+//
+// Split-K instance (pgemm_kernel<BN, 0, 5>, b2_gemm_splitk_f16): work item t = s * tiles_mn + (output tile) accumulates the K blocks
+// [s * nkb / S, (s + 1) * nkb / S) of that tile and stores its raw fp32 accumulators into slice s of a workspace [S][M][ldw] (no
+// affine, no staging, no TMA store).  splitk_reduce_kernel then sums the S slices of each element in the order 0..S-1, applies the
+// per-column affine and ReLU and writes fp16 or fp32.  The fully connected classifiers of VGG / AlexNet have M = batch rows, so
+// their 128-row output tiles number fewer than the SMs while each walks a K of up to 25088; the splits put the idle SMs to work on
+// the same weight stream.  No atomics: the result does not depend on the schedule.
 #pragma once
 
 #include "b2_ptx.cuh"
@@ -83,6 +90,9 @@ struct PgemmParams {
   // second-operand maps this instance never reads).  Each map spans only its destination's columns, so TMA drops the
   // padding columns of a ragged last box and nothing outside the slice is written.
   int split_box[4];
+  // pgemm_kernel<BN, 0, 5> only: K splits, output tiles per split (tiles_total = splits * tiles_mn), fp32 workspace [splits][M][ldw]
+  int splits, tiles_mn, ldw;
+  float* ws;
 };
 
 template <int BN, int GAN, int C2 = GAN>   // C2: a second-output staging tile (generator and dual instances)
@@ -115,7 +125,8 @@ __device__ __forceinline__ uint32_t pg_sw_off(int row, int j, int c) {
 template <int BN, int GAN, int EPI = 0>    // GAN = 1: instance with the generator extras (res_up gather, res_pre, dual output, A transform);
                                            // 0: the classic epilogue.  With GAN = 0, EPI = 1: ReLU-derivative mask operand (fine-tuning
                                            // backward); EPI = 2: per-sample affine resolved per fragment row (see PgemmParams::fd_aff);
-                                           // EPI = 3: column-slice destinations; EPI = 4: second output from the accumulator (dual)
+                                           // EPI = 3: column-slice destinations; EPI = 4: second output from the accumulator (dual);
+                                           // EPI = 5: split-K partial accumulators into the workspace (see PgemmParams::splits)
 __global__ void __launch_bounds__(GAN ? kPgThreadsGan : kPgThreads, 1)
 pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -148,8 +159,10 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     // ================================ producer ==========================================
     int it = 0, lt = 0;
     for (int tile = blockIdx.x; tile < p.tiles_total; tile += gridDim.x, ++lt) {
-      const int m0 = (tile / p.tiles_n) * 128, n0 = (tile % p.tiles_n) * BN;
-      for (int kb = 0; kb < p.nkb + p.nkb2; ++kb, ++it) {
+      const int tmn = EPI == 5 ? tile % p.tiles_mn : tile, sp = EPI == 5 ? tile / p.tiles_mn : 0;
+      const int m0 = (tmn / p.tiles_n) * 128, n0 = (tmn % p.tiles_n) * BN;
+      const int kb_lo = EPI == 5 ? sp * p.nkb / p.splits : 0, kb_hi = EPI == 5 ? (sp + 1) * p.nkb / p.splits : p.nkb + p.nkb2;
+      for (int kb = kb_lo; kb < kb_hi; ++kb, ++it) {
         const int s = it % kSt;
         mbar_wait(&empty[s], ((it / kSt) & 1) ^ 1);
         if (elect_one()) {
@@ -206,10 +219,12 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     float acc[BN / 2];
     int it = 0, lt = 0;
     for (int tile = blockIdx.x; tile < p.tiles_total; tile += gridDim.x, ++lt) {
-      const int m0 = (tile / p.tiles_n) * 128, n0 = (tile % p.tiles_n) * BN;
+      const int tmn = EPI == 5 ? tile % p.tiles_mn : tile, sp = EPI == 5 ? tile / p.tiles_mn : 0;
+      const int m0 = (tmn / p.tiles_n) * 128, n0 = (tmn % p.tiles_n) * BN;
+      const int kb_lo = EPI == 5 ? sp * nkb / p.splits : 0, kb_hi = EPI == 5 ? (sp + 1) * nkb / p.splits : nkb_all;
       // the tile's affine, fetched before the main loop and stored after it
       float aff[4] = {0.f, 0.f, 0.f, 0.f};
-      if (EPI != 2 && wt < BN && n0 + wt < p.Ncols) {
+      if (EPI != 2 && EPI != 5 && wt < BN && n0 + wt < p.Ncols) {
         // per-sample affine (class-conditional BN of the consumer): a 128-row tile never straddles two samples
         const size_t arow = p.aff_ld ? static_cast<size_t>(m0 / p.aff_rows) * p.aff_ld : 0;
         aff[0] = __ldg(&p.scale[arow + n0 + wt]);
@@ -224,7 +239,7 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       for (int k = 0; k < BN / 2; ++k) acc[k] = 0.f;
       reg_fence(acc);
       int prev_s = -1;
-      for (int kb = 0; kb < nkb_all; ++kb, ++it) {
+      for (int kb = kb_lo; kb < kb_hi; ++kb, ++it) {
         const int s = it % kSt;
         if (xform && kb < nkb) mbar_wait(&xf_full[s], (it / kSt) & 1);     // operands landed AND the A tile was rewritten
         else mbar_wait(&full[s], (it / kSt) & 1);
@@ -251,6 +266,21 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       // ---- epilogue math on the fragments, in place (fp32) ----
       const int rb = lt & 1;
       mbar_wait(&res_full[rb], (lt >> 1) & 1);
+      if constexpr (EPI == 5) {
+        // raw accumulators of split sp; rows past M and columns past ldw (ragged last tiles) are dropped
+        float* ws = p.ws + static_cast<size_t>(sp) * p.M * p.ldw;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n0 + 8 * j + fc;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int row = m0 + fr + 8 * i;
+            if (row < p.M && col < p.ldw)
+              *reinterpret_cast<float2*>(ws + static_cast<size_t>(row) * p.ldw + col) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+          }
+        }
+        continue;
+      }
       uint8_t* stage = smem + S::kResOff + rb * S::kTile;
       uint8_t* stage2 = smem + S::kC2Off;                  // second output (generator / dual instances): free since the bar above
       int rsrc[2] = {fr, fr + 8};                          // row of the residual box each fragment row adds
@@ -415,6 +445,39 @@ pgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         }
       }
     }
+  }
+}
+
+// The second pass of the split-K GEMM: d[m][n] = act(scale[n] * (ws[0][m][n] + ws[1][m][n] + ... + ws[S-1][m][n]) + shift[n]), the
+// slices summed in that order in fp32, one fma with the affine, one rounding (fp16) or none (fp32).  Four columns per thread.
+// fp16: columns [N, ldd) are written as zero; fp32: only columns [0, N) are written.
+__global__ void __launch_bounds__(256)
+splitk_reduce_kernel(const float* __restrict__ ws, int S, int M, int N, int ldw, const float* __restrict__ scale,
+                     const float* __restrict__ shift, int relu, void* __restrict__ d, int ldd, int out_f32, int quads) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= static_cast<long long>(M) * quads) return;
+  const int m = static_cast<int>(idx / quads), c0 = static_cast<int>(idx % quads) * 4;
+  const size_t slice = static_cast<size_t>(M) * ldw;
+  float v[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int c = c0 + q;
+    v[q] = 0.f;
+    if (c < N) {
+      const float* src = ws + static_cast<size_t>(m) * ldw + c;
+      float sum = 0.f;
+      for (int s = 0; s < S; ++s) sum += __ldg(src + s * slice);
+      sum = fmaf(sum, __ldg(scale + c), __ldg(shift + c));
+      v[q] = relu ? fmaxf(sum, 0.f) : sum;
+    }
+  }
+  if (out_f32) {
+    float* y = static_cast<float*>(d) + static_cast<size_t>(m) * ldd;
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      if (c0 + q < N) y[c0 + q] = v[q];
+  } else {
+    *reinterpret_cast<uint2*>(static_cast<__half*>(d) + static_cast<size_t>(m) * ldd + c0) = make_uint2(pack_half2(v[0], v[1]), pack_half2(v[2], v[3]));
   }
 }
 

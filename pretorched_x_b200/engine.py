@@ -31,6 +31,7 @@ import torch.nn as nn
 
 from . import ops
 from . import ops_dual
+from . import ops_vgg
 from . import functions as Fn
 from .ops import Act
 
@@ -1284,6 +1285,129 @@ def run_densenet_head(model, a, bn=None):
     else:
         s, t = _bn_affine(bn, a.ld)
     return _head_on_pooled(model.last_linear, ops.avgpool_global_affine(a, s, t), a.C)
+
+
+# ---------------------------------------------------------------------------------------------
+# VGG / AlexNet (torchvision vgg.py / alexnet.py behind torchvision_models.py:195-248, 597-725)
+# ---------------------------------------------------------------------------------------------
+def _check_224(x):
+    if x.dim() != 4 or tuple(x.shape[2:]) != (224, 224):
+        # the reference skips torchvision's avgpool, so its view(B, -1) only fits fc6 for a 224x224 input
+        raise ValueError("VGG / AlexNet take 224x224 images (the classifier reads the 7x7 / 6x6 final map as is), got %s"
+                         % (tuple(x.shape),))
+
+
+def _plain_stack_body(mods, a, i=0):
+    """Conv2d [-> BatchNorm2d] -> ReLU units and MaxPool2d layers of a torchvision ``features`` Sequential from layer ``i`` on: each
+    convolution on the convolution path with its bias (+ folded BatchNorm) and the ReLU in the epilogue, each pool on the pooling
+    kernel (floor mode)."""
+    while i < len(mods):
+        m = mods[i]
+        if isinstance(m, nn.Conv2d):
+            bn = mods[i + 1] if i + 1 < len(mods) and isinstance(mods[i + 1], nn.BatchNorm2d) else None
+            j = i + 1 + (bn is not None)
+            if j >= len(mods) or not isinstance(mods[j], nn.ReLU):
+                raise NotImplementedError("VGG / AlexNet convolutions are followed by a ReLU")
+            a = conv_bn_act(m, bn, a, relu=True)
+            i = j + 1
+        elif isinstance(m, nn.MaxPool2d):
+            if m.ceil_mode or m.dilation not in (1, (1, 1)):
+                raise NotImplementedError("the engine runs floor-mode, undilated max pools here")
+            a = ops.maxpool3d(a, *_pool_args(m))
+            i += 1
+        else:
+            raise NotImplementedError("unsupported layer %r in a VGG / AlexNet trunk" % (m,))
+    return a
+
+
+def _vgg_trunk_body(features, a):
+    """VGG's ``_features`` on the pitch-8 image ``a``: an Act [N*7*7][512] at 224x224."""
+    return _plain_stack_body(list(features), a)
+
+
+def _alexnet_trunk_body(features, a):
+    """AlexNet's ``_features`` on the space-to-depth image ``a`` (ops_vgg.space_to_depth4): conv1 (11x11, stride 4, padding 2) as
+    the valid 3x3 convolution with the regrouped filter, then the rest of the stack.  An Act [N*6*6][256] at 224x224."""
+    mods = list(features)
+    conv = mods[0]
+    if (not isinstance(conv, nn.Conv2d) or tuple(conv.kernel_size) != (11, 11) or tuple(conv.stride) != (4, 4)
+            or tuple(conv.padding) != (2, 2) or conv.in_channels != 3 or not isinstance(mods[1], nn.ReLU)):
+        raise NotImplementedError("AlexNet's conv1 is Conv2d(3, K, 11, stride=4, padding=2) -> ReLU")
+    if a.ld != 48:
+        raise ValueError("AlexNet's trunk takes the 48-channel space-to-depth image, got %r" % (a,))
+    pc = _cached(conv, "s2d", _sig(conv.weight, conv.bias),
+                 lambda: ops.PackedConv(ops_vgg.s2d_filter(conv.weight.detach().float()), conv.bias, None, (1, 1, 1), (0, 0, 0),
+                                        in_pitch=48))
+    return _plain_stack_body(mods, ops.conv(a, pc, relu=True), 2)
+
+
+def run_vgg_trunk(features, x):
+    """VGG ``_features`` through its Function: fp32 NCHW 224x224 images in, the last pool's output (an Act) out."""
+    _check_224(x)
+    return Fn.VGGTrunkFunction.run(features, ops.from_ncdhw(x, pitch=8))
+
+
+def run_alexnet_trunk(features, x):
+    """AlexNet ``_features`` through its Function: fp32 NCHW 224x224 images in, the last pool's output (an Act) out."""
+    _check_224(x)
+    return Fn.AlexNetTrunkFunction.run(features, ops_vgg.space_to_depth4(x))
+
+
+def _fc6_pack(linear, C, H, W):
+    """fc6 as fp16 [4096][H*W*C] with its columns in the engine's (h, w, c) order (the reference flattens (c, h, w)), + bias."""
+    def build():
+        w = linear.weight.detach()
+        if w.shape[1] != C * H * W:
+            raise ValueError("fc6 takes %d features, the final map has %d x %d x %d" % (w.shape[1], C, H, W))
+        wp = w.reshape(w.shape[0], C, H, W).permute(0, 2, 3, 1).reshape(w.shape[0], H * W * C)
+        return ops.PackedLinear(wp.contiguous(), linear.bias)
+    return _cached(linear, "fc6_hwc", _sig(linear.weight, linear.bias) + (C, H, W), build)
+
+
+def _packed_linear(linear):
+    return _cached(linear, "pl", _sig(linear.weight, linear.bias), lambda: ops.PackedLinear(linear.weight, linear.bias))
+
+
+def classifier_gemm(x16, pl, relu=False, out_f32=False):
+    """One fully connected layer on fp16 rows ``x16``: split-K (ops_vgg.gemm_splitk) with the splits b2_gemm_splitk_plan picks
+    when the output tiles leave SMs idle, else the persistent GEMM."""
+    M, N, Kd = x16.shape[0], pl.out_features, pl.in_features
+    splits = ops_vgg.splitk_plan(M, N, Kd, _sm_count(x16.device))
+    if splits > 1:
+        return ops_vgg.gemm_splitk(x16, pl.w, pl.scale, pl.shift, M, N, Kd, splits, relu=relu, out_f32=out_f32)
+    return ops.gemm(x16, pl.w, pl.scale, pl.shift, M, N, Kd, relu=relu, out_f32=out_f32)
+
+
+_SM_COUNT = {}
+
+
+def _sm_count(dev):
+    idx = dev.index if dev.index is not None else torch.cuda.current_device()
+    if idx not in _SM_COUNT:
+        _SM_COUNT[idx] = torch.cuda.get_device_properties(idx).multi_processor_count
+    return _SM_COUNT[idx]
+
+
+def run_vgg_classifier(model, a):
+    """view(B, -1) -> linear0 -> relu0 -> linear1 on the trunk output ``a`` ([N*H*W][C] read as [N][H*W*C]): fc6 with bias + ReLU
+    into fp16, fc7 with its bias into fp32 -- ``features()``'s tensor [N][4096]."""
+    if a.ld != a.C:
+        raise ValueError("the classifier reads the final map as [N][H*W*C]: it needs a dense [M][C] map, got %r" % (a,))
+    x = a.data.view(a.N, a.H * a.W * a.C)
+    h = classifier_gemm(x, _fc6_pack(model.linear0, a.C, a.H, a.W), relu=True)
+    return classifier_gemm(h, _packed_linear(model.linear1), out_f32=True)
+
+
+def run_vgg_logits(model, features):
+    """relu1 -> last_linear on fp32 [N][4096] features: the ReLU is applied as the rows are cast to fp16 (or, for a trainable head,
+    inside functions.LinearFunction), then the classifier GEMM writes fp32 logits."""
+    head = model.last_linear
+    if not isinstance(head, nn.Linear):
+        # user-swapped head (TRN replaces it by Dropout): hand it relu1's output, as the reference does
+        return head(torch.relu(features))
+    if torch.is_grad_enabled() and any(p.requires_grad for p in head.parameters()):
+        return Fn.linear(features, head.weight, head.bias, relu_input=True)
+    return classifier_gemm(ops.cast_rows(features, relu=True), _packed_linear(head), out_f32=True)
 
 
 # ---------------------------------------------------------------------------------------------

@@ -207,6 +207,25 @@ class DenseNetTrunkFunction(_FrozenFunction):
         return DenseNetTrunkFunction._finish(ctx, engine._densenet_trunk_body(features, Act(x2d, *geom)))
 
 
+class VGGTrunkFunction(_FrozenFunction):
+    """VGG's ``_features`` (torchvision vgg.py): convolutions with bias (+ folded BatchNorm) and ReLU, 2x2 max pools."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, features):
+        from . import engine
+        return VGGTrunkFunction._finish(ctx, engine._vgg_trunk_body(features, Act(x2d, *geom)))
+
+
+class AlexNetTrunkFunction(_FrozenFunction):
+    """AlexNet's ``_features`` (torchvision alexnet.py) on the space-to-depth image: conv1 as a valid 3x3 convolution, then
+    convolutions with bias and ReLU and 3x3 stride-2 max pools."""
+
+    @staticmethod
+    def forward(ctx, x2d, geom, features):
+        from . import engine
+        return AlexNetTrunkFunction._finish(ctx, engine._alexnet_trunk_body(features, Act(x2d, *geom)))
+
+
 class GBlockFunction(_FrozenFunction):
     """BigGAN-deep GBlock: ccbn-ReLU-1x1 -> ccbn-ReLU-[up]-3x3 -> ccbn-ReLU-3x3 -> ccbn-ReLU-1x1 (+ skip)."""
 

@@ -61,6 +61,8 @@ case("slowfast18", lambda: P.slowfast.resnet18(mode="sf", num_classes=12), (1, 3
 case("densenet121", lambda: P.densenet121(pretrained=None), (2, 3, 224, 224))
 case("densenet161", lambda: P.densenet161(pretrained=None), (1, 3, 224, 224))
 case("inceptionv3", lambda: OV3.fan_in_scale_(P.inceptionv3(pretrained=None)), (1, 3, 299, 299))
+case("vgg16", lambda: P.vgg16(pretrained=None), (2, 3, 224, 224))
+case("alexnet", lambda: P.alexnet(pretrained=None), (2, 3, 224, 224))
 
 if not only or "trn" in only:
     torch.manual_seed(0)
