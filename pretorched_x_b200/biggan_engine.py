@@ -38,6 +38,7 @@ import os
 import torch
 import torch.nn.functional as F
 
+from . import functions as Fn
 from . import ops
 from .ops import Act, _round_up
 
@@ -218,13 +219,11 @@ def _next_affine(nxt, a_out_hw, aff, pk):
 
 
 def run_gblock(blk, a, aff, pk, fuse_output_bn=False, pre=None, nxt=None, out=None):
-    """One GBlock through its torch.autograd.Function (functions.GBlockFunction: forward = the launch sequence of
+    """One GBlock through the frozen torch.autograd.Function (``functions.frozen``: forward = the launch sequence of
     ``_gblock_body``, outputs non-differentiable).  Returns (block output, relu(bn1_next(output)) or None).  ``out``:
     preallocated rows for the block output (written by conv4's epilogue)."""
-    from .functions import GBlockFunction
-    d0, g0, d1, g1 = GBlockFunction.apply(a.data, (a.N, a.T, a.H, a.W, a.C), blk, aff, pk,
-                                          dict(fuse_output_bn=fuse_output_bn, pre=pre, nxt=nxt, out=out))
-    return Act(d0, *g0), (Act(d1, *g1) if d1 is not None else None)
+    y = Fn.frozen(lambda x, o: _gblock_body(blk, x, aff, pk, fuse_output_bn=fuse_output_bn, pre=pre, nxt=nxt, out=o), a, out)
+    return y if isinstance(y, tuple) else (y, None)
 
 
 def _gblock_body(blk, a, aff, pk, fuse_output_bn=False, pre=None, nxt=None, out=None):

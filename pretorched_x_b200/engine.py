@@ -18,10 +18,11 @@ parameter itself (``p.copy_()``, ``p.mul_()`` under ``no_grad``) rebuild the pac
 NOT seen: ``model.invalidate()`` / ``engine.invalidate(model)`` drops every packed copy, and it runs by itself on
 ``train()`` / ``eval()`` and on ``.to()`` / ``.half()`` / ``.cuda()`` (``_apply``).
 
-Every block body is entered through a ``torch.autograd.Function`` (``functions.py``, SURVEY.md section 8b-ii): the
-Function's ``forward`` is the ctypes call sequence, its outputs are marked non-differentiable (frozen-backbone
-semantics), except for the stages a ``fine_tune(k)`` call (``ResNet3D``, ``ResNet2D``, ``TRN``) made trainable (``block_backward``), and the dense heads (``last_linear``, the TRN
-relation MLPs) have a real backward on the same wgmma GEMM so that a head can be trained on engine features.
+Every block body is entered through one ``torch.autograd.Function`` (``functions.frozen``, SURVEY.md section 8b-ii): the
+body arrives as a callable, the Function's ``forward`` is its ctypes call sequence, and its outputs are marked
+non-differentiable (frozen-backbone semantics), except for the stages a ``fine_tune(k)`` call (``ResNet3D``, ``ResNet2D``,
+``TRN``) made trainable (``block_backward``), and the dense heads (``last_linear``, the TRN relation MLPs) have a real
+backward on the same wgmma GEMM so that a head can be trained on engine features.
 """
 import copy
 import os
@@ -194,7 +195,7 @@ def conv_bn_act(conv, bn, a, residual=None, relu=False, simt=False, pool_w=False
     """Run ``conv`` (Conv3d / Conv2d / SpatioTemporalConv-like) -> ``bn`` -> (+residual) -> (ReLU).  ``pool_w``: stem only, see
     ``_stem_body``.  ``out``: preallocated output rows (``ops.conv``)."""
     if hasattr(conv, "spatial_conv") and hasattr(conv, "temporal_conv"):
-        return Fn.SpatioTemporalConvFunction.run(conv, a, bn, residual, relu, simt, out)
+        return Fn.frozen(lambda x, o: _st_conv_body(conv, bn, x, residual, relu, simt, o), a, out)
     stem = a.ld == 4
     if stem and not _is_stem_shape(conv):
         raise NotImplementedError("NDHWC4 inputs are only supported by 7-wide stride-2 stem convolutions")
@@ -228,7 +229,7 @@ def _shortcut(block, a, simt):
 
 def run_basic(block, a, simt=False, out=None):
     """conv-BN-ReLU-conv-BN-(+shortcut)-ReLU (resnet3D.py:91-106)."""
-    return Fn.BasicBlockFunction.run(block, a, simt, out)
+    return Fn.frozen(lambda x, o: _basic_body(block, x, simt, o), a, out)
 
 
 def _basic_body(block, a, simt=False, out=None, keep=None):
@@ -318,7 +319,7 @@ def _fused_close_with_projection(block, a, h, out=None, nxt=None):
 def run_bottleneck(block, a, simt=False, out=None, h1=None, nxt=None):
     """1x1x1-BN-ReLU, 3x3x3(stride)-BN-ReLU, 1x1x1-BN-(+shortcut)-ReLU (resnet3D.py:125-143).  ``h1`` / ``nxt``: see
     ``_bottleneck_body``."""
-    return Fn.BottleneckFunction.run(block, a, simt, out, h1, nxt)
+    return Fn.frozen(lambda x, o: _bottleneck_body(block, x, simt, o, h1=h1, nxt=nxt), a, out)
 
 
 def _bottleneck_body(block, a, simt=False, out=None, keep=None, h1=None, nxt=None):
@@ -374,7 +375,7 @@ def run_block(block, a, simt=False, out=None, h1=None, nxt=None):
     if h1 is not None or nxt is not None:
         y = run_bottleneck(block, a, simt, bout, h1, nxt)
     elif getattr(block, "preactivation", False):
-        y = Fn.PreActBlockFunction.run(block, a, simt, bout)
+        y = Fn.frozen(lambda x, o: _preact_body(block, x, simt, o), a, bout)
     else:
         y = run_bottleneck(block, a, simt, bout) if hasattr(block, "conv3") else run_basic(block, a, simt, bout)
     if nl is not None:
@@ -403,7 +404,7 @@ def _pad_cols(x2d, cols):
 
 
 def run_nonlocal(nl, a, simt=False, out=None):
-    return Fn.NonLocalFunction.run(nl, a, simt, out)
+    return Fn.frozen(lambda x, o: _nonlocal_body(nl, x, simt, o), a, out)
 
 
 def _nonlocal_body(nl, a, simt=False, out=None):
@@ -581,12 +582,12 @@ def run_mobilenet_features(features, x):
     mods = list(features)
     for i, m in enumerate(mods):
         if hasattr(m, "use_res_connect"):
-            a = Fn.InvertedResidualFunction.run(m, a)
+            a = Fn.frozen(lambda x, o: _inverted_residual_body(m, x, o), a)
             continue
         nxt = mods[i + 1] if i + 1 < len(mods) else None
         # the output may skip the upper clamp only when a depthwise convolution is its sole reader
         feeds_dw = hasattr(nxt, "use_res_connect") and not nxt.use_res_connect and nxt.conv[0].groups > 1
-        a = Fn.ConvBNReLU6Function.run(m, a, not feeds_dw)
+        a = Fn.frozen(lambda x, o: _conv_bn_relu6_body(m, x, not feeds_dw), a)
     return a
 
 
@@ -634,8 +635,8 @@ def _se_pack(block, C2):
 
 
 def run_se_bottleneck(block, a, out=None):
-    """SEResNetBottleneck / SEResNeXtBottleneck (senet.py:107-131) through its Function."""
-    return Fn.SEBottleneckFunction.run(block, a, out)
+    """SEResNetBottleneck / SEResNeXtBottleneck (senet.py:107-131) through the frozen Function."""
+    return Fn.frozen(lambda x, o: _se_bottleneck_body(block, x, o), a, out)
 
 
 def _se_bottleneck_body(block, a, out=None):
@@ -681,7 +682,7 @@ def _se_stem_body(layer0, a, out=None):
 def run_senet_trunk(model, x):
     """layer0 .. layer4 of an SENet: fp32 NCHW images (or an NDHWC4 Act) in, Act out."""
     a = x if isinstance(x, Act) else ops.from_ncdhw(x)
-    a = Fn.SEStemFunction.run(model.layer0, a)
+    a = Fn.frozen(lambda x, o: _se_stem_body(model.layer0, x, o), a)
     for name in ("layer1", "layer2", "layer3", "layer4"):
         for blk in getattr(model, name):
             a = run_se_bottleneck(blk, a)
@@ -729,8 +730,8 @@ def _pool2d(pool):
 
 
 def run_inception(model, spec, a, out=None):
-    """One inception block of BNInception (``spec``: a row of models.bninception.BLOCKS) through its Function."""
-    return Fn.InceptionFunction.run(model, a, spec, out)
+    """One inception block of BNInception (``spec``: a row of models.bninception.BLOCKS) through the frozen Function."""
+    return Fn.frozen(lambda x, o: _inception_body(model, spec, x, o), a, out)
 
 
 def _inception_body(model, spec, a, out=None):
@@ -796,7 +797,7 @@ def run_bninception_trunk(model, x):
     """The BNInception trunk: fp32 NCHW images (or an NDHWC4 Act) in, the 5b block output (an Act) out."""
     from .models.bninception import BLOCKS
     a = x if isinstance(x, Act) else ops.from_ncdhw(x)
-    a = Fn.BNInceptionStemFunction.run(model, a)
+    a = Fn.frozen(lambda x, o: _bninception_stem_body(model, x, o), a)
     for spec in BLOCKS:
         a = run_inception(model, spec, a)
     return a
@@ -963,16 +964,19 @@ def _inception_block_body(block, a, out=None, row=None):
 def run_inception_trunk(n_stem, units, x):
     """The trunk of Inception-v4 (``units`` = ``features``), Inception-ResNet-v2 or Inception-v3: fp32 NCHW images (or an Act
     with channel pitch 8) in, the final 8x8 map (an Act; 1536 channels, 2048 for Inception-v3) out.  ``units[:n_stem]`` run as
-    one stem Function, every block as one ``InceptionBlockFunction``, a trailing BasicConv2d (conv2d_7b) as a stem Function of its
-    own."""
+    one frozen Function call of ``_inception_stem_body``, every block as one of ``_inception_block_body``, a trailing BasicConv2d
+    (conv2d_7b) as a stem call of its own."""
     from .models.inception import BasicConv2d
     a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
     if (a.H, a.W) != (299, 299):
         # the final pool is the reference's fixed AvgPool2d(8): only an 8x8 final map gives one vector per image
         raise ValueError("the final pool is AvgPool2d(8): it needs an 8x8 final map (299x299 inputs), got a %dx%d input" % (a.H, a.W))
-    a = Fn.InceptionStemFunction.run(tuple(units[:n_stem]), a)
+    a = Fn.frozen(lambda x, o: _inception_stem_body(tuple(units[:n_stem]), x, o), a)
     for u in units[n_stem:]:
-        a = Fn.InceptionStemFunction.run((u,), a) if isinstance(u, BasicConv2d) else Fn.InceptionBlockFunction.run(u, a)
+        if isinstance(u, BasicConv2d):
+            a = Fn.frozen(lambda x, o: _inception_stem_body((u,), x, o), a)
+        else:
+            a = Fn.frozen(lambda x, o: _inception_block_body(u, x, o), a)
     return a
 
 
@@ -1138,14 +1142,14 @@ def _polynet_block_body(module, a):
 
 def run_polynet_trunk(model, x):
     """The PolyNet trunk: fp32 NCHW images (or an Act with channel pitch 8) in, the 9x9x2048 stage_c output (an Act) out; every
-    module is one ``PolyNetBlockFunction``."""
+    module is one frozen Function call of ``_polynet_block_body``."""
     H, W = (x.H, x.W) if isinstance(x, Act) else tuple(x.shape[-2:])
     if (H, W) != (331, 331):
         # the final pool is the reference's fixed AvgPool2d(9): only a 9x9 final map gives one vector per image
         raise ValueError("the final pool is AvgPool2d(9): it needs a 9x9 final map (331x331 inputs), got a %dx%d input" % (H, W))
     a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
     for m in model.modules_in_order():
-        a = Fn.PolyNetBlockFunction.run(m, a)
+        a = Fn.frozen(lambda x, o: _polynet_block_body(m, x), a)
     return a
 
 
@@ -1261,10 +1265,10 @@ def _densenet_trunk_body(features, a):
 
 
 def run_densenet_trunk(features, x):
-    """DenseNet ``features`` up to norm5 through its Function: fp32 NCHW images (or an NDHWC4 Act) in, the last dense block's
+    """DenseNet ``features`` up to norm5 through the frozen Function: fp32 NCHW images (or an NDHWC4 Act) in, the last dense block's
     output (an Act, norm5 not applied) out."""
     a = x if isinstance(x, Act) else ops.from_ncdhw(x)
-    return Fn.DenseNetTrunkFunction.run(features, a)
+    return Fn.frozen(lambda x, o: _densenet_trunk_body(features, x), a)
 
 
 def densenet_norm5(features, a):
@@ -1342,15 +1346,15 @@ def _alexnet_trunk_body(features, a):
 
 
 def run_vgg_trunk(features, x):
-    """VGG ``_features`` through its Function: fp32 NCHW 224x224 images in, the last pool's output (an Act) out."""
+    """VGG ``_features`` through the frozen Function: fp32 NCHW 224x224 images in, the last pool's output (an Act) out."""
     _check_224(x)
-    return Fn.VGGTrunkFunction.run(features, ops.from_ncdhw(x, pitch=8))
+    return Fn.frozen(lambda x, o: _vgg_trunk_body(features, x), ops.from_ncdhw(x, pitch=8))
 
 
 def run_alexnet_trunk(features, x):
-    """AlexNet ``_features`` through its Function: fp32 NCHW 224x224 images in, the last pool's output (an Act) out."""
+    """AlexNet ``_features`` through the frozen Function: fp32 NCHW 224x224 images in, the last pool's output (an Act) out."""
     _check_224(x)
-    return Fn.AlexNetTrunkFunction.run(features, ops_vgg.space_to_depth4(x))
+    return Fn.frozen(lambda x, o: _alexnet_trunk_body(features, x), ops_vgg.space_to_depth4(x))
 
 
 def _fc6_pack(linear, C, H, W):
@@ -1425,7 +1429,7 @@ def _pool_args(mp):
 def run_stem(model, x, simt=False, out=None):
     """conv1 -> bn1 -> relu -> maxpool (torchvision_models.py:449-452)."""
     a = x if isinstance(x, Act) else ops.from_ncdhw(x)
-    return Fn.StemFunction.run(model, a, simt, out)
+    return Fn.frozen(lambda x, o: _stem_body(model, x, simt, o), a, out)
 
 
 def _stem_body(model, a, simt=False, out=None):

@@ -3,12 +3,12 @@
 
 Two kinds:
 
-* **Frozen block bodies** -- ``StemFunction``, ``BottleneckFunction`` (resnet3D.py:125-143), ``BasicBlockFunction``
-  (:91-106), ``SpatioTemporalConvFunction`` (r2plus1d.py:85-88), ``NonLocalFunction`` (nonlocalnet.py:143-243),
-  ``GBlockFunction`` (BigGAN-deep GBlock).  ``forward`` is the ctypes launch sequence of ``engine.py`` /
-  ``biggan_engine.py`` on fp16 NDHWC matrices; every output is marked non-differentiable, so the modules can sit inside
-  an autograd graph as a frozen feature extractor (the way the reference's zoo models are used with a replaced
-  ``last_linear``, README.md:520-547).  These frozen bodies have no backward: asking for one raises.
+* **Frozen block bodies** -- one ``FrozenFunction``, entered through ``frozen(body, a, out)``: every block body of
+  ``engine.py`` / ``biggan_engine.py`` (stem, residual and non-local blocks, inception blocks, whole trunks, BigGAN-deep
+  GBlocks) arrives as the callable ``body``, and its ``forward`` is that body's ctypes launch sequence on fp16 NDHWC
+  matrices.  Every output is marked non-differentiable, so the modules can sit inside an autograd graph as a frozen feature
+  extractor (the way the reference's zoo models are used with a replaced ``last_linear``, README.md:520-547).  These frozen
+  bodies have no backward: asking for one raises.
 * **Fine-tuned residual blocks** -- ``BlockTrainFunction`` / ``FineTunePoolFunction``, used instead of the frozen bodies for
   ``layer{k}..layer4`` after ``ResNet3D.fine_tune(k)`` (engine.block_backward).
 * **Dense heads with a real backward** -- ``LinearFunction`` (``last_linear`` / ``fc``: resnet3D.py:162,
@@ -17,8 +17,9 @@ Two kinds:
   head can be trained on engine features without leaving the library.
 
 Tensors cross a Function boundary as the raw ``[N*T*H*W][ld]`` fp16 matrix of an ``ops.Act`` plus its geometry tuple.
-``out`` (optional, last argument of the block bodies): a preallocated ``[rows][ld]`` fp16 row range the body's LAST kernel writes
-its result into -- how the depth-first trunk schedule (``engine.run_trunk``) assembles a full-batch tensor chunk by chunk.
+``out`` (optional, the second argument of a frozen ``body``): a preallocated ``[rows][ld]`` fp16 row range the body's LAST
+kernel writes its result into -- how the depth-first trunk schedule (``engine.run_trunk``) assembles a full-batch tensor chunk by
+chunk.
 """
 import torch
 
@@ -30,214 +31,33 @@ def _geom(a):
     return (a.N, a.T, a.H, a.W, a.C)
 
 
-class _FrozenFunction(torch.autograd.Function):
-    """Base: outputs are constants to autograd."""
+class FrozenFunction(torch.autograd.Function):
+    """One frozen block body as one autograd node: ``forward`` runs ``body(Act, out)`` and marks every tensor it returns
+    non-differentiable, so the result is a constant to autograd."""
+
+    @staticmethod
+    def forward(ctx, x2d, out, geom, body):
+        res = body(Act(x2d, *geom), out)
+        acts = res if isinstance(res, tuple) else (res,)
+        ctx.mark_non_differentiable(*(r.data for r in acts if r is not None))
+        flat = ()
+        for r in acts:
+            flat += (r.data, _geom(r)) if r is not None else (None, None)
+        return flat
 
     @staticmethod
     def backward(ctx, *grads):      # pragma: no cover - unreachable: every output is marked non-differentiable
         raise RuntimeError("pretorched_x_b200 is a forward-pass engine: the convolutional trunk has no backward "
                            "(frozen-backbone semantics); only LinearFunction / the relation MLP are differentiable")
 
-    @classmethod
-    def run(cls, module, a, *extra):
-        """Act in -> Act out through ``cls.apply``."""
-        data, geom = cls.apply(a.data, _geom(a), module, *extra)
-        return Act(data, *geom)
 
-    @classmethod
-    def _finish(cls, ctx, out):
-        ctx.mark_non_differentiable(out.data)
-        return out.data, _geom(out)
-
-
-class StemFunction(_FrozenFunction):
-    """conv1 -> bn1 -> relu -> maxpool (torchvision_models.py:449-452).  ``x`` is the NDHWC4 / NDHWC input matrix."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, model, simt=False, out=None):
-        from . import engine
-        return StemFunction._finish(ctx, engine._stem_body(model, Act(x2d, *geom), simt, out))
-
-
-class BottleneckFunction(_FrozenFunction):
-    """``h1``: the block's conv1 output, computed by the previous block's closing kernel.  ``nxt``: the next block, whose conv1
-    the closing kernel computes too (engine._chains); then the result is (block output, next block's h1), as in GBlockFunction."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, block, simt=False, out=None, h1=None, nxt=None):
-        from . import engine
-        out = engine._bottleneck_body(block, Act(x2d, *geom), simt, out, h1=h1, nxt=nxt)
-        if isinstance(out, tuple):
-            ctx.mark_non_differentiable(out[0].data, out[1].data)
-            return out[0].data, _geom(out[0]), out[1].data, _geom(out[1])
-        ctx.mark_non_differentiable(out.data)
-        return out.data, _geom(out), None, None
-
-    @classmethod
-    def run(cls, block, a, simt=False, out=None, h1=None, nxt=None):
-        y2d, geom, h2d, hgeom = cls.apply(a.data, _geom(a), block, simt, out, h1, nxt)
-        return (Act(y2d, *geom), Act(h2d, *hgeom)) if nxt is not None else Act(y2d, *geom)
-
-
-class BasicBlockFunction(_FrozenFunction):
-    @staticmethod
-    def forward(ctx, x2d, geom, block, simt=False, out=None):
-        from . import engine
-        return BasicBlockFunction._finish(ctx, engine._basic_body(block, Act(x2d, *geom), simt, out))
-
-
-class PreActBlockFunction(_FrozenFunction):
-    """Pre-activation residual blocks (pre_act_resnet3D.py:27-96)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, block, simt=False, out=None):
-        from . import engine
-        return PreActBlockFunction._finish(ctx, engine._preact_body(block, Act(x2d, *geom), simt, out))
-
-
-class SpatioTemporalConvFunction(_FrozenFunction):
-    """(1,k,k) conv -> BN -> ReLU -> (k,1,1) conv [-> outer BN -> +residual -> ReLU] (r2plus1d.py:85-88)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, conv, bn=None, residual=None, relu=False, simt=False, out=None):
-        from . import engine
-        return SpatioTemporalConvFunction._finish(ctx, engine._st_conv_body(conv, bn, Act(x2d, *geom), residual, relu, simt, out))
-
-
-class NonLocalFunction(_FrozenFunction):
-    @staticmethod
-    def forward(ctx, x2d, geom, nl, simt=False, out=None):
-        from . import engine
-        return NonLocalFunction._finish(ctx, engine._nonlocal_body(nl, Act(x2d, *geom), simt, out))
-
-
-class ConvBNReLU6Function(_FrozenFunction):
-    """MobileNetV2 conv_bn / conv_1x1_bn: conv -> BN -> ReLU6 (mobilenet.py:22-35)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, seq, clamp_out=True):
-        from . import engine
-        return ConvBNReLU6Function._finish(ctx, engine._conv_bn_relu6_body(seq, Act(x2d, *geom), clamp_out))
-
-
-class InvertedResidualFunction(_FrozenFunction):
-    """MobileNetV2 inverted residual: expand -> depthwise -> project (+ x) (mobilenet.py:38-76)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, block, out=None):
-        from . import engine
-        return InvertedResidualFunction._finish(ctx, engine._inverted_residual_body(block, Act(x2d, *geom), out))
-
-
-class SEStemFunction(_FrozenFunction):
-    """layer0 of the SENets: conv1 -> bn1 -> relu1 -> ceil-mode pool (senet.py:272-283)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, layer0, out=None):
-        from . import engine
-        return SEStemFunction._finish(ctx, engine._se_stem_body(layer0, Act(x2d, *geom), out))
-
-
-class SEBottleneckFunction(_FrozenFunction):
-    """SEResNetBottleneck / SEResNeXtBottleneck (senet.py:107-131): convolutions, squeeze-excite and the closing GEMM."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, block, out=None):
-        from . import engine
-        return SEBottleneckFunction._finish(ctx, engine._se_bottleneck_body(block, Act(x2d, *geom), out))
-
-
-class BNInceptionStemFunction(_FrozenFunction):
-    """The BNInception stem: conv1_7x7_s2 .. pool2_3x3_s2 (bninception.py:255-265)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, model, out=None):
-        from . import engine
-        return BNInceptionStemFunction._finish(ctx, engine._bninception_stem_body(model, Act(x2d, *geom), out))
-
-
-class InceptionFunction(_FrozenFunction):
-    """One BNInception block (``spec``: a row of models.bninception.BLOCKS): its branches written in place into the
-    concatenated output (bninception.py:266-483)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, model, spec, out=None):
-        from . import engine
-        return InceptionFunction._finish(ctx, engine._inception_body(model, spec, Act(x2d, *geom), out))
-
-
-class InceptionStemFunction(_FrozenFunction):
-    """Units of Inception-v4 / Inception-ResNet-v2 / Inception-v3 outside the blocks, in sequence (``units``: a tuple of
-    BasicConv2d / MaxPool2d): the stems (inceptionv4.py:274-276, inceptionresnetv2.py:305-311, torchvision_models.py:397-403)
-    and conv2d_7b (inceptionresnetv2.py:319)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, units, out=None):
-        from . import engine
-        return InceptionStemFunction._finish(ctx, engine._inception_stem_body(units, Act(x2d, *geom), out))
-
-
-class InceptionBlockFunction(_FrozenFunction):
-    """One block of Inception-v4 / Inception-ResNet-v2 / Inception-v3 (models.inception.BRANCHES): its branches written in place
-    into the concatenated output, and the residual close of Block35 / 17 / 8."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, block, out=None):
-        from . import engine
-        return InceptionBlockFunction._finish(ctx, engine._inception_block_body(block, Act(x2d, *geom), out))
-
-
-class PolyNetBlockFunction(_FrozenFunction):
-    """One module of the PolyNet trunk (polynet.py:71-371): the stem, a reduction, a 2-way module or a poly-3 module, every
-    branch written in place into its concatenation matrix."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, module):
-        from . import engine
-        return PolyNetBlockFunction._finish(ctx, engine._polynet_block_body(module, Act(x2d, *geom)))
-
-
-class DenseNetTrunkFunction(_FrozenFunction):
-    """The DenseNet trunk up to norm5 (torchvision densenet.py ``features`` without its last BatchNorm): every dense block as one
-    matrix that its layers and the preceding transition (or the stem's pool) write in place."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, features):
-        from . import engine
-        return DenseNetTrunkFunction._finish(ctx, engine._densenet_trunk_body(features, Act(x2d, *geom)))
-
-
-class VGGTrunkFunction(_FrozenFunction):
-    """VGG's ``_features`` (torchvision vgg.py): convolutions with bias (+ folded BatchNorm) and ReLU, 2x2 max pools."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, features):
-        from . import engine
-        return VGGTrunkFunction._finish(ctx, engine._vgg_trunk_body(features, Act(x2d, *geom)))
-
-
-class AlexNetTrunkFunction(_FrozenFunction):
-    """AlexNet's ``_features`` (torchvision alexnet.py) on the space-to-depth image: conv1 as a valid 3x3 convolution, then
-    convolutions with bias and ReLU and 3x3 stride-2 max pools."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, features):
-        from . import engine
-        return AlexNetTrunkFunction._finish(ctx, engine._alexnet_trunk_body(features, Act(x2d, *geom)))
-
-
-class GBlockFunction(_FrozenFunction):
-    """BigGAN-deep GBlock: ccbn-ReLU-1x1 -> ccbn-ReLU-[up]-3x3 -> ccbn-ReLU-3x3 -> ccbn-ReLU-1x1 (+ skip)."""
-
-    @staticmethod
-    def forward(ctx, x2d, geom, blk, aff, pk, kwargs):
-        from . import biggan_engine
-        out = biggan_engine._gblock_body(blk, Act(x2d, *geom), aff, pk, **kwargs)
-        if isinstance(out, tuple):          # (block output, pre-activated input of the next block)
-            ctx.mark_non_differentiable(out[0].data, out[1].data)
-            return out[0].data, _geom(out[0]), out[1].data, _geom(out[1])
-        ctx.mark_non_differentiable(out.data)
-        return out.data, _geom(out), None, None
+def frozen(body, a, out=None):
+    """``body(Act, out) -> Act``, or ``-> (Act, Act or None)``, run on ``a`` as one ``FrozenFunction`` node; returns what the
+    body returned.  ``body`` puts the module and its other arguments in the block body's own order, e.g.
+    ``frozen(lambda x, o: engine._stem_body(model, x, simt, o), a, out)``."""
+    flat = FrozenFunction.apply(a.data, out, _geom(a), body)
+    acts = tuple(Act(d, *g) if d is not None else None for d, g in zip(flat[0::2], flat[1::2]))
+    return acts if len(acts) > 1 else acts[0]
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -3,7 +3,7 @@
 The modules are parameter containers created under the reference's names and in its order, so the ``state_dict`` keys, their
 order and a seeded random init are the reference's and its checkpoint loads unchanged.  The forward runs on the engine
 (engine.run_bninception_trunk): the 7x7 stem on the stem kernel, the ceil-mode pools on the pooling kernel, and every inception
-block as one ``InceptionFunction`` whose branches write their columns of the concatenated block output in place -- the 1x1 heads
+block as one ``functions.frozen`` call whose branches write their columns of the concatenated block output in place -- the 1x1 heads
 that read the block input as one split GEMM, the 3x3 branches as slice convolutions, the pool branch as a slice pool (+ its
 projection GEMM).
 

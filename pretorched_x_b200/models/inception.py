@@ -2,7 +2,7 @@
 
 The modules are parameter containers created under the reference's names and in its order, so the ``state_dict`` keys, their
 order and a seeded random init are the reference's and its checkpoints load unchanged.  The forward runs on the engine
-(engine.run_inception_trunk): every block is one ``InceptionBlockFunction`` whose branches write their columns of the
+(engine.run_inception_trunk): every block is one ``functions.frozen`` call whose branches write their columns of the
 concatenated block output in place -- the 1x1 heads that read the block input as one split GEMM, the convolutions with taps
 (valid-padded 3x3, 1x7 / 7x1, 1x3 / 3x1, 5x5) as slab slice convolutions, the pool branches as slice pools -- and whose
 residual form (Block35 / 17 / 8) closes with the persistent GEMM: per-column scale, shift, the block input as residual, ReLU.

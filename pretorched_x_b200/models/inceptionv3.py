@@ -6,7 +6,7 @@ and seeded init; the blocks are torchvision's InceptionA-E classes, subclassed o
 models.inception.BRANCHES), and the forward runs on the engine (engine.run_inception_trunk), exactly as Inception-v4's:
 
 * the stem (Conv2d_1a_3x3 .. maxpool2) is Inception-ResNet-v2's stem, unit for unit;
-* every block is one ``InceptionBlockFunction`` whose branches write their columns of the concatenated output in place: the 1x1
+* every block is one ``functions.frozen`` call whose branches write their columns of the concatenated output in place: the 1x1
   units that read the block input as one split GEMM, every convolution with taps (3x3, 5x5, 1x7 / 7x1, 1x3 / 3x1) on the slab
   kernel's slice entry, the average-pool branches (F.avg_pool2d(3, 1, 1), padding counted) as a slice pool into a matrix that
   ``branch_pool`` reads, the max-pool branches (F.max_pool2d(3, 2)) as a slice pool into the pass-through columns;

@@ -2,7 +2,7 @@
 
 The modules are parameter containers created under the reference's names and in its order, so the ``state_dict`` keys (3104),
 their order and a seeded random init are the reference's and its checkpoint loads unchanged.  The forward runs on the engine
-(engine.run_polynet_trunk), one ``PolyNetBlockFunction`` per module, on the Inception block path of models/inception.py:
+(engine.run_polynet_trunk), one ``functions.frozen`` call per module, on the Inception block path of models/inception.py:
 
 * the stem and the two reductions are rows of ``BRANCHES`` below, walked by engine._inception_block_body: their 1x1 heads as
   one split GEMM, every convolution with taps on the slab kernel's slice entry, the max pools into their pass-through columns;
@@ -255,7 +255,7 @@ class PolyNet(engine.CacheOwner, nn.Module):
         self.last_linear = nn.Linear(2048, num_classes)
 
     def modules_in_order(self):
-        """The trunk's modules, each one PolyNetBlockFunction: stem, stage_a, reduction_a, stage_b, reduction_b, stage_c."""
+        """The trunk's modules, each one ``functions.frozen`` call: stem, stage_a, reduction_a, stage_b, reduction_b, stage_c."""
         return [self.stem, *self.stage_a, self.reduction_a, *self.stage_b, self.reduction_b, *self.stage_c]
 
     def features_act(self, x):

@@ -228,7 +228,7 @@ def test_block_matches_oracle(model, name):
 # 5. models against the reference fixtures
 # ---------------------------------------------------------------------------------------------
 def _stages(m, x):
-    a = Fn.BNInceptionStemFunction.run(m, ops.from_ncdhw(x))
+    a = Fn.frozen(lambda t, o: engine._bninception_stem_body(m, t, o), ops.from_ncdhw(x))
     out = {"stem": a}
     for spec in PB.BLOCKS:
         a = engine.run_inception(m, spec, a)
@@ -236,7 +236,7 @@ def _stages(m, x):
     return out, m.logits(a)
 
 
-def test_model_matches_reference_fixture():
+def test_model_stages_match_reference_fixture():
     fx = _load("bninception_b2_224.pt")
     m = OB.build_package_model(P, fx).to(dev)
     x = OF.seeded_input(fx["input_shape"], fx["seeds"]["input"]).to(dev)

@@ -209,13 +209,13 @@ BLOCKS = [("inceptionv4", "features.3", 147), ("inceptionv4", "features.4", 73),
 
 
 @pytest.mark.parametrize("arch,name,H", BLOCKS, ids=["%s-%s" % b[:2] for b in BLOCKS])
-def test_block_matches_oracle(models, arch, name, H):
+def test_frozen_block_matches_oracle(models, arch, name, H):
     m = models[arch]
     blk = m.get_submodule(name)
     cin = [mod for mod in blk.modules() if isinstance(mod, torch.nn.Conv2d)][0].in_channels
     x = torch.rand((2, cin, H, H), generator=torch.Generator().manual_seed(9)).to(torch.float16)
     with torch.no_grad():
-        y = engine.Fn.InceptionBlockFunction.run(blk, ops.from_ncdhw(x.to(dev)))
+        y = engine.Fn.frozen(lambda t, o: engine._inception_block_body(blk, t, o), ops.from_ncdhw(x.to(dev)))
     got = ops.to_ncdhw(y).squeeze(2).double().cpu()
     sd = {k: v.detach().double().cpu() for k, v in m.state_dict().items()}
     want = OI.block(x.double(), sd, blk, name + ".")

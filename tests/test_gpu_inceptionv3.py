@@ -56,15 +56,15 @@ BLOCKS = [("Mixed_5b", 35), ("Mixed_5c", 35), ("Mixed_5d", 35), ("Mixed_6a", 35)
 
 
 @pytest.mark.parametrize("name,H", BLOCKS, ids=[b[0] for b in BLOCKS])
-def test_block_matches_oracle(model, name, H):
+def test_frozen_block_matches_oracle(model, name, H):
     blk = model.get_submodule(name)
     cin = [mod for mod in blk.modules() if isinstance(mod, torch.nn.Conv2d)][0].in_channels
     x = (torch.rand((2, cin, H, H), generator=torch.Generator().manual_seed(9)) * 4).to(torch.float16)
     a = ops.from_ncdhw(x.to(dev))
     with torch.no_grad():
-        engine.Fn.InceptionBlockFunction.run(blk, a)          # the first call also packs the filters
+        engine.Fn.frozen(lambda t, o: engine._inception_block_body(blk, t, o), a)     # the first call also packs the filters
         c0 = _lib.launch_count()
-        y = engine.Fn.InceptionBlockFunction.run(blk, a)
+        y = engine.Fn.frozen(lambda t, o: engine._inception_block_body(blk, t, o), a)
     torch.cuda.synchronize()
     assert _lib.launch_count() - c0 == LAUNCHES[type(blk).kind]
     got = ops.to_ncdhw(y).squeeze(2).double().cpu()

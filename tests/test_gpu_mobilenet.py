@@ -150,16 +150,16 @@ def staged(m, x):
         mods = list(m.features)
         for i, blk in enumerate(mods):
             if hasattr(blk, "use_res_connect"):
-                a = Fn.InvertedResidualFunction.run(blk, a)
+                a = Fn.frozen(lambda t, o: engine._inverted_residual_body(blk, t, o), a)
             else:
-                a = Fn.ConvBNReLU6Function.run(blk, a, i == len(mods) - 1)
+                a = Fn.frozen(lambda t, o: engine._conv_bn_relu6_body(blk, t, i == len(mods) - 1), a)
             outs["features.%d" % i] = a
         logits = m.logits(a)
     return outs, logits
 
 
 @pytest.mark.parametrize("path", FIX, ids=[os.path.basename(p)[:-3] for p in FIX])
-def test_forward_matches_reference_golden(path):
+def test_staged_forward_matches_reference_golden(path):
     fx = _load(path)
     m = OM.build_package_model(P, fx).to(dev)
     x = OF.seeded_input(fx["input_shape"], fx["seeds"]["input"]).to(dev)

@@ -121,14 +121,14 @@ MODULES = [("stem", 3, 331), ("stage_a.0", 384, 39), ("reduction_a", 384, 39), (
 
 
 @pytest.mark.parametrize("name,C,H", MODULES, ids=[m[0] for m in MODULES])
-def test_module_matches_oracle(model, name, C, H):
+def test_frozen_module_matches_oracle(model, name, C, H):
     mod = model.get_submodule(name)
     x = (torch.rand((2, C, H, H), generator=torch.Generator().manual_seed(9)) * 4).to(torch.float16)
     a = ops.from_ncdhw(x.to(dev), pitch=8 if C == 3 else None)
     with torch.no_grad():
-        engine.Fn.PolyNetBlockFunction.run(mod, a)              # the first call also packs the filters
+        engine.Fn.frozen(lambda t, o: engine._polynet_block_body(mod, t), a)     # the first call also packs the filters
         c0 = _lib.launch_count()
-        y = engine.Fn.PolyNetBlockFunction.run(mod, a)
+        y = engine.Fn.frozen(lambda t, o: engine._polynet_block_body(mod, t), a)
     torch.cuda.synchronize()
     assert _lib.launch_count() - c0 == LAUNCHES[type(mod).__name__]
     got = ops.to_ncdhw(y).squeeze(2).double().cpu()

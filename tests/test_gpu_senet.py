@@ -224,7 +224,7 @@ def test_block_matches_oracle(name, cls, inplanes, planes, groups, stride, H):
 # 5. models against the reference fixtures
 # ---------------------------------------------------------------------------------------------
 def _stages(model, x):
-    a = Fn.SEStemFunction.run(model.layer0, ops.from_ncdhw(x))
+    a = Fn.frozen(lambda t, o: engine._se_stem_body(model.layer0, t, o), ops.from_ncdhw(x))
     out = {"layer0": a}
     for name in ("layer1", "layer2", "layer3", "layer4"):
         for blk in getattr(model, name):
@@ -234,7 +234,7 @@ def _stages(model, x):
 
 
 @pytest.mark.parametrize("fname", ["se_resnet50_b2_224.pt", "se_resnext50_32x4d_b2_224.pt"])
-def test_model_matches_reference_fixture(fname):
+def test_model_stages_match_reference_fixture(fname):
     fx = _load(fname)
     model = OS.build_package_model(P, fx).to(dev)
     x = OF.seeded_input(fx["input_shape"], fx["seeds"]["input"]).to(dev)
