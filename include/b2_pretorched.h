@@ -284,6 +284,12 @@ size_t b2_pack_grouped_conv_weight_elems(int K, int Cin_per_group, int groups, i
 int b2_pack_grouped_conv_weight(const float* w, void* w_packed, int K, int Cin_per_group, int groups, int kt, int kh, int kw,
                                 void* stream);
 int b2_conv_grouped_ndhwc_fprop(const b2_conv_args* a, int groups, void* stream);
+/* The input gradient of a grouped convolution (fine-tuning backward): the same group-aware kernel and contract as
+ * b2_conv_grouped_ndhwc_fprop at stride 1 (a strided gradient is zero-inserted first, b2_zero_insert_ndhwc), with the filter packed
+ * transposed within each group, flipped and BatchNorm-scaled by the caller, and the ReLU-derivative mask (required; mask pitch ldm
+ * a multiple of 8, >= ldy): y is zeroed where mask <= 0.  Residual, ReLU and every other extra must be zero.
+ * b2_debug_last_kernel: KID 10, as the forward. */
+int b2_conv_grouped_ndhwc_dgrad(const b2_conv_args* a, int groups, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Fine-tuning backward of the residual blocks (the backward of resnet3D.py:91-143 with eval-mode BatchNorm).  Gradients
@@ -311,6 +317,21 @@ size_t b2_conv_wgrad_thw_workspace_elems(int N, int T, int H, int W, int Cin, in
 int b2_conv_wgrad_thw(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
                       float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int Cin, int Cout, int kt,
                       int kh, int kw, int st, int s, int pt, int p, void* stream);
+/* Weight gradient of a grouped 1 x 3 x 3 convolution with C == K (C % 64 == 0, 4 / 8 / 16 / 32 channels per group, padding 1,
+ * stride s in {1, 2}; a 2-D filter at T = 1):
+ *     dw[k][c_local][tap] = scale[k] * G[k][g cg + c_local][tap] * inv_loss_scale   (fp32, nn.Conv2d grouped weight layout
+ *                                                                                     [C][C / groups][3][3], g = k / cg)
+ *     wdot[k]             = sum w[k][c_local][tap] * G * inv_loss_scale               (nullable; needs w, fp32 same layout)
+ * Only the diagonal 64 x 64 block of each 64-channel slice and tap is computed: 64 / cg times the algorithmic multiply-
+ * accumulates (position blocks of 8 x 8 aside), never the dense C x C product.  Deterministic split-K as b2_conv_wgrad_thw (ws:
+ * b2_conv_wgrad_grouped_workspace_elems floats).  b2_conv_wgrad_grouped_plan returns the executed and algorithmic
+ * multiply-accumulate counts and the split count of that plan.  b2_debug_last_kernel: KID 18, info = {cg, splits, position blocks}. */
+size_t b2_conv_wgrad_grouped_workspace_elems(int N, int T, int H, int W, int C, int groups, int s);
+int b2_conv_wgrad_grouped_plan(int N, int T, int H, int W, int C, int groups, int s, long long* executed_macs, long long* algorithmic_macs,
+                               int* splits);
+int b2_conv_wgrad_grouped(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
+                          float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int C, int groups, int s,
+                          void* stream);
 /* Adjoint of b2_shortcut_a_ndhwc: y[n, s*to, s*ho, s*wo, 0:C] = g[n, to, ho, wo, 0:C] for the low-resolution extent
  * To = (T-1)/s + 1 (etc.), every other pixel and channels [C, ldy) zero; y is [N*T*H*W][ldy].  The backward of the type-A
  * shortcut, the placement of the type-B projection gradient, and the zero-insertion that turns the input gradient of a

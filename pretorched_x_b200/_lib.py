@@ -103,6 +103,10 @@ SYMBOLS = {
     "b2_pack_grouped_conv_weight_elems": (ctypes.c_size_t, [c_int] * 6),
     "b2_pack_grouped_conv_weight": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
     "b2_conv_grouped_ndhwc_fprop": (c_int, [ctypes.POINTER(ConvArgs), c_int, c_void_p]),
+    "b2_conv_grouped_ndhwc_dgrad": (c_int, [ctypes.POINTER(ConvArgs), c_int, c_void_p]),
+    "b2_conv_wgrad_grouped_workspace_elems": (ctypes.c_size_t, [c_int] * 7),
+    "b2_conv_wgrad_grouped_plan": (c_int, [c_int] * 7 + [ctypes.POINTER(ctypes.c_longlong)] * 2 + [ctypes.POINTER(c_int)]),
+    "b2_conv_wgrad_grouped": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 6 + [ctypes.c_size_t] + [c_int] * 7 + [c_void_p]),
     "b2_gemm_sample_affine_f16": (c_int, [ctypes.POINTER(GemmArgs), c_void_p]),
     "b2_maxpool3d_ndhwc_out": (c_int, [c_void_p, c_void_p] + [c_int] * 17 + [c_void_p]),
     "b2_se_excite_workspace_elems": (ctypes.c_size_t, [c_int] * 3),

@@ -306,6 +306,8 @@ static int launch_slab(const b2_conv_args* a, SlabParams& p, int MT, int R, cuda
   p.scale = a->scale; p.shift = a->shift;
   p.residual = reinterpret_cast<const __half*>(a->residual);
   p.ldr = a->ldr;
+  p.mask = G ? reinterpret_cast<const __half*>(a->mask) : nullptr;
+  p.ldm = G ? a->ldm : 0;
   p.y = reinterpret_cast<__half*>(a->y);
   p.ldy = a->ldy;
   p.ldo = ldo;
@@ -597,6 +599,7 @@ static int launch_slab_t(const b2_conv_args* a, TPlan& t, cudaStream_t stream) {
   p.Ncols = a->K;
   p.scale = a->scale; p.shift = a->shift;
   p.residual = nullptr; p.ldr = 0;
+  p.mask = nullptr; p.ldm = 0;
   p.y = reinterpret_cast<__half*>(a->y);
   p.ldy = a->ldy;
   p.ldo = 0;
@@ -1519,6 +1522,8 @@ int b2_pack_grouped_conv_weight(const float* w, void* out, int K, int Cin_per_gr
   return B2_OK;
 }
 
+static int grouped_slab(const b2_conv_args* a, int groups, void* stream);
+
 int b2_conv_grouped_ndhwc_fprop(const b2_conv_args* a, int groups, void* stream) {
   set_last_kernel(KID_NONE);
   int rc = validate_conv(a);
@@ -1527,6 +1532,26 @@ int b2_conv_grouped_ndhwc_fprop(const b2_conv_args* a, int groups, void* stream)
                    !a->residual_pre && !a->y2 && !a->scale2 && !a->shift2 && !a->aff2_ld && !a->pool_w && !a->in_scale && !a->in_shift &&
                    !a->in_aff_ld && !a->mask && !a->ldm,
                "the grouped convolution takes a plain fp16 call: mode, fp32 output, per-sample affines, generator and fine-tuning fields must be zero");
+  return grouped_slab(a, groups, stream);
+}
+
+int b2_conv_grouped_ndhwc_dgrad(const b2_conv_args* a, int groups, void* stream) {
+  set_last_kernel(KID_NONE);
+  int rc = validate_conv(a);
+  if (rc != B2_OK) return rc;
+  B2_CHECK_ARG(a->mode == B2_CONV_AUTO && !a->out_f32 && !a->accumulate && !a->aff_ld && !a->upsample && !a->residual_up &&
+                   !a->residual_pre && !a->y2 && !a->scale2 && !a->shift2 && !a->aff2_ld && !a->pool_w && !a->in_scale && !a->in_shift &&
+                   !a->in_aff_ld && !a->residual && !a->ldr && !a->relu,
+               "the grouped input gradient takes a plain fp16 call with a mask: mode, fp32 output, residual, ReLU, per-sample affines "
+               "and generator fields must be zero");
+  B2_CHECK_ARG(a->mask, "the grouped input gradient needs the ReLU-derivative mask");
+  B2_CHECK_ARG(a->ldm % 8 == 0 && a->ldm >= a->ldy, "mask pitch %d must be a multiple of 8 and >= ldy %d", a->ldm, a->ldy);
+  B2_CHECK_ARG(a->st == 1 && a->sh == 1 && a->sw == 1, "the input gradient is a stride-1 convolution (zero-insert a strided gradient)");
+  return grouped_slab(a, groups, stream);
+}
+
+static int grouped_slab(const b2_conv_args* a, int groups, void* stream) {
+  int rc;
   B2_CHECK_ARG(groups > 0, "groups must be positive");
   const int cg = a->C / groups;
   if (a->C != a->K || a->C % groups || !grouped_filter_ok(a->K, cg, groups, a->kt, a->kh, a->kw) || a->pt != a->kt / 2 || a->ph != 1 ||

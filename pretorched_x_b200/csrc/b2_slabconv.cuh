@@ -80,6 +80,10 @@ struct SlabParams {
   const float* shift;
   const __half* residual;  // nullable, dense [M][ldr]; only columns < Ncols are read
   int ldr;
+  // slabconv_kernel<64, G> (grouped) only, nullable: fp16 [M][ldm]; the output is zeroed where mask <= 0 (the ReLU derivative of
+  // the fine-tuning backward, b2_conv_grouped_ndhwc_dgrad)
+  const __half* mask;
+  int ldm;
   __half* y;               // dense [M][ldy]
   int ldy;
   int relu;
@@ -517,6 +521,14 @@ slabconv_kernel(const __grid_constant__ CUtensorMap tmX,   // input as (C, W, H,
                                                        fmaf(v[2 * e + 1], sc[c + 1], sh[c + 1]));
                         if (p.relu) hv = __hmax2(hv, zero2);
                         o[e] = *reinterpret_cast<uint32_t*>(&hv);
+                      }
+                      if constexpr (G_ > 0) {
+                        if (p.mask) {                          // uniform
+                          const uint4 mv = *reinterpret_cast<const uint4*>(p.mask + static_cast<size_t>(row[j]) * p.ldm + c0 + c8 * 8);
+                          const uint32_t mm[4] = {mv.x, mv.y, mv.z, mv.w};
+#pragma unroll
+                          for (int e = 0; e < 4; ++e) o[e] &= __hgt2_mask(*reinterpret_cast<const __half2*>(&mm[e]), zero2);
+                        }
                       }
                       *reinterpret_cast<uint4*>(yrow + c8 * 8) = ov;
                     }

@@ -174,6 +174,138 @@ static WgradPlan wgrad_plan(int N, int T, int H, int W, int Cin, int Cout, int k
   return q;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Grouped weight gradient (C == K, 4 / 8 / 16 / 32 channels per group, 1 x 3 x 3 filters): every group lies inside one 64-channel
+// slice, so only the diagonal 64 x 64 block of each slice and tap is computed -- one consumer warpgroup, A = g^T, B = x^T over
+// the same position blocks and TMA boxes as wgrad_kernel -- 64 / cg times the algorithmic multiply-accumulates instead of the
+// K x C (= groups times) of the dense product.  Workspace [splits][taps][C][64] (column = input channel within the slice); the
+// reduce keeps the group's own cg columns:
+//     dw[k][c_local][tap] = scale[k] * G[k][g cg + c_local][tap] / loss_scale,  wdot[k] = <w[k], G[k]> / loss_scale
+// ---------------------------------------------------------------------------------------------------------------------------
+constexpr int kWgdThreads = 160;          // warps 0-3: one consumer warpgroup, warp 4: TMA producer
+constexpr int kWgdStageBytes = 2 * kWgTileBytes;
+constexpr int kWgdSmem = kWgStages * kWgdStageBytes + 1024 + 2 * kWgStages * 8;
+
+__global__ void __launch_bounds__(kWgdThreads, 1)
+wgrad_diag_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX, const WgradParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_align<1024>(smem_raw);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kWgStages * kWgdStageBytes);
+  uint64_t* empty = full + kWgStages;
+  const int c0 = blockIdx.x * 64;
+  const int tap = blockIdx.y % p.taps, split = blockIdx.y / p.taps;
+  const int b0 = static_cast<int>(static_cast<long long>(p.nbox) * split / p.splits);
+  const int b1 = static_cast<int>(static_cast<long long>(p.nbox) * (split + 1) / p.splits);
+  const int warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kWgStages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 1);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp == 4) {
+    if ((threadIdx.x & 31) == 0) {
+      tma_prefetch_desc(&tmG);
+      tma_prefetch_desc(&tmX);
+      const int dh = tap / p.kw, dw = tap % p.kw;
+      for (int b = b0, i = 0; b < b1; ++b, ++i) {
+        const int s = i % kWgStages;
+        if (i >= kWgStages) mbar_wait(&empty[s], ((i / kWgStages) - 1) & 1);
+        int q = b;
+        const int wbi = q % p.wb; q /= p.wb;
+        const int hbi = q % p.hb; q /= p.hb;
+        const int t = q % p.To;
+        const int n = q / p.To;
+        const int h0 = hbi * 8, w0 = wbi * 8;
+        uint8_t* st = smem + s * kWgdStageBytes;
+        mbar_expect_tx(&full[s], kWgdStageBytes);
+        tma_load_5d(st, &tmG, &full[s], c0, w0, h0, t, n);
+        tma_load_5d(st + kWgTileBytes, &tmX, &full[s], c0, w0 * p.s + dw - p.p, h0 * p.s + dh - p.p, t, n);
+      }
+    }
+    return;
+  }
+
+  float acc[32];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  for (int b = b0, i = 0; b < b1; ++b, ++i) {
+    const int s = i % kWgStages;
+    mbar_wait(&full[s], (i / kWgStages) & 1);
+    const uint32_t st = smem_u32(smem + s * kWgdStageBytes);
+    const uint64_t da = wg_desc_mn(st), db = wg_desc_mn(st + kWgTileBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_n64_ss_mn(acc, da + k * 128, db + k * 128);
+    wgmma_commit();
+    wgmma_wait0();
+    if (threadIdx.x == 0) mbar_arrive(&empty[s]);
+  }
+
+  const int wt = threadIdx.x;
+  const int row = c0 + (wt >> 5) * 16 + ((wt & 31) >> 2);
+  float* out = p.ws + (static_cast<size_t>(split) * p.taps + tap) * p.Cout * 64;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int col = 8 * j + 2 * (wt & 3);
+    *reinterpret_cast<float2*>(out + static_cast<size_t>(row) * 64 + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(out + static_cast<size_t>(row + 8) * 64 + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
+}
+
+// One CTA per output channel, fixed-order sums as wgrad_reduce_kernel, over the cg x taps entries of the channel's own group.
+__global__ void __launch_bounds__(kWgReduceThreads)
+wgrad_diag_reduce_kernel(const float* __restrict__ ws, int splits, int C, int cg, int taps, const float* __restrict__ w,
+                         const float* __restrict__ scale, const float* __restrict__ inv_loss_scale, float* __restrict__ dw,
+                         float* __restrict__ wdot) {
+  __shared__ float part[kWgReduceThreads / 32];
+  const int k = blockIdx.x;
+  const float inv = inv_loss_scale ? *inv_loss_scale : 1.f;
+  const float sc = scale ? scale[k] : 1.f;
+  const int n = cg * taps;
+  const int base = (k & 63) / cg * cg;                 // the group's first input channel within the 64-channel slice
+  const size_t slice = static_cast<size_t>(C) * 64;
+  float dot = 0.f;
+  for (int i = threadIdx.x; i < n; i += kWgReduceThreads) {
+    const int tap = i / cg, cl = i - tap * cg;
+    const float* src = ws + static_cast<size_t>(tap) * slice + static_cast<size_t>(k) * 64 + base + cl;
+    float g = 0.f;
+    for (int j = 0; j < splits; ++j) g += src[static_cast<size_t>(j) * taps * slice];
+    g *= inv;
+    const size_t o = static_cast<size_t>(k) * n + static_cast<size_t>(cl) * taps + tap;
+    dw[o] = sc * g;
+    if (w) dot += w[o] * g;
+  }
+  if (!wdot) return;
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) dot += __shfl_down_sync(0xffffffffu, dot, off);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = dot;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int j = 0; j < kWgReduceThreads / 32; ++j) t += part[j];
+    wdot[k] = t;
+  }
+}
+
+static WgradPlan wgrad_diag_plan(int N, int T, int H, int W, int C, int s) {
+  WgradPlan q = wgrad_plan(N, T, H, W, C, C, 1, 3, 3, 1, s, 0, 1);
+  q.tiles = (C / 64) * 9;
+  int sp = (2 * sm_count() + q.tiles - 1) / q.tiles;
+  sp = sp < q.nbox / 4 ? sp : q.nbox / 4;
+  sp = sp < 64 ? sp : 64;
+  q.splits = sp > 1 ? sp : 1;
+  return q;
+}
+
+static bool wgrad_diag_ok(int N, int T, int H, int W, int C, int groups, int s) {
+  return N > 0 && T > 0 && H > 0 && W > 0 && groups > 0 && C % 64 == 0 && C % groups == 0 && (s == 1 || s == 2) &&
+         (C / groups == 4 || C / groups == 8 || C / groups == 16 || C / groups == 32);
+}
+
 }  // namespace b2
 
 using namespace b2;
@@ -223,6 +355,59 @@ int b2_conv_wgrad_thw(const void* g, int ldg, const void* x, int ldx, const floa
   B2_CHECK_LAUNCH("wgrad");
   wgrad_reduce_kernel<<<Cout, kWgReduceThreads, 0, stm>>>(ws, q.splits, Cout, Cin, taps, w, scale, inv_loss_scale, dw, wdot);
   B2_CHECK_LAUNCH("wgrad_reduce");
+  return B2_OK;
+}
+
+size_t b2_conv_wgrad_grouped_workspace_elems(int N, int T, int H, int W, int C, int groups, int s) {
+  if (!wgrad_diag_ok(N, T, H, W, C, groups, s)) return 0;
+  return static_cast<size_t>(wgrad_diag_plan(N, T, H, W, C, s).splits) * 9 * C * 64;
+}
+
+int b2_conv_wgrad_grouped_plan(int N, int T, int H, int W, int C, int groups, int s, long long* executed_macs, long long* algorithmic_macs,
+                               int* splits) {
+  B2_CHECK_ARG(executed_macs && algorithmic_macs && splits, "null pointer");
+  if (!wgrad_diag_ok(N, T, H, W, C, groups, s))
+    return set_error(B2_ERR_UNSUPPORTED, "grouped weight gradient needs C %% 64 == 0, 4 / 8 / 16 / 32 channels per group, stride 1 or 2");
+  const WgradPlan q = wgrad_diag_plan(N, T, H, W, C, s);
+  *executed_macs = static_cast<long long>(q.nbox) * 64 * 9 * (C / 64) * 64 * 64;
+  *algorithmic_macs = static_cast<long long>(N) * T * q.Ho * q.Wo * 9 * C * (C / groups);
+  *splits = q.splits;
+  return B2_OK;
+}
+
+int b2_conv_wgrad_grouped(const void* g, int ldg, const void* x, int ldx, const float* w, const float* scale, const float* inv_loss_scale,
+                          float* dw, float* wdot, float* ws, size_t ws_elems, int N, int T, int H, int W, int C, int groups, int s,
+                          void* stream) {
+  set_last_kernel(KID_NONE);
+  B2_CHECK_ARG(g && x && dw && ws, "null pointer");
+  B2_CHECK_ARG(!wdot || w, "wdot needs the weight");
+  if (!wgrad_diag_ok(N, T, H, W, C, groups, s))
+    return set_error(B2_ERR_UNSUPPORTED, "grouped weight gradient needs C %% 64 == 0, 4 / 8 / 16 / 32 channels per group and stride 1 "
+                                         "or 2 (got C=%d groups=%d stride %d)", C, groups, s);
+  B2_CHECK_ARG(ldg >= C && ldx >= C && ldg % 8 == 0 && ldx % 8 == 0, "pitches must be multiples of 8 and >= C");
+  const WgradPlan q = wgrad_diag_plan(N, T, H, W, C, s);
+  B2_CHECK_ARG(q.Ho > 0 && q.Wo > 0, "empty output");
+  B2_CHECK_ARG(ws_elems >= static_cast<size_t>(q.splits) * 9 * C * 64, "workspace too small (see b2_conv_wgrad_grouped_workspace_elems)");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  CUtensorMap tmG, tmX;
+  if ((rc = make_tmap_ndhwc_5d(&tmG, g, (uint64_t)C, (uint64_t)ldg, (uint64_t)q.Wo, (uint64_t)q.Ho, (uint64_t)T, (uint64_t)N, 8, 8, 1)) !=
+      B2_OK)
+    return rc;
+  if ((rc = make_tmap_ndhwc_5d(&tmX, x, (uint64_t)C, (uint64_t)ldx, (uint64_t)W, (uint64_t)H, (uint64_t)T, (uint64_t)N, 8, 8,
+                               (uint32_t)s)) != B2_OK)
+    return rc;
+  WgradParams prm;
+  prm.Cout = C; prm.Cin = C; prm.taps = 9; prm.kh = 3; prm.kw = 3;
+  prm.To = T; prm.Ho = q.Ho; prm.Wo = q.Wo; prm.hb = (q.Ho + 7) / 8; prm.wb = (q.Wo + 7) / 8;
+  prm.nbox = q.nbox; prm.splits = q.splits; prm.st = 1; prm.s = s; prm.pt = 0; prm.p = 1; prm.ws = ws;
+  cudaStream_t stm = reinterpret_cast<cudaStream_t>(stream);
+  B2_OPT_IN_SMEM(wgrad_diag_kernel, kWgdSmem);
+  wgrad_diag_kernel<<<dim3(C / 64, 9 * q.splits), kWgdThreads, kWgdSmem, stm>>>(tmG, tmX, prm);
+  B2_CHECK_LAUNCH("wgrad_diag");
+  wgrad_diag_reduce_kernel<<<C, kWgReduceThreads, 0, stm>>>(ws, q.splits, C, C / groups, 9, w, scale, inv_loss_scale, dw, wdot);
+  B2_CHECK_LAUNCH("wgrad_diag_reduce");
+  set_last_kernel(KID_WGRAD_GROUPED, C / groups, q.splits, q.nbox);
   return B2_OK;
 }
 

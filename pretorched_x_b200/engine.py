@@ -33,6 +33,7 @@ import torch.nn as nn
 from . import ops
 from . import ops_dual
 from . import ops_vgg
+from . import ops_grouped
 from . import functions as Fn
 from .ops import Act
 
@@ -1558,9 +1559,10 @@ class TrainAct(Act):
     __slots__ = ("loss_scale",)
 
 
-def _check_trainable_2d(block):
-    """torchvision BasicBlock / Bottleneck (the 2-D ResNets): Conv2d 1x1 / 3x3 with padding k // 2, stride 1 or 2, no groups,
-    bias or dilation, BatchNorm2d, identity or (Conv2d 1x1, BatchNorm2d) shortcut."""
+def _check_trainable_2d(block, grouped=False):
+    """torchvision BasicBlock / Bottleneck (the 2-D ResNets) and ResNeXt-101's bottleneck: Conv2d 1x1 / 3x3 with padding k // 2,
+    stride 1 or 2, no bias or dilation, no groups except (``grouped``, ResNeXt-101) a 3x3 inside the group-aware kernels'
+    contract (C == K, 4 / 8 / 16 / 32 channels per group), BatchNorm2d, identity or (Conv2d 1x1, BatchNorm2d) shortcut."""
     convs = [(block.conv1, block.bn1), (block.conv2, block.bn2)] + ([(block.conv3, block.bn3)] if hasattr(block, "conv3") else [])
     ds = block.downsample
     ok = True
@@ -1571,7 +1573,8 @@ def _check_trainable_2d(block):
         ok = False
     for conv, bn in convs if ok else ():
         k = tuple(conv.weight.shape[2:])
-        ok = ok and type(conv) is nn.Conv2d and conv.groups == 1 and conv.bias is None and all(d == 1 for d in conv.dilation)
+        ok = ok and type(conv) is nn.Conv2d and conv.bias is None and all(d == 1 for d in conv.dilation)
+        ok = ok and (conv.groups == 1 or (grouped and k == (3, 3) and grouped_route(conv)))   # the group-aware kernels' contract
         ok = ok and k in ((1, 1), (3, 3)) and tuple(conv.padding) == (k[0] // 2,) * 2
         ok = ok and len(set(conv.stride)) == 1 and conv.stride[0] in (1, 2)
         ok = ok and isinstance(bn, nn.BatchNorm2d) and bn.affine and bn.running_var is not None
@@ -1585,8 +1588,9 @@ def check_trainable_block(block):
     BasicBlock / Bottleneck the backward covers."""
     import torchvision.models.resnet as tvresnet
     from .models.resnet3d import BasicBlock, Bottleneck, ShortcutA
-    if type(block) in (tvresnet.BasicBlock, tvresnet.Bottleneck):
-        return _check_trainable_2d(block)
+    from .models.resnext import ResNeXt101Bottleneck
+    if type(block) in (tvresnet.BasicBlock, tvresnet.Bottleneck, ResNeXt101Bottleneck):
+        return _check_trainable_2d(block, grouped=type(block) is ResNeXt101Bottleneck)
     name = type(block).__name__
     ok = type(block) in (BasicBlock, Bottleneck) and getattr(block, "nonlocalblock", None) is None
     convs = [(block.conv1, block.bn1), (block.conv2, block.bn2)] + ([(block.conv3, block.bn3)] if ok and hasattr(block, "conv3") else [])
@@ -1664,6 +1668,25 @@ def _gemm_dgrad(g, wt, residual=None, second=None, mask=None):
     return Act(y, g.N, g.T, g.H, g.W, C)
 
 
+def _dgrad_grouped(conv, s):
+    """The input gradient of a grouped 2-D 3x3 convolution (C == K) as a stride-1 grouped convolution with the same groups: its
+    filter transposed within each group, flipped and s-folded, on the group-aware kernel."""
+    K, cg = conv.weight.shape[:2]
+    G = conv.groups
+    w = (conv.weight.detach().float() * s.view(-1, 1, 1, 1)).view(G, cg, cg, 3, 3).transpose(1, 2).flip(3, 4).reshape(K, cg, 3, 3)
+    return ops.PackedGroupedConv(w.contiguous(), G, None, None, (1, 1, 1), (0, 1, 1))
+
+
+def _conv_dgrad_masked(conv, s, g, x):
+    """Gradient at the input ``x`` of a 3x3x3 (or 2-D 3x3, grouped or not) convolution for the gradient ``g`` at its (BN-scaled)
+    output, times the ReLU mask [x > 0]."""
+    stride = _inplane_stride(conv)
+    z = g if stride == 1 else ops.zero_insert(g, x.T, x.H, x.W, stride)
+    if conv.groups > 1:
+        return ops_grouped.conv_grouped_dgrad(z, _dgrad_grouped(conv, s), mask=x)
+    return ops.conv(z, _dgrad_3x3(conv, s, z.ld), mask=x)
+
+
 def _conv_dgrad(conv, s, g, x):
     """Gradient at the input ``x`` of a 3x3x3 convolution for the gradient ``g`` at its (BN-scaled) output, before any residual."""
     stride = _inplane_stride(conv)
@@ -1678,8 +1701,12 @@ def _param_grads(conv, bn, g, x, ls, needs):
     inv = ls[1:]
     if need_w or need_g:
         stride, pad = _conv_geometry(conv)
-        dw, wdot = ops.conv_wgrad(g, x, _kernel_thw(conv), stride, pad, weight=conv.weight if need_g else None, scale=_bn_scale(bn),
-                                  inv_loss_scale=inv)
+        if conv.groups > 1:
+            dw, wdot = ops_grouped.conv_wgrad_grouped(g, x, conv.groups, stride[1], weight=conv.weight if need_g else None, scale=_bn_scale(bn),
+                                              inv_loss_scale=inv)
+        else:
+            dw, wdot = ops.conv_wgrad(g, x, _kernel_thw(conv), stride, pad, weight=conv.weight if need_g else None,
+                                      scale=_bn_scale(bn), inv_loss_scale=inv)
         dw = dw.view(conv.weight.shape)
     if need_b or need_g:
         dbeta = ops.colsum(g, inv)
@@ -1711,8 +1738,7 @@ def block_backward(block, x, hs, gy, ls, need_x, needs):
         grads[6:9] = _param_grads(block.conv3, block.bn3, gy, h2, ls, needs[6:9])
         g2 = _gemm_dgrad(gy, _dgrad_1x1(block.conv3, _bn_scale(block.bn3)), mask=h2)
         grads[3:6] = _param_grads(block.conv2, block.bn2, g2, h1, ls, needs[3:6])
-        z, pc = _conv_dgrad(block.conv2, _bn_scale(block.bn2), g2, h1)
-        g1 = ops.conv(z, pc, mask=h1)
+        g1 = _conv_dgrad_masked(block.conv2, _bn_scale(block.bn2), g2, h1)
     else:
         (h1,) = hs
         grads[3:6] = _param_grads(block.conv2, block.bn2, gy, h1, ls, needs[3:6])

@@ -154,11 +154,15 @@ class FineTunable:
         for i in range(k, 5):
             for blk in getattr(self, 'layer%d' % i):
                 engine.check_trainable_block(blk)
-        trainable = tuple('layer%d.' % i for i in range(k, 5)) + ('%s.' % self.head_name,)
+        trainable = tuple(self._stage_prefix(i) for i in range(k, 5)) + ('%s.' % self.head_name,)
         for name, p in self.named_parameters():
             p.requires_grad_(name.startswith(trainable))
         self.ft_begin_index = k
         return self
+
+    def _stage_prefix(self, i):
+        """Parameter-name prefix of stage ``layer{i}`` (ResNeXt101: ``features.{3 + i}.``, its reference's names)."""
+        return 'layer%d.' % i
 
     def _fine_tuning(self):
         return self.ft_begin_index is not None and self.ft_begin_index <= 4 and torch.is_grad_enabled()
