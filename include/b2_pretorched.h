@@ -262,6 +262,18 @@ int b2_dwconv3x3_ndhwc(const void* x, const float* w, const float* scale, const 
 int b2_relu6_inplace_ndhwc(void* x, long long rows, int ld, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Xception (xception.py:50-233)
+ * ------------------------------------------------------------------------------------------- */
+/* Depthwise 3x3 convolution, stride 1, padding 1 (conv1 of SeparableConv2d, xception.py:50-60) of ReLU(x), with no affine:
+ *     y[n, h, w, c] = sum_{kh,kw} max(x[n, h + kh - 1, w + kw - 1, c], 0) * w[kh*3 + kw][c]
+ * with zero padding, fp32 accumulation in the fixed tap order (kh, kw) and one fp16 rounding.  The ReLU is the one that opens
+ * every separable convolution of an Xception block, whose input is the signed residual sum; the BatchNorm that follows is applied
+ * by the pointwise GEMM.  x, y: fp16 [N*H*W][ld], channels [C, ld) of y written as zero; w: fp32 [9][C] (tap-major).
+ * C % 8 == 0, ld % 8 == 0, ld >= C, every pointer 16-byte aligned.  A compile-time variant of b2_dwconv3x3_ndhwc's kernel
+ * (4 output columns per thread).  b2_debug_last_kernel: KID 19, info = {1, 4}. */
+int b2_dwconv3x3_relu_in_ndhwc(const void* x, const float* w, void* y, int N, int H, int W, int C, int ld, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * ResNeXt-3D (resnext3D.py:76-121)
  * ------------------------------------------------------------------------------------------- */
 /* Grouped convolution (nn.Conv3d(C, C, 3, stride, 1, groups=32), conv2 of ResNeXtBottleneck, resnext3D.py:86-93) -> BatchNorm

@@ -9,6 +9,11 @@
 // rows above and below, and the edge columns shared with the neighbouring run) is served by L1 / L2: each input byte
 // comes from HBM once.  Every output element accumulates its taps in the fixed order (kh, kw) in fp32; the folded BN
 // affine and the clamp run in fp32 before the single fp16 rounding.
+//
+// The RELU_IN instance is the depthwise half of Xception's separable convolutions (xception.py:50-60, 93-112): it reads
+// max(x, 0) and has no affine and no activation (the BatchNorm follows the pointwise 1x1, in its GEMM epilogue), so it rounds
+// the fp32 tap sum itself.  Xception needs the ReLU on load because a block's input is the signed residual sum, which the
+// skip path reads raw.
 #include "b2_host.h"
 
 #include <cuda_fp16.h>
@@ -36,8 +41,9 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
 }
 
 // x, y: fp16 [N*H*W][ld] resp. [N*Ho*Wo][ld] as uint4 (ld8 = ld / 8 vectors per pixel); w: fp32 [9][C] (tap-major);
-// scale / shift: fp32 [C].  Thread i -> (n, ho, run of R output columns, 8-channel group), channel group fastest.
-template <int S, int R>
+// scale / shift: fp32 [C] (unused by RELU_IN).  Thread i -> (n, ho, run of R output columns, 8-channel group), channel group
+// fastest.
+template <int S, int R, bool RELU_IN>
 __global__ void __launch_bounds__(256) dwconv3x3_kernel(const uint4* __restrict__ x, const float* __restrict__ w,
                                                          const float* __restrict__ scale, const float* __restrict__ shift,
                                                          uint4* __restrict__ y, int H, int W, int Ho, int Wo, int runs, int C8,
@@ -85,7 +91,10 @@ __global__ void __launch_bounds__(256) dwconv3x3_kernel(const uint4* __restrict_
       if (wi < 0 || wi >= W) continue;                  // zero padding column
       float xv[8];
       unpack8(__ldg(xrow + (long long)wi * ld8), xv);
-      if (clamp_in) {
+      if constexpr (RELU_IN) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) xv[e] = fmaxf(xv[e], 0.f);
+      } else if (clamp_in) {
 #pragma unroll
         for (int e = 0; e < 8; ++e) xv[e] = fminf(xv[e], 6.f);
       }
@@ -99,6 +108,12 @@ __global__ void __launch_bounds__(256) dwconv3x3_kernel(const uint4* __restrict_
     }
   }
 
+  if constexpr (RELU_IN) {
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+      if (wo0 + r < Wo) y[(orow + wo0 + r) * ld8 + c8] = pack8(acc[r]);
+    return;
+  }
   float sc[8], sh[8];
   {
     const float4* sp = reinterpret_cast<const float4*>(scale + c8 * 8);
@@ -132,15 +147,15 @@ __global__ void relu6_inplace_kernel(uint4* __restrict__ x, long long vecs) {
   x[i] = v;
 }
 
-template <int S, int R>
+template <int S, int R, bool RELU_IN = false>
 static int launch_dwconv(const void* x, const float* w, const float* scale, const float* shift, void* y, int N, int H, int W,
                          int C, int ld, int clamp_in, int relu6, cudaStream_t stream) {
   const int Ho = (H - 1) / S + 1, Wo = (W - 1) / S + 1;
   const int runs = (Wo + R - 1) / R;
   const long long total = (long long)N * Ho * runs * (ld / 8);
-  dwconv3x3_kernel<S, R><<<div_up(total, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), w, scale, shift,
-                                                                 reinterpret_cast<uint4*>(y), H, W, Ho, Wo, runs, C / 8, ld / 8,
-                                                                 clamp_in, relu6, total);
+  dwconv3x3_kernel<S, R, RELU_IN><<<div_up(total, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(x), w, scale, shift,
+                                                                          reinterpret_cast<uint4*>(y), H, W, Ho, Wo, runs, C / 8,
+                                                                          ld / 8, clamp_in, relu6, total);
   B2_CHECK_LAUNCH("dwconv3x3_kernel");
   return B2_OK;
 }
@@ -165,6 +180,21 @@ int b2_dwconv3x3_ndhwc(const void* x, const float* w, const float* scale, const 
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   return stride == 1 ? launch_dwconv<1, 4>(x, w, scale, shift, y, N, H, W, C, ld, clamp_in, relu6, st)
                      : launch_dwconv<2, 2>(x, w, scale, shift, y, N, H, W, C, ld, clamp_in, relu6, st);
+}
+
+int b2_dwconv3x3_relu_in_ndhwc(const void* x, const float* w, void* y, int N, int H, int W, int C, int ld, void* stream) {
+  B2_CHECK_ARG(x && w && y, "null tensor pointer");
+  B2_CHECK_ARG(N > 0 && H > 0 && W > 0 && C > 0, "empty output (N %d, H %d, W %d, C %d)", N, H, W, C);
+  B2_CHECK_ARG(C % 8 == 0, "channel count %d is not a multiple of 8", C);
+  B2_CHECK_ARG(ld % 8 == 0 && ld >= C, "channel pitch %d must be a multiple of 8 and >= C %d", ld, C);
+  B2_CHECK_ARG(((uintptr_t)x | (uintptr_t)y | (uintptr_t)w) % 16 == 0, "tensors must be 16-byte aligned");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  constexpr int R = 4;
+  if ((rc = launch_dwconv<1, R, true>(x, w, nullptr, nullptr, y, N, H, W, C, ld, 0, 0, reinterpret_cast<cudaStream_t>(stream))) != B2_OK)
+    return rc;
+  set_last_kernel(KID_DWCONV_RELU_IN, 1, R);
+  return B2_OK;
 }
 
 int b2_relu6_inplace_ndhwc(void* x, long long rows, int ld, void* stream) {

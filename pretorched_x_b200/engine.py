@@ -24,6 +24,7 @@ non-differentiable (frozen-backbone semantics), except for the stages a ``fine_t
 ``TRN``) made trainable (``block_backward``), and the dense heads (``last_linear``, the TRN relation MLPs) have a real
 backward on the same wgmma GEMM so that a head can be trained on engine features.
 """
+import collections
 import copy
 import os
 
@@ -34,6 +35,7 @@ from . import ops
 from . import ops_dual
 from . import ops_vgg
 from . import ops_grouped
+from . import ops_xception
 from . import functions as Fn
 from .ops import Act
 
@@ -595,17 +597,18 @@ def run_mobilenet_features(features, x):
 # ---------------------------------------------------------------------------------------------
 # SE-ResNet / SE-ResNeXt (senet.py:85-366)
 # ---------------------------------------------------------------------------------------------
-def _strided_1x1(conv, bn, a, relu):
-    """A 1x1 Conv2d of stride s > 1 (SE-ResNet's conv1, senet.py:166-167, and every stage's projection): the strided pixel
-    subset is gathered once (1/s^2 of the input, b2_shortcut_a_ndhwc at T = 1) and the convolution runs as a stride-1 GEMM."""
+def _strided_1x1(conv, bn, a, relu, residual=None, out=None):
+    """A 1x1 Conv2d of stride s > 1 (SE-ResNet's conv1, senet.py:166-167, every stage's projection, Xception's skips): the
+    strided pixel subset is gathered once (1/s^2 of the input, b2_shortcut_a_ndhwc at T = 1) and the convolution runs as a
+    stride-1 GEMM, with ``residual`` added in its epilogue."""
     s = _conv_geometry(conv)[0]
     if s[1] == 1:
-        return conv_bn_act(conv, bn, a, relu=relu)
+        return conv_bn_act(conv, bn, a, residual=residual, relu=relu, out=out)
     if not (_plain_1x1(conv) and s[1] == s[2] and a.T == 1):
         raise NotImplementedError("strided 1x1 convolutions need equal in-plane strides on images")
     sub = ops.shortcut_a(a, s[1], a.C)
     pc = packed_conv(conv, bn, sub.ld, stride=(1, 1, 1))
-    return ops.conv(sub, pc, relu=relu)
+    return ops.conv(sub, pc, residual=residual, relu=relu, out=out)
 
 
 def _se_pack(block, C2):
@@ -1413,6 +1416,129 @@ def run_vgg_logits(model, features):
     if torch.is_grad_enabled() and any(p.requires_grad for p in head.parameters()):
         return Fn.linear(features, head.weight, head.bias, relu_input=True)
     return classifier_gemm(ops.cast_rows(features, relu=True), _packed_linear(head), out_f32=True)
+
+
+# ---------------------------------------------------------------------------------------------
+# Xception (xception.py:50-233)
+# ---------------------------------------------------------------------------------------------
+# Every separable convolution is two launches: the depthwise 3x3 on CUDA cores, then the pointwise 1x1 on the persistent GEMM with
+# the BatchNorm that follows it and a ReLU (the next op is another separable convolution) or the block's identity residual in its
+# epilogue.  A separable convolution that a ReLU of ``rep`` opens runs its depthwise pass on max(x, 0)
+# (ops_xception.dwconv3x3_relu_in): the first one reads the block input, the previous block's signed residual sum, which the skip
+# path reads raw; on the later ones (a pointwise output stored after its ReLU) the max is the identity.  One that no ReLU opens (the
+# first of a block built with start_with_relu=False, block1) and conv3, which reads block12's signed sum, run their depthwise pass on
+# b2_dwconv3x3_ndhwc with a unit affine.
+_XUnit = collections.namedtuple("_XUnit", "conv bn")
+
+
+def _xception_dw(conv):
+    """(fp32 [9][C] taps, unit scale, zero shift) of SeparableConv2d.conv1: a depthwise 3x3, stride 1, padding 1, no bias."""
+    C = conv.weight.shape[0]
+    stride, padding = _conv_geometry(conv)
+    if (conv.groups != C or tuple(conv.weight.shape[1:]) != (1, 3, 3) or stride != (1, 1, 1) or padding != (0, 1, 1)
+            or conv.bias is not None or any(d != 1 for d in conv.dilation)):
+        raise NotImplementedError("Xception's depthwise pass covers 3x3 convolutions with groups = channels, stride 1, padding 1 "
+                                  "and no bias")
+    dev = conv.weight.device
+    return _cached(conv, "dw9", _sig(conv.weight),
+                   lambda: (conv.weight.detach().reshape(C, 9).t().float().contiguous(),) + ops.fold_affine(C, None, None, dev))
+
+
+def _separable(sep, bn, a, relu_in=True, residual=None, relu=False, out=None):
+    """SeparableConv2d ``sep`` -> BatchNorm ``bn`` (xception.py:50-60) of max(a, 0) (of ``a`` itself without ``relu_in``): the
+    depthwise pass, then the pointwise GEMM with the BatchNorm, ``residual`` and ``relu`` in its epilogue."""
+    if a.C != sep.conv1.weight.shape[0]:
+        raise ValueError("separable convolution over %d channels got %r" % (sep.conv1.weight.shape[0], a))
+    w9, one, zero = _xception_dw(sep.conv1)
+    if relu_in:
+        h = ops_xception.dwconv3x3_relu_in(a, w9)
+    else:
+        h = ops.dwconv3x3(a, w9, one, zero, 1, relu6=False)
+    return conv_bn_act(sep.pointwise, bn, h, residual=residual, relu=relu, out=out)
+
+
+def _xception_rep(block):
+    """The separable convolutions of ``block.rep`` as (SeparableConv2d, BatchNorm2d, whether a ReLU opens it) triples, and its
+    closing pool (or None).  The layout must be the reference's: [ReLU, SeparableConv2d, BatchNorm2d] per repetition, the first ReLU
+    absent only in a block built with start_with_relu=False, then MaxPool2d(3, 2, 1) in the blocks with a projection skip."""
+    rep = list(block.rep)
+    pool = rep.pop() if rep and isinstance(rep[-1], nn.MaxPool2d) else None
+    seps, i = [], 0
+    while i < len(rep):
+        relu = isinstance(rep[i], nn.ReLU)
+        if relu:
+            i += 1
+        elif seps:
+            break
+        if i + 1 >= len(rep) or not hasattr(rep[i], "pointwise") or not isinstance(rep[i + 1], nn.BatchNorm2d):
+            break
+        seps.append((rep[i], rep[i + 1], relu))
+        i += 2
+    ok = bool(seps) and i == len(rep)
+    if pool is not None:
+        ok = (ok and block.skip is not None and not pool.ceil_mode and pool.dilation in (1, (1, 1))
+              and _pool_args(pool) == ((1, 3, 3), (1, 2, 2), (0, 1, 1)))
+    else:
+        ok = ok and block.skip is None
+    if not ok:
+        raise NotImplementedError("the engine runs Xception blocks as the reference builds them: [ReLU, SeparableConv2d, BatchNorm2d] "
+                                  "repetitions, closed by MaxPool2d(3, 2, 1) with a projection skip or by the identity skip")
+    return seps, pool
+
+
+def _xception_stem_body(model, a):
+    """conv1 (3x3, stride 2, valid) -> bn1 -> ReLU -> conv2 (3x3, valid) -> bn2 -> ReLU (xception.py:163-169), each on the slab
+    kernel's slice entry as Inception-v3's stem (``_basic_unit``)."""
+    a = _basic_unit(_XUnit(model.conv1, model.bn1), a)
+    return _basic_unit(_XUnit(model.conv2, model.bn2), a)
+
+
+def _xception_block_body(block, a, out=None):
+    """Block (xception.py:63-112): the separable convolutions of ``rep``, the first on max(x, 0) only when a ReLU opens it, each
+    but the last with the ReLU that opens the next in its GEMM epilogue; the last adds the block input (blocks 4-11) in its epilogue, or, in a strided block, is pooled
+    (MaxPool2d(3, 2, 1)) and the skip's 1x1 stride-2 convolution + skipbn adds the pooled tensor as its residual
+    (``x += skip``): the strided pixels are gathered and the projection runs as a GEMM (``_strided_1x1``)."""
+    seps, pool = _xception_rep(block)
+    h = a
+    for i, (sep, bn, relu_in) in enumerate(seps):
+        if i < len(seps) - 1:
+            h = _separable(sep, bn, h, relu_in=relu_in, relu=True)
+        elif pool is None:
+            h = _separable(sep, bn, h, relu_in=relu_in, residual=a, out=out)
+        else:
+            h = _separable(sep, bn, h, relu_in=relu_in)
+    if pool is None:
+        return h
+    pooled = ops.maxpool3d(h, *_pool_args(pool))
+    return _strided_1x1(block.skip, block.skipbn, a, relu=False, residual=pooled, out=out)
+
+
+def _xception_exit_body(model, a):
+    """conv3 -> bn3 -> ReLU -> conv4 -> bn4 (xception.py:183-192): bn4's output, before the head's ReLU."""
+    h = _separable(model.conv3, model.bn3, a, relu_in=False, relu=True)
+    return _separable(model.conv4, model.bn4, h)
+
+
+def run_xception_trunk(model, x):
+    """Xception's ``features`` on the engine: fp32 NCHW images (or an Act with channel pitch 8) in, bn4's output (an Act) out.  The
+    stem, each block and the exit flow are one frozen Function call each."""
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
+    if a.T != 1 or a.H < 7 or a.W < 7:
+        # conv1 and conv2 are valid 3x3 convolutions: below 7x7 the reference's conv2 has no output either
+        raise ValueError("Xception takes images of at least 7x7, got %r" % (a,))
+    a = Fn.frozen(lambda x, o: _xception_stem_body(model, x), a)
+    for i in range(1, 13):
+        blk = getattr(model, "block%d" % i)
+        a = Fn.frozen(lambda x, o: _xception_block_body(blk, x, o), a)
+    return Fn.frozen(lambda x, o: _xception_exit_body(model, x), a)
+
+
+def run_xception_head(model, a):
+    """ReLU -> adaptive mean -> view -> last_linear (xception.py:195-202) on bn4's output ``a``: the ReLU and the mean are one pass
+    (b2_avgpool_global_affine_ndhwc with a unit affine), so any final map size works."""
+    dev = a.data.device
+    s, t = _cached(model, "head_unit", (a.ld, dev), lambda: ops.fold_affine(a.ld, None, None, dev))
+    return _head_on_pooled(model.last_linear, ops.avgpool_global_affine(a, s, t), a.C)
 
 
 # ---------------------------------------------------------------------------------------------
