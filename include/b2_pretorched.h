@@ -274,6 +274,34 @@ int b2_relu6_inplace_ndhwc(void* x, long long rows, int ld, void* stream);
 int b2_dwconv3x3_relu_in_ndhwc(const void* x, const float* w, void* y, int N, int H, int W, int C, int ld, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * PNASNet-5 (pnasnet.py:49-146)
+ * ------------------------------------------------------------------------------------------- */
+/* Depthwise K x K convolution (K = 3, 5 or 7; stride 1 or 2) of ReLU(x), with no affine: the relu_1 / relu_2 + depthwise_conv2d of
+ * BranchSeparables (pnasnet.py:67-97):
+ *     y[n, ho, wo, c] = sum_{kh,kw} max(x[n, ho*stride + kh - pad, wo*stride + kw - pad, c], 0) * w[kh*K + kw][c]
+ * Taps outside the H x W map read zero; the output extent Ho x Wo is the caller's (a window may run past the bottom / right
+ * edge).  The ZeroPad2d((1, 0, 1, 0)) -> convolution at padding K/2 -> [1:, 1:] crop of a reduction cell with zero_pad (cell_4) is
+ * this convolution at pad = K/2 - 1 with the ceil extent (42 -> 21).  fp32 accumulation in the fixed tap order (kh, kw), one fp16
+ * rounding.  x: fp16 rows of pitch ldx (channels [0, C) read); y: the column slice (y, ldy, C) of N*Ho*Wo rows -- columns [0, C)
+ * written, the rest of each row untouched; w: fp32 [K*K][C] (tap-major).  C % 8 == 0, ldx and ldy multiples of 8 and >= C,
+ * 0 <= pad <= K/2, every window overlapping the input ((Ho - 1) * stride - pad < H, likewise W), x / y / w 16-byte aligned, and y's address
+ * range (first row to the last row's column C) disjoint from x's: two column slices of one matrix are refused even where their
+ * columns do not meet (B2_ERR_INVALID otherwise).  Output columns per thread: 2 at stride 2; 6 (K = 3) or 4 (K = 5, 7) at stride 1.
+ * b2_debug_last_kernel: KID 20,
+ * info = {K, stride, pad, output columns per thread}. */
+int b2_dwconv_kxk_relu_in_ndhwc(const void* x, int ldx, const float* w, void* y, int ldy, int N, int H, int W, int C, int K, int stride,
+                                int pad, int Ho, int Wo, void* stream);
+/* b2_shortcut_a_ndhwc on images with the sampled grid shifted by `offset` (0 <= offset < stride), and max(x, 0) when relu != 0:
+ *     y[n, ho, wo, 0:C] = [relu] x[n, ho*stride + offset, wo*stride + offset, 0:C]   (zero where the row or column is past the map)
+ *     y[n, ho, wo, C:Cout] = 0,   Ho = (H - 1) / stride + 1, Wo likewise
+ * x: fp16 [N*H*W][C], y: fp16 [N*Ho*Wo][Cout].  Offset 1 at stride 2 is path_2 of FactorizedReduction (pnasnet.py:117-146):
+ * ZeroPad2d((0, 1, 0, 1)) -> [1:, 1:] -> AvgPool2d(1, stride 2) reads x[2i + 1, 2j + 1], zero past the far edge of an odd map; the
+ * ReLU is the one that opens FactorizedReduction.
+ * C, Cout multiples of 8, Cout >= C, stride 1 or 2, x / y 16-byte aligned (B2_ERR_INVALID otherwise). */
+int b2_shortcut_a_offset_ndhwc(const void* x, void* y, int N, int H, int W, int C, int stride, int offset, int relu, int Cout,
+                               void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * ResNeXt-3D (resnext3D.py:76-121)
  * ------------------------------------------------------------------------------------------- */
 /* Grouped convolution (nn.Conv3d(C, C, 3, stride, 1, groups=32), conv2 of ResNeXtBottleneck, resnext3D.py:86-93) -> BatchNorm

@@ -34,6 +34,7 @@ from .models.vgg import (alexnet, vgg11, vgg11_bn, vgg13, vgg13_bn, vgg16, vgg16
                          vgg19_bn)                          # pretorched/__init__.py (torchvision_models.py:23-31)
 from .models.resnext import resnext101_32x4d, resnext101_64x4d  # noqa: F401  (pretorched/__init__.py:14-15)
 from .models.xception import xception  # noqa: F401  (pretorched/__init__.py:47)
+from .models.pnasnet import pnasnet5large  # noqa: F401  (pretorched/__init__.py)
 from .models.trn import Relation, MultiScaleRelation, HierarchicalRelation, TRN, trn  # noqa: F401
 from .models.utils import Identity  # noqa: F401
 # BigGAN-deep generator (BASELINE.json configs[4]; not in the reference tree -- see models/biggan_deep.py)

@@ -101,6 +101,8 @@ SYMBOLS = {
     "b2_dwconv3x3_ndhwc": (c_int, [c_void_p] * 5 + [c_int] * 8 + [c_void_p]),
     "b2_relu6_inplace_ndhwc": (c_int, [c_void_p, ctypes.c_longlong, c_int, c_void_p]),
     "b2_dwconv3x3_relu_in_ndhwc": (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_void_p]),
+    "b2_dwconv_kxk_relu_in_ndhwc": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 10 + [c_void_p]),
+    "b2_shortcut_a_offset_ndhwc": (c_int, [c_void_p, c_void_p] + [c_int] * 8 + [c_void_p]),
     "b2_pack_grouped_conv_weight_elems": (ctypes.c_size_t, [c_int] * 6),
     "b2_pack_grouped_conv_weight": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
     "b2_conv_grouped_ndhwc_fprop": (c_int, [ctypes.POINTER(ConvArgs), c_int, c_void_p]),

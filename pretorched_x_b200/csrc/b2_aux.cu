@@ -440,9 +440,10 @@ __global__ void cast_kernel(const float* __restrict__ x, int ldx, __half* __rest
   y[i] = __float2half_rn(v);
 }
 
-// type-A shortcut: y[n,to,ho,wo,0:C] = x[n,to*s,ho*s,wo*s,:], y[..., C:Cout] = 0
+// type-A shortcut: y[n,to,ho,wo,0:C] = x[n,to*s,ho*s+off,wo*s+off,:] (zero where ho*s+off or wo*s+off is past the map; max(x, 0)
+// with relu), y[..., C:Cout] = 0
 __global__ void shortcut_a_kernel(const __half* __restrict__ x, __half* __restrict__ y, int T, int H, int W, int C8,
-                                  int s, int To, int Ho, int Wo, int Co8, long long total) {
+                                  int s, int off, int relu, int To, int Ho, int Wo, int Co8, long long total) {
   long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int c8 = (int)(i % Co8);
@@ -452,7 +453,14 @@ __global__ void shortcut_a_kernel(const __half* __restrict__ x, __half* __restri
   const int to = (int)(q % To);
   const long long n = q / To;
   uint4 v = make_uint4(0, 0, 0, 0);
-  if (c8 < C8) v = __ldg(reinterpret_cast<const uint4*>(x + (((n * T + (long long)to * s) * H + (long long)ho * s) * W + (long long)wo * s) * (C8 * 8)) + c8);
+  const int hi = ho * s + off, wi = wo * s + off;
+  if (c8 < C8 && hi < H && wi < W)
+    v = __ldg(reinterpret_cast<const uint4*>(x + (((n * T + (long long)to * s) * H + hi) * W + wi) * (C8 * 8)) + c8);
+  if (relu) {
+    __half2* h = reinterpret_cast<__half2*>(&v);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) h[e] = __hmax2(h[e], __float2half2_rn(0.f));
+  }
   reinterpret_cast<uint4*>(y)[i] = v;
 }
 
@@ -846,7 +854,25 @@ int b2_shortcut_a_ndhwc(const void* x, void* y, int N, int T, int H, int W, int 
   const int To = (T - 1) / stride + 1, Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
   const long long total = (long long)N * To * Ho * Wo * (Cout / 8);
   shortcut_a_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      (const __half*)x, (__half*)y, T, H, W, C / 8, stride, To, Ho, Wo, Cout / 8, total);
+      (const __half*)x, (__half*)y, T, H, W, C / 8, stride, 0, 0, To, Ho, Wo, Cout / 8, total);
+  B2_CHECK_LAUNCH("shortcut_a");
+  return B2_OK;
+}
+
+int b2_shortcut_a_offset_ndhwc(const void* x, void* y, int N, int H, int W, int C, int stride, int offset, int relu, int Cout,
+                               void* stream) {
+  B2_CHECK_ARG(x && y, "null tensor pointer");
+  B2_CHECK_ARG(N > 0 && H > 0 && W > 0, "empty input (N %d, H %d, W %d)", N, H, W);
+  B2_CHECK_ARG(stride == 1 || stride == 2, "stride %d is not 1 or 2", stride);
+  B2_CHECK_ARG(offset >= 0 && offset < stride, "offset %d is outside [0, stride %d)", offset, stride);
+  B2_CHECK_ARG(C > 0 && C % 8 == 0 && Cout % 8 == 0 && Cout >= C, "channel pitches must be multiples of 8 with Cout >= C");
+  B2_CHECK_ARG(((uintptr_t)x | (uintptr_t)y) % 16 == 0, "tensors must be 16-byte aligned");
+  int rc;
+  if ((rc = require_sm90()) != B2_OK) return rc;
+  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  const long long total = (long long)N * Ho * Wo * (Cout / 8);
+  shortcut_a_kernel<<<div_up(total, 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      (const __half*)x, (__half*)y, 1, H, W, C / 8, stride, offset, relu ? 1 : 0, 1, Ho, Wo, Cout / 8, total);
   B2_CHECK_LAUNCH("shortcut_a");
   return B2_OK;
 }

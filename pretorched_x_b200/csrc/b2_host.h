@@ -84,7 +84,8 @@ enum LastKernel : int {
   KID_SLAB_T64 = 16 /* the slab kernel's 64-wide transposed form (b2_slab_t128.cuh): info = {NP, items, R} */,
   KID_PGEMM_SPLITK = 17 /* b2_gemm_splitk_f16: info = {N tile, splits} */,
   KID_WGRAD_GROUPED = 18 /* b2_conv_wgrad_grouped: info = {channels per group, splits, position blocks} */,
-  KID_DWCONV_RELU_IN = 19 /* b2_dwconv3x3_relu_in_ndhwc: info = {stride, output columns per thread} */
+  KID_DWCONV_RELU_IN = 19 /* b2_dwconv3x3_relu_in_ndhwc: info = {stride, output columns per thread} */,
+  KID_DWCONV_KXK = 20 /* b2_dwconv_kxk_relu_in_ndhwc: info = {K, stride, pad, output columns per thread} */
 };
 void set_last_kernel(int id, int i0 = 0, int i1 = 0, int i2 = 0, int i3 = 0, int i4 = 0);
 

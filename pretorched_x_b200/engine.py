@@ -36,6 +36,7 @@ from . import ops_dual
 from . import ops_vgg
 from . import ops_grouped
 from . import ops_xception
+from . import ops_pnasnet
 from . import functions as Fn
 from .ops import Act
 
@@ -1536,6 +1537,210 @@ def run_xception_trunk(model, x):
 def run_xception_head(model, a):
     """ReLU -> adaptive mean -> view -> last_linear (xception.py:195-202) on bn4's output ``a``: the ReLU and the mean are one pass
     (b2_avgpool_global_affine_ndhwc with a unit affine), so any final map size works."""
+    dev = a.data.device
+    s, t = _cached(model, "head_unit", (a.ld, dev), lambda: ops.fold_affine(a.ld, None, None, dev))
+    return _head_on_pooled(model.last_linear, ops.avgpool_global_affine(a, s, t), a.C)
+
+
+# ---------------------------------------------------------------------------------------------
+# PNASNet-5-Large (pnasnet.py:33-369)
+# ---------------------------------------------------------------------------------------------
+# Channel layouts.  A tensor of ``seg * n`` logical channels is stored as n segments of ``seg`` channels at a pitch of ``pitch``
+# columns each (pad columns zero): a cell output is five combinations side by side, and the 54- and 108-wide combinations of the
+# stem cells sit at pitches 56 and 112 so that every segment starts on a 16-byte column.  Filters that read such a tensor get zero
+# rows at the pad columns when they are packed (``_scatter``).  Every other tensor is one dense segment.
+# A combination is the sum of two operands: its separable branch's closing pointwise GEMM adds the other operand as its residual
+# into a dense [M][pitch] matrix, which is then copied into the combination's columns of the cell output by the slice pool kernel as
+# a 1x1 window (no GEMM entry writes a column slice and adds a residual; b2_gemm_f16 stores whole rows of pitch ldd).
+def _dense_layout(C):
+    return (C, ops._round_up(C, 8), 1)
+
+
+def _scatter(w, layout, width):
+    """fp32 [rows][seg * n] -> [rows][width]: logical column c at (c // seg) * pitch + c % seg, zeros elsewhere."""
+    seg, pitch, n = layout
+    if w.shape[1] != seg * n or pitch * n != width:
+        raise ValueError("a filter over %d channels does not read the layout %s of width %d" % (w.shape[1], layout, width))
+    out = w.new_zeros((w.shape[0], width))
+    for j in range(n):
+        out[:, j * pitch:j * pitch + seg] = w[:, j * seg:(j + 1) * seg]
+    return out
+
+
+def _pn_pointwise(conv, bn, layout, width):
+    """(fp16 [K][width] filter with zero pad rows, scale, shift) of a 1x1 Conv2d + BatchNorm reading ``layout``."""
+    K = conv.weight.shape[0]
+
+    def build():
+        w = _scatter(conv.weight.detach().reshape(K, -1).float(), layout, width)
+        return (w.half().contiguous(),) + ops.fold_affine(K, None, bn, w.device)
+    return _cached(conv, "pn1x1", (_sig(conv.weight) + _sig(*_bn_tensors(bn)), layout, width), build, reads=_bn_tensors(bn))
+
+
+def _pn_unit_affine(width, dev, owner):
+    """The pre-activation GEMM's input affine for a bare ReLU: ones over ``width`` columns, zero past them up to round_up(width, 64)."""
+    def build():
+        n = ops._round_up(width, 64)
+        one = torch.zeros(n, dtype=torch.float32, device=dev)
+        one[:width] = 1.0
+        return one, torch.zeros(n, dtype=torch.float32, device=dev)
+    return _cached(owner, "pn_unit", (width, dev), build)
+
+
+def _pn_gemm(a, conv, bn, layout, relu=False, residual=None, preact=False):
+    """1x1 Conv2d + BatchNorm of ``a`` (stored in ``layout``) on the persistent GEMM: ``preact`` applies ReLU to the A operand
+    (ReluConvBn), ``relu`` to the output; ``residual`` (an Act of the output's shape) joins in the epilogue."""
+    w, scale, shift = _pn_pointwise(conv, bn, layout, a.ld)
+    K = w.shape[0]
+    if preact:
+        one, zero = _pn_unit_affine(a.ld, a.data.device, conv)
+        y = ops.gemm_preact(a.data, w, scale, shift, one, zero, a.M, K, a.ld, relu=relu)
+    else:
+        y = ops.gemm(a.data, w, scale, shift, a.M, K, a.ld, residual=residual.data if residual is not None else None, relu=relu)
+    return Act(y, a.N, 1, a.H, a.W, y.shape[1])
+
+
+def _pn_depthwise(a, conv, layout, zero_pad=False):
+    """SeparableConv2d.depthwise_conv2d of max(a, 0) (ops_pnasnet.dwconv_kxk_relu_in), the taps scattered to ``layout``.  A branch
+    built with zero_pad (ZeroPad2d((1, 0, 1, 0)) before the stride-2 convolution, [1:, 1:] after) runs at padding k // 2 - 1 with the
+    cropped extent H // 2."""
+    k, s = conv.kernel_size[0], conv.stride[0]
+    C = conv.weight.shape[0]
+    if conv.groups != C or conv.kernel_size != (k, k) or conv.stride != (s, s) or conv.padding != (k // 2, k // 2) or conv.bias is not None:
+        raise NotImplementedError("PNASNet's depthwise pass covers square k x k depthwise convolutions with padding k // 2")
+    wk = _cached(conv, "pn_dw", (_sig(conv.weight), layout, a.C),
+                 lambda: _scatter(conv.weight.detach().reshape(C, k * k).t().float(), layout, a.C).contiguous())
+    if zero_pad:
+        pad, Ho, Wo = k // 2 - 1, a.H // 2, a.W // 2
+    else:
+        pad = k // 2
+        Ho, Wo = (a.H + 2 * pad - k) // s + 1, (a.W + 2 * pad - k) // s + 1
+    return ops_pnasnet.dwconv_kxk_relu_in(a, wk, k, s, pad, Ho, Wo)
+
+
+def _pn_branch(br, a, layout, residual=None):
+    """BranchSeparables ``br`` (pnasnet.py:67-97) of ``a``: depthwise (ReLU on load) -> pointwise + bn_sep_1 + ReLU -> depthwise ->
+    pointwise + bn_sep_2 (+ ``residual``).  Returns a dense Act of the output width."""
+    sep1, sep2 = br.separable_1, br.separable_2
+    h = _pn_depthwise(a, sep1.depthwise_conv2d, layout, zero_pad=br.zero_pad is not None)
+    h = _pn_gemm(h, sep1.pointwise_conv2d, br.bn_sep_1, layout, relu=True)
+    mid = _dense_layout(sep1.pointwise_conv2d.weight.shape[0])
+    h = _pn_depthwise(h, sep2.depthwise_conv2d, mid)
+    return _pn_gemm(h, sep2.pointwise_conv2d, br.bn_sep_2, mid, residual=residual)
+
+
+def _pn_relu_conv_bn(u, a, layout):
+    """ReluConvBn (pnasnet.py:100-114): the pre-activation GEMM with a unit affine; at stride 2 the strided pixels are gathered
+    first (b2_shortcut_a_ndhwc)."""
+    s = u.conv.stride[0]
+    if u.conv.kernel_size != (1, 1) or u.conv.stride != (s, s) or s not in (1, 2):
+        raise NotImplementedError("ReluConvBn runs 1x1 convolutions at stride 1 or 2")
+    if s == 2:
+        a = ops.shortcut_a(a, 2, a.ld)
+    return _pn_gemm(a, u.conv, u.bn, layout, preact=True)
+
+
+def _pn_factorized_reduction(u, a, layout):
+    """FactorizedReduction (pnasnet.py:117-146): ReLU and the gathers x[2i, 2j] / x[2i + 1, 2j + 1] (ops_pnasnet.gather_offset), then
+    one two-operand GEMM whose filters hold path_1's rows in the first half and path_2's in the second (zeros elsewhere), with
+    final_path_bn: the concatenation of the two half-width convolutions at any half width (54 and 108 do not start on a 16-byte
+    column)."""
+    c1, c2 = u.path_1.conv, u.path_2.conv
+    h, K = c1.weight.shape[0], 2 * c1.weight.shape[0]
+
+    def build():
+        w1 = _scatter(c1.weight.detach().reshape(h, -1).float(), layout, a.ld)
+        w2 = _scatter(c2.weight.detach().reshape(h, -1).float(), layout, a.ld)
+        b1, b2 = w1.new_zeros((K, a.ld)), w1.new_zeros((K, a.ld))
+        b1[:h], b2[h:] = w1, w2
+        return (b1.half().contiguous(), b2.half().contiguous()) + ops.fold_affine(K, None, u.final_path_bn, w1.device)
+    b1, b2, scale, shift = _cached(u, "pn_fr", (_sig(c1.weight, c2.weight) + _sig(*_bn_tensors(u.final_path_bn)), layout, a.ld),
+                                   build, reads=_bn_tensors(u.final_path_bn))
+    g1 = ops_pnasnet.gather_offset(a, 2, 0, relu=True)
+    g2 = ops_pnasnet.gather_offset(a, 2, 1, relu=True)
+    y = ops.gemm(g1.data, b1, scale, shift, g1.M, K, a.ld, second=(g2.data, b2, a.ld))
+    return Act(y, g1.N, 1, g1.H, g1.W, y.shape[1])
+
+
+def _pn_pool(m, a):
+    """MaxPool (pnasnet.py:33-46) on the slice pool: the zero-pad form is the ceil-extent 3x3 pool without padding."""
+    k, s, p = m.pool.kernel_size, m.pool.stride, m.pool.padding
+    if m.zero_pad is not None:
+        return ops.pool_slice(a, k, s, 0, False)
+    return ops.pool_slice(a, k, s, p, False)
+
+
+def _pn_cell_body(cell, left, left_layout, right, right_layout):
+    """One cell (pnasnet.py:149-288): (output Act, its layout).  ``left`` / ``right``: the cell's two inputs (CellStem0: conv_0's
+    output and None)."""
+    from .models.pnasnet import CellStem0
+    stem0 = isinstance(cell, CellStem0)
+    if stem0:
+        x_left, l_lay = left, left_layout
+        x_right = _pn_relu_conv_bn(cell.conv_1x1, left, left_layout)
+    else:
+        if cell.match_prev_layer_dimensions:
+            x_left = _pn_factorized_reduction(cell.conv_prev_1x1, left, left_layout)
+        else:
+            x_left = _pn_relu_conv_bn(cell.conv_prev_1x1, left, left_layout)
+        l_lay = _dense_layout(cell.comb_iter_0_left.bn_sep_2.num_features)
+        x_right = _pn_relu_conv_bn(cell.conv_1x1, right, right_layout)
+    r_lay = _dense_layout(cell.conv_1x1.bn.num_features)
+    Cb = cell.comb_iter_1_left.bn_sep_2.num_features
+    Cp = ops._round_up(Cb, 8)
+    lay = (Cb, Cp, 1)
+    c0 = _pn_pool(cell.comb_iter_0_right.max_pool if stem0 else cell.comb_iter_0_right, x_left)
+    if stem0:
+        c0 = _pn_gemm(c0, cell.comb_iter_0_right.conv, cell.comb_iter_0_right.bn, l_lay)
+    c0 = _pn_branch(cell.comb_iter_0_left, x_left, l_lay, residual=c0)
+    out = torch.empty((c0.M, 5 * Cp), dtype=torch.float16, device=c0.data.device)
+
+    def put(j, c):
+        ops.pool_slice(Act(c.data, c.N, 1, c.H, c.W, c.ld), 1, 1, 0, False, y=out[:, j * Cp:(j + 1) * Cp])
+
+    put(0, c0)
+    put(1, _pn_branch(cell.comb_iter_1_left, x_right, r_lay, residual=_pn_pool(cell.comb_iter_1_right, x_right)))
+    c2 = _pn_branch(cell.comb_iter_2_right, x_right, r_lay)
+    put(2, _pn_branch(cell.comb_iter_2_left, x_right, r_lay, residual=c2))
+    slot2 = Act(out[:, 2 * Cp:3 * Cp], c0.N, 1, c0.H, c0.W, Cp)
+    put(3, _pn_branch(cell.comb_iter_3_left, slot2, lay, residual=_pn_pool(cell.comb_iter_3_right, x_right)))
+    r4 = x_right if cell.comb_iter_4_right is None else _pn_relu_conv_bn(cell.comb_iter_4_right, x_right, r_lay)
+    put(4, _pn_branch(cell.comb_iter_4_left, x_left, l_lay, residual=r4))
+    return Act(out, c0.N, 1, c0.H, c0.W, 5 * Cp), (Cb, Cp, 5)
+
+
+def pnasnet_stages(model, a):
+    """conv_0, cell_stem_0, cell_stem_1, cell_0 .. cell_11 of ``a`` (an NHWC Act with channel pitch 8): a list of (name, Act,
+    layout).  conv_0 (3x3, stride 2, valid) + BN runs on the slab kernel's slice entry without a ReLU."""
+    from .models.pnasnet import CELLS
+    pc = packed_conv(model.conv_0.conv, model.conv_0.bn, a.ld)
+    Ho, Wo = (a.H - 3) // 2 + 1, (a.W - 3) // 2 + 1
+    y = torch.empty((a.N * Ho * Wo, pc.K), dtype=torch.float16, device=a.data.device)
+    x0 = ops.conv_slice(a, pc, y, relu=False)
+    stages = [("conv_0", x0, _dense_layout(96))]
+    s0 = _pn_cell_body(model.cell_stem_0, x0, stages[0][2], None, None)
+    stages.append(("cell_stem_0",) + s0)
+    for name, *_ in CELLS:
+        (_, pa, pl), (_, ca, cl) = stages[-2], stages[-1]
+        stages.append((name,) + _pn_cell_body(getattr(model, name), pa, pl, ca, cl))
+    return stages
+
+
+def run_pnasnet_trunk(model, x):
+    """PNASNet-5-Large's ``features`` on the engine: fp32 NCHW 331x331 images (or an Act with channel pitch 8) in, cell_11's output
+    (an Act) out, in one frozen Function call."""
+    a = x if isinstance(x, Act) else ops.from_ncdhw(x, pitch=8)
+    if a.T != 1 or (a.H, a.W) != (331, 331):
+        # the reference's head is a fixed AvgPool2d(11): only 331x331 inputs reach it with an 11x11 map
+        raise ValueError("PNASNet-5-Large takes 331x331 images, got %r" % (a,))
+    return Fn.frozen(lambda x, o: pnasnet_stages(model, x)[-1][1], a)
+
+
+def run_pnasnet_head(model, a):
+    """ReLU -> AvgPool2d(11) -> view -> dropout (identity in eval) -> last_linear (pnasnet.py:358-364) on cell_11's output: the ReLU
+    and the mean in one pass (b2_avgpool_global_affine_ndhwc with a unit affine)."""
+    if (a.H, a.W) != (11, 11):
+        raise ValueError("PNASNet-5-Large's head pools an 11x11 map, got %r" % (a,))
     dev = a.data.device
     s, t = _cached(model, "head_unit", (a.ld, dev), lambda: ops.fold_affine(a.ld, None, None, dev))
     return _head_on_pooled(model.last_linear, ops.avgpool_global_affine(a, s, t), a.C)

@@ -1,5 +1,5 @@
 from . import (resnet3d, r2plus1d, nonlocalnet, resnet2d, resnext3d, trn, slowfast, mobilenet, senet, bninception,  # noqa: F401
-               inception, densenet, inceptionv3, polynet, vgg, resnext, xception,
+               inception, densenet, inceptionv3, polynet, vgg, resnext, xception, pnasnet,
                utils, settings)
 
 # the reference spells the module `resnet3D` (capital D); keep that import path working

@@ -14,10 +14,11 @@ from .polynet import pretrained_settings as polynet_settings          # polynet.
 from .vgg import pretrained_settings as vgg_settings                  # torchvision_models.py:64-119
 from .resnext import pretrained_settings as resnext_settings          # resnext.py:12-35 (settings.py:4,23 of the reference)
 from .xception import pretrained_settings as xception_settings      # xception.py:33-47
+from .pnasnet import pretrained_settings as pnasnet_settings        # pnasnet.py:9-30
 
 all_settings = [resnet2d_settings, resnet3d_settings, resnext3d_settings, nonlocal_settings, mobilenet_settings, senet_settings,
                 bninception_settings, inception_settings, densenet_settings, inceptionv3_settings, polynet_settings,
-                vgg_settings, resnext_settings, xception_settings]
+                vgg_settings, resnext_settings, xception_settings, pnasnet_settings]
 
 model_names = []
 pretrained_settings = {}
